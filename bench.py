@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the hot path on BASELINE.json's headline config.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 Workload (config.workload): BASELINE.json configs[1] -- PPO, synthetic 64-dim observations, 1024 actors x
 horizon 128 (n_step = stride = 128), 2x256 MLP actor + critic, clip mode, z-filter on, A = 8.
@@ -19,6 +19,11 @@ surrogate policy epochs with KL early stop -> 10 value epochs), then publish + a
 Timing: CUDA events on the launching stream, >= 3 warm-up steps, max over ranks; inputs of every step are
 freshly generated on the device (the 47 MB batch and ~60 MB of staging/replay traffic per step exceed any
 reuse window together with the explicit L2 flush between timed steps).
+--dump-outputs DIR: after the timed steps, what the last of them computed is written as DIR/<name>.npy (rank 0): the
+learner's statistics (stat_<name>, float64), parameters after the update (actor / critic / log_var / z-filter), the
+critic values, advantages and returns of its batch, and a fixed sample of 128 of the windows the overlapped rollout
+put into the replay FIFO.  Every input derives from fixed seeds (per rank), so two runs with the same arguments compute
+the same arrays and two builds can be compared array for array.
 """
 import argparse
 import copy
@@ -43,7 +48,7 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'], bf16_tflops_sustained=d.get('bf16_tflops_sustained'),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=None, source='H100 SXM data sheet (dense, 700 W)')
 
 
 def build_configs(n_actors=N_ACTORS, horizon=HORIZON):
@@ -164,7 +169,7 @@ def run_ours(args):
     dev = torch.device('cuda', local)
     if world > 1:
         # small messages (600 KB gradients, scalars): a few channels are plenty, and a collective kernel must always
-        # find free SMs next to the persistent rollout kernel (128 of 148 SMs) and the other branch's collective
+        # find free SMs next to the persistent rollout kernel (128 of 132 SMs) and the other branch's collective
         os.environ.setdefault('NCCL_MAX_NCHANNELS', '4')
         dist.init_process_group('nccl', device_id=dev)
     import __graft_entry__
@@ -179,14 +184,24 @@ def run_ours(args):
     from surreal_b200.replay import FIFOReplay
     from surreal_b200.distributed import LocalHub
     _lib.lib()
+    # identical inputs from run to run: the initial weights come from the global RNGs
+    import random
+    import numpy as np
+    random.seed(rank)
+    np.random.seed(rank)
+    torch.manual_seed(rank)
     lc, ec, sc = build_configs(N_ACTORS, HORIZON)
     ec.seed = rank
     la = SurrealDefaultLauncher(PPOAgent, PPOLearner, FIFOReplay, sc, ec, lc)
     agent, replay, learner = la.setup_engine()
+    # the launcher seeds numpy from the clock before it builds the agent (as the reference does), so the per-actor noise
+    # constants are redrawn here from a fixed seed, with the agent's own distribution
+    r = float(lc.algo.consts.log_sig_range)
+    agent.set_noise(np.random.default_rng(1000 + rank).uniform(-r, r, N_ACTORS))
     if world > 1:
         learner.enable_data_parallel(dist.group.WORLD)
     N, T, D, A = N_ACTORS, HORIZON, OBS_DIM, ACT_DIM
-    flush = torch.empty(192 * 1024 * 1024 // 4, device=dev)       # > 126 MB L2
+    flush = torch.empty(192 * 1024 * 1024 // 4, device=dev)       # > 50 MB L2
     launches = {'n': 0}
 
     from surreal_b200.launch import PipelinedEngine
@@ -198,7 +213,7 @@ def run_ours(args):
 
     def seq_step():
         agent.main_loop(max_steps=T)
-        learner.main_loop()
+        return learner.main_loop()
 
     one_step = eng.step if eng is not None else seq_step
     tstream = eng.sL if eng is not None else torch.cuda.current_stream()
@@ -217,18 +232,21 @@ def run_ours(args):
     torch.cuda.synchronize()
     clocks.start()
     t_wall0 = time.time()
+    last_stats = None
     for _ in range(args.steps):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         with torch.cuda.stream(tstream):
             flush.fill_(1.0)                                      # L2 flush between timed iterations
             e0.record()
-        one_step()
+        last_stats = one_step()
         with torch.cuda.stream(tstream):
             e1.record()
         times.append((e0, e1))
     torch.cuda.synchronize()
     t_wall = time.time() - t_wall0
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, agent, replay, learner, last_stats)
     ms = [a.elapsed_time(b) for a, b in times]
     total_ms = sum(ms)
     if world > 1:
@@ -295,8 +313,8 @@ def run_ours(args):
     roof_critic = None
     if 'sb200_mlp_forward_tc5_f32' in per_step:
         roof_critic = mlp_roof('sb200_mlp_forward_tc5_f32', rows, 1,
-                               'tc5_prep_kernel + mlp3_tc5_kernel (fused critic pass over %d rows: tcgen05.mma kind::tf32 tiles of '
-                               '128 rows, accumulators in TMEM, weight images streamed by the TMA engine, 3xTF32)' % rows)
+                               'tc5_prep_kernel + mlp3_wgmma_kernel (fused critic pass over %d rows: wgmma tf32 tiles of 128 rows, '
+                               'accumulators in registers, weight images streamed by the TMA engine, 3xTF32)' % rows)
         roof_critic['note'] = ('fp32-accurate 3xTF32: every algorithmic product is 3 tensor-core MMAs, so the tensor pipe executes 3x '
                                'the algorithmic FLOP counted here; denominator = measured dense bf16 peak (the mandated one), the '
                                'tf32 pipe peaks at half of it')
@@ -311,7 +329,7 @@ def run_ours(args):
         flop = 2.0 * N * T * (w_params + HIDDEN[1] * A + D * (D + A))          # policy forward + env step, all T steps
         byts = N * T * (D + 3 * A + 2) * 4 + 2 * N * ((T + 1) * D + 3 * T * A + 2 * T) * 4   # staging writes + window copy
         ach = flop / (avg_ms / 1e3) / 1e12
-        ffma_peak = 148 * 128 * 2 * 1.9e9 / 1e12
+        ffma_peak = 67.0                                                     # H100 SXM data sheet, FP32
         roof_roll = {'kernel': 'ppo_rollout2_kernel (persistent: %d env steps of %d actors per launch; 4-CTA clusters, '
                                'resident weights, warp-specialised env warps, st.async / mbarrier DSMEM hand-offs)' % (T, N),
                      'bound': 'tensor', 'achieved': ach, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s',
@@ -321,10 +339,9 @@ def run_ours(args):
                      'fp32_ffma_peak_tflops': ffma_peak, 'frac_of_fp32_ffma_peak': ach / ffma_peak,
                      'peak_source': peaks['source'],
                      'note': 'fp32 FFMA by necessity (1e-5 parity with the fp32 reference); the dense-bf16 tensor peak is '
-                             'the mandated denominator, the fp32 FFMA ceiling (148 SMs x 128 lanes x 2 x 1.9 GHz) the '
-                             'meaningful one (tools/fma_bench.cu measures 127 FMA/clk/SM for FFMA and FFMA2 alike).  Per '
-                             'step the kernel is a dependent chain: layer -> hand-off -> layer -> hand-off -> '
-                             'head / sample / env -> hand-off (profiles/r02b_rollout_trace_*.txt)'}
+                             'the mandated denominator, the fp32 FFMA ceiling (H100 SXM data sheet, 67 TFLOP/s) the '
+                             'meaningful one.  Per step the kernel is a dependent chain: layer -> hand-off -> layer -> '
+                             'hand-off -> head / sample / env -> hand-off'}
     # dram__bytes_read.sum + dram__bytes_write.sum per launch, from one `ncu --set full` capture each (profiles/)
     if roof_roll is not None:
         roof_roll['traffic'] = load_profile_traffic('rollout')
@@ -479,6 +496,33 @@ def run_extras(dev, peaks, flush):
                                    'batch_1M_frac_of_hbm_peak': big * (2 * rec + 8) / (big_ms / 1e3) / 1e9 / peaks['hbm_gbs'],
                                    'peak': peaks['hbm_gbs'], 'unit': 'GB/s'}}
     return out
+
+
+def dump_outputs(out_dir, agent, replay, learner, stats):
+    """--dump-outputs: the arrays the last timed step produced, float32 (float64 for the statistics), < 64 MB in all."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+
+    def save(name, t):
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        np.save(os.path.join(out_dir, name + '.npy'), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
+    for k, v in sorted((stats or {}).items()):
+        if isinstance(v, (int, float)):
+            save('stat_' + k.lstrip('_'), np.float64(v))
+    m = learner.model
+    save('actor_params', m.actor.params)
+    save('critic_params', m.critic.params)
+    save('log_var', m.log_var)
+    if m.z_stats is not None:
+        save('z_stats', m.z_stats)
+    save('values', learner._values)
+    save('advantages', learner._adv)
+    save('returns', learner._ret)
+    idx = torch.randperm(replay.r_obs.shape[0], generator=torch.Generator().manual_seed(0))[:128].to(replay.r_obs.device)
+    for name in ('r_obs', 'r_act', 'r_pd', 'r_rew', 'r_done'):
+        save('window_' + name[2:], getattr(replay, name).index_select(0, idx))
 
 
 def dp_parity_check(learner, dev, rank, world):
@@ -862,7 +906,9 @@ if __name__ == '__main__':
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', type=str, default='ours', choices=['ours', 'reference'])
     ap.add_argument('--sequential', action='store_true', help='rollout then learn on one stream (no actor/learner overlap)')
-    ap.add_argument('--lite', action='store_true', help='skip the e2e and CPU-baseline legs (profiling runs under ncu)')
+    ap.add_argument('--lite', action='store_true', help='skip the e2e and CPU-baseline legs')
+    ap.add_argument('--dump-outputs', type=str, default=None, metavar='DIR',
+                    help='write what the last timed step computed to DIR/<name>.npy')
     ap.add_argument('--workload', type=str, default='cfg2', choices=['cfg2', 'cfg5'],
                     help='cfg2: BASELINE configs[1] (the metric; weak scaling).  cfg5: configs[4], 4096 actors x horizon 256 in total, '
                          'sharded over the ranks (strong scaling; use with --lite)')

@@ -1,4 +1,4 @@
-/* libsurreal_b200 -- C-ABI of the B200-native actor -> replay -> learner hot path.
+/* libsurreal_b200 -- C-ABI of the H100-native actor -> replay -> learner hot path.
  *
  * The reference (SurrealAI/surreal) is pure Python and has NO FFI / operator registry: its plugin
  * surface is three Python base classes (Agent / Replay / Learner, SURVEY.md §8b).  This header is
@@ -35,7 +35,7 @@ extern "C" {
 #define SB200_MAX_LAYERS 4
 
 int sb200_version(void);
-/* One-time per-process setup on the current device (kernel attributes); fails on non-sm_100 devices.
+/* One-time per-process setup on the current device (kernel attributes); fails on devices other than sm_90 (H100).
  * Must run before any compute entry (and before CUDA-graph capture). */
 int sb200_init(void);
 const char* sb200_status_string(int status);
@@ -109,11 +109,11 @@ size_t sb200_mlp_pack_floats(const sb200_mlp* net);
 int sb200_mlp_pack_tf32(const sb200_mlp* net, float* packed, void* stream);
 int sb200_mlp_forward_packed_f32(const sb200_mlp* net, const float* packed, const sb200_zfilter* zf,
                                  const sb200_rows* in, float* out, int64_t ld_out, void* stream);
-/* Blackwell-native large-batch forward (csrc/mlp_fwd_tc5.cu): tcgen05.mma kind::tf32 tiles of 128 rows with the
- * accumulators in tensor memory, weights streamed by the TMA engine (cp.async.bulk), 3xTF32 split for fp32-level
+/* Hopper large-batch forward (csrc/mlp_fwd_tc5.cu): wgmma tf32 tiles of 128 rows (two warpgroups of 64) with the
+ * accumulators in registers, weights streamed by the TMA engine (cp.async.bulk), 3xTF32 split for fp32-level
  * accuracy, both hidden layers and the narrow head fused in one persistent kernel (one CTA per SM).  The critic pass of
  * PPOLearner._gae_and_return (ppo.py:376-387: B*(n+1) rows through D-256-256-1) is its customer.
- *   supported: 3 layers, ReLU-ReLU-any, dims[0] a multiple of 32 up to 256, dims[1] multiple of 32 and dims[2] multiple of 64 (both
+ *   supported: 3 layers, ReLU-ReLU-any, dims[0] a multiple of 32 up to 256, dims[1] and dims[2] multiples of 32 (both
  *     <= 256), dims[3] <= 8, no aux input, rows >= 128.  Returns 1 / 0.
  *   workspace_bytes: caller-owned scratch for the per-call weight images (hi / lo planes in operand layout); 0 when
  *     unsupported.  One workspace must not be shared by calls that may run concurrently.

@@ -1,6 +1,6 @@
 """ctypes binding of libsurreal_b200.so (the C-ABI declared in include/surreal_b200.h).
 
-The library is built in-tree by ``surreal_b200/build.py`` (nvcc, sm_100a).  There is NO fallback:
+The library is built in-tree by ``surreal_b200/build.py`` (nvcc, sm_90a).  There is NO fallback:
 if the shared object is missing or a kernel call fails, an exception is raised.
 """
 import ctypes as C

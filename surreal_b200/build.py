@@ -1,4 +1,4 @@
-"""Build libsurreal_b200.so in-tree with nvcc for sm_100a (no torch headers: pure C-ABI)."""
+"""Build libsurreal_b200.so in-tree with nvcc for sm_90a (no torch headers: pure C-ABI)."""
 import glob
 import hashlib
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libsurreal_b200.so')
 STAMP = LIB + '.stamp'      # source digest the .so was built from: git-ignored, travels with the .so to the GPU box
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-Xptxas', '-v']
 
 
@@ -54,7 +54,7 @@ def build(force=False, verbose=False):
         fp.write('\n'.join(log))
     if verbose:
         print('\n'.join(log))
-    subprocess.check_call([NVCC, '-shared', '-o', LIB] + objs + ['-lcudart'])
+    subprocess.check_call([NVCC, '-shared'] + FLAGS[:2] + ['-o', LIB] + objs + ['-lcudart'])
     with open(STAMP, 'w') as fp:
         fp.write(dig)
     return LIB

@@ -35,8 +35,8 @@ extern "C" int sb200_init(void) {
     SB200_CUDA(cudaGetDevice(&dev));
     cudaDeviceProp prop;
     SB200_CUDA(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 10) {
-        fprintf(stderr, "[surreal_b200] built for sm_100a (B200); found compute capability %d.%d\n", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        fprintf(stderr, "[surreal_b200] built for sm_90a (H100); found compute capability %d.%d\n", prop.major, prop.minor);
         return SB200_ERR_UNSUPPORTED;
     }
     int rc = sb200_mlp_fwd_init();

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libsurreal_b200 (sm_100a only).
+// Shared device/host helpers for libsurreal_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,6 +6,11 @@
 #include "../../include/surreal_b200.h"
 
 #define SB200_THREADS 256
+
+// c + a * b on a pair of fp32 lanes: two IEEE fmas (sm_90 has no packed fp32 fma)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+    return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
 
 extern unsigned long long g_sb200_launches;     // kernels launched by this library (api.cu)
 

@@ -253,8 +253,8 @@ __device__ __forceinline__ void rb_gemm(const float* __restrict__ As, int lda, i
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const float2 aa = make_float2(av[i], av[i]);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w[i].x, w[i].y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w[i].z, w[i].w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w[i].x, w[i].y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w[i].z, w[i].w), acc[r][1]);
             }
         }
 #pragma unroll
@@ -1257,7 +1257,7 @@ int e2_grid(const sb200_epochs* a) {
     static int n_sm = 0;
     if (n_sm == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 132;
     }
     int g = (a != nullptr && a->grid >= 1) ? a->grid : n_sm;
     g = std::min(g, n_sm);

@@ -13,7 +13,7 @@
 namespace {
 
 constexpr int GAE_WARPS = 8;
-constexpr int GAE_MAX_GRID = 1184;          // persistent grid: 148 SMs x 8 resident CTAs
+constexpr int GAE_MAX_GRID = 1056;          // persistent grid: 132 SMs x 8 resident CTAs
 constexpr int GAE_FUSED_NORM_MAX = 16384;   // up to here the last CTA normalises alone (one launch); above: a parallel pass
 
 struct GaeWs {
@@ -255,7 +255,7 @@ static int gae_resident_ctas(int n, size_t smem) {
     static int cache[5] = {0, 0, 0, 0, 0};
     if (n_sm == 0) {
         int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 148;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 132;
     }
     const int cls = (n == 32) ? 1 : (n == 64) ? 2 : (n == 128) ? 3 : (n == 256) ? 4 : 0;
     if (cache[cls] == 0) {

@@ -135,7 +135,7 @@ extern "C" int sb200_rows_zfilter_f32(const float* x, int64_t row_stride, int64_
     SB200_REQUIRE(x && out && B >= 1 && L >= 1 && D >= 1 && ldo >= D);
     const long long total = (long long)B * L * D;
     int grid = (int)((total + 255) / 256);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     rows_zfilter_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, row_stride, batch_stride, B, L, D, zf_stats, (float)eps, out, ldo);
     return sb200_launch_status();
 }

@@ -757,8 +757,8 @@ static int mlp_forward_impl(const sb200_mlp* net, const sb200_zfilter* zf, const
     if (force_tm == 1 && fits(8, 64)) return launch_fwd<1, 64>(p, maxw, st);
     // largest row tile that still yields >= ~1 CTA per SM; small batches take 16-row tiles with 64-row W stages
     const long long want = 120;
-    // measured on B200 (tools/bench_kernels.py critic): 32-row tiles at 2 CTAs/SM (16 warps hide the LDS->FFMA
-    // dependency chains) beat 64-row tiles at 1 CTA/SM: 800 us vs 914 us on the 132 096-row critic pass
+    // 32-row tiles at 2 CTAs/SM (16 warps hide the LDS->FFMA dependency chains) before 64-row tiles at 1 CTA/SM
+    // (tools/bench_kernels.py critic times both)
     if (fits(32, 16) && (p.rows + 31) / 32 >= 2 * want) return launch_fwd<4, 16>(p, maxw, st);
     if (fits(64, 16) && (p.rows + 63) / 64 >= want) return launch_fwd<8, 16>(p, maxw, st);
     if (fits(32, 16) && (p.rows + 31) / 32 >= want) return launch_fwd<4, 16>(p, maxw, st);

@@ -3,12 +3,11 @@
 // fp32 accumulate), which restores fp32-level accuracy (~1e-6 relative) -- plain TF32 (~1e-3) would miss the 1e-5
 // parity bar.  Included by mlp_fwd.cu (shares FwdParams / apply_act / round_up).
 //
-// Why mma.sync and not tcgen05 here: these are skinny problems.  One env step of all actors is 1024 rows, a learner
-// minibatch 1024-4096 rows; a tcgen05 tile is 128 rows issued by one thread with TMEM allocation and mbarrier
-// hand-offs, which would leave >130 SMs idle and add microseconds of fixed latency to a kernel whose whole budget is
-// a few microseconds.  m16n8k8 fragments give 16-row tiles, and -- the point of the exercise -- the A fragments are
+// Why mma.sync and not wgmma here: these are skinny problems.  One env step of all actors is 1024 rows, a learner
+// minibatch 1024-4096 rows; a wgmma tile is 64 rows per warpgroup fed through an mbarrier pipeline, which would leave
+// most SMs idle and add microseconds of fixed latency to a kernel whose whole budget is a few microseconds.  m16n8k8 fragments give 16-row tiles, and -- the point of the exercise -- the A fragments are
 // DISTRIBUTED over the lanes of a warp, so the activation rows are read from shared memory once per warp instead of
-// once per thread (the FFMA version was bound by exactly that LDS return traffic; see profiles/).
+// once per thread (the FFMA version was bound by exactly that LDS return traffic).
 //
 // Tile: CTA = 8 warps, BM = 16*MT rows; warp w owns output columns [n0 + 32w, n0 + 32w + 32) of a 256-column pass
 // (4 n-tiles) for all MT m-tiles.  B fragments (weights, kernel layout W[k][n]) are loaded straight from L2 into a

@@ -1,9 +1,8 @@
 // Inference forward for SMALL batches (one env step of all co-located actors: ~1K rows) on pre-packed weights.
 //
-// At this size the forward is a chain of dependent latencies, not a throughput problem.  ncu on the earlier
-// variants (profiles/r01c_small_forward.md): two warps per scheduler, each retiring one instruction per ~5
-// cycles, every CTA pulling ALL the weights (330 KB) through a register ring that keeps only ~24 KB in flight
-// per SM -- the L2 round trip, not bandwidth or math, sets the time.  This kernel attacks exactly that:
+// At this size the forward is a chain of dependent latencies, not a throughput problem: in the earlier variants
+// every CTA pulled ALL the weights (330 KB) through a register ring that keeps only ~24 KB in flight per SM --
+// the L2 round trip, not bandwidth or math, sets the time.  This kernel attacks exactly that:
 //   * a thread-block CLUSTER of 4 CTAs owns 32 rows; each CTA computes a QUARTER of every layer's output
 //     columns, so it needs only a quarter of the weights (~80 KB for 64-256-256), and it fetches that slice
 //     with cp.async in one burst at kernel entry -- the whole slice is in flight at once and then RESIDENT in

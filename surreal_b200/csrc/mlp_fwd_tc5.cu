@@ -1,41 +1,40 @@
-// Blackwell-native fused MLP forward for LARGE row counts (the critic pass of _gae_and_return, ppo.py:376-387:
-// B*(n+1) = 132 096 rows through 64 -> 256 -> 256 -> 1): tcgen05.mma (kind::tf32) with accumulators in tensor
-// memory, operands staged in shared memory, weights streamed by the TMA engine (cp.async.bulk + mbarrier), fp32-level
-// accuracy through the 3xTF32 split (x = hi + lo;  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi, fp32 accumulate).
+// Tensor-core fused MLP forward for LARGE row counts (the critic pass of _gae_and_return, ppo.py:376-387:
+// B*(n+1) = 132 096 rows through 64 -> 256 -> 256 -> 1) on Hopper: wgmma (tf32, fp32 accumulators in registers), weights
+// streamed by the TMA engine (cp.async.bulk + mbarrier ring), fp32-level accuracy through the 3xTF32 split
+// (x = hi + lo;  a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi, fp32 accumulate).
 //
-// One persistent CTA per SM walks 128-row tiles.  Per tile both hidden layers are a sequence of K-chunks of 32:
+// One persistent CTA per SM walks 128-row tiles; each of its two consumer warpgroups owns 64 rows of the tile, and the two
+// share every weight stage.  A stage is one K-chunk of 32 of one column half (128 columns) of a layer's weights, hi and lo
+// planes (2 x 16 KB), copied from a per-call "image" of the weights (already in the SWIZZLE_128B K-major operand layout,
+// built by tc5_prep_kernel from the flat parameter buffer).  Per tile:
 //
-//     chunk c:  A_c [128 rows x 32 k] (hi, lo planes)   x   B_c [N x 32 k] (hi, lo planes)   -> 12 tcgen05.mma (M128 N256 K8)
+//   layer 1:  A = z-filtered observation columns, loaded from global memory straight into the wgmma A-fragment
+//             registers and split there                                     -> acc1 (128 registers: 64 rows x 256 columns)
+//   layer 2:  A = relu(acc1 + b1), taken from the accumulator registers as they are: the accumulator holds columns
+//             8i + 2t, 8i + 2t + 1 where the A fragment wants k = t, t + 4, so the layer-2 weight image stores each group
+//             of 8 k in the order (0 2 4 6 1 3 5 7) and the two agree      -> acc2 (64 registers, one column half at a time)
+//   head   :  relu(acc2 + b2) . W3 + b3 on the CUDA cores after each column half, quad-reduced by shuffles (n_out <= 8)
 //
-//   layer 1:  A_c = z-filtered observation columns, split on the fly by the producer warps        -> accumulator 1 (TMEM cols 0..255)
-//   layer 2:  A_c = relu(accumulator 1 + b1) columns 32c.., read back with tcgen05.ld, split      -> accumulator 2 (TMEM cols 256..511)
-//   head   :  relu(accumulator 2 + b2) . W3 + b3 on the CUDA cores of the epilogue warps (n_out <= 8 columns)
-//
-// B_c comes from a per-call "image" of the weights (hi / lo planes, already in the SWIZZLE_128B operand layout, built by
-// tc5_prep_kernel from the flat parameter buffer) with one 32 KB bulk copy per plane.  Two 96 KB stages
-// {A_hi, A_lo, B_hi, B_lo} form the ring; chunk q uses stage q & 1.
-//
-// Warp roles (12 warps): 0 = weight loader (one lane), 1 = MMA issuer (one lane), 2 = TMEM allocator, 3 = idle,
-// 4..11 = producer / epilogue warps (warp % 4 selects the TMEM lane quarter a warp may read; every warp converts a slice of
-// every operand chunk).
+// 8 warps = two consumer warpgroups; thread 0 also issues the bulk copies that refill the ring.
 //
 // Algorithmic HBM bytes per row: 4*D read + 4*n_out written; weights (640 KB of images per call) stay in L2.
 #include "common.cuh"
-#include "tc5.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-using namespace tc5;
+using namespace wg;
 
-constexpr int TM = 128;                    // rows per tile (UMMA M)
+constexpr int TM = 128;                    // rows per tile: 64 per consumer warpgroup
 constexpr int KC = 32;                     // k per chunk = one 128-byte swizzle row
-constexpr int MAXN = 256;                  // widest hidden layer (UMMA N <= 256)
+constexpr int MAXN = 256;                  // widest hidden layer
+constexpr int HN = 128;                    // columns per wgmma (one half of the widest layer)
 constexpr int MAX_OUT = 8;
-constexpr int A_PLANE = TM * 128;          // 16 KB
-constexpr int B_PLANE = MAXN * 128;        // 32 KB
-constexpr int STAGE_BYTES = 2 * A_PLANE + 2 * B_PLANE;     // 96 KB
-constexpr int NTHREADS = 384;
-constexpr int EPI_WARP0 = 4;
+constexpr int B_PLANE = MAXN * 128;        // 32 KB: one plane of one chunk of the image
+constexpr int HALF_PLANE = HN * 128;       // 16 KB: one column half of it
+constexpr int STAGE_BYTES = 2 * HALF_PLANE;            // hi | lo
+constexpr int NSTAGE = 6;
+constexpr int NTHREADS = 256;
 constexpr int MAX_K0 = 256;
 
 struct Tc5Params {
@@ -59,32 +58,20 @@ struct Tc5Params {
     long long n_tiles;
 };
 
-// Optional timeline trace (harness builds with -DTC5_TRACE): CTA 0 stamps clock64() at pipeline events of its first tiles.
-#ifdef TC5_TRACE
-__device__ long long g_tc5_trace[4096];
-#define TC5_STAMP(slot) do { if (blockIdx.x == 0 && (slot) < 4096) g_tc5_trace[(slot)] = clock64(); } while (0)
-#else
-#define TC5_STAMP(slot) do { } while (0)
-#endif
-// trace slots: role*1024 + (tile_iter*NC + chunk)*4 + event;  role 0 = loader, 1 = mma, 2 = producer warp 0, 3 = head (per tile)
-
 struct SmemSmall {
-    uint64_t full[2], empty[2];
-    uint64_t acc1_full, acc2_full, acc1_empty, acc2_empty;
-    uint32_t tmem_base;
-    uint32_t pad_;
+    uint64_t full[NSTAGE], empty[NSTAGE];
     alignas(16) float zmean[MAX_K0];
     alignas(16) float zstd[MAX_K0];
-    alignas(16) float b1[MAXN];
-    alignas(16) float b2[MAXN];
-    alignas(16) float w3[MAXN * MAX_OUT];
+    alignas(16) float b1[MAXN];             // zero past N1
+    alignas(16) float b2[MAXN];             // zero past N2
+    alignas(16) float w3[MAXN * MAX_OUT];   // w3[col][8], zero-padded
     float b3[MAX_OUT];
-    float part[2][TM * MAX_OUT];
 };
 
 // ---- weight images ------------------------------------------------------------------------------------------------------
 // W is the kernel layout [K][ldw] (k-major rows, n contiguous).  Chunk c of a layer covers k in [32c, 32c+32); its image is
-// the operand tile B[n][kk] = W[32c + kk][n] in the SWIZZLE_128B K-major layout, as a hi plane and a lo plane.
+// the operand tile B[n][kk] = W[32c + kk'][n] in the SWIZZLE_128B K-major layout, as a hi plane and a lo plane, rows past N
+// zero.  Layer 1: kk' = kk.  Layer 2: within each group of 8, kk' = (0 2 4 6 1 3 5 7)[kk % 8] (see the header comment).
 __global__ void __launch_bounds__(256) tc5_prep_kernel(const float* __restrict__ W1, int ldw1, int K0, int N1,
                                                        const float* __restrict__ W2, int ldw2, int N2,
                                                        unsigned char* __restrict__ img) {
@@ -98,18 +85,19 @@ __global__ void __launch_bounds__(256) tc5_prep_kernel(const float* __restrict__
         const float* W = l1 ? W1 : W2;
         const int ldw = l1 ? ldw1 : ldw2;
         const int N = l1 ? N1 : N2;
-        const int k0 = (l1 ? c : c - NC1) * KC + c16 * 4;
-        float4 hi = make_float4(0.f, 0.f, 0.f, 0.f), lo = hi;
+        const int kb = (l1 ? c : c - NC1) * KC;
+        int k[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) k[j] = l1 ? kb + c16 * 4 + j : kb + (c16 >> 1) * 8 + 2 * j + (c16 & 1);
+        uint32_t hi[4] = {0u, 0u, 0u, 0u}, lo[4] = {0u, 0u, 0u, 0u};
         if (n < N) {
-            split_tf32(W[(long long)(k0 + 0) * ldw + n], hi.x, lo.x);
-            split_tf32(W[(long long)(k0 + 1) * ldw + n], hi.y, lo.y);
-            split_tf32(W[(long long)(k0 + 2) * ldw + n], hi.z, lo.z);
-            split_tf32(W[(long long)(k0 + 3) * ldw + n], hi.w, lo.w);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) split_tf32(W[(long long)k[j] * ldw + n], hi[j], lo[j]);
         }
         unsigned char* base = img + (size_t)c * 2 * B_PLANE;
         const uint32_t off = sw128_off((uint32_t)n, (uint32_t)(c16 * 4));
-        *reinterpret_cast<float4*>(base + off) = hi;
-        *reinterpret_cast<float4*>(base + B_PLANE + off) = lo;
+        *reinterpret_cast<uint4*>(base + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+        *reinterpret_cast<uint4*>(base + B_PLANE + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     }
 }
 
@@ -122,39 +110,42 @@ __device__ __forceinline__ const float* row_ptr(const Tc5Params& p, long long r)
     return p.x + r * p.ldx;
 }
 
-__global__ void __launch_bounds__(NTHREADS, 1) mlp3_tc5_kernel(const __grid_constant__ Tc5Params p) {
+// the three products of one k-slice, small terms first; `first` starts the accumulator
+__device__ __forceinline__ void mma3(float (&d)[64], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint64_t bh, uint64_t bl,
+                                     bool first) {
+    wgmma_m64n128k8_tf32_rs(d, al[0], al[1], al[2], al[3], bh, first ? 0u : 1u);
+    wgmma_m64n128k8_tf32_rs(d, ah[0], ah[1], ah[2], ah[3], bl, 1u);
+    wgmma_m64n128k8_tf32_rs(d, ah[0], ah[1], ah[2], ah[3], bh, 1u);
+}
+
+// MO: output columns the head keeps per row (1 for the critic, MAX_OUT otherwise)
+template <int MO>
+__global__ void __launch_bounds__(NTHREADS, 1) mlp3_wgmma_kernel(const __grid_constant__ Tc5Params p) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // stage s: [A_hi | A_lo | B_hi | B_lo]; the 1024-byte alignment of every plane is what the swizzle relies on
     unsigned char* stage_base = smem_raw;
     if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();      // the dynamic segment must start 1024-aligned (no static smem here)
-    SmemSmall* sm = reinterpret_cast<SmemSmall*>(stage_base + 2 * STAGE_BYTES);
+    SmemSmall* sm = reinterpret_cast<SmemSmall*>(stage_base + NSTAGE * STAGE_BYTES);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NC1 = p.K0 / KC, NC2 = p.N1 / KC, NC = NC1 + NC2;
+    const int NC1 = p.K0 / KC, NC2 = p.N1 / KC;
+    const int nh1 = (p.N1 + HN - 1) / HN, nh2 = (p.N2 + HN - 1) / HN;
 
     // ---- one-time setup ---------------------------------------------------------------------------------------------
     if (tid == 0) {
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&sm->full[s], 9);            // 8 producer warps (operand A slices) + the loader's arrive.expect_tx (B bytes)
-            mbar_init(&sm->empty[s], 1);           // tcgen05.commit
+        for (int s = 0; s < NSTAGE; ++s) {
+            mbar_init(&sm->full[s], 1);            // thread 0's arrive.expect_tx (both planes' bytes)
+            mbar_init(&sm->empty[s], 8);           // every consumer warp, after its wgmmas on the stage completed
         }
-        mbar_init(&sm->acc1_full, 1);
-        mbar_init(&sm->acc2_full, 1);
-        mbar_init(&sm->acc1_empty, 8);             // all 8 producer / epilogue warps
-        mbar_init(&sm->acc2_empty, 8);
         mbar_init_fence();
     }
-    if (warp == 2) tmem_alloc(&sm->tmem_base, 512);
-    for (int i = tid; i < p.N1; i += NTHREADS) sm->b1[i] = p.b1[i];
-    for (int i = tid; i < p.N2; i += NTHREADS) sm->b2[i] = p.b2[i];
-    if (p.n_out == 1) {
-        for (int i = tid; i < p.N2; i += NTHREADS) sm->w3[i] = p.W3[(long long)i * p.ldw3];            // w3[col]
-    } else {
-        for (int i = tid; i < p.N2 * MAX_OUT; i += NTHREADS) {                                          // w3[col][8], zero-padded
-            const int k = i / MAX_OUT, o = i - k * MAX_OUT;
-            sm->w3[i] = (o < p.n_out) ? p.W3[(long long)k * p.ldw3 + o] : 0.0f;
-        }
+    for (int i = tid; i < MAXN; i += NTHREADS) {
+        sm->b1[i] = (i < p.N1) ? p.b1[i] : 0.0f;
+        sm->b2[i] = (i < p.N2) ? p.b2[i] : 0.0f;
     }
-    if (tid < p.n_out) sm->b3[tid] = p.b3[tid];
+    for (int i = tid; i < MAXN * MAX_OUT; i += NTHREADS) {
+        const int k = i / MAX_OUT, o = i - k * MAX_OUT;
+        sm->w3[i] = (k < p.N2 && o < p.n_out) ? p.W3[(long long)k * p.ldw3 + o] : 0.0f;
+    }
+    if (tid < MAX_OUT) sm->b3[tid] = (tid < p.n_out) ? p.b3[tid] : 0.0f;
     if (p.zf != nullptr) {
         const float cnt = p.zf[2 * p.K0];
         for (int k = tid; k < p.K0; k += NTHREADS) {
@@ -164,234 +155,164 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp3_tc5_kernel(const __grid_cons
             sm->zstd[k] = 1.0f / fmaxf(sqrtf(var), p.zf_eps);       // reciprocal: the filter multiplies (1 ulp vs the division)
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sm->tmem_base;
-    const uint32_t acc1 = tmem, acc2 = tmem + 256;
     const long long my_tiles = (p.n_tiles > (long long)blockIdx.x) ? (p.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
-    if (warp == 0) {
-        // ================= weight loader: one bulk copy per plane per chunk =================
-        if (lane == 0) {
-            const uint32_t bytes1 = (uint32_t)p.N1 * 128u, bytes2 = (uint32_t)p.N2 * 128u;
-            long long q = 0;
-            for (long long it = 0; it < my_tiles; ++it) {
-                for (int c = 0; c < NC; ++c, ++q) {
-                    const int s = (int)(q & 1);
-                    const uint32_t u = (uint32_t)(q >> 1);
-                    TC5_STAMP(0 * 1024 + (int)q * 4 + 0);
-                    mbar_wait(&sm->empty[s], (u & 1u) ^ 1u);
-                    TC5_STAMP(0 * 1024 + (int)q * 4 + 1);
-                    const uint32_t bytes = (c < NC1) ? bytes1 : bytes2;
-                    unsigned char* st = stage_base + (size_t)s * STAGE_BYTES + 2 * A_PLANE;
-                    const unsigned char* src = p.wimg + (size_t)c * 2 * B_PLANE;
-                    mbar_arrive_expect_tx(&sm->full[s], 2 * bytes);
-                    bulk_g2s(st, src, bytes, &sm->full[s]);
-                    bulk_g2s(st + B_PLANE, src + B_PLANE, bytes, &sm->full[s]);
-                }
-            }
-        }
+    // ================= consumer warpgroups =================
+    const int wgi = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
+    float acc1[2][64];
+    float acc2[64];
+    // stage q of this CTA: tile q / QT; within a tile, layer 1 runs chunk-major (c, h) and layer 2 half-major (h, c)
+    const int QT = NC1 * nh1 + nh2 * NC2;
+    const long long n_stages = my_tiles * QT;
+    // thread 0 also feeds the ring: stage q + NSTAGE goes into the slot stage q leaves, once all 8 consumer warps left it
+    auto load = [&](long long qq) {
+        const int r = (int)(qq % QT);
+        const int chunk = (r < NC1 * nh1) ? r / nh1 : NC1 + (r - NC1 * nh1) % NC2;
+        const int h = (r < NC1 * nh1) ? r % nh1 : (r - NC1 * nh1) / NC2;
+        const int s = (int)(qq % NSTAGE);
+        unsigned char* st = stage_base + (size_t)s * STAGE_BYTES;
+        const unsigned char* src = p.wimg + (size_t)chunk * 2 * B_PLANE + (size_t)h * HALF_PLANE;
+        mbar_arrive_expect_tx(&sm->full[s], 2 * HALF_PLANE);
+        bulk_g2s(st, src, HALF_PLANE, &sm->full[s]);
+        bulk_g2s(st + HALF_PLANE, src + B_PLANE, HALF_PLANE, &sm->full[s]);
+    };
+    if (tid == 0)
+        for (long long qq = 0; qq < NSTAGE && qq < n_stages; ++qq) load(qq);
+    long long q = 0;
+    // waits for the next stage; returns the descriptors of its hi / lo planes at k-slice 0
+    auto acquire = [&](uint64_t& dh, uint64_t& dl) {
+        const int s = (int)(q % NSTAGE);
+        mbar_wait(&sm->full[s], (uint32_t)(q / NSTAGE) & 1u);
+        const uint32_t a = smem_u32(stage_base + (size_t)s * STAGE_BYTES);
+        dh = smem_desc_sw128(a);
+        dl = smem_desc_sw128(a + HALF_PLANE);
+    };
+    auto release = [&]() {
         __syncwarp();
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            const uint32_t id1 = idesc_tf32(TM, (uint32_t)p.N1), id2 = idesc_tf32(TM, (uint32_t)p.N2);
-            long long q = 0;
-            for (long long it = 0; it < my_tiles; ++it) {
-                const uint32_t tph = (uint32_t)(it & 1);
-                for (int c = 0; c < NC; ++c, ++q) {
-                    const int s = (int)(q & 1);
-                    const uint32_t u = (uint32_t)(q >> 1);
-                    if (it > 0 && c == 0) mbar_wait(&sm->acc1_empty, tph ^ 1u);      // previous tile's accumulator 1 was read
-                    if (it > 0 && c == NC1) mbar_wait(&sm->acc2_empty, tph ^ 1u);    // previous tile's accumulator 2 was read
-                    TC5_STAMP(1 * 1024 + (int)q * 4 + 0);
-                    mbar_wait(&sm->full[s], u & 1u);                                  // operand A written AND operand B landed
-                    TC5_STAMP(1 * 1024 + (int)q * 4 + 2);
-                    tc_fence_after();
-                    const uint32_t a_hi = smem_u32(stage_base + (size_t)s * STAGE_BYTES);
-                    const uint32_t a_lo = a_hi + A_PLANE, b_hi = a_hi + 2 * A_PLANE, b_lo = b_hi + B_PLANE;
-                    const bool l1 = c < NC1;
-                    const uint32_t acc = l1 ? acc1 : acc2;
-                    const uint32_t idesc = l1 ? id1 : id2;
-                    const bool first = (c == 0) || (c == NC1);
+        const int s = (int)(q % NSTAGE);
+        if (lane == 0) mbar_arrive(&sm->empty[s]);
+        if (tid == 0 && q + NSTAGE < n_stages) {
+            mbar_wait(&sm->empty[s], (uint32_t)(q / NSTAGE) & 1u);
+            load(q + NSTAGE);
+        }
+        ++q;
+    };
+
+    for (long long it = 0; it < my_tiles; ++it) {
+        const long long tile = (long long)blockIdx.x + it * gridDim.x;
+        const long long ra = tile * TM + wgi * 64 + w * 16 + g, rb = ra + 8;
+        const float* xa = (ra < p.rows) ? row_ptr(p, ra) : nullptr;
+        const float* xb = (rb < p.rows) ? row_ptr(p, rb) : nullptr;
+
+        // ---- layer 1 ------------------------------------------------------------------------------------------------
+#pragma unroll 1
+        for (int c = 0; c < NC1; ++c) {
+            uint32_t ah[4][4], al[4][4];
 #pragma unroll
-                    for (int ks = 0; ks < KC / 8; ++ks) {
-                        const uint64_t dah = smem_desc_sw128(a_hi + ks * 32), dal = smem_desc_sw128(a_lo + ks * 32);
-                        const uint64_t dbh = smem_desc_sw128(b_hi + ks * 32), dbl = smem_desc_sw128(b_lo + ks * 32);
-                        mma_tf32_ss(acc, dal, dbh, idesc, (first && ks == 0) ? 0u : 1u);     // small terms first
-                        mma_tf32_ss(acc, dah, dbl, idesc, 1u);
-                        mma_tf32_ss(acc, dah, dbh, idesc, 1u);
+            for (int ks = 0; ks < 4; ++ks) {
+                const int k0 = c * KC + ks * 8 + t;
+                float v[4] = {xa ? __ldg(xa + k0) : 0.0f, xb ? __ldg(xb + k0) : 0.0f,
+                              xa ? __ldg(xa + k0 + 4) : 0.0f, xb ? __ldg(xb + k0 + 4) : 0.0f};
+                if (p.zf != nullptr) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int k = k0 + (j >> 1) * 4;
+                        v[j] = fminf(fmaxf((v[j] - sm->zmean[k]) * sm->zstd[k], -5.0f), 5.0f);
                     }
-                    mma_commit(&sm->empty[s]);                                        // stage s may be refilled
-                    TC5_STAMP(1 * 1024 + (int)q * 4 + 3);
-                    if (c == NC1 - 1) mma_commit(&sm->acc1_full);
-                    if (c == NC - 1) mma_commit(&sm->acc2_full);
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) split_tf32(v[j], ah[ks][j], al[ks][j]);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (h < nh1) {
+                    uint64_t dh, dl;
+                    acquire(dh, dl);
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks)
+                        mma3(acc1[h], ah[ks], al[ks], dh + 2 * ks, dl + 2 * ks, c == 0 && ks == 0);   // +32 bytes per k-slice
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    fence_regs(acc1[h]);
+                    release();
                 }
             }
         }
-        __syncwarp();
-    } else if (warp >= EPI_WARP0) {
-        // ================= producer / epilogue warps =================
-        // All 8 warps work on EVERY chunk (halves the empty -> full latency of a stage): warp = (lane quarter qd, column
-        // half hf).  Layer-1 chunks are staged by the 256 threads together; of a layer-2 chunk a warp converts its 32 rows x
-        // 16 columns of accumulator 1.
-        const int w8 = warp - EPI_WARP0;
-        const int hf = w8 >> 2;                         // column half of a chunk / of the head
-        const int qd = warp & 3;                        // TMEM lane quarter of this warp
-        const int t256 = w8 * 32 + lane;
-        const int row = qd * 32 + lane;                 // tile row this thread owns in TMEM
-        const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-        // the first XPF layer-1 chunks of the NEXT tile are loaded into registers before the head of the current one, so
-        // that their global-memory latency hides behind the head instead of sitting on the tile boundary
-        constexpr int XPF = 2;
-        float4 xpf[XPF][4];
-        auto prefetch_x = [&](long long r0) {
+        // hidden activations in place: acc1[h][4i + e] holds column 128h + 8i + 2t + (e & 1)
 #pragma unroll
-            for (int c = 0; c < XPF; ++c)
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int pss = 0; pss < 4; ++pss) {
-                    const int idx = pss * 256 + t256;
-                    const long long gr = r0 + (idx >> 3);
-                    xpf[c][pss] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (c < NC1 && gr < p.rows) xpf[c][pss] = ld_stream4(row_ptr(p, gr) + c * KC + (idx & 7) * 4);
-                }
-        };
-        // one operand chunk (tile iteration `it`, chunk c) into stage (q & 1)
-        auto produce = [&](long long it, int c) {
-            const long long q = it * NC + c;
-            const long long row0 = ((long long)blockIdx.x + it * gridDim.x) * TM;
-            const int s = (int)(q & 1);
-            const uint32_t u = (uint32_t)(q >> 1);
-            unsigned char* a_hi = stage_base + (size_t)s * STAGE_BYTES;
-            unsigned char* a_lo = a_hi + A_PLANE;
-            if (w8 == 0 && lane == 0) TC5_STAMP(2 * 1024 + (int)q * 4 + 0);
-            mbar_wait(&sm->empty[s], (u & 1u) ^ 1u);      // the MMAs that read this stage's previous content are done
-            if (w8 == 0 && lane == 0) TC5_STAMP(2 * 1024 + (int)q * 4 + 1);
-            if (c < NC1) {
-                // ---- layer-1 operand: 128 rows x 32 input columns, z-filtered, split into hi / lo planes
-                const int kbase = c * KC;
+            for (int i = 0; i < 16; ++i) {
+                const float2 bb = *reinterpret_cast<const float2*>(sm->b1 + h * HN + 8 * i + 2 * t);
+                acc1[h][4 * i + 0] = fmaxf(acc1[h][4 * i + 0] + bb.x, 0.0f);
+                acc1[h][4 * i + 1] = fmaxf(acc1[h][4 * i + 1] + bb.y, 0.0f);
+                acc1[h][4 * i + 2] = fmaxf(acc1[h][4 * i + 2] + bb.x, 0.0f);
+                acc1[h][4 * i + 3] = fmaxf(acc1[h][4 * i + 3] + bb.y, 0.0f);
+            }
+
+        // ---- layer 2 + head -----------------------------------------------------------------------------------------
+        float o[2][MO];
 #pragma unroll
-                for (int pss = 0; pss < 4; ++pss) {
-                    const int idx = pss * 256 + t256;
-                    const int r = idx >> 3, c16 = idx & 7;
-                    const long long gr = row0 + r;
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (gr < p.rows) {
-                        if (c < XPF) v = (c == 0) ? xpf[0][pss] : xpf[1][pss];
-                        else v = ld_stream4(row_ptr(p, gr) + kbase + c16 * 4);
-                        if (p.zf != nullptr) {
-                            const int k = kbase + c16 * 4;
-                            v.x = fminf(fmaxf((v.x - sm->zmean[k + 0]) * sm->zstd[k + 0], -5.0f), 5.0f);
-                            v.y = fminf(fmaxf((v.y - sm->zmean[k + 1]) * sm->zstd[k + 1], -5.0f), 5.0f);
-                            v.z = fminf(fmaxf((v.z - sm->zmean[k + 2]) * sm->zstd[k + 2], -5.0f), 5.0f);
-                            v.w = fminf(fmaxf((v.w - sm->zmean[k + 3]) * sm->zstd[k + 3], -5.0f), 5.0f);
-                        }
+        for (int k = 0; k < MO; ++k) o[0][k] = o[1][k] = 0.0f;
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+            if (h2 >= nh2) break;
+#pragma unroll
+            for (int c = 0; c < MAXN / KC; ++c) {
+                if (c < NC2) {
+                    uint64_t dh, dl;
+                    acquire(dh, dl);
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks) {
+                        const int sl = c * 4 + ks, hs = sl >> 4, i = sl & 15;       // source k-slice = 8 columns of acc1
+                        uint32_t ah[4], al[4];
+                        split_tf32(acc1[hs][4 * i + 0], ah[0], al[0]);
+                        split_tf32(acc1[hs][4 * i + 2], ah[1], al[1]);
+                        split_tf32(acc1[hs][4 * i + 1], ah[2], al[2]);
+                        split_tf32(acc1[hs][4 * i + 3], ah[3], al[3]);
+                        mma3(acc2, ah, al, dh + 2 * ks, dl + 2 * ks, c == 0 && ks == 0);
                     }
-                    float4 hi, lo;
-                    split_tf32(v.x, hi.x, lo.x); split_tf32(v.y, hi.y, lo.y);
-                    split_tf32(v.z, hi.z, lo.z); split_tf32(v.w, hi.w, lo.w);
-                    const uint32_t off = sw128_off((uint32_t)r, (uint32_t)(c16 * 4));
-                    *reinterpret_cast<float4*>(a_hi + off) = hi;
-                    *reinterpret_cast<float4*>(a_lo + off) = lo;
-                }
-            } else {
-                // ---- layer-2 operand: relu(acc1[:, 32j + 16hf .. +16) + b1), this thread's row
-                const int j = c - NC1;
-                float v[16];
-                tmem_ld16(acc1 + lane_base + (uint32_t)(j * KC + hf * 16), v);
-                const float* bb = sm->b1 + j * KC + hf * 16;
-#pragma unroll
-                for (int i4 = 0; i4 < 4; ++i4) {
-                    float4 hi, lo;
-                    split_tf32(fmaxf(v[i4 * 4 + 0] + bb[i4 * 4 + 0], 0.0f), hi.x, lo.x);
-                    split_tf32(fmaxf(v[i4 * 4 + 1] + bb[i4 * 4 + 1], 0.0f), hi.y, lo.y);
-                    split_tf32(fmaxf(v[i4 * 4 + 2] + bb[i4 * 4 + 2], 0.0f), hi.z, lo.z);
-                    split_tf32(fmaxf(v[i4 * 4 + 3] + bb[i4 * 4 + 3], 0.0f), hi.w, lo.w);
-                    const uint32_t off = sw128_off((uint32_t)row, (uint32_t)(hf * 16 + i4 * 4));
-                    *reinterpret_cast<float4*>(a_hi + off) = hi;
-                    *reinterpret_cast<float4*>(a_lo + off) = lo;
+                    wgmma_commit();
+                    wgmma_wait_all();
+                    fence_regs(acc2);
+                    release();
                 }
             }
-            fence_async_smem();                           // generic-proxy stores -> visible to tcgen05.mma
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm->full[s]);
-            if (w8 == 0 && lane == 0) TC5_STAMP(2 * 1024 + (int)q * 4 + 2);
-        };
-        // Order per tile: [layer-2 operands of tile it] -> [layer-1 operands of tile it+1] -> [head of tile it]: the next
-        // tile's first MMAs start while this tile's head is still being computed.
-        if (my_tiles > 0) {
-            prefetch_x((long long)blockIdx.x * TM);
-            for (int c = 0; c < NC1; ++c) produce(0, c);
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = h2 * HN + 8 * i + 2 * t + e;
+                    const float bb = sm->b2[col];
+                    const float ya = fmaxf(acc2[4 * i + e] + bb, 0.0f), yb = fmaxf(acc2[4 * i + 2 + e] + bb, 0.0f);
+#pragma unroll
+                    for (int k = 0; k < MO; ++k) {
+                        const float wk = sm->w3[col * MAX_OUT + k];
+                        o[0][k] = fmaf(ya, wk, o[0][k]);
+                        o[1][k] = fmaf(yb, wk, o[1][k]);
+                    }
+                }
         }
-        for (long long it = 0; it < my_tiles; ++it) {
-            const long long tile = (long long)blockIdx.x + it * gridDim.x;
-            const long long row0 = tile * TM;
-            const uint32_t tph = (uint32_t)(it & 1);
-            if (it + 1 < my_tiles) prefetch_x((tile + gridDim.x) * TM);      // lands while layer 2 of this tile is converted
-            mbar_wait(&sm->acc1_full, tph);               // accumulator 1 of this tile is complete
-            tc_fence_after();
-            for (int c = NC1; c < NC; ++c) produce(it, c);
-            // every layer-2 operand has been read out of accumulator 1
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm->acc1_empty);
-            if (it + 1 < my_tiles)
-                for (int c = 0; c < NC1; ++c) produce(it + 1, c);
-            // ---- head: relu(acc2 + b2) . W3 + b3; column half hf covers [hf*N2/2, (hf+1)*N2/2)
-            mbar_wait(&sm->acc2_full, tph);
-            tc_fence_after();
-            if (w8 == 0 && lane == 0) TC5_STAMP(3 * 1024 + (int)it * 4 + 0);
-            float o[MAX_OUT];
+        // the 4 lanes of a quad hold disjoint columns of the same two rows
 #pragma unroll
-            for (int k = 0; k < MAX_OUT; ++k) o[k] = 0.0f;
-            const int half = p.N2 >> 1;
-            if (p.n_out == 1) {
-                for (int cc = hf * half; cc < (hf + 1) * half; cc += 32) {
-                    float v[32];
-                    tmem_ld32(acc2 + lane_base + (uint32_t)cc, v);
+        for (int r = 0; r < 2; ++r)
 #pragma unroll
-                    for (int i4 = 0; i4 < 8; ++i4) {
-                        const float4 b4 = *reinterpret_cast<const float4*>(sm->b2 + cc + i4 * 4);
-                        const float4 w4 = *reinterpret_cast<const float4*>(sm->w3 + cc + i4 * 4);     // n_out == 1: w3[col]
-                        o[0] = fmaf(fmaxf(v[i4 * 4 + 0] + b4.x, 0.0f), w4.x, o[0]);
-                        o[0] = fmaf(fmaxf(v[i4 * 4 + 1] + b4.y, 0.0f), w4.y, o[0]);
-                        o[0] = fmaf(fmaxf(v[i4 * 4 + 2] + b4.z, 0.0f), w4.z, o[0]);
-                        o[0] = fmaf(fmaxf(v[i4 * 4 + 3] + b4.w, 0.0f), w4.w, o[0]);
-                    }
-                }
-            } else {
-                for (int cc = hf * half; cc < (hf + 1) * half; cc += 32) {
-                    float v[32];
-                    tmem_ld32(acc2 + lane_base + (uint32_t)cc, v);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const float h = fmaxf(v[i] + sm->b2[cc + i], 0.0f);
-                        const float4 wa = *reinterpret_cast<const float4*>(sm->w3 + (cc + i) * MAX_OUT);       // zero-padded
-                        const float4 wb = *reinterpret_cast<const float4*>(sm->w3 + (cc + i) * MAX_OUT + 4);
-                        o[0] = fmaf(h, wa.x, o[0]); o[1] = fmaf(h, wa.y, o[1]); o[2] = fmaf(h, wa.z, o[2]); o[3] = fmaf(h, wa.w, o[3]);
-                        o[4] = fmaf(h, wb.x, o[4]); o[5] = fmaf(h, wb.y, o[5]); o[6] = fmaf(h, wb.z, o[6]); o[7] = fmaf(h, wb.w, o[7]);
-                    }
-                }
+            for (int k = 0; k < MO; ++k) {
+                o[r][k] += __shfl_xor_sync(0xffffffffu, o[r][k], 1);
+                o[r][k] += __shfl_xor_sync(0xffffffffu, o[r][k], 2);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&sm->acc2_empty);
-            if (w8 == 0 && lane == 0) TC5_STAMP(3 * 1024 + (int)it * 4 + 1);
-            float* part = sm->part[it & 1];
-            if (hf == 1) {
+        if (t == 0) {
 #pragma unroll
-                for (int k = 0; k < MAX_OUT; ++k)
-                    if (k < p.n_out) part[row * MAX_OUT + k] = o[k];
-            }
-            asm volatile("bar.sync 1, 256;" ::: "memory");          // the 8 epilogue warps only
-            if (hf == 0) {
-                const long long gr = row0 + row;
+            for (int r = 0; r < 2; ++r) {
+                const long long gr = r ? rb : ra;
                 if (gr < p.rows) {
 #pragma unroll
-                    for (int k = 0; k < MAX_OUT; ++k)
+                    for (int k = 0; k < MO; ++k)
                         if (k < p.n_out) {
-                            float y = (o[k] + part[row * MAX_OUT + k]) + sm->b3[k];
+                            float y = o[r][k] + sm->b3[k];
                             if (p.act_out == SB200_ACT_RELU) y = fmaxf(y, 0.0f);
                             else if (p.act_out == SB200_ACT_TANH) y = tanhf(y);
                             p.out[gr * p.ld_out + k] = y;
@@ -400,19 +321,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) mlp3_tc5_kernel(const __grid_cons
             }
         }
     }
-    // ---- teardown -------------------------------------------------------------------------------------------------------
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (warp == 2) tmem_dealloc(tmem, 512);
 }
 
-constexpr size_t TC5_SMEM = 2 * (size_t)STAGE_BYTES + sizeof(SmemSmall);
+constexpr size_t TC5_SMEM = (size_t)NSTAGE * STAGE_BYTES + sizeof(SmemSmall);
 
 }  // namespace
 
 int sb200_mlp_tc5_init() {
-    SB200_CUDA(cudaFuncSetAttribute(mlp3_tc5_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC5_SMEM));
+    SB200_CUDA(cudaFuncSetAttribute(mlp3_wgmma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC5_SMEM));
+    SB200_CUDA(cudaFuncSetAttribute(mlp3_wgmma_kernel<MAX_OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC5_SMEM));
     return SB200_OK;
 }
 
@@ -421,7 +338,7 @@ static bool tc5_net_ok(const sb200_mlp* net) {
     const int K0 = net->dims[0], N1 = net->dims[1], N2 = net->dims[2], NO = net->dims[3];
     if (K0 % KC != 0 || K0 < KC || K0 > MAX_K0) return false;
     if (N1 % KC != 0 || N1 < KC || N1 > MAXN) return false;
-    if (N2 % 64 != 0 || N2 < 64 || N2 > MAXN) return false;     // the head splits the columns between the two groups
+    if (N2 % KC != 0 || N2 < KC || N2 > MAXN) return false;
     if (NO < 1 || NO > MAX_OUT) return false;
     if (net->act[0] != SB200_ACT_RELU || net->act[1] != SB200_ACT_RELU) return false;
     return true;
@@ -441,8 +358,7 @@ extern "C" int sb200_mlp_forward_tc5_f32(const sb200_mlp* net, const sb200_zfilt
     SB200_REQUIRE(net && in && out && workspace);
     if (!tc5_net_ok(net)) return SB200_ERR_UNSUPPORTED;
     SB200_REQUIRE(in->x != nullptr && in->rows >= 0 && in->aux == nullptr && in->save_x == nullptr);
-    SB200_REQUIRE((in->ldx % 4) == 0 && (((uintptr_t)in->x) & 15) == 0);
-    SB200_REQUIRE(in->win_n == 0 || (in->x_next != nullptr && (((uintptr_t)in->x_next) & 15) == 0));
+    SB200_REQUIRE(in->win_n == 0 || in->x_next != nullptr);
     SB200_REQUIRE((((uintptr_t)workspace) & 15) == 0 && ld_out >= net->dims[3]);
     if (in->rows == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)stream;
@@ -466,6 +382,7 @@ extern "C" int sb200_mlp_forward_tc5_f32(const sb200_mlp* net, const sb200_zfilt
     tc5_prep_kernel<<<(units + 255) / 256, 256, 0, st>>>(net->W[0], net->ldw[0], p.K0, p.N1, net->W[1], net->ldw[1], p.N2,
                                                         (unsigned char*)workspace);
     const long long grid = p.n_tiles < n_sm ? p.n_tiles : n_sm;
-    mlp3_tc5_kernel<<<(unsigned)grid, NTHREADS, TC5_SMEM, st>>>(p);
+    if (p.n_out == 1) mlp3_wgmma_kernel<1><<<(unsigned)grid, NTHREADS, TC5_SMEM, st>>>(p);
+    else mlp3_wgmma_kernel<MAX_OUT><<<(unsigned)grid, NTHREADS, TC5_SMEM, st>>>(p);
     return sb200_launch_status(2);
 }

@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(OT) soft_update_kernel(float* __restrict__ tar
 
 inline int grid_for(long long n) {
     long long b = (n + 4 * OT - 1) / (4 * OT);   // >= 4 elements per thread: small nets finish in one short wave
-    if (b > 296) b = 296;          // 2 x 148 SMs, grid-stride
+    if (b > 264) b = 264;          // 2 x 132 SMs, grid-stride
     if (b < 1) b = 1;
     return (int)b;
 }

@@ -308,7 +308,7 @@ extern "C" int sb200_replay_gather_f32(const float* src, int64_t record_floats, 
     SB200_REQUIRE(src && out && (idx32 || idx64) && batch >= 1 && record_floats >= 1);
     const int vec = (record_floats % 4 == 0) && ((((uintptr_t)src) | ((uintptr_t)out)) & 15) == 0;
     int blocks = (batch + 7) / 8;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     gather_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, record_floats, idx32, (const long long*)idx64, batch, out,
                                                             vec);
     return sb200_launch_status();
@@ -333,7 +333,7 @@ extern "C" int sb200_replay_gather_multi_f32(const float* const* srcs, float* co
     for (int k = nfields; k < GATHER_MAX_FIELDS; ++k) { f.src[k] = nullptr; f.out[k] = nullptr; f.rec[k] = 0; f.unit[k] = 1; f.chunk_end[k] = end; }
     f.nf = nfields;
     int blocks = (batch + 7) / 8;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     gather_multi_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(f, idx32, (const long long*)idx64, batch);
     return sb200_launch_status();
 }

@@ -1,8 +1,8 @@
 // Persistent rollout kernel: T env steps of ALL co-located actors in ONE launch.
 //
 // The per-step launch sequence (policy forward -> sample -> env step -> window staging) is bound by fixed costs:
-// every launch re-fetches the policy weights from L2 (a chain of dependent round trips, profiles/r01c) and pays
-// launch + drain; 128 steps x 3 launches cost ~4.3 ms per rollout for ~0.2 ms of arithmetic.  Actors are
+// every launch re-fetches the policy weights from L2 (a chain of dependent round trips) and pays
+// launch + drain, 128 steps x 3 launches per rollout for a fraction of that in arithmetic.  Actors are
 // independent of one another, so the loop over time can move INSIDE the kernel:
 //   * a thread-block cluster of 4 CTAs owns 32 actors for the whole chunk;
 //   * each CTA keeps a QUARTER of every hidden layer's weights resident in shared memory for all T steps (fetched
@@ -120,7 +120,7 @@ __device__ __forceinline__ void rf_st_cluster_v4(unsigned addr, const float4& v)
 //   tiles are summed in a fixed order (deterministic) through `Part` [4][32][Nc].
 //   ALL_ROWS: the result is stored in every CTA's copy of Hout [32][ldout] (input of the next hidden layer);
 //   otherwise each row goes only to the CTA that owns the actor, into its Hout [8][ldout] (input of the head).
-template <bool ALL_ROWS, bool F2>
+template <bool ALL_ROWS>
 __device__ __forceinline__ void rf_layer(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
                                          int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
                                          int ldout, int col0, float* __restrict__ Part, unsigned smem_base,
@@ -133,42 +133,6 @@ __device__ __forceinline__ void rf_layer(const float* __restrict__ Xin, int ldin
     for (int c4 = tx; c4 < nq; c4 += 16) {
         const float* xr = Xin + (ty * 4) * ldin;
         const float* wp = Ws + c4 * 4;
-        if constexpr (F2) {
-            // packed fma.rn.f32x2 (sm_100): two columns per instruction; each half is an IEEE fma, so the result is
-            // bit-identical to the scalar path -- it only halves the FFMA issue slots
-            float2 acc[4][2];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) acc[r][0] = acc[r][1] = make_float2(0.0f, 0.0f);
-#pragma unroll 2
-            for (int k = k_lo; k < k_hi; k += 4) {
-                float4 a[4];
-#pragma unroll
-                for (int r = 0; r < 4; ++r) a[r] = *reinterpret_cast<const float4*>(xr + r * ldin + k);
-                const float4 w0 = *reinterpret_cast<const float4*>(wp + (k + 0) * Nc);
-                const float4 w1 = *reinterpret_cast<const float4*>(wp + (k + 1) * Nc);
-                const float4 w2 = *reinterpret_cast<const float4*>(wp + (k + 2) * Nc);
-                const float4 w3 = *reinterpret_cast<const float4*>(wp + (k + 3) * Nc);
-#pragma unroll
-                for (int r = 0; r < 4; ++r) {
-                    float2 aa = make_float2(a[r].x, a[r].x);
-                    acc[r][0] = __ffma2_rn(aa, make_float2(w0.x, w0.y), acc[r][0]);
-                    acc[r][1] = __ffma2_rn(aa, make_float2(w0.z, w0.w), acc[r][1]);
-                    aa = make_float2(a[r].y, a[r].y);
-                    acc[r][0] = __ffma2_rn(aa, make_float2(w1.x, w1.y), acc[r][0]);
-                    acc[r][1] = __ffma2_rn(aa, make_float2(w1.z, w1.w), acc[r][1]);
-                    aa = make_float2(a[r].z, a[r].z);
-                    acc[r][0] = __ffma2_rn(aa, make_float2(w2.x, w2.y), acc[r][0]);
-                    acc[r][1] = __ffma2_rn(aa, make_float2(w2.z, w2.w), acc[r][1]);
-                    aa = make_float2(a[r].w, a[r].w);
-                    acc[r][0] = __ffma2_rn(aa, make_float2(w3.x, w3.y), acc[r][0]);
-                    acc[r][1] = __ffma2_rn(aa, make_float2(w3.z, w3.w), acc[r][1]);
-                }
-            }
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-                *reinterpret_cast<float4*>(Part + ((q * RF_ROWS + ty * 4 + r) * Nc + c4 * 4)) =
-                    make_float4(acc[r][0].x, acc[r][0].y, acc[r][1].x, acc[r][1].y);
-        } else {
         float acc[4][4];
 #pragma unroll
         for (int r = 0; r < 4; ++r)
@@ -199,7 +163,6 @@ __device__ __forceinline__ void rf_layer(const float* __restrict__ Xin, int ldin
         for (int r = 0; r < 4; ++r)
             *reinterpret_cast<float4*>(Part + ((q * RF_ROWS + ty * 4 + r) * Nc + c4 * 4)) =
                 make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
-        }
     }
     RF_STAMP(rf_id, 0);
     __syncthreads();
@@ -232,7 +195,6 @@ __device__ __forceinline__ void rf_layer(const float* __restrict__ Xin, int ldin
     }
 }
 
-template <bool F2>
 __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     ppo_rollout_kernel(const __grid_constant__ RfParams p) {
     cg::cluster_group cluster = cg::this_cluster();
@@ -333,11 +295,11 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
         const bool final_step = (t == p.T - 1);
         const int rf_t = t;
         RF_STAMP(0, 0);
-        rf_layer<true, F2>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, Part, smem_base, crank, rf_t, 1);
+        rf_layer<true>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, Part, smem_base, crank, rf_t, 1);
         RF_STAMP(3, 0);
         cluster.sync();
         RF_STAMP(4, 0);
-        rf_layer<false, F2>(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5);
+        rf_layer<false>(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5);
         RF_STAMP(7, 0);
         cluster.sync();
         RF_STAMP(8, 0);
@@ -608,17 +570,17 @@ __device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldi
             for (int r = 0; r < 8; ++r) {
                 const float4 a = *reinterpret_cast<const float4*>(xr + r * ldin + k);
                 float2 aa = make_float2(a.x, a.x);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w0.x, w0.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w0.z, w0.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w0.x, w0.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w0.z, w0.w), acc[r][1]);
                 aa = make_float2(a.y, a.y);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w1.x, w1.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w1.z, w1.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w1.x, w1.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w1.z, w1.w), acc[r][1]);
                 aa = make_float2(a.z, a.z);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w2.x, w2.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w2.z, w2.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w2.x, w2.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w2.z, w2.w), acc[r][1]);
                 aa = make_float2(a.w, a.w);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w3.x, w3.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w3.z, w3.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w3.x, w3.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w3.z, w3.w), acc[r][1]);
             }
         }
 #pragma unroll
@@ -700,17 +662,17 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
             for (int r = 0; r < 4; ++r) {
                 const float4 a = *reinterpret_cast<const float4*>(xr + r * ldin + k);
                 float2 aa = make_float2(a.x, a.x);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w0.x, w0.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w0.z, w0.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w0.x, w0.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w0.z, w0.w), acc[r][1]);
                 aa = make_float2(a.y, a.y);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w1.x, w1.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w1.z, w1.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w1.x, w1.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w1.z, w1.w), acc[r][1]);
                 aa = make_float2(a.z, a.z);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w2.x, w2.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w2.z, w2.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w2.x, w2.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w2.z, w2.w), acc[r][1]);
                 aa = make_float2(a.w, a.w);
-                acc[r][0] = __ffma2_rn(aa, make_float2(w3.x, w3.y), acc[r][0]);
-                acc[r][1] = __ffma2_rn(aa, make_float2(w3.z, w3.w), acc[r][1]);
+                acc[r][0] = fma2(aa, make_float2(w3.x, w3.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w3.z, w3.w), acc[r][1]);
             }
         }
         const float4 bv = *reinterpret_cast<const float4*>(bias_s + (on ? c4 : 0) * 4);
@@ -754,7 +716,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     __shared__ __align__(8) unsigned long long s_bar[3];      // ASYNC: hidden layer 1 | last hidden layer rows | next input tile
 
     // (tried: the two roles on swapped warp halves, in case the scheduler's preference for one end of the warp index range
-    // starved the layers -- no difference, profiles/r02b_rollout_trace_*)
+    // starved the layers -- no difference in clock64 traces)
     const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
     const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
     const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
@@ -1238,8 +1200,7 @@ bool rf_plan(const sb200_mlp* net, int D, int A, RfParams* p, size_t* smem_bytes
 }  // namespace
 
 int sb200_rollout_fused_init() {
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     return SB200_OK;
@@ -1316,9 +1277,6 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     p.T = a->T;
     p.step_ctr = (const unsigned long long*)a->step_counter;
     const long long clusters = ((long long)a->N + RF_ROWS - 1) / RF_ROWS;
-    // packed fma.rn.f32x2 in the hidden layers (default; bit-identical results, fewer issue slots: 1.764 -> 1.696 ms per
-    // 128-step chunk of 1024 actors).  SB200_RF_FFMA2=0 selects the scalar-FFMA instantiation.
-    static const int f2 = [] { const char* e = getenv("SB200_RF_FFMA2"); return e ? atoi(e) : 1; }();
     // v2 (warp-specialised env warps, 8x4 register tiles) is the default; SB200_RF_V2=0 selects the v1 kernel
     static const int v2 = [] { const char* e = getenv("SB200_RF_V2"); return e ? atoi(e) : 1; }();
     static const int l1_direct = [] { const char* e = getenv("SB200_RF_L1DIRECT"); return e ? atoi(e) : 1; }();
@@ -1332,8 +1290,7 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     if (v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20))
         ppo_rollout2_kernel<true><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     else if (v2) ppo_rollout2_kernel<false><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else if (f2) ppo_rollout_kernel<true><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else ppo_rollout_kernel<false><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    else ppo_rollout_kernel<<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     return sb200_launch_status();
 }
 

@@ -1,6 +1,6 @@
 // CNN stem of the pixel path (surreal/model/model_builders/builders.py:8-33, ppo_net.py:268-273,368-375):
 //   uint8 frames / 255 -> Conv2d(16, k8, s4) + ReLU -> Conv2d(32, k4, s2) + ReLU -> Flatten -> Linear(cnn_feature_dim) + ReLU
-// (VALID padding; the Linear layer runs on the MLP kernels / the tcgen05 linear kernel).  This file holds the two
+// (VALID padding; the Linear layer runs on the MLP kernels).  This file holds the two
 // convolutions, forward and backward, as direct fp32 FFMA kernels:
 //
 //   conv_fwd_kernel   one frame per CTA iteration, the frame (converted to float, x 1/255 for uint8 input) and the layer's
@@ -218,7 +218,7 @@ int launch_fwd(const void* x, int frames, int CIN, int H, int W, const float* Wk
                cudaStream_t st) {
     const size_t smem = ((size_t)CIN * KS * KS * COUT + (size_t)CIN * H * row_pitch<KS, ST>(W)) * sizeof(float);
     if (smem > STEM_SMEM_MAX) return SB200_ERR_UNSUPPORTED;
-    const int grid = frames < 148 * 4 ? frames : 148 * 4;
+    const int grid = frames < 132 * 4 ? frames : 132 * 4;
     conv_fwd_kernel<KS, ST, COUT, IN_T><<<grid, CT, smem, st>>>((const IN_T*)x, frames, CIN, H, W, Wk, bias, in_scale, y);
     return sb200_launch_status();
 }
@@ -288,7 +288,7 @@ extern "C" int sb200_conv_backward_dx_f32(int layer, const float* dy, const floa
     const int HO = (H - 4) / 2 + 1, WO = (W - 4) / 2 + 1;
     const size_t smem = ((size_t)CIN * 16 * 32 + (size_t)HO * WO * 32) * sizeof(float);
     if (smem > STEM_SMEM_MAX) return SB200_ERR_UNSUPPORTED;
-    const int grid = frames < 148 * 4 ? (int)frames : 148 * 4;
+    const int grid = frames < 132 * 4 ? (int)frames : 132 * 4;
     conv_bwd_dx_kernel<4, 2, 32><<<grid, CT, smem, (cudaStream_t)stream>>>(dy, Wk, act, (int)frames, CIN, H, W, dx);
     return sb200_launch_status();
 }

@@ -38,7 +38,7 @@ class Launcher:
 
 
 class PipelinedEngine:
-    """Actors and learner as two concurrent CUDA streams of ONE process (the B200 form of Surreal's asynchronous
+    """Actors and learner as two concurrent CUDA streams of ONE process (the single-GPU form of Surreal's asynchronous
     actor / learner processes): while the learner works on batch k, the actors already roll out batch k+1 with the
     weights published after batch k-1 -- exactly the policy lag Surreal's actors run with (docs/ppo.md:16).
 

@@ -1,5 +1,5 @@
 """PPOLearner: drop-in for surreal/learner/ppo.py:12-682 whose learn() runs entirely as hand-written
-sm_100a kernels (critic pass -> windowed GAE -> fused loss+grad -> backward GEMMs -> clip+Adam).
+sm_90a kernels (critic pass -> windowed GAE -> fused loss+grad -> backward GEMMs -> clip+Adam).
 
 Same constructor, config keys, method names, statistics names and control flow as the reference
 (clip / adapt modes, KL early stop ppo.py:556, publish-time adaptation ppo.py:637-666).  The batch a
@@ -197,7 +197,7 @@ class PPOLearner(Learner):
         self._graph = ops.GraphRunner()
         self._graph_head = ops.GraphRunner()
         self.before_epochs_hook = None                    # see _optimize
-        self._tc5 = ops.Tc5Forward(self.model.critic)     # critic pass on tcgen05 / TMEM when the shape qualifies
+        self._tc5 = ops.Tc5Forward(self.model.critic)     # critic pass on the wgmma kernel when the shape qualifies
         self.tc5_min_rows = int(os.environ.get('SB200_TC5_MIN_ROWS', '4096'))
         self.dp = None
         self.dp_v = None
@@ -353,7 +353,7 @@ class PPOLearner(Learner):
             else:
                 ops.mlp_forward(m.critic, feat, out=self._values)
         elif rows >= self.tc5_min_rows and self._tc5.supported(rows):
-            # Blackwell-native path: tcgen05.mma tiles, accumulators in TMEM, weights streamed by the TMA engine
+            # Hopper path: wgmma tiles, accumulators in registers, weights streamed by the TMA engine
             self._tc5(self._obs_full.view(rows, -1), self._values.view(rows, 1), zf_stats=m.z_stats, zf_eps=m.z_eps)
         elif self.dual_critic and rows >= 32768:
             ops.mlp_forward_dual(m.critic, self._obs_full.view(rows, -1), zf_stats=m.z_stats, zf_eps=m.z_eps,

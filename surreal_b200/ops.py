@@ -162,7 +162,7 @@ def mlp_forward_packed(packed, x, zf_stats=None, zf_eps=1e-5, aux=None, out=None
 
 
 class Tc5Forward:
-    """Large-batch forward of a FlatNet on the tcgen05 / TMEM kernel (sb200_mlp_forward_tc5_f32).  Owns the workspace of
+    """Large-batch forward of a FlatNet on the wgmma kernel (sb200_mlp_forward_tc5_f32).  Owns the workspace of
     the per-call weight images; ``supported(rows)`` says whether the shape qualifies (else callers use mlp_forward)."""
 
     def __init__(self, net):
@@ -533,7 +533,7 @@ class EpochPair:
 
 
 class GraphRunner:
-    """Capture a fixed launch sequence once into a CUDA graph and replay it (B200: a launch-bound inner loop of
+    """Capture a fixed launch sequence once into a CUDA graph and replay it (a launch-bound inner loop of
     hundreds of small kernels becomes ONE submission).  Capture records without executing, so state is advanced
     exactly once per call: the first call captures and immediately replays."""
 

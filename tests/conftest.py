@@ -14,7 +14,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 def pytest_configure(config):
     import torch
     torch.set_num_threads(min(8, os.cpu_count() or 1))      # the CPU oracle does not scale to 100+ threads on tiny GEMMs
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100: pytest -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):

@@ -206,15 +206,15 @@ def test_gae_matches_oracle(B, n, H, norm):
 
 
 @pytest.mark.parametrize('dims,rows,zf,win', [
-    ([64, 256, 256, 1], 132096, True, 0),      # the cfg2 critic pass: 1032 tiles of 128 rows, 7 tiles per CTA
+    ([64, 256, 256, 1], 132096, True, 0),      # the cfg2 critic pass: 1032 tiles of 128 rows, 7-8 tiles per CTA
     ([64, 256, 256, 1], 128 * 5 + 77, True, 0),   # ragged last tile
     ([64, 256, 256, 8], 4096, True, 0),        # 8 output columns, tanh head
-    ([32, 128, 64, 3], 19205, False, 0),       # narrower layers (UMMA N = 128 / 64), single layer-1 chunk (odd chunk count)
+    ([32, 128, 64, 3], 19205, False, 0),       # narrower layers (one 128-column half each, layer 2 zero-padded), single layer-1 chunk
     ([128, 256, 256, 1], 1000, True, 0),       # four layer-1 chunks
     ([64, 256, 256, 1], 0, True, 16),          # virtual cat([obs, obs_next]) rows of ppo.py:376-383 (B = 600 windows)
 ])
 def test_tcgen05_forward_matches_oracle(dims, rows, zf, win):
-    """sb200_mlp_forward_tc5_f32 (tcgen05.mma kind::tf32, accumulators in TMEM, 3xTF32 split) against the fp32 oracle
+    """sb200_mlp_forward_tc5_f32 (wgmma tf32, accumulators in registers, 3xTF32 split) against the fp32 oracle
     network at 1e-5 * max(1, rms): same bar as the mma.sync / FFMA forward kernels."""
     from surreal_b200 import ops
     gen = torch.Generator().manual_seed(sum(dims) + rows + win)
@@ -248,7 +248,7 @@ def test_tcgen05_forward_matches_oracle(dims, rows, zf, win):
         for l, (w, b) in enumerate(layers):
             h = torch.nn.functional.linear(h, w, b)
             h = torch.relu(h) if acts[l] == ops.ACT_RELU else (torch.tanh(h) if acts[l] == ops.ACT_TANH else h)
-    assert_close_scale(out, h, 1e-5, 'tcgen05 forward')
+    assert_close_scale(out, h, 1e-5, 'wgmma forward')
     # and the same rows through the default dispatcher (mma.sync / FFMA kernels) agree to the same bar
     ref = ops.mlp_forward(net, x.to(_dev()), zf_stats=stats)
-    assert_close_scale(out, ref, 1e-5, 'tcgen05 vs default forward')
+    assert_close_scale(out, ref, 1e-5, 'wgmma vs default forward')

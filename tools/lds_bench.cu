@@ -1,6 +1,6 @@
 // Micro-benchmark (dev tool, not shipped): cycles per warp-wide shared-memory load as a function of width and of the
 // number of DISTINCT addresses in the warp -- decides the register-tile shape of the persistent rollout kernel.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/lds_bench tools/lds_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/lds_bench tools/lds_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

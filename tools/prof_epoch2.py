@@ -56,7 +56,7 @@ def main():
     print('  %-12s CTA 0 %8.1f us   last CTA %8.1f us' % ('sum', tot0, tot1))
     cp = pair.cta_profile()
     print('per-CTA us per launch: P1 | P2 | forward (GEMMs) | loss rows + d2 | d1 GEMM')
-    for c in list(range(0, 148, 8)) + [60, 61, 62, 63, 123, 124, 125, 126, 127]:
+    for c in list(range(0, 132, 8)) + [60, 61, 62, 63, 123, 124, 125, 126, 127]:
         v = [x / reps / mhz for x in cp[c]]
         print('  CTA %3d: %7.1f | %7.1f | %7.1f (%7.1f) | %7.1f | %7.1f' % (c, v[0], v[1], v[2], v[3], v[4], v[5]))
 

@@ -9,9 +9,6 @@ echo "launch list rc=$?"
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:ppo_rollout2?_kernel -s 2 -c 1 \
     -o gpurun_out/prof_rollout -f python tools/prof_rollout.py 128 1 > gpurun_out/prof_rollout.log 2>&1
 echo "rollout capture rc=$?"
-timeout 300 ncu --set full --clock-control none --import-source on -k regex:mlp3_tc5 -s 2 -c 1 -f -o gpurun_out/prof_tc5 \
-    tools/tc5_harness prof > gpurun_out/prof_tc5.log 2>&1
-echo "tc5 capture rc=$?"
 ls -la gpurun_out | head -40
 # round 2b: the one-launch learner kernel, the v2 rollout kernel (matched by the ppo_rollout regex above), GAE at 2^18 windows
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:ppo_epochs2 -s 2 -c 1 -f -o gpurun_out/prof_epochs2 \

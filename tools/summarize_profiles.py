@@ -101,7 +101,7 @@ def traffic(pairs):
 
 
 def sass_excerpt(tag, obj, out_name, patterns):
-    """The SASS mnemonics that prove a Blackwell-native kernel (B200_PROFILING.md): UTC*MMA, LDTM, UBLKCP / UTMALDG."""
+    """Counts of the listed SASS mnemonics in one object file, with the lines that carry them."""
     sass = subprocess.run(['cuobjdump', '-sass', obj], capture_output=True, text=True).stdout.splitlines()
     hits = collections.Counter()
     lines = []
@@ -132,4 +132,4 @@ if __name__ == '__main__':
     traffic([('rollout', 'prof_rollout'), ('critic', 'prof_tc5'), ('epochs2', 'prof_epochs2'), ('gae_large', 'prof_gae_large')])
     obj = os.path.join(ROOT, 'surreal_b200', 'build', 'mlp_fwd_tc5.o')
     if os.path.exists(obj):
-        sass_excerpt(tag, obj, 'sass_tc5', ['UTC', 'LDTM', 'STTM', 'UBLKCP', 'UTMA', 'SYNCS', 'HMMA'])
+        sass_excerpt(tag, obj, 'sass_tc5', ['HGMMA', 'UBLKCP', 'SYNCS', 'WARPGROUP'])
