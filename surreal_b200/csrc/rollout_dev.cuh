@@ -103,14 +103,23 @@ __device__ __forceinline__ void copy_floats(float* __restrict__ dst, const float
 // step (SLOT_NONE: not complete, SLOT_DROPPED: complete but not stored).  Appends (reward, done) at
 // deque position p and obs_next at p+1; if the window completed, copies it into its replay slot and pops
 // `stride` items; if the episode ended, clears the deque (exp_sender_wrapper.py:204-207) and seeds position 0
-// with the reset observation.  Barriers are block-wide and executed by EVERY thread (valid or not).
+// with the reset observation.  `barrier` is executed by EVERY thread of the barrier's group (valid or not): block-wide by
+// default; a caller whose commit group is one warp and whose other warps are busy elsewhere passes WarpBarrier.
+struct BlockBarrier {
+    __device__ __forceinline__ void operator()() const { __syncthreads(); }
+};
+struct WarpBarrier {
+    __device__ __forceinline__ void operator()() const { __syncwarp(); }
+};
+template <class Barrier = BlockBarrier>
 __device__ void commit_actor(bool valid, int i, int g, int G, const float* __restrict__ next_row,
                              const float* __restrict__ reset_row, float rew, float dn, int n_step, int stride, int D,
                              int A, int* __restrict__ pos, int slot, float* __restrict__ stage_obs,
                              float* __restrict__ stage_act, float* __restrict__ stage_pd,
                              float* __restrict__ stage_rew, float* __restrict__ stage_done,
                              float* __restrict__ r_obs, float* __restrict__ r_act,
-                             float* __restrict__ r_pd, float* __restrict__ r_rew, float* __restrict__ r_done) {
+                             float* __restrict__ r_pd, float* __restrict__ r_rew, float* __restrict__ r_done,
+                             Barrier barrier = Barrier()) {
     const long long ii = valid ? i : 0;
     const int p = valid ? *pos : 0;
     float* so = stage_obs + ii * (n_step + 1) * D;
@@ -125,7 +134,7 @@ __device__ void commit_actor(bool valid, int i, int g, int G, const float* __res
             sd[p] = dn;
         }
     }
-    __syncthreads();
+    barrier();
     int len = p + 1;
     if (!valid) slot = SLOT_NONE;
     const bool complete = (slot != SLOT_NONE);               // len == n_step
@@ -136,7 +145,7 @@ __device__ void commit_actor(bool valid, int i, int g, int G, const float* __res
         copy_floats(r_rew + (long long)slot * n_step, sr, n_step, g, G);
         copy_floats(r_done + (long long)slot * n_step, sd, n_step, g, G);
     }
-    __syncthreads();
+    barrier();
     const int pop = min(stride, n_step);                     // uniform: every completing deque holds n_step items
     const int keep = n_step - pop;
     if (keep > 0) {                                          // overlapping windows: slide the deque down
@@ -145,33 +154,33 @@ __device__ void commit_actor(bool valid, int i, int g, int G, const float* __res
             const bool on = complete && k < (keep + 1) * D;
             float v = 0.f;
             if (on) v = so[(long long)pop * D + k];
-            __syncthreads();
+            barrier();
             if (on) so[k] = v;
-            __syncthreads();
+            barrier();
         }
         for (int k0 = 0; k0 < keep * 2 * A; k0 += G) {
             const int k = k0 + g;
             float va = 0.f, vp = 0.f;
             if (complete && k < keep * A) va = sa[(long long)pop * A + k];
             if (complete && k < keep * 2 * A) vp = sp[(long long)pop * 2 * A + k];
-            __syncthreads();
+            barrier();
             if (complete && k < keep * A) sa[k] = va;
             if (complete && k < keep * 2 * A) sp[k] = vp;
-            __syncthreads();
+            barrier();
         }
         for (int k0 = 0; k0 < keep; k0 += G) {
             const int k = k0 + g;
             float vr = 0.f, vd = 0.f;
             if (complete && k < keep) { vr = sr[pop + k]; vd = sd[pop + k]; }
-            __syncthreads();
+            barrier();
             if (complete && k < keep) { sr[k] = vr; sd[k] = vd; }
-            __syncthreads();
+            barrier();
         }
     } else if (complete) {
         for (int d = g; d < D; d += G) so[d] = next_row[d];                 // obs_next -> next window's first obs
     }
     if (complete) len = keep;
-    __syncthreads();
+    barrier();
     if (valid && dn > 0.5f) {                                // episode over: deque cleared, new episode's first obs
         for (int d = g; d < D; d += G) so[d] = reset_row[d];
         len = 0;

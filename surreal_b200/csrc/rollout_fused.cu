@@ -19,6 +19,7 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <mutex>
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -45,8 +46,24 @@ __device__ long long g_rf_trace[RF_CS][RF_TR_STEPS][RF_TR_IDS];
         if (blockIdx.x < RF_CS && RF_TID == (who) && rf_t >= 2 && rf_t < 2 + RF_TR_STEPS)           \
             g_rf_trace[blockIdx.x][rf_t - 2][id] = clock64();                                       \
     } while (0)
+// per CTA of the last launch: %smid, %globaltimer at entry, %globaltimer at exit (shows how many waves the grid ran in)
+constexpr int RF_TR_CTAS = 4096;
+__device__ long long g_rf_cta[RF_TR_CTAS][3];
+__device__ __forceinline__ void rf_cta_stamp(int slot) {
+    if (threadIdx.x != 0 || blockIdx.x >= RF_TR_CTAS) return;
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    if (slot == 1) {
+        unsigned sm;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+        g_rf_cta[blockIdx.x][0] = sm;
+    }
+    g_rf_cta[blockIdx.x][slot] = (long long)t;
+}
+#define RF_CTA_STAMP(slot) rf_cta_stamp(slot)
 #else
 #define RF_STAMP(id, who) do { } while (0)
+#define RF_CTA_STAMP(slot) do { } while (0)
 #endif
 
 struct RfParams {
@@ -90,6 +107,8 @@ struct RfParams {
     const unsigned long long* step_ctr;
     // shared-memory plan (float offsets)
     int oW1, oW2, oWh, oB, oX0, oH1, oH2, oPart, oZf, oEnv, oS, oNext, oAct, oPre;
+    int oHs;                        // two groups per cluster: head slice sums [16][8][ldw[2]]
+    int gstride;                    // two groups per cluster: floats between group 0's and group 1's X0 .. Pre
     int ldx0, ldh1, ldh2;
     int l1_direct;                  // v2: reduction-free first layer (rf2_layer1)
     int head_mode;                  // v2: 1 = k-sliced head over all owned actors, 0 = two warps per actor
@@ -702,9 +721,471 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
     RF_STAMP(2, 0);
 }
 
-template <bool ASYNC>
+// Last hidden layer on the 8 math warps WITHOUT the shared-memory reduction of rf2_layer<false, true>, with the same
+// result bit for bit: the same four k quarters, each accumulated in the same order by one lane, meet through two rounds of
+// shuffles as ((p0 + p1) + (p2 + p3)) + bias (fp32 addition is commutative, so which lane of a pair adds does not
+// matter).  Warp = (row group rg = warp & 3: rows 8rg..8rg+7, column half ch = warp >> 2), lane = (column quad cq = lane & 7,
+// k quarter ks = lane >> 3).  Each row goes to the CTA that owns its actor, as in rf2_layer<false, .>.
+__device__ __forceinline__ void rf2_layer2_direct(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
+                                                  int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
+                                                  int ldout, int col0, unsigned smem_base, unsigned crank, unsigned bar_off) {
+    const int tid = (int)RF_TID, warp = tid >> 5, lane = tid & 31;
+    const int rg = warp & 3, ch = warp >> 2, cq = lane & 7, ks = lane >> 3;
+    const bool u3 = (lane & 8) != 0, u4 = (lane & 16) != 0;
+    const int kq = (((K >> 2) + 3) >> 2) << 2;               // k span of one quarter, as in rf2_layer
+    const int k_lo = ks * kq, k_hi = min(K, k_lo + kq);
+    const int nq = Nc >> 2;
+    const float* xr = Xin + (rg * 8) * ldin;
+    for (int cb = ch * 8; cb < nq; cb += 16) {               // uniform trip count: the shuffles need the whole warp
+        const int c4 = cb + cq;
+        const bool on = c4 < nq;
+        const float* wp = Ws + (on ? c4 : 0) * 4;
+        float2 acc[8][2];
+#pragma unroll
+        for (int r = 0; r < 8; ++r) acc[r][0] = acc[r][1] = make_float2(0.0f, 0.0f);
+#pragma unroll 2
+        for (int k = k_lo; k < k_hi; k += 4) {
+            const float4 w0 = *reinterpret_cast<const float4*>(wp + (k + 0) * Nc);
+            const float4 w1 = *reinterpret_cast<const float4*>(wp + (k + 1) * Nc);
+            const float4 w2 = *reinterpret_cast<const float4*>(wp + (k + 2) * Nc);
+            const float4 w3 = *reinterpret_cast<const float4*>(wp + (k + 3) * Nc);
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+                const float4 a = *reinterpret_cast<const float4*>(xr + r * ldin + k);
+                float2 aa = make_float2(a.x, a.x);
+                acc[r][0] = fma2(aa, make_float2(w0.x, w0.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w0.z, w0.w), acc[r][1]);
+                aa = make_float2(a.y, a.y);
+                acc[r][0] = fma2(aa, make_float2(w1.x, w1.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w1.z, w1.w), acc[r][1]);
+                aa = make_float2(a.z, a.z);
+                acc[r][0] = fma2(aa, make_float2(w2.x, w2.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w2.z, w2.w), acc[r][1]);
+                aa = make_float2(a.w, a.w);
+                acc[r][0] = fma2(aa, make_float2(w3.x, w3.y), acc[r][0]);
+                acc[r][1] = fma2(aa, make_float2(w3.z, w3.w), acc[r][1]);
+            }
+        }
+        // round 1, quarters 0 <-> 1 and 2 <-> 3: lanes with bit 3 clear keep rows 0..3, the others rows 4..7
+        float2 s[4][2];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float2 snd = u3 ? acc[r][h] : acc[r + 4][h], kp = u3 ? acc[r + 4][h] : acc[r][h];
+                s[r][h].x = kp.x + __shfl_xor_sync(0xffffffffu, snd.x, 8);
+                s[r][h].y = kp.y + __shfl_xor_sync(0xffffffffu, snd.y, 8);
+            }
+        // round 2, (p0 + p1) <-> (p2 + p3): lanes with bit 4 clear keep the first two of their four rows
+        const float4 bv = *reinterpret_cast<const float4*>(bias_s + (on ? c4 : 0) * 4);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2 snd0 = u4 ? s[r][0] : s[r + 2][0], kp0 = u4 ? s[r + 2][0] : s[r][0];
+            const float2 snd1 = u4 ? s[r][1] : s[r + 2][1], kp1 = u4 ? s[r + 2][1] : s[r][1];
+            float4 o;
+            o.x = rf_act((kp0.x + __shfl_xor_sync(0xffffffffu, snd0.x, 16)) + bv.x, act);
+            o.y = rf_act((kp0.y + __shfl_xor_sync(0xffffffffu, snd0.y, 16)) + bv.y, act);
+            o.z = rf_act((kp1.x + __shfl_xor_sync(0xffffffffu, snd1.x, 16)) + bv.z, act);
+            o.w = rf_act((kp1.y + __shfl_xor_sync(0xffffffffu, snd1.y, 16)) + bv.w, act);
+            if (on) {
+                const int row = rg * 8 + (u3 ? 4 : 0) + (u4 ? 2 : 0) + r;
+                const unsigned owner = (unsigned)(row / RF_OWN);
+                float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
+                if (owner == crank) *reinterpret_cast<float4*>(qd) = o;
+                else {
+                    const unsigned pb = rf_mapa(smem_base, owner);
+                    rf_st_async_v4(pb + (rf_smem_u32(qd) - smem_base), o, pb + bar_off);
+                }
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void rf_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void rf_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+
+// Two groups of 32 actors per cluster (G = 2), software-pipelined, so that a chunk of N actors needs half as many
+// clusters.  Warps 0..7 ("layer warps") run hidden layers 1 and 2 for group 0, then for group 1, step after step.
+// Warps 8..15 ("tail warps", warp 8 + a for owned actor a of each group) take the whole tail of a group -- the
+// action-independent env precompute, head, sampling, env step, window staging, the push of the next input rows -- while
+// the layer warps compute the other group.  Arithmetic, operand order and Philox keys are those of the G = 1 schedule
+// (head_mode 1, reduction-free layer 1, rf2_layer2_direct = rf2_layer<false> bit for bit), so both give the same results.
+//
+// Hand-offs, per group g (each group has its own tiles, state and three mbarriers):
+//   layer -> peers: H1 rows (all 32) and H2 rows (owners' only) by st.async, counted on the receiver's h1[g] / h2[g];
+//   layer -> tail:  own H2 rows, named barrier 2 + g (layer warps bar.arrive, tail warps bar.sync; 512 threads);
+//   tail  -> peers: next X0 rows by st.async, counted on x0[g];
+//   tail  -> layer: own next X0 rows, named barrier 4 + g (tail warps bar.arrive, layer warps bar.sync).
+// No reverse "buffer free" signal is needed: every buffer of group g is rewritten only behind a chain of hand-offs that
+// starts after its last reader is done.
+//   * X0[g], step t+1: a peer pushes it after its head of step t, which needs this CTA's H2 rows of step t, which the
+//     layer warps push only after all of them passed layer 1 (rf_bar_math), the last reader of X0[g].  The tail warps
+//     rewrite their own rows after their head, i.e. after named barrier 2 + g, which every layer warp reaches after layer 2.
+//   * H1[g], step t+1: a peer pushes it after its layer 1 of step t+1, which needs this CTA's X0 rows of step t+1, which
+//     the tail warps push after named barrier 2 + g: after every layer warp has finished layer 2, the reader of H1[g].
+//   * H2[g], step t+1: written by layer 2 of step t+1 (peers' and own), behind layer 1 of step t+1, behind the X0 rows of
+//     step t+1 of every CTA of the cluster, which this CTA's tail pushes after its head of step t, the reader of H2[g].
+//   * the same chains order every st.async of step t+1 after the mbarrier wait of step t, so no phase receives bytes of
+//     the next one.  Each phase is armed once (expect_tx; arrival count 1) by thread 0 after the previous phase is known
+//     complete: h1[g] and h2[g] after the layer warps' wait on named barrier 4 + g (the tail waited h2[g] of the step
+//     before), x0[g] after the layer warps' own wait on x0[g].
+//   * named barriers 2 + g and 4 + g never see two generations of arrivals at once: each arrival of step t+1 sits behind
+//     the other side's arrival of step t on the other barrier.
+//   * the head slice buffer is used by the tail warps only, between named barrier 6 (tail warps, 256 threads) and the
+//     next group's named barrier 2 + g', which all 256 tail threads must reach.
+__device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
+    constexpr int G = 2;
+    cg::cluster_group cluster = cg::this_cluster();
+    const unsigned crank = cluster.block_rank();
+    extern __shared__ __align__(16) float smem[];
+    const unsigned smem_base = rf_smem_u32(smem);
+    unsigned peer_base[RF_CS - 1];
+#pragma unroll
+    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
+    __shared__ int s_pos[G][RF_OWN], s_ep[G][RF_OWN], s_cnt[G][RF_OWN];
+    __shared__ __align__(8) unsigned long long s_bar[G][3];   // per group: hidden layer 1 | last hidden layer rows | next input tile
+
+    const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
+    const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
+    const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
+    const int ldwh = p.ldw[2];
+    const int gs = p.gstride;
+    float* W1s = smem + p.oW1;
+    float* W2s = smem + p.oW2;
+    float* Whs = smem + p.oWh;
+    float* B1s = smem + p.oB;
+    float* B2s = B1s + Nc1;
+    float* Bhs = B2s + Nc2;
+    float* Zm = smem + p.oZf;
+    float* Zs = Zm + D;
+    float* Hs = smem + p.oHs;
+    const float* __restrict__ EWs = p.WsT;   // env matrices: global memory, through L1
+    const float* __restrict__ EWa = p.WaT;
+    const long long row0 = (long long)(blockIdx.x / RF_CS) * (G * RF_ROWS);
+
+    // ---- one-time loads (as G = 1, without the env matrices; tiles and state of both groups)
+    for (int f = tid; f < D * (Nc1 >> 2); f += RF_THREADS) {
+        const int k = f / (Nc1 >> 2), q = f - k * (Nc1 >> 2);
+        cp_async16(W1s + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
+    }
+    for (int f = tid; f < H1 * (Nc2 >> 2); f += RF_THREADS) {
+        const int k = f / (Nc2 >> 2), q = f - k * (Nc2 >> 2);
+        cp_async16(W2s + k * Nc2 + q * 4, p.W[1] + (long long)k * p.ldw[1] + crank * Nc2 + q * 4, 16);
+    }
+    for (int f = tid; f < (H2 * ldwh) >> 2; f += RF_THREADS) cp_async16(Whs + f * 4, p.W[2] + f * 4, 16);
+    cp_async_commit();
+    for (int n = tid; n < Nc1; n += RF_THREADS) B1s[n] = p.b[0][crank * Nc1 + n];
+    for (int n = tid; n < Nc2; n += RF_THREADS) B2s[n] = p.b[1][crank * Nc2 + n];
+    for (int n = tid; n < ldwh; n += RF_THREADS) Bhs[n] = (n < A) ? p.b[2][n] : 0.0f;
+    if (p.zf != nullptr) {
+        const float cnt = p.zf[2 * D];
+        for (int k = tid; k < D; k += RF_THREADS) {
+            const float mean = p.zf[k] / cnt;
+            const float var = p.zf[D + k] / cnt - mean * mean;
+            Zm[k] = mean;
+            Zs[k] = fmaxf(sqrtf(var), p.zf_eps);
+        }
+    }
+    if (tid < G * RF_OWN) {
+        const int g = tid / RF_OWN, a = tid - g * RF_OWN;
+        const long long i = row0 + g * RF_ROWS + crank * RF_OWN + a;
+        s_pos[g][a] = (i < p.N) ? p.stage_pos[i] : 0;
+        s_ep[g][a] = (i < p.N) ? p.ep_step[i] : 0;
+        s_cnt[g][a] = 0;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < G * RF_ROWS * D; idx += RF_THREADS) {
+        const int gm = idx / D, k = idx - gm * D;
+        const int g = gm / RF_ROWS, m = gm - g * RF_ROWS;
+        const long long i = row0 + g * RF_ROWS + m;
+        float v = (i < p.N) ? p.state[i * D + k] : 0.0f;
+        const int own = m - (int)crank * RF_OWN;
+        if (own >= 0 && own < RF_OWN) smem[p.oS + g * gs + own * D + k] = v;
+        if (p.zf != nullptr) v = fminf(fmaxf((v - Zm[k]) / Zs[k], -5.0f), 5.0f);
+        smem[p.oX0 + g * gs + m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
+    }
+    const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
+    if (tid == 0) {
+        for (int g = 0; g < G; ++g)
+            for (int i = 0; i < 3; ++i) rf_mbar_init(&s_bar[g][i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    // bytes a CTA receives from its three peers per step and group (as G = 1)
+    const unsigned tx_h1 = 3u * RF_ROWS * Nc1 * 4u, tx_h2 = 3u * RF_OWN * Nc2 * 4u, tx_x0 = 3u * RF_OWN * D * 4u;
+    const bool layer = warp < RF_OWN;
+    const int own = warp & (RF_OWN - 1);              // tail warp 8 + own: owned actor `own` of each group
+    if (!layer && lane < A) {
+        for (int g = 0; g < G; ++g) {
+            const long long i = row0 + g * RF_ROWS + crank * RF_OWN + own;
+            const float sc = (i < p.N && p.log_noise != nullptr) ? expf(p.log_noise[i]) : 1.0f;
+            smem[p.oAct + g * gs + 2 * RF_OWN * A + own * A + lane] = __fmul_rn(expf(p.log_var[lane]), sc);
+        }
+    }
+    cp_async_wait<0>();
+    cluster.sync();
+
+    if (layer) {
+        for (int t = 0; t < p.T; ++t) {
+            const bool final_step = (t == p.T - 1);
+            const int rf_t = t;
+            RF_STAMP(0, 0);
+            for (int g = 0; g < G; ++g) {
+                float* X0 = smem + p.oX0 + g * gs;
+                float* Hb1 = smem + p.oH1 + g * gs;
+                float* Hb2 = smem + p.oH2 + g * gs;
+                if (t > 0) {                                   // own rows from the tail warps, the peers' rows by st.async
+                    rf_bar_sync(4 + g, 2 * 256);
+                    rf_mbar_wait(&s_bar[g][2], (unsigned)(t - 1) & 1u);
+                }
+                if (tid == 0) {
+                    rf_mbar_arm(&s_bar[g][0], tx_h1);
+                    rf_mbar_arm(&s_bar[g][1], tx_h2);
+                    if (!final_step) rf_mbar_arm(&s_bar[g][2], tx_x0);
+                }
+                rf2_layer1<true>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank,
+                                 rf_smem_u32(&s_bar[g][0]) - smem_base, rf_t);
+                rf_bar_math();
+                rf_mbar_wait(&s_bar[g][0], (unsigned)t & 1u);
+                RF_STAMP(3 + 2 * g, 0);
+                rf2_layer2_direct(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, smem_base, crank,
+                                  rf_smem_u32(&s_bar[g][1]) - smem_base);
+                RF_STAMP(4 + 2 * g, 0);
+                rf_bar_arrive(2 + g, 2 * 256);
+            }
+        }
+    } else {
+        for (int t = 0; t < p.T; ++t) {
+            const unsigned long long ctr = ctr0 + (unsigned long long)t;
+            const bool final_step = (t == p.T - 1);
+            const int rf_t = t;
+            for (int g = 0; g < G; ++g) {
+                float* X0 = smem + p.oX0 + g * gs;
+                float* Hb2 = smem + p.oH2 + g * gs;
+                float* S = smem + p.oS + g * gs;
+                float* Nx = smem + p.oNext + g * gs;
+                float* Ac = smem + p.oAct + g * gs;
+                float* Sd = Ac + 2 * RF_OWN * A;
+                float* Zn = Sd + RF_OWN * A;
+                float* Eacc = smem + p.oPre + g * gs;
+                float* Egx = Eacc + RF_OWN * D;
+                float* Erz = Egx + RF_OWN * D;
+                float* Eq = Erz + RF_OWN * D;
+                const int m_own = (int)crank * RF_OWN + own;
+                const long long i_own = row0 + g * RF_ROWS + m_own;
+                const bool valid = i_own < p.N;
+                RF_STAMP(8 + 4 * g, 256);
+                // ---- everything of the step that does not depend on the action: the env warps' arithmetic of G = 1, but a
+                // lane takes the adjacent columns d, d + 1 together (two independent FMA chains, float2 weight and float4
+                // state loads): here this work is on the step's critical path, next to layer warps that keep the
+                // shared-memory pipe busy, so its loads and dependent latencies are what count
+                {
+                    const float* sh = S + own * D;
+                    float q = 0.0f;
+                    for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
+                    q = warp_sum(q);
+                    const bool h_done = (p.max_steps > 0) && (s_ep[g][own] + 1 >= p.max_steps);
+                    for (int d = 2 * lane; d < D; d += 64) {          // D % 4 == 0: d + 1 < D
+                        float acc0 = 0.0f, acc1 = 0.0f;
+#pragma unroll 4
+                        for (int k = 0; k < D; k += 4) {
+                            const float4 s4 = *reinterpret_cast<const float4*>(sh + k);
+                            const float2 w0 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 0) * D + d));
+                            const float2 w1 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 1) * D + d));
+                            const float2 w2 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 2) * D + d));
+                            const float2 w3 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 3) * D + d));
+                            acc0 = fmaf(w0.x, s4.x, acc0); acc1 = fmaf(w0.y, s4.x, acc1);
+                            acc0 = fmaf(w1.x, s4.y, acc0); acc1 = fmaf(w1.y, s4.y, acc1);
+                            acc0 = fmaf(w2.x, s4.z, acc0); acc1 = fmaf(w2.y, s4.z, acc1);
+                            acc0 = fmaf(w3.x, s4.w, acc0); acc1 = fmaf(w3.y, s4.w, acc1);
+                        }
+                        const unsigned long long key = ((unsigned long long)i_own << 20) | (unsigned long long)d;
+                        const Philox4 r0 = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr, key);
+                        const Philox4 r1 = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr, key + 1);
+                        const float2 gz0 = box_muller(r0.x, r0.y), gz1 = box_muller(r1.x, r1.y);
+                        *reinterpret_cast<float2*>(Eacc + own * D + d) = make_float2(acc0, acc1);
+                        *reinterpret_cast<float2*>(Egx + own * D + d) = make_float2(gz0.x, gz1.x);
+                        *reinterpret_cast<float2*>(Erz + own * D + d) =
+                            h_done ? make_float2(box_muller(r0.z, r0.w).x, box_muller(r1.z, r1.w).x) : make_float2(0.0f, 0.0f);
+                        if (d == 0) {
+                            Eq[2 * own] = q;
+                            Eq[2 * own + 1] = gz0.y;
+                        }
+                    }
+                    if (!p.deterministic && lane < A) {
+                        const int j = lane;
+                        const Philox4 r = philox4x32_10(p.agent_seed, ctr, ((unsigned long long)i_own << 16) | (unsigned long long)(j >> 2));
+                        const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
+                        const int c = j & 3;
+                        Zn[own * A + j] = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
+                    }
+                }
+                rf_bar_sync(2 + g, 2 * 256);                   // own rows of the last hidden layer, then the peers' rows
+                rf_mbar_wait(&s_bar[g][1], (unsigned)t & 1u);
+                RF_STAMP(9 + 4 * g, 256);
+                // ---- head, head_mode 1: the 16 k slices of G = 1, two per tail warp, same lane layout and sums
+                {
+                    const int ks = H2 >> 4;
+                    const int a8 = lane >> 2, ksub = lane & 3;
+                    const bool u1 = (lane & 2) != 0, u0 = (lane & 1) != 0;
+                    for (int sl = own; sl < 16; sl += RF_OWN) {
+                        const float* hrow = Hb2 + a8 * p.ldh2 + sl * ks;
+                        const float* wbase = Whs + (sl * ks) * ldwh;
+                        for (int n8 = 0; n8 < A; n8 += 8) {
+                            float s8[8];
+#pragma unroll
+                            for (int jj = 0; jj < 8; ++jj) s8[jj] = 0.0f;
+                            const bool second = (n8 + 4 < ldwh);
+                            for (int k = ksub; k < ks; k += 4) {
+                                const float hv = hrow[k];
+                                const float* wr = wbase + k * ldwh + n8;
+                                const float4 w0 = *reinterpret_cast<const float4*>(wr);
+                                s8[0] = fmaf(hv, w0.x, s8[0]); s8[1] = fmaf(hv, w0.y, s8[1]);
+                                s8[2] = fmaf(hv, w0.z, s8[2]); s8[3] = fmaf(hv, w0.w, s8[3]);
+                                if (second) {
+                                    const float4 w1 = *reinterpret_cast<const float4*>(wr + 4);
+                                    s8[4] = fmaf(hv, w1.x, s8[4]); s8[5] = fmaf(hv, w1.y, s8[5]);
+                                    s8[6] = fmaf(hv, w1.z, s8[6]); s8[7] = fmaf(hv, w1.w, s8[7]);
+                                }
+                            }
+                            float t4[4], t2[2];
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const float recv = __shfl_xor_sync(0xffffffffu, u1 ? s8[i] : s8[i + 4], 2);
+                                t4[i] = (u1 ? s8[i + 4] : s8[i]) + recv;
+                            }
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                const float recv = __shfl_xor_sync(0xffffffffu, u0 ? t4[i] : t4[i + 2], 1);
+                                t2[i] = (u0 ? t4[i + 2] : t4[i]) + recv;
+                            }
+                            const int j0 = n8 + (u1 ? 4 : 0) + (u0 ? 2 : 0);
+                            float* dst = Hs + ((sl * RF_OWN + a8) * ldwh);
+                            if (j0 < A) dst[j0] = t2[0];
+                            if (j0 + 1 < A) dst[j0 + 1] = t2[1];
+                        }
+                    }
+                }
+                rf_bar_sync(6, 256);
+                RF_STAMP(10 + 4 * g, 256);
+                // ---- action, env step, bookkeeping (the owner warps' code of G = 1)
+                float rew, dn;
+                int slot = SLOT_NONE;
+                {
+                    const int pos = s_pos[g][own];
+                    if (lane < A) {
+                        const int j = lane;
+                        float pre = 0.0f;
+#pragma unroll 4
+                        for (int w = 0; w < RF_THREADS / 32; ++w) pre += Hs[(w * RF_OWN + own) * ldwh + j];
+                        const float mu = rf_act(pre + Bhs[j], p.act[2]);
+                        const float sd = Sd[own * A + j];
+                        float a = mu;
+                        if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
+                        a = fminf(fmaxf(a, -1.0f), 1.0f);
+                        Ac[own * A + j] = a;
+                        if (valid) {
+                            p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
+                            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + j] = mu;
+                            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + A + j] = sd;
+                            if (final_step) {
+                                p.action[i_own * A + j] = a;
+                                p.pd[i_own * 2 * A + j] = mu;
+                                p.pd[i_own * 2 * A + A + j] = sd;
+                            }
+                        }
+                    }
+                    __syncwarp();
+                    float* sown = S + own * D;
+                    const int ep = s_ep[g][own] + 1;
+                    const bool is_done = (p.max_steps > 0) && (ep >= p.max_steps);
+                    dn = is_done ? 1.0f : 0.0f;
+                    rew = -Eq[2 * own] / (float)D + 0.1f * Eq[2 * own + 1];
+                    for (int d = lane; d < D; d += 32) {
+                        float acc = Eacc[own * D + d];
+#pragma unroll 4
+                        for (int k = 0; k < A; ++k) acc = fmaf(__ldg(EWa + k * D + d), Ac[own * A + k], acc);
+                        const float nxt = tanhf(acc) + 0.01f * Egx[own * D + d];
+                        Nx[own * D + d] = nxt;
+                        sown[d] = is_done ? Erz[own * D + d] : nxt;
+                        if (valid && final_step) p.obs_next[i_own * D + d] = nxt;
+                    }
+                    if (lane == 0) {
+                        s_ep[g][own] = is_done ? 0 : ep;
+                        if (valid && final_step) {
+                            p.reward[i_own] = rew;
+                            p.done[i_own] = dn;
+                        }
+                        if (valid && pos + 1 == p.n_step) {
+                            const int w = s_cnt[g][own];
+                            if (w < p.Wout) {
+                                slot = (int)(i_own * p.Wout + w);
+                                p.ev_step[slot] = t;
+                                s_cnt[g][own] = w + 1;
+                            } else {
+                                slot = SLOT_DROPPED;
+                            }
+                        }
+                    }
+                    slot = __shfl_sync(0xffffffffu, slot, 0);
+                    __syncwarp();
+                }
+                commit_actor(valid, (int)i_own, lane, 32, Nx + own * D, S + own * D, rew, dn, p.n_step, p.stride, D, A,
+                             &s_pos[g][own], slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew, p.stage_done, p.o_obs,
+                             p.o_act, p.o_pd, p.o_rew, p.o_done, WarpBarrier());
+                RF_STAMP(11 + 4 * g, 256);
+                if (!final_step) {                             // next observation -> z-filter -> every CTA's input tile
+                    const int q4 = lane;
+                    if (q4 < (D >> 2)) {
+                        float4 v = *reinterpret_cast<const float4*>(S + own * D + q4 * 4);
+                        if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (p.zf != nullptr) {
+                            const float4 zm = *reinterpret_cast<const float4*>(Zm + q4 * 4);
+                            const float4 zs = *reinterpret_cast<const float4*>(Zs + q4 * 4);
+                            v.x = fminf(fmaxf((v.x - zm.x) / zs.x, -5.0f), 5.0f);
+                            v.y = fminf(fmaxf((v.y - zm.y) / zs.y, -5.0f), 5.0f);
+                            v.z = fminf(fmaxf((v.z - zm.z) / zs.z, -5.0f), 5.0f);
+                            v.w = fminf(fmaxf((v.w - zm.w) / zs.w, -5.0f), 5.0f);
+                            if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
+                        }
+                        float* qx = X0 + m_own * p.ldx0 + q4 * 4;
+                        *reinterpret_cast<float4*>(qx) = v;
+                        const unsigned off = rf_smem_u32(qx) - smem_base;
+                        const unsigned bar_off = rf_smem_u32(&s_bar[g][2]) - smem_base;
+#pragma unroll
+                        for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off);
+                    }
+                    rf_bar_arrive(4 + g, 2 * 256);
+                }
+            }
+        }
+    }
+    cluster.sync();                                           // nobody leaves while a peer may still address its shared memory
+
+    if (!layer) {
+        for (int g = 0; g < G; ++g) {
+            const long long i_own = row0 + g * RF_ROWS + (int)crank * RF_OWN + own;
+            if (i_own >= p.N) continue;
+            const float* S = smem + p.oS + g * gs;
+            for (int d = lane; d < D; d += 32) p.state[i_own * D + d] = S[own * D + d];
+            if (lane == 0) {
+                p.stage_pos[i_own] = s_pos[g][own];
+                p.ep_step[i_own] = s_ep[g][own];
+                p.ev_count[i_own] = s_cnt[g][own];
+            }
+        }
+    }
+}
+
+template <bool ASYNC, int G>
 __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     ppo_rollout2_kernel(const __grid_constant__ RfParams p) {
+    static_assert(G == 1 || (G == 2 && ASYNC), "two groups per cluster use the mbarrier hand-offs");
+    RF_CTA_STAMP(1);
+    if constexpr (G == 2) {
+        rf2_two_groups(p);
+        RF_CTA_STAMP(2);
+        return;
+    }
     cg::cluster_group cluster = cg::this_cluster();
     const unsigned crank = cluster.block_rank();
     extern __shared__ __align__(16) float smem[];
@@ -1085,6 +1566,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
             p.ev_count[i_own] = s_cnt[own];
         }
     }
+    RF_CTA_STAMP(2);
 }
 
 // ---- post-pass 1 (one block): rank the chunk's window completions in (step, actor) order, give them FIFO slots
@@ -1170,7 +1652,12 @@ __global__ void __launch_bounds__(256) ppo_rollout_copy_kernel(const int* __rest
     copy_floats(r_done + (long long)slot * n_step, o_done + e * n_step, n_step, g, G);
 }
 
-bool rf_plan(const sb200_mlp* net, int D, int A, RfParams* p, size_t* smem_bytes) {
+// Shared-memory plan of ppo_rollout2_kernel<., G>.  G = 1: weights, the cluster's activation tiles, the k-split partial
+// tiles (Part), the env matrices and the owned actors' state.  G = 2: no Part (both layers are reduction-free), the env
+// matrices stay in global memory (read through L1 by the tail warps, off the layers' path), a 4 KB head slice buffer,
+// and the per-group tiles and state twice, `gstride` floats apart.  At the configs[1] shape [64, 256, 256, 8]:
+// G = 1 204 512 B, G = 2 219 552 B.
+bool rf_plan(const sb200_mlp* net, int D, int A, int G, RfParams* p, size_t* smem_bytes) {
     if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0) return false;
     const int H1 = net->dims[1], H2 = net->dims[2];
     if (net->dims[0] != D || net->dims[3] != A) return false;
@@ -1181,15 +1668,28 @@ bool rf_plan(const sb200_mlp* net, int D, int A, RfParams* p, size_t* smem_bytes
     const int oW1 = take((long long)D * Nc1), oW2 = take((long long)H1 * Nc2), oWh = take((long long)H2 * ldwh);
     const int oB = take(Nc1 + Nc2 + ldwh);
     const int ldx0 = D + 4, ldh1 = H1 + 4, ldh2 = H2 + 4;
-    const int oX0 = take(RF_ROWS * ldx0), oH1 = take(RF_ROWS * ldh1), oH2 = take(RF_OWN * ldh2);
-    const int oPart = take(4LL * RF_ROWS * (Nc1 > Nc2 ? Nc1 : Nc2));
-    const int oZf = take(2 * D), oEnv = take((long long)D * D + A * D);
-    const int oS = take(RF_OWN * D), oNext = take(RF_OWN * D), oAct = take(6 * RF_OWN * A);
-    const int oPre = take(3 * RF_OWN * D + 2 * RF_OWN);
+    int oX0, oH1, oH2, oPart = -1, oZf, oEnv = -1, oS, oNext, oAct, oPre, oHs = -1, gstride = 0;
+    if (G == 1) {
+        oX0 = take(RF_ROWS * ldx0); oH1 = take(RF_ROWS * ldh1); oH2 = take(RF_OWN * ldh2);
+        oPart = take(4LL * RF_ROWS * (Nc1 > Nc2 ? Nc1 : Nc2));
+        oZf = take(2 * D); oEnv = take((long long)D * D + A * D);
+        oS = take(RF_OWN * D); oNext = take(RF_OWN * D); oAct = take(6 * RF_OWN * A);
+        oPre = take(3 * RF_OWN * D + 2 * RF_OWN);
+    } else {
+        oZf = take(2 * D);
+        oHs = take(16LL * RF_OWN * ldwh);
+        const long long g0 = off;
+        oX0 = take(RF_ROWS * ldx0); oH1 = take(RF_ROWS * ldh1); oH2 = take(RF_OWN * ldh2);
+        oS = take(RF_OWN * D); oNext = take(RF_OWN * D); oAct = take(6 * RF_OWN * A);
+        oPre = take(3 * RF_OWN * D + 2 * RF_OWN);
+        gstride = (int)(off - g0);
+        off += (long long)(G - 1) * gstride;
+    }
     if ((size_t)off * sizeof(float) > 224 * 1024) return false;
     if (p != nullptr) {
         p->oW1 = oW1; p->oW2 = oW2; p->oWh = oWh; p->oB = oB; p->oX0 = oX0; p->oH1 = oH1; p->oH2 = oH2; p->oPart = oPart;
         p->oZf = oZf; p->oEnv = oEnv; p->oS = oS; p->oNext = oNext; p->oAct = oAct; p->oPre = oPre;
+        p->oHs = oHs; p->gstride = gstride;
         p->ldx0 = ldx0; p->ldh1 = ldh1; p->ldh2 = ldh2;
         p->D = D; p->H1 = H1; p->H2 = H2; p->A = A;
     }
@@ -1197,25 +1697,84 @@ bool rf_plan(const sb200_mlp* net, int D, int A, RfParams* p, size_t* smem_bytes
     return true;
 }
 
+template <int G>
+cudaError_t rf_query_clusters(size_t smem, int* n) {
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = RF_CS;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.gridDim = dim3(RF_CS);
+    cfg.blockDim = dim3(RF_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    return cudaOccupancyMaxActiveClusters(n, ppo_rollout2_kernel<true, G>, &cfg);
+}
+
+// How many 4-CTA clusters of ppo_rollout2_kernel<true, G> with `smem` dynamic bytes the current device runs at once.
+// A cluster must sit inside one GPC, and an H100's GPCs have uneven SM counts, so this is below SMs / 4 (30 on an H100
+// SXM with 132 SMs at the configs[1] plan).  Queried once per (device, G, bytes).
+int rf_max_clusters(int G, size_t smem, int* n_out) {
+    struct Entry { int dev, G; size_t smem; int n; };
+    static std::mutex mu;
+    static Entry cache[16];
+    static int n_cache = 0;
+    int dev = 0;
+    SB200_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(mu);
+    for (int i = 0; i < n_cache; ++i)
+        if (cache[i].dev == dev && cache[i].G == G && cache[i].smem == smem) {
+            *n_out = cache[i].n;
+            return SB200_OK;
+        }
+    int n = 0;
+    SB200_CUDA(G == 2 ? rf_query_clusters<2>(smem, &n) : rf_query_clusters<1>(smem, &n));
+    if (n_cache < 16) cache[n_cache++] = Entry{dev, G, smem, n};
+    *n_out = n;
+    return SB200_OK;
+}
+
 }  // namespace
 
 int sb200_rollout_fused_init() {
     SB200_CUDA(cudaFuncSetAttribute(ppo_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     return SB200_OK;
 }
 
 #ifdef RF_TRACE
+static unsigned g_rf_last_grid = 0;
+static size_t g_rf_last_smem = 0;
+static int g_rf_last_groups = 0;
+
 extern "C" int sb200_debug_rf_trace(long long* host_out) {
     SB200_CUDA(cudaDeviceSynchronize());
     SB200_CUDA(cudaMemcpyFromSymbol(host_out, g_rf_trace, sizeof(g_rf_trace)));
     return SB200_OK;
 }
+
+// per-CTA [smid, entry ns, exit ns] of the last persistent launch (RF_TR_CTAS rows); info = {grid CTAs, dynamic shared
+// bytes, groups per cluster G, cudaOccupancyMaxActiveClusters of ppo_rollout2_kernel<true, G> at that configuration}
+extern "C" int sb200_debug_rf_ctas(long long* host_out, long long* info) {
+    SB200_CUDA(cudaDeviceSynchronize());
+    SB200_CUDA(cudaMemcpyFromSymbol(host_out, g_rf_cta, sizeof(g_rf_cta)));
+    int n = 0;
+    const int rc = rf_max_clusters(g_rf_last_groups, g_rf_last_smem, &n);
+    if (rc != SB200_OK) return rc;
+    info[0] = g_rf_last_grid;
+    info[1] = (long long)g_rf_last_smem;
+    info[2] = g_rf_last_groups;
+    info[3] = n;
+    return SB200_OK;
+}
 #endif
 
 extern "C" int sb200_ppo_rollout_supported(const sb200_mlp* net, int D, int A) {
-    return rf_plan(net, D, A, nullptr, nullptr) ? 1 : 0;
+    return rf_plan(net, D, A, 1, nullptr, nullptr) ? 1 : 0;
 }
 
 extern "C" size_t sb200_ppo_rollout_scratch_ints(int N, int W, int T) {
@@ -1227,7 +1786,7 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     SB200_REQUIRE(a != nullptr && a->net != nullptr);
     RfParams p;
     size_t smem = 0;
-    if (!rf_plan(a->net, a->D, a->A, &p, &smem)) return SB200_ERR_UNSUPPORTED;
+    if (!rf_plan(a->net, a->D, a->A, 1, &p, &smem)) return SB200_ERR_UNSUPPORTED;
     SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->n_step >= 1 && a->stride >= 1 && a->W >= 1);
     SB200_REQUIRE(a->state && a->WsT && a->WaT && a->ep_step && a->action && a->pd && a->obs_next && a->reward && a->done);
     SB200_REQUIRE(a->log_var && a->stage_pos && a->stage_obs && a->stage_act && a->stage_pd && a->stage_rew && a->stage_done);
@@ -1287,10 +1846,40 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     // default: mbarrier-signalled st.async hand-offs instead of the three cluster barriers per step (1.47 -> 1.38 ms per
     // 128-step chunk of 1024 actors, same results bit for bit); SB200_RF_ASYNC=0 selects the barrier.cluster variant
     static const int rf_async = [] { const char* e = getenv("SB200_RF_ASYNC"); return e ? atoi(e) : 1; }();
-    if (v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20))
-        ppo_rollout2_kernel<true><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else if (v2) ppo_rollout2_kernel<false><<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else ppo_rollout_kernel<<<(unsigned)(clusters * RF_CS), RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    const bool async = v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20);
+    // Two groups of 32 actors per cluster when the device cannot hold all ceil(N / 32) one-group clusters at once (the
+    // clusters that do not fit run as a whole further wave of the chunk) AND two groups at least halve the number of
+    // waves: a two-group step does both groups' work, 1.74x the time of a one-group step at the configs[1] shape on an
+    // H100 (38 K vs 22 K cycles), so fewer waves pay only when they are at most half as many (1024 actors: 2 -> 1
+    // wave; 4096 actors: 5 -> 3 waves would be slower).  Same results as one group: same arithmetic (head_mode 1,
+    // reduction-free layer 1, rf2_layer2_direct).
+    int groups = 1;
+    RfParams p2 = p;
+    size_t smem2 = 0;
+    if (async && p.l1_direct && p.head_mode == 1 && rf_plan(a->net, a->D, a->A, 2, &p2, &smem2)) {
+        int fit1 = 0, fit2 = 0;
+        int rc = rf_max_clusters(1, smem, &fit1);
+        if (rc == SB200_OK) rc = rf_max_clusters(2, smem2, &fit2);
+        if (rc != SB200_OK) return rc;
+        if (fit1 >= 1 && fit2 >= 1 && clusters > fit1) {
+            const long long waves1 = (clusters + fit1 - 1) / fit1, waves2 = ((clusters + 1) / 2 + fit2 - 1) / fit2;
+            if (2 * waves2 <= waves1) {
+                groups = 2;
+                p = p2;
+                smem = smem2;
+            }
+        }
+    }
+    const long long ctas = (clusters + groups - 1) / groups * RF_CS;
+#ifdef RF_TRACE
+    g_rf_last_grid = (unsigned)ctas;
+    g_rf_last_smem = smem;
+    g_rf_last_groups = groups;
+#endif
+    if (groups == 2) ppo_rollout2_kernel<true, 2><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    else if (async) ppo_rollout2_kernel<true, 1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    else if (v2) ppo_rollout2_kernel<false, 1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    else ppo_rollout_kernel<<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     return sb200_launch_status();
 }
 

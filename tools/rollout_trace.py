@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """clock64 timeline of the persistent rollout kernel: builds a -DRF_TRACE variant of the library under tools/_trace/
-(never the shipped .so), runs one chunk at the bench shape and prints, per phase, the cycles cluster 0's CTAs spent.
+(never the shipped .so), runs one chunk at the bench shape and prints how many clusters the device holds at once, in
+how many waves the chunk's CTAs ran (every CTA's SM and %globaltimer at entry and exit), and, per phase, the cycles
+cluster 0's CTAs spent.
 
     python tools/rollout_trace.py build      # here (nvcc only)
     python tools/rollout_trace.py            # on the GPU box
@@ -40,6 +42,53 @@ def build():
     print(LIB)
 
 
+def waves(L, np):
+    """Residency of the last chunk's launch: how many 4-CTA clusters the device can hold at once at this launch
+    configuration, and in how many waves the CTAs actually ran (a CTA that starts after another has exited belongs
+    to a later wave)."""
+    cta = np.zeros((4096, 3), dtype=np.int64)
+    info = np.zeros(4, dtype=np.int64)
+    L.sb200_debug_rf_ctas.argtypes = [C.c_void_p, C.c_void_p]
+    assert L.sb200_debug_rf_ctas(cta.ctypes.data_as(C.c_void_p), info.ctypes.data_as(C.c_void_p)) == 0
+    grid, smem, groups, max_clusters = (int(v) for v in info)
+    cta = cta[:grid]
+    print('launch: %d CTAs = %d clusters of 4 (%d group(s) of 32 actors each), 512 threads, %d B dynamic shared memory; '
+          'cudaOccupancyMaxActiveClusters = %d' % (grid, grid // 4, groups, smem, max_clusters))
+    t0 = cta[:, 1].min()
+    start, end = cta[:, 1] - t0, cta[:, 2] - t0
+    wave = np.zeros(grid, dtype=np.int64)
+    order = np.argsort(start, kind='stable')
+    first_end = None
+    w = 0
+    for i in order:                                   # a new wave begins at the first CTA that starts after an exit
+        if first_end is not None and start[i] >= first_end:
+            w += 1
+            first_end = None
+        wave[i] = w
+        first_end = end[i] if first_end is None else min(first_end, end[i])
+    print('%d distinct SMs; %d wave(s); kernel span %.3f ms' % (len(set(cta[:, 0].tolist())), w + 1, end.max() / 1e6))
+    for k in range(w + 1):
+        sel = wave == k
+        print('   wave %d: %3d CTAs, start %.3f..%.3f ms, end %.3f..%.3f ms, duration %.3f ms'
+              % (k, sel.sum(), start[sel].min() / 1e6, start[sel].max() / 1e6, end[sel].min() / 1e6, end[sel].max() / 1e6,
+                 (end[sel].max() - start[sel].min()) / 1e6))
+    return groups
+
+
+def two_groups(tr, np):
+    """Cycle stamps of the two-group schedule, relative to the layer warps' step top (group 0's layer 1 begins)."""
+    marks = [(3, 'layer warps: g0 layer 1 + H1 wait'), (4, 'layer warps: g0 layer 2'), (5, 'layer warps: g1 x0 wait + layer 1 + H1 wait'),
+             (6, 'layer warps: g1 layer 2'), (8, 'tail warps: g0 tail starts'), (9, 'tail warps: g0 precompute + H2 wait'),
+             (10, 'tail warps: g0 head'), (11, 'tail warps: g0 sample+env+commit'), (12, 'tail warps: g1 tail starts'),
+             (13, 'tail warps: g1 precompute + H2 wait'), (14, 'tail warps: g1 head'), (15, 'tail warps: g1 sample+env+commit')]
+    for cta in range(4):
+        d = tr[cta]
+        step = np.median(d[1:, 0] - d[:-1, 0])
+        print('CTA %d: step period %.0f cycles (cycles since step top)' % (cta, step))
+        for i, name in marks:
+            print('   %-46s %7.0f' % (name, np.median(d[:, i] - d[:, 0])))
+
+
 def main():
     import numpy as np
     import torch
@@ -62,8 +111,12 @@ def main():
     torch.cuda.synchronize()
     tr = np.zeros((4, 8, 32), dtype=np.int64)
     L = _lib.lib()
+    groups = waves(L, np)
     L.sb200_debug_rf_trace.argtypes = [C.c_void_p]
     assert L.sb200_debug_rf_trace(tr.ctypes.data_as(C.c_void_p)) == 0
+    if groups == 2:
+        two_groups(tr, np)
+        return
     for cta in range(4):
         print('CTA %d (cycles since step top; delta)' % cta)
         d = tr[cta]
