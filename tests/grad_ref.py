@@ -154,6 +154,85 @@ def value(layers, x, ret):
     return out
 
 
+def lstm(x, h0, c0, w_ih, w_hh, b_ih, b_hh):
+    """One torch.nn.LSTM layer (batch_first, gate order i, f, g, o) as a plain cell loop, differentiable: no copies, so
+    callers pass float64 leaves.  x [B, L, D]; h0 / c0 [B, H] or None (zeros).  -> dict: ``h`` / ``c`` [B, L, H] (the
+    output and cell sequences), ``gates`` [B, L, 4H] (activated: sigmoid i, f, o and tanh g), ``pre`` (list of L
+    [B, 4H] gate pre-activations, to take gradients with respect to), ``h_last`` / ``c_last`` [B, H]."""
+    B, L, _ = x.shape
+    H = w_hh.shape[1]
+    h = x.new_zeros(B, H) if h0 is None else h0
+    c = x.new_zeros(B, H) if c0 is None else c0
+    hs, cs, gs, pres = [], [], [], []
+    for t in range(L):
+        pre = F.linear(x[:, t], w_ih, b_ih) + F.linear(h, w_hh, b_hh)
+        i, f, g, o = torch.sigmoid(pre[:, :H]), torch.sigmoid(pre[:, H:2 * H]), torch.tanh(pre[:, 2 * H:3 * H]), \
+            torch.sigmoid(pre[:, 3 * H:])
+        c = f * c + i * g
+        h = o * torch.tanh(c)
+        pres.append(pre)
+        gs.append(torch.cat((i, f, g, o), 1))
+        hs.append(h)
+        cs.append(c)
+    return {'h': torch.stack(hs, 1), 'c': torch.stack(cs, 1), 'gates': torch.stack(gs, 1), 'pre': pres, 'h_last': h,
+            'c_last': c}
+
+
+def _rnn_features(stem, x, h0, c0, zs):
+    """z-filter (``zs`` = its statistics, or None: off) -> LSTM from the DETACHED initial cells (ppo.py:507-510) -> rows
+    b*L + t.  ``stem`` = (w_ih, w_hh, b_ih, b_hh) float64 leaves."""
+    x = f64(x)
+    if zs is not None:
+        x = zfilter(x, zs)
+    B, L = x.shape[:2]
+    r = lstm(x, None if h0 is None else f64(h0).to(x.device), None if c0 is None else f64(c0).to(x.device), *stem)
+    return r['h'].reshape(B * L, -1)
+
+
+def rnn_features(stem, x, h0, c0, zs=None):
+    """The head input of RNN mode in float64, without gradients: rows b*L + t of the LSTM outputs."""
+    with torch.no_grad():
+        return _rnn_features([f64(t) for t in stem], x, h0, c0, zs)
+
+
+_STEM_NAMES = ['g_w_ih', 'g_w_hh', 'g_b_ih', 'g_b_hh']
+
+
+def ppo_policy_rnn(stem, layers, log_var, x, h0, c0, actions, adv, behave, mode, zs=None, masks=None, **hyper):
+    """RNN mode's policy loss (ppo.py:507-556): raw observations x [B, L, D] -> z-filter -> LSTM from (h0, c0) -> actor
+    head -> loss, over the B*L rows b*L + t.  ``grads`` per head layer, ``g_log_var``, ``stem`` = the gradients of
+    (W_ih, W_hh, b_ih, b_hh) in torch's layout, ``g_pre`` and the loss statistics.  ``masks`` as in trunk."""
+    S = [f64(t).requires_grad_(True) for t in stem]
+    L = _leaves(layers)
+    lv = f64(log_var).reshape(-1).requires_grad_(True)
+    pre = trunk(_rnn_features(S, x, h0, c0, zs), L, masks=masks)
+    A = pre.shape[1]
+    ref = hyper.pop('ref', None)
+    loss, st = _policy_loss(pre, lv, f64(actions).reshape(-1, A), f64(adv).reshape(-1), f64(behave).reshape(-1, 2 * A),
+                            mode, ref=f64(ref).reshape(-1, 2 * A) if ref is not None else None, **hyper)
+    nl = 2 * len(L)
+    out = _result(loss, st, _flat(L) + [lv, pre] + S, ['_g%d' % i for i in range(nl)] + ['g_log_var', 'g_pre'] + _STEM_NAMES)
+    out['grads'] = _pairs([out.pop('_g%d' % i) for i in range(nl)])
+    out['stem'] = tuple(out.pop(k) for k in _STEM_NAMES)
+    return out
+
+
+def value_rnn(stem, layers, x, h0, c0, ret, zs=None, masks=None):
+    """RNN mode's value loss mean((v - ret)^2) over the B*L rows (ppo.py:311-353): ``grads`` per critic layer,
+    ``stem`` as in ppo_policy_rnn, ``g_pre`` = dL/dv."""
+    S = [f64(t).requires_grad_(True) for t in stem]
+    L = _leaves(layers)
+    v = trunk(_rnn_features(S, x, h0, c0, zs), L, masks=masks)
+    ret = f64(ret).reshape(-1, 1).to(v.device)
+    loss = (v - ret).pow(2).mean()
+    st = {'loss': loss, 'explained_var': 1 - torch.var(ret - v) / torch.var(ret)}
+    nl = 2 * len(L)
+    out = _result(loss, st, _flat(L) + [v] + S, ['_g%d' % i for i in range(nl)] + ['g_pre'] + _STEM_NAMES)
+    out['grads'] = _pairs([out.pop('_g%d' % i) for i in range(nl)])
+    out['stem'] = tuple(out.pop(k) for k in _STEM_NAMES)
+    return out
+
+
 def ddpg_critic(layers, x, actions, y, aux_layer=1):
     """nn.MSELoss()(Q(s, a), y) of oracle/ddpg.py: ``grads`` per critic layer, ``g_pre`` = dL/dQ, stat ``q_mean``."""
     L = _leaves(layers)
