@@ -118,11 +118,12 @@ int sb200_mlp_forward_packed_f32(const sb200_mlp* net, const float* packed, cons
  *   workspace_bytes: caller-owned scratch for the per-call weight images (hi / lo planes in operand layout); 0 when
  *     unsupported.  One workspace must not be shared by calls that may run concurrently.
  *   forward: out[rows][ld_out] = network output (only the last layer is written: no saved activations, no save_x).
- *     SB200_ERR_UNSUPPORTED for other shapes -- callers then use sb200_mlp_forward_f32. */
+ *     SB200_ERR_UNSUPPORTED for other shapes -- callers then use sb200_mlp_forward_f32.  max_grid >= 1 caps the
+ *     persistent grid below one CTA per SM (0: no cap); tiles and their arithmetic do not depend on it. */
 int sb200_mlp_tc5_supported(const sb200_mlp* net, int64_t rows);
 size_t sb200_mlp_tc5_workspace_bytes(const sb200_mlp* net);
 int sb200_mlp_forward_tc5_f32(const sb200_mlp* net, const sb200_zfilter* zf, const sb200_rows* in, float* out,
-                              int64_t ld_out, void* workspace, void* stream);
+                              int64_t ld_out, void* workspace, int max_grid, void* stream);
 /* ---------------------------------------------------------------------------------------------
  * CNN stem of the pixel path (CNNStemNetwork, builders.py:8-33; used by PPOModel / DDPGModel with pixel input,
  * ppo_net.py:136-140,268-273,368-375): Conv2d(16, k8, s4)+ReLU -> Conv2d(32, k4, s2)+ReLU -> Flatten -> Linear+ReLU.
@@ -229,6 +230,9 @@ typedef struct {
  * DIFFERENT sb200_par channels (both exchange in the same phase). */
 int sb200_ppo_epochs2_supported(const sb200_epochs* policy, const sb200_epochs* value);
 size_t sb200_ppo_epochs2_workspace_bytes(const sb200_epochs* policy, const sb200_epochs* value);
+/* the launch plan: {grid, squared-norm chunks, s, rows per split (policy), s, rows per split (value; 0 without one)}.
+ * `grid` caps the launch below one CTA per SM; everything else is sized for one CTA per SM, so results do not depend on it. */
+int sb200_ppo_epochs2_plan(const sb200_epochs* policy, const sb200_epochs* value, int* out6);
 int sb200_ppo_epochs2_f32(const sb200_epochs* policy, const sb200_epochs* value, void* workspace, void* stream);
 /* accumulated clock64 cycles per phase of the launches on `workspace` (2 x 16: CTA 0, last CTA; see epoch2.cu) */
 int sb200_ppo_epochs2_profile(void* workspace, uint64_t* out32, int reset, void* stream);
@@ -521,6 +525,9 @@ typedef struct {
 int sb200_ppo_rollout_supported(const sb200_mlp* net, int D, int A);
 size_t sb200_ppo_rollout_scratch_ints(int N, int W, int T);
 int sb200_ppo_rollout_f32(const sb200_ppo_rollout* args, void* stream);
+/* SMs that sb200_ppo_rollout_f32 with these net / N / D / A holds for the whole chunk when all its CTAs are resident at
+ * once (one wave, one CTA per SM) -> *sms; 0 when the chunk runs in several waves or residency is not known. */
+int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* args, int* sms);
 int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, void* fifo_state, float* r_obs,
                                  float* r_act, float* r_pd, float* r_rew, float* r_done, uint64_t* step_counter,
                                  void* stream);

@@ -92,7 +92,7 @@ def _declare(lib):
                                               C.POINTER(P), C.POINTER(L), I, P]),
         'sb200_mlp_tc5_supported': (I, [C.POINTER(Mlp), L]),
         'sb200_mlp_tc5_workspace_bytes': (S, [C.POINTER(Mlp)]),
-        'sb200_mlp_forward_tc5_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), C.POINTER(Rows), P, L, P, P]),
+        'sb200_mlp_forward_tc5_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), C.POINTER(Rows), P, L, P, I, P]),
         'sb200_synth_pixel_env_step_u8': (I, [P, P, I, L, I, I, P, C.c_uint64, P, P, P, P, P]),
         'sb200_par_buffer_bytes': (S, [L]),
         'sb200_par_alloc': (I, [L, C.POINTER(C.c_void_p), P]),
@@ -102,6 +102,7 @@ def _declare(lib):
         'sb200_par_allreduce_f64': (I, [C.POINTER(Par), P, P, I, D, P]),
         'sb200_ppo_epochs2_supported': (I, [C.POINTER(Epochs), C.POINTER(Epochs)]),
         'sb200_ppo_epochs2_workspace_bytes': (S, [C.POINTER(Epochs), C.POINTER(Epochs)]),
+        'sb200_ppo_epochs2_plan': (I, [C.POINTER(Epochs), C.POINTER(Epochs), C.POINTER(C.c_int)]),
         'sb200_ppo_epochs2_f32': (I, [C.POINTER(Epochs), C.POINTER(Epochs), P, P]),
         'sb200_ppo_epochs2_profile': (I, [P, C.POINTER(C.c_uint64), I, P]),
         'sb200_ppo_epochs2_cta_profile': (I, [P, C.POINTER(C.c_uint64), P]),
@@ -121,6 +122,7 @@ def _declare(lib):
         'sb200_ppo_rollout_supported': (I, [C.POINTER(Mlp), I, I]),
         'sb200_ppo_rollout_scratch_ints': (S, [I, I, I]),
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),
+        'sb200_ppo_rollout_footprint': (I, [C.POINTER(PPORollout), C.POINTER(C.c_int)]),
         'sb200_ppo_rollout_commit_f32': (I, [C.POINTER(PPORollout), P, P, P, P, P, P, P, P, P]),
         'sb200_linear_bwd_dx_f32': (I, [P, L, P, I, P, L, P, L, I, I, I, P]),
         'sb200_linear_bwd_dw_f32': (I, [P, L, P, L, P, P, L, I, I, I, I, I, P]),

@@ -350,6 +350,21 @@ class PPOAgent(Agent):
         d = self.model.actor.desc()
         return bool(_lib.lib().sb200_ppo_rollout_supported(C.byref(d), self.model.low_dim, self.action_dim))
 
+    def rollout_footprint(self):
+        """SMs the persistent rollout kernel holds for a whole chunk when it runs in one wave (one CTA per SM); 0 when the
+        chunk takes several waves or does not run on that kernel."""
+        if not self.rollout_chunk_supported():
+            return 0
+        m = self.model
+        a = _lib.PPORollout()
+        d = m.actor.desc()
+        a.net = C.pointer(d)
+        a.N, a.D, a.A = self.num_envs, m.low_dim, self.action_dim
+        n = C.c_int(0)
+        _lib.ensure_device()
+        check(_lib.lib().sb200_ppo_rollout_footprint(C.byref(a), C.byref(n)), 'sb200_ppo_rollout_footprint')
+        return int(n.value)
+
     def rollout_chunk(self, steps):
         """``steps`` iterations of the actor loop (agent/base.py:244-262) in one launch + the ordered commit pass."""
         w = self.env

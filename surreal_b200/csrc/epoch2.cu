@@ -119,7 +119,7 @@ struct Job {                          // one optimiser
     int epochs;
     double* kl_part;                  // [n_rb]
     double* loss_part;                // [n_rb][E2_SLOTS]
-    double* sq_part;                  // [G]
+    double* sq_part;                  // [n_sq]
     double* kl_global;
     int n_rb;                         // row blocks
     int s;                            // row splits of the weight-gradient phase (slabs used)
@@ -130,6 +130,7 @@ struct Job {                          // one optimiser
 struct E2Params {
     Job job[2];
     int n_jobs;
+    int n_sq;                         // chunks of the squared-norm sum (fixed per device: the sum does not depend on the grid)
     unsigned int* bar;
     unsigned long long* prof;         // [2][16] clock64 cycles per phase, accumulated by CTA 0 and the last CTA
     unsigned long long* cta_prof;     // [G][8] per-CTA cycles: 0 P1, 1 P2, 2 forward, 3 GEMMs of forward, 4 loss rows + d2, 5 d1 GEMM
@@ -974,25 +975,28 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
         E2_STAMP(4);
         grid_bar(P.bar, bar_target);
         E2_STAMP(5);
-        // ---------------- P3: slabs -> grad (fixed order), squared-norm partials
+        // ---------------- P3: slabs -> grad (fixed order), squared-norm partials of P.n_sq chunks (CTA c takes chunks
+        // c, c + G, ...: every partial, and so the norm, is the same at any grid)
         for (int j = 0; j < NJ; ++j) {
             const Job& p = P.job[j];
             if (!train[j]) continue;
-            double sq = 0.0;
-            for (long long i4 = (long long)c * E2T + tid; i4 < (p.n_params >> 2); i4 += (long long)G * E2T) {    // one quad per thread
-                float4 g = gt::ldcg4(p.slabs + i4 * 4);
-                for (int z = 1; z < p.s; ++z) {
-                    const float4 t4 = gt::ldcg4(p.slabs + (long long)z * p.n_params + i4 * 4);
-                    g.x += t4.x; g.y += t4.y; g.z += t4.z; g.w += t4.w;
+            for (int k = c; k < P.n_sq; k += G) {
+                double sq = 0.0;
+                for (long long i4 = (long long)k * E2T + tid; i4 < (p.n_params >> 2); i4 += (long long)P.n_sq * E2T) {    // one quad per thread
+                    float4 g = gt::ldcg4(p.slabs + i4 * 4);
+                    for (int z = 1; z < p.s; ++z) {
+                        const float4 t4 = gt::ldcg4(p.slabs + (long long)z * p.n_params + i4 * 4);
+                        g.x += t4.x; g.y += t4.y; g.z += t4.z; g.w += t4.w;
+                    }
+                    *reinterpret_cast<float4*>(p.grad + i4 * 4) = g;
+                    sq += (double)g.x * (double)g.x;
+                    sq += (double)g.y * (double)g.y;
+                    sq += (double)g.z * (double)g.z;
+                    sq += (double)g.w * (double)g.w;
                 }
-                *reinterpret_cast<float4*>(p.grad + i4 * 4) = g;
-                sq += (double)g.x * (double)g.x;
-                sq += (double)g.y * (double)g.y;
-                sq += (double)g.z * (double)g.z;
-                sq += (double)g.w * (double)g.w;
+                const double t = block_sum(sq, s_red);
+                if (tid == 0) p.sq_part[k] = (p.par.world > 1) ? 0.0 : t;
             }
-            const double t = block_sum(sq, s_red);
-            if (tid == 0) p.sq_part[c] = (p.par.world > 1) ? 0.0 : t;
         }
         E2_STAMP(6);
         grid_bar(P.bar, bar_target);
@@ -1051,7 +1055,7 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
             if (!train[j]) continue;
             steps_done[j] += 1;
             double a = 0.0;
-            for (int k = tid; k < G; k += E2T) a += __ldcg(&p.sq_part[k]);
+            for (int k = tid; k < P.n_sq; k += E2T) a += __ldcg(&p.sq_part[k]);
             const double acc = block_sum(a, s_red);                            // same tree in every CTA: identical coefficients
             if (tid == 0) {
                 const float total_norm = (float)sqrt(acc);
@@ -1115,10 +1119,24 @@ struct Plan {
     int o_xs, o_h1, o_h2, o_d2, o_out, o_dp, o_part, o_w3, o_rows, ld_xs, ld_h1s, ld_h2s, ldp;
     size_t smem_bytes;
     int s[2], rps[2];
+    int n_sq;
 };
 
-// shared-memory plan + row-split choice for up to two jobs on a grid of G CTAs
-bool e2_plan(const sb200_epochs* const* a, int n_jobs, int G, Plan* pl) {
+// SMs of the current device (at most E2_MAX_G): the full grid, and what the plan is sized for at any grid
+int e2_n_sm() {
+    static int n_sm = 0;
+    if (n_sm == 0) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 132;
+    }
+    return std::min(n_sm, E2_MAX_G);
+}
+
+// shared-memory plan + row-split choice for up to two jobs.  Sized for one CTA per SM whatever grid the launch gets, so that a
+// capped grid (a learner sharing the GPU with the actors) computes the same slabs and sums as the full one.
+bool e2_plan(const sb200_epochs* const* a, int n_jobs, Plan* pl) {
+    const int G = e2_n_sm();
+    pl->n_sq = G;
     int ld_xs = 4, ld_h1 = 4, ld_h2 = 4, ldp = 4, max_as = 0, max_w3 = 4;
     int blocks = 0;
     for (int j = 0; j < n_jobs; ++j) {
@@ -1254,14 +1272,8 @@ int e2_fill_job(const sb200_epochs* a, Job* p, unsigned char* ws, const WsLayout
 }
 
 int e2_grid(const sb200_epochs* a) {
-    static int n_sm = 0;
-    if (n_sm == 0) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n_sm = 132;
-    }
-    int g = (a != nullptr && a->grid >= 1) ? a->grid : n_sm;
-    g = std::min(g, n_sm);
-    return std::min(g, E2_MAX_G);
+    const int n_sm = e2_n_sm();
+    return (a != nullptr && a->grid >= 1) ? std::min(a->grid, n_sm) : n_sm;
 }
 
 }  // namespace
@@ -1276,7 +1288,22 @@ extern "C" int sb200_ppo_epochs2_supported(const sb200_epochs* a, const sb200_ep
     const int n = (b != nullptr) ? 2 : 1;
     if (a == nullptr) return 0;
     Plan pl;
-    return e2_plan(jobs, n, e2_grid(a), &pl) ? 1 : 0;
+    return e2_plan(jobs, n, &pl) ? 1 : 0;
+}
+
+extern "C" int sb200_ppo_epochs2_plan(const sb200_epochs* a, const sb200_epochs* b, int* out6) {
+    SB200_REQUIRE(a != nullptr && out6 != nullptr);
+    const sb200_epochs* jobs[2] = {a, b};
+    const int n = (b != nullptr) ? 2 : 1;
+    Plan pl;
+    if (!e2_plan(jobs, n, &pl)) return SB200_ERR_UNSUPPORTED;
+    out6[0] = e2_grid(a);
+    out6[1] = pl.n_sq;
+    for (int j = 0; j < 2; ++j) {
+        out6[2 + 2 * j] = j < n ? pl.s[j] : 0;
+        out6[3 + 2 * j] = j < n ? pl.rps[j] : 0;
+    }
+    return SB200_OK;
 }
 
 extern "C" size_t sb200_ppo_epochs2_workspace_bytes(const sb200_epochs* a, const sb200_epochs* b) {
@@ -1292,10 +1319,11 @@ extern "C" int sb200_ppo_epochs2_f32(const sb200_epochs* a, const sb200_epochs* 
     const int n = (b != nullptr) ? 2 : 1;
     const int G = e2_grid(a);
     Plan pl;
-    if (!e2_plan(jobs, n, G, &pl)) return SB200_ERR_UNSUPPORTED;
+    if (!e2_plan(jobs, n, &pl)) return SB200_ERR_UNSUPPORTED;
     const WsLayout wl = e2_ws(jobs, n);
     E2Params P;
     P.n_jobs = n;
+    P.n_sq = pl.n_sq;
     for (int j = 0; j < n; ++j) {
         const int rc = e2_fill_job(jobs[j], &P.job[j], (unsigned char*)workspace, wl, j, pl);
         if (rc != SB200_OK) return rc;

@@ -354,7 +354,7 @@ extern "C" size_t sb200_mlp_tc5_workspace_bytes(const sb200_mlp* net) {
 }
 
 extern "C" int sb200_mlp_forward_tc5_f32(const sb200_mlp* net, const sb200_zfilter* zf, const sb200_rows* in, float* out,
-                                         int64_t ld_out, void* workspace, void* stream) {
+                                         int64_t ld_out, void* workspace, int max_grid, void* stream) {
     SB200_REQUIRE(net && in && out && workspace);
     if (!tc5_net_ok(net)) return SB200_ERR_UNSUPPORTED;
     SB200_REQUIRE(in->x != nullptr && in->rows >= 0 && in->aux == nullptr && in->save_x == nullptr);
@@ -381,7 +381,8 @@ extern "C" int sb200_mlp_forward_tc5_f32(const sb200_mlp* net, const sb200_zfilt
     const int units = (p.K0 / KC + p.N1 / KC) * MAXN * 8;
     tc5_prep_kernel<<<(units + 255) / 256, 256, 0, st>>>(net->W[0], net->ldw[0], p.K0, p.N1, net->W[1], net->ldw[1], p.N2,
                                                         (unsigned char*)workspace);
-    const long long grid = p.n_tiles < n_sm ? p.n_tiles : n_sm;
+    const int cap = (max_grid >= 1 && max_grid < n_sm) ? max_grid : n_sm;
+    const long long grid = p.n_tiles < cap ? p.n_tiles : cap;
     if (p.n_out == 1) mlp3_wgmma_kernel<1><<<(unsigned)grid, NTHREADS, TC5_SMEM, st>>>(p);
     else mlp3_wgmma_kernel<MAX_OUT><<<(unsigned)grid, NTHREADS, TC5_SMEM, st>>>(p);
     return sb200_launch_status(2);

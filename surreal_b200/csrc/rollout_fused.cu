@@ -1710,6 +1710,10 @@ cudaError_t rf_query_clusters(size_t smem, int* n) {
     cfg.dynamicSmemBytes = smem;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
+    // without the opt-in to > 48 KB of dynamic shared memory the answer is 0 clusters (and it is cached): set it here too,
+    // so that a query made before sb200_init() is right
+    const cudaError_t e = cudaFuncSetAttribute(ppo_rollout2_kernel<true, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    if (e != cudaSuccess) return e;
     return cudaOccupancyMaxActiveClusters(n, ppo_rollout2_kernel<true, G>, &cfg);
 }
 
@@ -1733,6 +1737,62 @@ int rf_max_clusters(int G, size_t smem, int* n_out) {
     SB200_CUDA(G == 2 ? rf_query_clusters<2>(smem, &n) : rf_query_clusters<1>(smem, &n));
     if (n_cache < 16) cache[n_cache++] = Entry{dev, G, smem, n};
     *n_out = n;
+    return SB200_OK;
+}
+
+// Launch shape of a chunk: kernel variant, groups per cluster, CTAs, and whether they are all resident at once.
+struct RfShape {
+    bool v2, async;
+    int groups;
+    long long ctas;
+    bool one_wave;                    // known to run in one wave (false also when residency was not queried)
+};
+
+// `p` / `smem` hold the G = 1 plan of rf_plan on entry; on return the plan of the chosen shape (l1_direct and head_mode set).
+int rf_shape(const sb200_ppo_rollout* a, RfParams* p, size_t* smem, RfShape* sh) {
+    const long long clusters = ((long long)a->N + RF_ROWS - 1) / RF_ROWS;
+    // v2 (warp-specialised env warps, 8x4 register tiles) is the default; SB200_RF_V2=0 selects the v1 kernel
+    static const int v2 = [] { const char* e = getenv("SB200_RF_V2"); return e ? atoi(e) : 1; }();
+    static const int l1_direct = [] { const char* e = getenv("SB200_RF_L1DIRECT"); return e ? atoi(e) : 1; }();
+    p->l1_direct = (l1_direct && RF_ROWS == 4 * RF_OWN) ? 1 : 0;
+    static const int head_mode = [] { const char* e = getenv("SB200_RF_HEAD"); return e ? atoi(e) : 1; }();
+    // the slice sums need 16 warps x 8 actors x ldw[2] floats of the Part buffer (4 x 32 x max(Nc1, Nc2))
+    p->head_mode = (head_mode == 1 && 16 * RF_OWN * a->net->ldw[2] <= 4 * RF_ROWS * std::max(a->net->dims[1], a->net->dims[2]) / RF_CS) ? 1 : 0;
+    // default: mbarrier-signalled st.async hand-offs instead of the three cluster barriers per step (1.47 -> 1.38 ms per
+    // 128-step chunk of 1024 actors, same results bit for bit); SB200_RF_ASYNC=0 selects the barrier.cluster variant
+    static const int rf_async = [] { const char* e = getenv("SB200_RF_ASYNC"); return e ? atoi(e) : 1; }();
+    const bool async = v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20);
+    // Two groups of 32 actors per cluster when the device cannot hold all ceil(N / 32) one-group clusters at once (the
+    // clusters that do not fit run as a whole further wave of the chunk) AND two groups at least halve the number of
+    // waves: a two-group step does both groups' work, 1.74x the time of a one-group step at the configs[1] shape on an
+    // H100 (38 K vs 22 K cycles), so fewer waves pay only when they are at most half as many (1024 actors: 2 -> 1
+    // wave; 4096 actors: 5 -> 3 waves would be slower).  Same results as one group: same arithmetic (head_mode 1,
+    // reduction-free layer 1, rf2_layer2_direct).
+    int groups = 1, fit1 = 0, fit2 = 0;
+    if (async) {
+        const int rc = rf_max_clusters(1, *smem, &fit1);
+        if (rc != SB200_OK) return rc;
+    }
+    RfParams p2 = *p;
+    size_t smem2 = 0;
+    if (async && p->l1_direct && p->head_mode == 1 && rf_plan(a->net, a->D, a->A, 2, &p2, &smem2)) {
+        const int rc = rf_max_clusters(2, smem2, &fit2);
+        if (rc != SB200_OK) return rc;
+        if (fit1 >= 1 && fit2 >= 1 && clusters > fit1) {
+            const long long waves1 = (clusters + fit1 - 1) / fit1, waves2 = ((clusters + 1) / 2 + fit2 - 1) / fit2;
+            if (2 * waves2 <= waves1) {
+                groups = 2;
+                *p = p2;
+                *smem = smem2;
+            }
+        }
+    }
+    const long long launched = (clusters + groups - 1) / groups;
+    sh->v2 = v2 != 0;
+    sh->async = async;
+    sh->groups = groups;
+    sh->ctas = launched * RF_CS;
+    sh->one_wave = async && launched <= (groups == 2 ? fit2 : fit1);
     return SB200_OK;
 }
 
@@ -1835,42 +1895,12 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     p.stride = a->stride;
     p.T = a->T;
     p.step_ctr = (const unsigned long long*)a->step_counter;
-    const long long clusters = ((long long)a->N + RF_ROWS - 1) / RF_ROWS;
-    // v2 (warp-specialised env warps, 8x4 register tiles) is the default; SB200_RF_V2=0 selects the v1 kernel
-    static const int v2 = [] { const char* e = getenv("SB200_RF_V2"); return e ? atoi(e) : 1; }();
-    static const int l1_direct = [] { const char* e = getenv("SB200_RF_L1DIRECT"); return e ? atoi(e) : 1; }();
-    p.l1_direct = (l1_direct && RF_ROWS == 4 * RF_OWN) ? 1 : 0;
-    static const int head_mode = [] { const char* e = getenv("SB200_RF_HEAD"); return e ? atoi(e) : 1; }();
-    // the slice sums need 16 warps x 8 actors x ldw[2] floats of the Part buffer (4 x 32 x max(Nc1, Nc2))
-    p.head_mode = (head_mode == 1 && 16 * RF_OWN * a->net->ldw[2] <= 4 * RF_ROWS * std::max(a->net->dims[1], a->net->dims[2]) / RF_CS) ? 1 : 0;
-    // default: mbarrier-signalled st.async hand-offs instead of the three cluster barriers per step (1.47 -> 1.38 ms per
-    // 128-step chunk of 1024 actors, same results bit for bit); SB200_RF_ASYNC=0 selects the barrier.cluster variant
-    static const int rf_async = [] { const char* e = getenv("SB200_RF_ASYNC"); return e ? atoi(e) : 1; }();
-    const bool async = v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20);
-    // Two groups of 32 actors per cluster when the device cannot hold all ceil(N / 32) one-group clusters at once (the
-    // clusters that do not fit run as a whole further wave of the chunk) AND two groups at least halve the number of
-    // waves: a two-group step does both groups' work, 1.74x the time of a one-group step at the configs[1] shape on an
-    // H100 (38 K vs 22 K cycles), so fewer waves pay only when they are at most half as many (1024 actors: 2 -> 1
-    // wave; 4096 actors: 5 -> 3 waves would be slower).  Same results as one group: same arithmetic (head_mode 1,
-    // reduction-free layer 1, rf2_layer2_direct).
-    int groups = 1;
-    RfParams p2 = p;
-    size_t smem2 = 0;
-    if (async && p.l1_direct && p.head_mode == 1 && rf_plan(a->net, a->D, a->A, 2, &p2, &smem2)) {
-        int fit1 = 0, fit2 = 0;
-        int rc = rf_max_clusters(1, smem, &fit1);
-        if (rc == SB200_OK) rc = rf_max_clusters(2, smem2, &fit2);
-        if (rc != SB200_OK) return rc;
-        if (fit1 >= 1 && fit2 >= 1 && clusters > fit1) {
-            const long long waves1 = (clusters + fit1 - 1) / fit1, waves2 = ((clusters + 1) / 2 + fit2 - 1) / fit2;
-            if (2 * waves2 <= waves1) {
-                groups = 2;
-                p = p2;
-                smem = smem2;
-            }
-        }
-    }
-    const long long ctas = (clusters + groups - 1) / groups * RF_CS;
+    RfShape sh;
+    const int rc = rf_shape(a, &p, &smem, &sh);
+    if (rc != SB200_OK) return rc;
+    const int groups = sh.groups;
+    const bool async = sh.async, v2 = sh.v2;
+    const long long ctas = sh.ctas;
 #ifdef RF_TRACE
     g_rf_last_grid = (unsigned)ctas;
     g_rf_last_smem = smem;
@@ -1881,6 +1911,19 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     else if (v2) ppo_rollout2_kernel<false, 1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     else ppo_rollout_kernel<<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     return sb200_launch_status();
+}
+
+extern "C" int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* a, int* sms) {
+    SB200_REQUIRE(a != nullptr && a->net != nullptr && sms != nullptr && a->N >= 1);
+    *sms = 0;
+    RfParams p;
+    size_t smem = 0;
+    if (!rf_plan(a->net, a->D, a->A, 1, &p, &smem)) return SB200_ERR_UNSUPPORTED;
+    RfShape sh;
+    const int rc = rf_shape(a, &p, &smem, &sh);
+    if (rc != SB200_OK) return rc;
+    if (sh.one_wave) *sms = (int)sh.ctas;             // > 200 KB of shared memory per CTA: one CTA per SM
+    return SB200_OK;
 }
 
 extern "C" int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* a, int* scratch, void* fifo_state, float* r_obs,

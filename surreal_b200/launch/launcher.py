@@ -45,8 +45,10 @@ class PipelinedEngine:
       stream A:  [wait pop_k, pub]  rollout_{k+1} .........................  -> roll_{k+1}
       stream L:  [wait roll_k] pop+gather_k -> pop_k | learn_k (CUDA graph) ... publish -> pub
 
-    The rollout is a chain of small latency-bound kernels that occupies a handful of SMs; the learner's kernels fill
-    the rest, so the step time tends to max(rollout, learn) instead of their sum.  Ordering between the streams is
+    The rollout is one persistent kernel (or a chain of small kernels) and the learner's persistent kernels want SMs of
+    their own: when the rollout runs in one wave on at most half of the SMs, the learner gets the rest as its grid
+    budget and learn() runs beside the rollout, so the step time tends to max(rollout, learn) instead of their sum.
+    Otherwise the learner's epochs wait for the rollout (before_epochs_hook).  Ordering between the streams is
     carried by events only (FIFO control block: push happens-before pop happens-before next push; parameter
     snapshot: publish happens-before fetch happens-before next publish)."""
 
@@ -54,12 +56,20 @@ class PipelinedEngine:
         import torch
         self.torch = torch
         self.agent, self.replay, self.learner, self.T = agent, replay, learner, rollout_steps
-        self.sA, self.sL = torch.cuda.Stream(), torch.cuda.Stream()
+        # the actors' stream has the higher priority: when a rollout and a learn() become ready together, the rollout's
+        # clusters are placed first and find whole GPCs free (placed after the learner's CTAs they may not fit in one wave)
+        self.sA, self.sL = torch.cuda.Stream(priority=-1), torch.cuda.Stream()
         self.ev_roll = self.ev_pop = self.ev_pub = self.ev_fetch = None
         self.iterations = 0
+        self.overlap = False
+        if hasattr(learner, 'set_sm_budget'):
+            n_sm = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+            footprint = agent.rollout_footprint() if hasattr(agent, 'rollout_footprint') else 0
+            self.overlap = 0 < footprint and 2 * footprint <= n_sm and getattr(learner, 'dp', None) is None
+            learner.set_sm_budget(n_sm - footprint if self.overlap else 0)
         if hasattr(learner, 'before_epochs_hook'):
             # learners whose epochs are ONE all-SM persistent kernel take the GPU after the rollout, not beside it
-            learner.before_epochs_hook = self._wait_rollout
+            learner.before_epochs_hook = None if self.overlap else self._wait_rollout
         cur = torch.cuda.current_stream()
         self.sA.wait_stream(cur)
         self.sL.wait_stream(cur)

@@ -197,6 +197,7 @@ class PPOLearner(Learner):
         self._graph = ops.GraphRunner()
         self._graph_head = ops.GraphRunner()
         self.before_epochs_hook = None                    # see _optimize
+        self.sm_budget = 0                                # see set_sm_budget
         self._tc5 = ops.Tc5Forward(self.model.critic)     # critic pass on the wgmma kernel when the shape qualifies
         self.tc5_min_rows = int(os.environ.get('SB200_TC5_MIN_ROWS', '4096'))
         self.dp = None
@@ -618,7 +619,7 @@ class PPOLearner(Learner):
                                  self.epoch_policy, norm_out=self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop_flag=self._stop,
                                  actions=self._actions, lda=n * A, adv=self._adv, behave_pd=self._pds, ldb=n * 2 * A,
                                  ref_pd=self._ref_pd, ldr=2 * A, hyper=self._hyper, eta=self.eta, kl_target=self.kl_target,
-                                 stop_threshold=4.0 * self.kl_target, cta_shift=0)
+                                 stop_threshold=4.0 * self.kl_target, cta_shift=0, grid=self.sm_budget)
             vk = ops.EpochKernel(self.critic_optim, 2, self._obs_full, (n + 1) * D, B, m.z_stats, m.z_eps, self._stats,
                                  self.epoch_baseline, norm_out=self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1],
                                  returns=self._ret)
@@ -633,6 +634,20 @@ class PPOLearner(Learner):
         if self._ek[3] is None:
             return None                                           # shape the kernel rejects: launch chain
         return self._ek[1], self._ek[2], self._ek[3]
+
+    def set_sm_budget(self, n_sm):
+        """Run the learner's persistent kernels (critic pass, epoch kernel) on at most ``n_sm`` CTAs (0: one per SM), for a
+        caller that keeps the other SMs busy with the actors' persistent rollout.  Results do not depend on the budget; the
+        learn() graphs are captured again with the new one."""
+        n_sm = int(n_sm)
+        if n_sm == self.sm_budget:
+            return
+        self.sm_budget = n_sm
+        self._tc5.grid = n_sm
+        if self._ek is not None:
+            self._ek[1].args.grid = n_sm                          # e2_grid reads the policy block's grid
+        self._graph = ops.GraphRunner()
+        self._graph_head = ops.GraphRunner()
 
     def _optimize_device(self):
         """The whole of ppo.py:487-586 as one fixed launch sequence (CUDA-graph body).  The KL early stop
@@ -681,8 +696,10 @@ class PPOLearner(Learner):
                 # The one-launch learner kernel wants every SM (a grid barrier needs all its CTAs resident), and so does the
                 # actors' persistent rollout kernel: launched side by side each holds SMs the other one waits for
                 # (measured: the rollout stretched from 1.5 to 2.5 ms).  A caller that runs actors concurrently
-                # (PipelinedEngine) therefore gets two graphs with a hook in between: the head overlaps the rollout on the
-                # SMs it leaves free, the hook waits for the rollout, then the epochs have the GPU to themselves.
+                # (PipelinedEngine) therefore either caps the learner's grids to the SMs the rollout leaves free
+                # (set_sm_budget, no hook), or, when the rollout leaves too few, gets two graphs with a hook in between: the
+                # head overlaps the rollout on the SMs it leaves free, the hook waits for the rollout, then the epochs have
+                # the GPU to themselves.
                 self._graph_head.run(self._optimize_head)
                 self.before_epochs_hook()
                 self._graph.run(self._optimize_epochs)

@@ -163,13 +163,15 @@ def mlp_forward_packed(packed, x, zf_stats=None, zf_eps=1e-5, aux=None, out=None
 
 class Tc5Forward:
     """Large-batch forward of a FlatNet on the wgmma kernel (sb200_mlp_forward_tc5_f32).  Owns the workspace of
-    the per-call weight images; ``supported(rows)`` says whether the shape qualifies (else callers use mlp_forward)."""
+    the per-call weight images; ``supported(rows)`` says whether the shape qualifies (else callers use mlp_forward).
+    ``grid`` caps the persistent grid (0: one CTA per SM); the output does not depend on it."""
 
     def __init__(self, net):
         self.net = net
         d = net.desc()
         n = int(_lib.lib().sb200_mlp_tc5_workspace_bytes(C.byref(d)))
         self.ws = torch.zeros(n, dtype=torch.uint8, device=net.device) if n > 0 else None
+        self.grid = 0
 
     def supported(self, rows):
         if self.ws is None or os.environ.get('SB200_TC5', '1') == '0':
@@ -192,7 +194,7 @@ class Tc5Forward:
         zf = zfilter_desc(zf_stats, zf_eps)
         d = net.desc(params)
         check(_lib.lib().sb200_mlp_forward_tc5_f32(C.byref(d), C.byref(zf), C.byref(r), _ptr(out), out.stride(0), _ptr(self.ws),
-                                                   _stream()), 'sb200_mlp_forward_tc5_f32')
+                                                   int(self.grid), _stream()), 'sb200_mlp_forward_tc5_f32')
         return out
 
 
@@ -512,6 +514,14 @@ class EpochPair:
     @staticmethod
     def supported(policy, value=None):
         return bool(_lib.lib().sb200_ppo_epochs2_supported(C.byref(policy.args), C.byref(value.args) if value is not None else None))
+
+    @staticmethod
+    def plan(policy, value=None):
+        """{grid, norm_chunks, s, rps} of a launch (s / rps: per optimiser).  Only the grid follows ``policy.args.grid``."""
+        out = (C.c_int * 6)()
+        check(_lib.lib().sb200_ppo_epochs2_plan(C.byref(policy.args), C.byref(value.args) if value is not None else None, out),
+              'sb200_ppo_epochs2_plan')
+        return {'grid': out[0], 'norm_chunks': out[1], 's': (out[2], out[4]), 'rps': (out[3], out[5])}
 
     def run(self):
         check(_lib.lib().sb200_ppo_epochs2_f32(self._pa, self._va, C.c_void_p(self._ws_ptr), _stream()), 'sb200_ppo_epochs2_f32')

@@ -4,8 +4,9 @@
 how many waves the chunk's CTAs ran (every CTA's SM and %globaltimer at entry and exit), and, per phase, the cycles
 cluster 0's CTAs spent.
 
-    python tools/rollout_trace.py build      # here (nvcc only)
-    python tools/rollout_trace.py            # on the GPU box
+    python tools/rollout_trace.py build      # nvcc only, no GPU needed
+    python tools/rollout_trace.py            # one chunk of the agent alone
+    python tools/rollout_trace.py engine     # every rollout of a few PipelinedEngine steps (learner running beside it)
 """
 import ctypes as C
 import glob
@@ -133,8 +134,37 @@ def main():
                   % (np.median(d[1:, 18] - d[1:, 0]), np.median(d[:, 19] - d[:, 10]), np.median(d[:, 20] - d[:, 19]), np.median(d[:, 21] - d[:, 20]), np.median(d[:, 11] - d[:, 21])))
 
 
+def engine(steps=8):
+    """Waves of the rollout launched by each PipelinedEngine step at the bench shape: with the learner overlapped, its CTAs
+    are resident next to the rollout's, and every step's rollout must still run in one wave."""
+    import numpy as np
+    import torch
+    from surreal_b200 import _lib
+    _lib.LIB_PATH = LIB
+    import bench
+    from surreal_b200.launch import SurrealDefaultLauncher, PipelinedEngine
+    from surreal_b200.agent import PPOAgent
+    from surreal_b200.learner import PPOLearner
+    from surreal_b200.replay import FIFOReplay
+    lc, ec, sc = bench.build_configs(bench.N_ACTORS, bench.HORIZON)
+    agent, replay, learner = SurrealDefaultLauncher(PPOAgent, PPOLearner, FIFOReplay, sc, ec, lc).setup_engine()
+    eng = PipelinedEngine(agent, replay, learner, bench.HORIZON)
+    print('overlap: %s; learner SM budget %d (0: all SMs)' % (eng.overlap, learner.sm_budget))
+    eng.prime()
+    for _ in range(3):
+        eng.step()
+    torch.cuda.synchronize()
+    L = _lib.lib()
+    for k in range(steps):
+        eng.step()
+        print('step %d:' % k)
+        waves(L, np)                                  # the rollout this step launched (synchronises the device)
+
+
 if __name__ == '__main__':
     if len(sys.argv) > 1 and sys.argv[1] == 'build':
         build()
+    elif len(sys.argv) > 1 and sys.argv[1] == 'engine':
+        engine()
     else:
         main()
