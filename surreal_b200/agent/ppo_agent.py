@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from .. import _lib, ops
+from .. import utils as U
 from .._lib import check
 from ..model.ppo_net import PPOModel, DiagGauss
 from ..env import ExpSenderWrapperMultiStepMovingWindowWithInfo
@@ -146,26 +147,33 @@ class PPOAgent(Agent):
 
     # -- RNN policy (the reference's default PPO config) ------------------------------------------------------------
     def _rnn_state(self):
-        """LSTM cells of all N actors, zero-initialised (ppo_agent.py:84-93).  NOTE: like the reference -- whose
-        ``reset()`` no caller ever invokes -- the cells carry over from episode to episode."""
+        """LSTM cells of all N actors, zero-initialised (ppo_agent.py:84-93), held as torch holds them: ``_hs`` / ``_cs``
+        [L, N, H], each layer's cells one contiguous [N, H] block.  ``_h`` / ``_c`` (returned) are the same storage with
+        the layer dimension dropped at one layer.  NOTE: like the reference -- whose ``reset()`` no caller ever invokes --
+        the cells carry over from episode to episode."""
         if getattr(self, '_h', None) is None:
-            N, H, D = self.num_envs, self.model.rnn_stem.H, self.model.low_dim
+            N, H, D, L = self.num_envs, self.model.rnn_stem.H, self.model.low_dim, self.model.rnn_stem.layers
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
-            self._h, self._c, self._h_before, self._c_before = z(N, H), z(N, H), z(N, H), z(N, H)
+            self._hs, self._cs, self._hs_before, self._cs_before = z(L, N, H), z(L, N, H), z(L, N, H), z(L, N, H)
+            self._h, self._c = self._hs.squeeze(0), self._cs.squeeze(0)
+            self._h_before, self._c_before = self._hs_before.squeeze(0), self._cs_before.squeeze(0)
             self._xf = z(N, ops._ru(D, 4))[:, :D]
             self._rnn_bufs = self.model.rnn_stem.buffers(N, 1, save=False)
-            self._aug_bufs = [z(N, D + 2 * H), z(N, D + 2 * H)]
+            self._cell_layout = U.rnn_cell_layout(self.learner_config, self.env_config)
+            self._aug_bufs = [z(N, self._cell_layout.width), z(N, self._cell_layout.width)]
         return self._h, self._c
 
     def _augment(self, o, which=0):
         """Observation rows + the cells this agent holds right now (what it will act FROM on that observation): the rows the
-        HBM staging / replay carry in RNN mode (utils.record_obs_dim)."""
-        h, c = self._rnn_state()
-        D, H = self.model.low_dim, self.model.rnn_stem.H
+        HBM staging / replay carry in RNN mode (utils.rnn_cell_layout)."""
+        self._rnn_state()
+        D, lay = self.model.low_dim, self._cell_layout
         buf = self._aug_bufs[which]
         buf[:, :D].copy_(o.reshape(self.num_envs, D), non_blocking=True)
-        buf[:, D:D + H].copy_(h, non_blocking=True)
-        buf[:, D + H:].copy_(c, non_blocking=True)
+        for k in range(lay.layers):
+            lay.h(buf, k).copy_(self._hs[k], non_blocking=True)
+        for k in range(lay.layers):
+            lay.c(buf, k).copy_(self._cs[k], non_blocking=True)
         return buf
 
     def _act_rnn(self, obs, eps=None):
@@ -190,7 +198,8 @@ class PPOAgent(Agent):
         self._h_before.copy_(h, non_blocking=True)
         self._c_before.copy_(c, non_blocking=True)
         rows_zfilter(x, D, x.stride(0), N, 1, D, m.z_stats, m.z_eps, self._xf)
-        feat = stem.forward(self._xf, h, c, h.stride(0), N, 1, self._rnn_bufs, h_last=h, c_last=c)     # cells updated in place
+        # every layer steps from its own cells, which it updates in place
+        feat = stem.forward(self._xf, h, c, stem.H, N, 1, self._rnn_bufs, h_last=h, c_last=c)
         ops.mlp_forward(m.actor, feat, out=self._mean)
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
         env = self.env
@@ -217,12 +226,12 @@ class PPOAgent(Agent):
             torch.cuda.current_stream().synchronize()
             action = self._action.cpu().numpy().astype(np.float64)
             pd = self._pd.cpu().numpy()
-            onetime = [self._h_before.cpu().numpy()[:, None, :], self._c_before.cpu().numpy()[:, None, :]]   # [N, layers, H]
+            onetime = [self._hs_before.cpu().numpy().transpose(1, 0, 2), self._cs_before.cpu().numpy().transpose(1, 0, 2)]   # [N, layers, H]
             if N == 1:
                 action, pd, onetime = action.reshape(-1), pd.reshape(-1), [onetime[0][0], onetime[1][0]]
         else:
             action, pd = self._action, self._pd
-            onetime = [self._h_before.unsqueeze(1), self._c_before.unsqueeze(1)]
+            onetime = [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)]                          # [N, layers, H]
         if self.agent_mode != 'training':
             return action
         if self.env_config.sleep_time:
@@ -407,15 +416,16 @@ class PPOAgent(Agent):
     def reset(self):
         """reset of LSTM hidden and cell states (ppo_agent.py:169-183; nothing in the reference calls it)."""
         if self.model.rnn_stem is not None and getattr(self, '_h', None) is not None:
-            self._h.zero_()
-            self._c.zero_()
+            self._hs.zero_()
+            self._cs.zero_()
 
     def prepare_env_agent(self, env):
         env = super().prepare_env_agent(env)
         if self.model.rnn_stem is not None:
             self._rnn_state()
+            lay = self._cell_layout
             w = ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config,
-                                                              obs_extra=2 * self.model.rnn_stem.H)
+                                                              obs_extra=lay.width - lay.obs_dim)
             w.obs_augment = self._augment
             w.persistent_rollout = False
             return w

@@ -112,6 +112,7 @@ class PPOLearner(Learner):
         # frame as 32-bit words
         D = U.record_obs_dim(lc, self.env_config)
         self.low_dim = D
+        self.cell_layout = U.rnn_cell_layout(lc, self.env_config) if self.rnn else None
         self.eff_len = (n - self.horizon + 1) if self.rnn else 1
         M = B * self.eff_len                                      # rows the heads train on (ppo.py:518-537)
         self._rows = M
@@ -303,11 +304,11 @@ class PPOLearner(Learner):
         elif isinstance(obs, torch.Tensor):
             own['obs_full'][:, :n, :od].copy_(obs.reshape(B, n, od), non_blocking=True)
             own['obs_full'][:, n:, :od].copy_(obs_next.reshape(B, 1, od), non_blocking=True)
-            if self.rnn:                                          # onetime_infos = [h0, c0] of the window's first step
-                hc = get('onetime_infos')
-                Hh = self.model.rnn_stem.H
-                own['obs_full'][:, 0, od:od + Hh].copy_(torch.as_tensor(hc[0]).reshape(B, Hh), non_blocking=True)
-                own['obs_full'][:, 0, od + Hh:od + 2 * Hh].copy_(torch.as_tensor(hc[1]).reshape(B, Hh), non_blocking=True)
+            if self.rnn:                          # onetime_infos = [h0, c0] [B, L, H] of the window's first step
+                hc, cl = get('onetime_infos'), self.cell_layout
+                LH = cl.layers * cl.hidden
+                cl.h(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[0]).reshape(B, LH), non_blocking=True)
+                cl.c(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[1]).reshape(B, LH), non_blocking=True)
         else:
             if 'obs_full' not in self._pin:
                 self._pin['obs_full'] = torch.zeros(B, n + 1, D, dtype=torch.float32).pin_memory()
@@ -315,10 +316,10 @@ class PPOLearner(Learner):
             pf[:, :n, :od] = np.asarray(obs).reshape(B, n, od)
             pf[:, n:, :od] = np.asarray(obs_next).reshape(B, 1, od)
             if self.rnn:
-                hc = get('onetime_infos')
-                Hh = self.model.rnn_stem.H
-                pf[:, 0, od:od + Hh] = np.asarray(hc[0], dtype=np.float32).reshape(B, Hh)
-                pf[:, 0, od + Hh:od + 2 * Hh] = np.asarray(hc[1], dtype=np.float32).reshape(B, Hh)
+                hc, cl = get('onetime_infos'), self.cell_layout
+                LH = cl.layers * cl.hidden
+                cl.h(pf[:, 0])[...] = np.asarray(hc[0], dtype=np.float32).reshape(B, LH)
+                cl.c(pf[:, 0])[...] = np.asarray(hc[1], dtype=np.float32).reshape(B, LH)
             own['obs_full'].copy_(self._pin['obs_full'], non_blocking=True)
             nbytes += own['obs_full'].numel() * 4
         nbytes += self._h2d('actions', get('actions'), own['actions'])
@@ -385,10 +386,11 @@ class PPOLearner(Learner):
 
     # -- RNN mode helpers ---------------------------------------------------------------------------------
     def _cells(self):
-        """(h0, c0, ld): the LSTM cells at the first step of every window; they ride in row 0 of the observation records
-        (the reference ships them as onetime_infos, ppo_agent.py:133-137, ppo.py:507-510)."""
-        od, Hh = self.obs_dim, self.model.rnn_stem.H
-        return self._obs_full[:, 0, od:od + Hh], self._obs_full[:, 0, od + Hh:od + 2 * Hh], self._obs_full.stride(0)
+        """(h0, c0, ld): per layer, the LSTM cells at the first step of every window; they ride in row 0 of the observation
+        records (utils.rnn_cell_layout; the reference ships them as onetime_infos, ppo_agent.py:133-137, ppo.py:507-510)."""
+        cl, row0 = self.cell_layout, self._obs_full[:, 0]
+        return ([cl.h(row0, k) for k in range(cl.layers)], [cl.c(row0, k) for k in range(cl.layers)],
+                self._obs_full.stride(0))
 
     def _rnn_prepare(self):
         """Once per learn(): contiguous, z-filtered sequence rows -- all n+1 steps for the critic pass, the first eff_len
@@ -815,6 +817,8 @@ class PPOLearner(Learner):
         ck = self.session_config.checkpoint.learner
         if 'include_optimizer' in ck and ck.include_optimizer:
             attrs += ['actor_optim', 'critic_optim', 'adapt_state']
+            if self.rnn:                                          # each optimiser's Adam moments over the shared LSTM stem
+                attrs += ['actor_rnn', 'critic_rnn']
         return attrs
 
     @property

@@ -25,8 +25,8 @@ def _default_linear_init(dims, seed_gen=None):
 
 
 class PPOModel:
-    """Same constructor keywords as the reference's PPOModel (ppo_net.py:110-118).  The LSTM stem is a
-    'next' row of SURVEY §8f and raises here; the CNN stem (pixel input) is model/cnn_stem.py."""
+    """Same constructor keywords as the reference's PPOModel (ppo_net.py:110-118).  The LSTM stem (rnn_layer layers) is
+    model/lstm_stem.py; the CNN stem (pixel input) is model/cnn_stem.py."""
 
     def __init__(self, obs_spec, action_dim, model_config, use_cuda=True, init_log_sig=0, use_z_filter=False,
                  if_pixel_input=False, rnn_config=None, device=None):
@@ -56,6 +56,9 @@ class PPOModel:
             if if_pixel_input:
                 raise NotImplementedError('CNN + LSTM stems together (pixel input with if_rnn_policy) are not built')
             from .lstm_stem import LSTMStem
+            if int(rnn_config.rnn_layer) < 1:
+                from ..session import ConfigError
+                raise ConfigError('algo.rnn.rnn_layer must be at least 1, got %d' % int(rnn_config.rnn_layer))
             self.rnn_stem = LSTMStem(in_dim, rnn_config.rnn_hidden, self.device, layers=rnn_config.rnn_layer)
             in_dim = rnn_config.rnn_hidden
         D, A = in_dim, action_dim

@@ -40,8 +40,9 @@ class FIFOReplay(Replay):
             raise RuntimeError('surreal_b200.FIFOReplay lives in HBM: a CUDA device is required')
         self.device = torch.device('cuda', torch.cuda.current_device())
         self.n_step = self.learner_config.algo.n_step
-        from ..utils import record_obs_dim, obs_packed_dim, obs_is_pixel
+        from ..utils import record_obs_dim, obs_packed_dim, obs_is_pixel, rnn_cell_layout
         self.D = record_obs_dim(self.learner_config, self.env_config)   # pixel frames: opaque 32-bit words; RNN: + LSTM cells
+        self.cells = rnn_cell_layout(self.learner_config, self.env_config)
         self.obs_dim = obs_packed_dim(self.env_config.obs_spec)
         self.pixel_shape = tuple(self.env_config.obs_spec['pixel']['camera0']) if obs_is_pixel(self.env_config.obs_spec) else None
         self.A = self.env_config.action_spec.dim[0]
@@ -97,10 +98,14 @@ class FIFOReplay(Replay):
         od = self.obs_dim
         rows[:n, :od] = np.stack([flat(x) for x in exp['obs']])
         rows[n, :od] = flat(exp['obs_next'])
-        if D > od and exp.get('onetime_infos'):                 # [h, c] of the window's first step (ppo_agent.py:133-137)
-            Hh = (D - od) // 2
-            rows[0, od:od + Hh] = np.asarray(exp['onetime_infos'][0], dtype=np.float32).reshape(-1)[:Hh]
-            rows[0, od + Hh:] = np.asarray(exp['onetime_infos'][1], dtype=np.float32).reshape(-1)[:Hh]
+        cl = self.cells
+        if cl is not None and exp.get('onetime_infos'):         # [h, c] [L, H] of the window's first step (ppo_agent.py:133-137)
+            for i, blk in enumerate((cl.h(rows[0]), cl.c(rows[0]))):
+                v = np.asarray(exp['onetime_infos'][i], dtype=np.float32)
+                if v.size != blk.size:
+                    raise ValueError('onetime_infos[%d] holds %d floats; a %d-layer LSTM(%d) window carries [%d, %d]'
+                                     % (i, v.size, cl.layers, cl.hidden, cl.layers, cl.hidden))
+                blk[:] = v.reshape(-1)
         buf[o:o + (n + 1) * D] = rows.reshape(-1); o += (n + 1) * D
         buf[o:o + n * A] = np.stack(exp['actions']).astype(np.float32).reshape(-1); o += n * A
         buf[o:o + n * 2 * A] = np.stack([p[-1] for p in exp['persistent_infos']]).astype(np.float32).reshape(-1)
@@ -144,9 +149,10 @@ class FIFOReplay(Replay):
                     'persistent_infos': [out['pd']], 'onetime_infos': None}
         od = self.obs_dim
         onetime = None
-        if D > od:                 # RNN policy: the LSTM cells of the window's first step ride behind the observation
-            Hh = (D - od) // 2
-            onetime = [obs_full[:, 0, od:od + Hh].unsqueeze(1), obs_full[:, 0, od + Hh:od + 2 * Hh].unsqueeze(1)]
+        cl = self.cells
+        if cl is not None:         # RNN policy: the LSTM cells of the window's first step ride behind the observation
+            onetime = [cl.h(obs_full[:, 0]).unflatten(1, (cl.layers, cl.hidden)),
+                       cl.c(obs_full[:, 0]).unflatten(1, (cl.layers, cl.hidden))]       # [B, L, H] views
         return {'obs': {'low_dim': {'flat_inputs': obs_full[:, :n, :od]}},
                 'obs_next': {'low_dim': {'flat_inputs': obs_full[:, n:, :od]}},
                 'obs_full': obs_full, 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'],

@@ -3,6 +3,7 @@
 AutoInitializeMeta mirrors the reference's constructor protocol (surreal/utils/common.py:232-275):
 ``_initialize()`` runs after the most-derived ``__init__``.  The timers keep the names the reference
 reports under (learner/base.py:160-162, replay/base.py:139-141)."""
+import collections
 import logging
 import threading
 import time
@@ -169,13 +170,52 @@ def obs_flat(obs):
     return obs
 
 
+class CellLayout(collections.namedtuple('CellLayout', 'layers hidden obs_dim')):
+    """Where an RNN actor's LSTM cells sit in an observation row of the HBM staging / replay records and the learner's
+    batch buffers: ``[obs (obs_dim) | h_0 .. h_{L-1} (L*H) | c_0 .. c_{L-1} (L*H)]``, i.e. the reference's
+    ``onetime_infos[0 | 1]`` of shape [L, H] flattened layer-major (ppo_agent.py:133-135).  h_col / c_col: first column
+    of the h / c block; width: floats per row.  At one layer this is ``[obs | h | c]``."""
+    __slots__ = ()
+
+    @property
+    def h_col(self):
+        return self.obs_dim
+
+    @property
+    def c_col(self):
+        return self.obs_dim + self.layers * self.hidden
+
+    @property
+    def width(self):
+        return self.obs_dim + 2 * self.layers * self.hidden
+
+    def h(self, rows, k=None):
+        """The h block of ``rows`` [..., width] as [..., L*H], or layer k's [..., H]."""
+        o = self.h_col if k is None else self.h_col + k * self.hidden
+        return rows[..., o:o + (self.layers * self.hidden if k is None else self.hidden)]
+
+    def c(self, rows, k=None):
+        o = self.c_col if k is None else self.c_col + k * self.hidden
+        return rows[..., o:o + (self.layers * self.hidden if k is None else self.hidden)]
+
+
+def rnn_cell_layout(learner_config, env_config):
+    """The CellLayout of an RNN policy's records (None for a feed-forward policy): rnn_layer x rnn_hidden cells behind
+    obs_packed_dim observation floats.  Raises ConfigError for rnn_layer < 1."""
+    rnn = learner_config.algo.rnn if 'rnn' in learner_config.algo else None
+    if rnn is None or not rnn.if_rnn_policy:
+        return None
+    layers = int(rnn.rnn_layer) if 'rnn_layer' in rnn else 1
+    if layers < 1:
+        from .session import ConfigError
+        raise ConfigError('algo.rnn.rnn_layer must be at least 1, got %d' % layers)
+    return CellLayout(layers, int(rnn.rnn_hidden), obs_packed_dim(env_config.obs_spec))
+
+
 def record_obs_dim(learner_config, env_config):
     """Floats per observation row of the HBM staging / replay records and the learner's batch buffers: obs_packed_dim, plus
-    -- for an RNN policy -- 2 * rnn_hidden trailing floats that carry the actor's LSTM cells (h | c) BEFORE it acted on that
-    observation.  The reference ships the cells of a window's first step as ``onetime_infos``
+    -- for an RNN policy -- 2 * rnn_layer * rnn_hidden trailing floats that carry the actor's LSTM cells (rnn_cell_layout)
+    BEFORE it acted on that observation.  The reference ships the cells of a window's first step as ``onetime_infos``
     (ppo_agent.py:133-137, exp_sender_wrapper.py:244-264); here they simply ride with every observation row."""
-    d = obs_packed_dim(env_config.obs_spec)
-    rnn = learner_config.algo.rnn if 'rnn' in learner_config.algo else None
-    if rnn is not None and rnn.if_rnn_policy:
-        d += 2 * int(rnn.rnn_hidden)
-    return d
+    lay = rnn_cell_layout(learner_config, env_config)
+    return lay.width if lay is not None else obs_packed_dim(env_config.obs_spec)
