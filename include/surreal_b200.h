@@ -474,6 +474,76 @@ int sb200_ppo_window_step_host_f32(const float* obs_next_host, const float* obs_
                                    float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
                                    float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
                                    uint64_t* step_counter, int slots_assigned, void* stream);
+/*   ddpg_act_host: DDPGAgent.act on a host observation batch: [H2D obs_host -> obs_dev unless obs_host is NULL] -> actor
+ *     forward -> ddpg_ou_noise (when ou_state != NULL, with sigma64) or ddpg_noise (with sigma) -> D2H action -> ONE stream
+ *     synchronisation.  unit_noise: injected N(0,1) draws [N][A] or NULL (Philox).  2 kernels below 2048 actors. */
+int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* obs_dev, int N, float* mean_dev,
+                            const float* sigma, const double* sigma64, const float* unit_noise, int deterministic,
+                            uint64_t seed, const uint64_t* step_counter, double theta, double dt, double* ou_state,
+                            float* action_dev, float* action_host, void* stream);
+
+/* RNN-mode PPOAgent.act (ppo_net.py:317-351, ppo_agent.py:133-149) for host or device observations, one call:
+ *   [H2D obs_host -> obs unless obs_host is NULL] -> h, c copied to h_before, c_before (the step's onetime_infos) ->
+ *   rows_zfilter -> per layer k: input projection (mlp_forward of ih[k] into pre_x) and lstm_forward from layer k's cells,
+ *   updated in place -> head forward -> ppo_sample (ppo_sample_assign when fifo_state != NULL) -> [when action_host is not
+ *   NULL: D2H action / pd, and h_before / c_before when h_before_host is not NULL, then ONE stream synchronisation].
+ *   Cells are [layers][N][H] (h_before_host / c_before_host receive that layout).  Layer k writes h_out[(layers-1-k) % 2].
+ *   Kernels: 2 * layers + 3 while every forward stays below 2048 rows (one kernel each).  With the host pointers NULL no
+ *   copy to or from the host and no synchronisation is issued: the call is graph-capturable. */
+#define SB200_MAX_RNN_LAYERS 8
+typedef struct {
+    const sb200_mlp* head;              /* actor head: H -> ... -> A */
+    sb200_zfilter zf;                   /* z-filter of the observation rows */
+    const sb200_mlp* ih[SB200_MAX_RNN_LAYERS];  /* input projection of layer k: in -> 4H (W_ih^T, b_ih) */
+    const float* whh[SB200_MAX_RNN_LAYERS];     /* W_hh^T [H][4H] of layer k */
+    const float* bhh[SB200_MAX_RNN_LAYERS];     /* b_hh [4H] of layer k */
+    int layers, N, D, H;
+    const float* obs_host;              /* [N][D] pinned, or NULL: obs already holds this step's observations */
+    float* obs;                         /* [N][ld_obs] */
+    int64_t ld_obs;
+    float* xf;                          /* [N][ld_xf] z-filtered rows */
+    int64_t ld_xf;
+    float* pre_x;                       /* [N][4H] */
+    float* h_out[2];                    /* [N][ldh] each; h_out[1] only for layers > 1 */
+    int ldh;
+    float* h;                           /* [layers][N][H] cells, updated in place */
+    float* c;
+    float* h_before;                    /* [layers][N][H] cells before the step */
+    float* c_before;
+    float* mean;                        /* [N][A] head output */
+    const float* log_var;
+    const float* log_noise;
+    const float* eps;                   /* injected N(0,1) draws [N][A] or NULL (Philox) */
+    int deterministic;
+    uint64_t seed;
+    uint64_t* step_counter;
+    float* action;
+    float* pd;
+    const int* stage_pos;               /* window staging rows of this step (NULL: not staged), see ppo_sample */
+    float* stage_act;
+    float* stage_pd;
+    int n_step;
+    void* fifo_state;                   /* non-NULL: ppo_sample_assign with dest */
+    int* dest;
+    float* action_host;                 /* pinned; NULL: no D2H and no synchronisation */
+    float* pd_host;
+    float* h_before_host;               /* pinned; NULL: the cells stay on the device */
+    float* c_before_host;
+} sb200_ppo_act_rnn;
+int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* args, void* stream);
+/*   ppo_window_step_rnn: ppo_window_step for an RNN policy, whose record rows are [obs (obs_dim) | h_0 .. h_{layers-1} |
+ *     c_0 .. c_{layers-1}] (D = obs_dim + 2 * layers * H).  The commit kernel assembles the successor row and the reset row
+ *     from the env's [N][obs_dim] rows and the agent's [layers][N][H] cells h / c as they are now, i.e. the cells the
+ *     agent acts from on the next observation.  With the host pointers non-NULL (all four) they are uploaded first into
+ *     obs_next / obs_reset / reward / done, as ppo_window_step_host does (obs_next_host == obs_reset_host: one upload, into
+ *     obs_reset).  Same kernels and launch count as ppo_window_step. */
+int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const float* obs_reset_host, const float* reward_host,
+                                  const float* done_host, float* obs_next, float* obs_reset, float* reward, float* done,
+                                  int N, int n_step, int stride, int obs_dim, int layers, int H, const float* h,
+                                  const float* c, int A, int* stage_pos, float* stage_obs, float* stage_act,
+                                  float* stage_pd, float* stage_rew, float* stage_done, int* dest_scratch,
+                                  void* fifo_state, float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
+                                  uint64_t* step_counter, int slots_assigned, void* stream);
 
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N
  * actors in ONE launch (a 4-CTA cluster owns 32 actors for the whole chunk; the policy weights stay resident in
@@ -567,6 +637,16 @@ int sb200_ssar_step_f32(const float* obs, const float* action, const float* obs_
                         float* dq_obs, float* dq_act, double* dq_rew, int* dest_scratch, float* emit_scratch,
                         void* uniform_state, float* r_obs, float* r_obs_next, float* r_act, float* r_rew,
                         float* r_done, uint64_t* step_counter, void* stream);
+/*   ssar_step_host: ssar_step for a host env, one call: H2D of obs_next, action, done and the rewards AS FLOAT64 (the
+ *     reference sums Python floats; the record's reward is rounded to float32 once, at emission), then the ssar_step
+ *     kernels, then obs <- the reset observation (obs_reset_host, or obs_next when obs_reset_host == obs_next_host).
+ *     obs [N][D] holds s_t on entry and the next s_t on return.  Host pointers must be pinned. */
+int sb200_ssar_step_host_f32(const float* obs_next_host, const float* obs_reset_host, const float* action_host,
+                             const double* reward_host, const float* done_host, float* obs, float* obs_next_dev,
+                             float* action_dev, double* reward_dev, float* done_dev, int N, int n_step, double gamma,
+                             int D, int A, int* dq_len, float* dq_obs, float* dq_act, double* dq_rew, int* dest_scratch,
+                             float* emit_scratch, void* uniform_state, float* r_obs, float* r_obs_next, float* r_act,
+                             float* r_rew, float* r_done, uint64_t* step_counter, void* stream);
 /* CPython random.Random-compatible MT19937 on the HOST (uniform_replay.py:43-45 draws
  * random.randint(0, len-1) per sample; SURVEY Appendix A.6).  state_h: sb200_mt19937_state_bytes() bytes. */
 size_t sb200_mt19937_state_bytes(void);

@@ -43,6 +43,28 @@ class PPORollout(C.Structure):
                 ('n_step', C.c_int), ('stride', C.c_int), ('T', C.c_int), ('step_counter', C.c_void_p)]
 
 
+MAX_RNN_LAYERS = 8
+
+
+class ZFilter(C.Structure):
+    _fields_ = [('stats', C.c_void_p), ('eps', C.c_float)]
+
+
+class PPOActRnn(C.Structure):
+    """sb200_ppo_act_rnn (include/surreal_b200.h)."""
+    _fields_ = [('head', C.POINTER(Mlp)), ('zf', ZFilter), ('ih', C.POINTER(Mlp) * MAX_RNN_LAYERS),
+                ('whh', C.c_void_p * MAX_RNN_LAYERS), ('bhh', C.c_void_p * MAX_RNN_LAYERS), ('layers', C.c_int),
+                ('N', C.c_int), ('D', C.c_int), ('H', C.c_int), ('obs_host', C.c_void_p), ('obs', C.c_void_p),
+                ('ld_obs', C.c_int64), ('xf', C.c_void_p), ('ld_xf', C.c_int64), ('pre_x', C.c_void_p),
+                ('h_out', C.c_void_p * 2), ('ldh', C.c_int), ('h', C.c_void_p), ('c', C.c_void_p), ('h_before', C.c_void_p),
+                ('c_before', C.c_void_p), ('mean', C.c_void_p), ('log_var', C.c_void_p), ('log_noise', C.c_void_p),
+                ('eps', C.c_void_p), ('deterministic', C.c_int), ('seed', C.c_uint64), ('step_counter', C.c_void_p),
+                ('action', C.c_void_p), ('pd', C.c_void_p), ('stage_pos', C.c_void_p), ('stage_act', C.c_void_p),
+                ('stage_pd', C.c_void_p), ('n_step', C.c_int), ('fifo_state', C.c_void_p), ('dest', C.c_void_p),
+                ('action_host', C.c_void_p), ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p),
+                ('c_before_host', C.c_void_p)]
+
+
 class Par(C.Structure):
     """sb200_par (include/surreal_b200.h)."""
     _fields_ = [('peers', C.c_void_p * 8), ('world', C.c_int), ('rank', C.c_int), ('max_floats', C.c_int64)]
@@ -61,10 +83,6 @@ class Epochs(C.Structure):
                 ('returns', C.c_void_p), ('hyper', C.c_void_p), ('eta', C.c_double), ('kl_target', C.c_double),
                 ('stop_threshold', C.c_double), ('stats', C.c_void_p), ('stop_flag', C.c_void_p), ('epochs', C.c_int),
                 ('workspace', C.c_void_p), ('grid', C.c_int), ('cta_shift', C.c_int), ('par', C.c_void_p)]
-
-
-class ZFilter(C.Structure):
-    _fields_ = [('stats', C.c_void_p), ('eps', C.c_float)]
 
 
 class Rows(C.Structure):
@@ -119,6 +137,10 @@ def _declare(lib):
                                        I, P, P, P, P, P]),
         'sb200_ppo_window_step_host_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P,
                                                P, I, P]),
+        'sb200_ddpg_act_host_f32': (I, [C.POINTER(Mlp), P, P, I, P, P, P, P, I, C.c_uint64, P, D, D, P, P, P, P]),
+        'sb200_ppo_act_rnn_f32': (I, [C.POINTER(PPOActRnn), P]),
+        'sb200_ppo_window_step_rnn_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P, P, P, P, P, P, P, P,
+                                              P, P, P, P, P, P, I, P]),
         'sb200_ppo_rollout_supported': (I, [C.POINTER(Mlp), I, I]),
         'sb200_ppo_rollout_scratch_ints': (S, [I, I, I]),
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),
@@ -157,6 +179,8 @@ def _declare(lib):
         'sb200_replay_gather_multi_f32': (I, [P, P, P, I, P, P, I, P]),
         'sb200_uniform_state_bytes': (S, []),
         'sb200_ssar_step_f32': (I, [P, P, P, P, P, I, I, D, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P]),
+        'sb200_ssar_step_host_f32': (I, [P, P, P, P, P, P, P, P, P, P, I, I, D, I, I, P, P, P, P, P, P, P, P, P, P, P, P,
+                                         P, P]),
         'sb200_mt19937_state_bytes': (S, []),
         'sb200_mt19937_seed_h': (I, [P, P, I]),
         'sb200_mt19937_set_state_h': (I, [P, P, I]),

@@ -156,6 +156,26 @@ class Agent(metaclass=U.AutoInitializeMeta):
         self._obs = obs
         self.post_episode()
 
+    def _host_obs(self, x, D):
+        """(host pointer, device buffer) of a numpy observation batch ``x`` for the one-call act entries: (None, the
+        wrapper's device copy) when the wrapper already uploaded this very array (``cached_device_obs``), else ``x`` itself
+        when it lives in pinned memory, else a pinned staging copy of it; the entry uploads into ``self._obs_dev``."""
+        import ctypes as C
+        import numpy as np
+        import torch
+        env = self.env
+        cached = env.cached_device_obs(x) if hasattr(env, 'cached_device_obs') else None
+        if cached is not None:
+            return None, cached
+        src = x if (x.dtype == np.float32 and x.flags['C_CONTIGUOUS'] and x.flags['WRITEABLE'] and
+                    torch.from_numpy(x).is_pinned()) else None
+        if src is None:
+            if self._obs_pin is None:
+                self._obs_pin = torch.empty(self.num_envs, D, dtype=torch.float32, pin_memory=True)
+            self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.float32).reshape(self.num_envs, D)
+            src = self._obs_pin.numpy()
+        return C.c_void_p(src.ctypes.data), self._obs_dev
+
     def _device_resident(self, obs):
         """The chunked path needs every buffer of the step to live at a fixed device address: true for the in-tree
         device env (its obs tensor is its state buffer), false for host envs."""

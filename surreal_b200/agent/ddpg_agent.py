@@ -72,13 +72,8 @@ class DDPGAgent(Agent):
         if self.sleep_time > 0.0:
             time.sleep(self.sleep_time)
         x = obs['low_dim']['flat_inputs'] if isinstance(obs, dict) else obs
-        host = not isinstance(x, torch.Tensor)
-        if host:
-            if self._obs_pin is None:
-                self._obs_pin = torch.empty(N, D, dtype=torch.float32, pin_memory=True)
-            self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.float32).reshape(N, D)
-            self._obs_dev.copy_(self._obs_pin, non_blocking=True)
-            x = self._obs_dev
+        if not isinstance(x, torch.Tensor):
+            return self._act_host(np.asarray(x), unit_noise)
         x = x.reshape(N, D)
         if self._in_chunk and self._packed.supported and x.stride(1) == 1:
             # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
@@ -101,10 +96,32 @@ class DDPGAgent(Agent):
                                                   _p(counter), _p(self._action), ops._stream()), 'sb200_ddpg_noise_f32')
         if counter is self._counter:
             self._counter += 1
-        if host:
-            a = self._action.cpu().numpy()
-            return a.reshape(-1) if (N == 1 and np.asarray(x.shape).size and np.asarray(obs['low_dim']['flat_inputs'] if isinstance(obs, dict) else obs).ndim == 1) else a
         return self._action
+
+    def _act_host(self, x, unit_noise):
+        """act() on a HOST observation batch through sb200_ddpg_act_host_f32 (H2D obs unless the wrapper already moved it
+        -> actor forward -> exploration noise -> D2H action -> one sync): numpy in, float32 numpy out."""
+        N, A, D = self.num_envs, self.action_dim, self.model.input_dim
+        obs_host, obs_dev = self._host_obs(x, D)
+        if getattr(self, '_act_pin', None) is None:
+            self._act_pin = torch.empty(N, A, dtype=torch.float32, pin_memory=True)
+        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
+        env = self.env
+        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
+        un = None
+        if unit_noise is not None:
+            un = torch.as_tensor(np.asarray(unit_noise, dtype=np.float32).reshape(N, A)).to(self.device)
+        ou = self._ou_state is not None
+        d = self.model.actor.desc()
+        check(_lib.lib().sb200_ddpg_act_host_f32(
+            C.byref(d), obs_host, _p(obs_dev), N, _p(self._mean), _p(self._sigma), _p(self._sigma64 if ou else None),
+            _p(un), int(det), self.seed, _p(counter), self.ou_theta if ou else 0.0, self.ou_dt if ou else 0.0,
+            _p(self._ou_state), _p(self._action), C.c_void_p(self._act_pin.data_ptr()), ops._stream()),
+            'sb200_ddpg_act_host_f32')
+        if counter is self._counter:
+            self._counter += 1
+        a = self._act_pin.numpy().copy()
+        return a.reshape(-1) if (N == 1 and x.ndim == 1) else a
 
     def pre_episode(self):
         super().pre_episode()

@@ -11,7 +11,6 @@ import numpy as np
 import torch
 
 from .. import _lib, ops
-from .. import utils as U
 from .._lib import check
 from ..model.ppo_net import PPOModel, DiagGauss
 from ..env import ExpSenderWrapperMultiStepMovingWindowWithInfo
@@ -159,76 +158,84 @@ class PPOAgent(Agent):
             self._h_before, self._c_before = self._hs_before.squeeze(0), self._cs_before.squeeze(0)
             self._xf = z(N, ops._ru(D, 4))[:, :D]
             self._rnn_bufs = self.model.rnn_stem.buffers(N, 1, save=False)
-            self._cell_layout = U.rnn_cell_layout(self.learner_config, self.env_config)
-            self._aug_bufs = [z(N, self._cell_layout.width), z(N, self._cell_layout.width)]
         return self._h, self._c
 
-    def _augment(self, o, which=0):
-        """Observation rows + the cells this agent holds right now (what it will act FROM on that observation): the rows the
-        HBM staging / replay carry in RNN mode (utils.rnn_cell_layout)."""
-        self._rnn_state()
-        D, lay = self.model.low_dim, self._cell_layout
-        buf = self._aug_bufs[which]
-        buf[:, :D].copy_(o.reshape(self.num_envs, D), non_blocking=True)
-        for k in range(lay.layers):
-            lay.h(buf, k).copy_(self._hs[k], non_blocking=True)
-        for k in range(lay.layers):
-            lay.c(buf, k).copy_(self._cs[k], non_blocking=True)
-        return buf
-
     def _act_rnn(self, obs, eps=None):
-        """act() with the LSTM stem: z-filter -> one LSTM step from each actor's cells -> actor head -> sampling
-        (ppo_net.py:317-351, ppo_agent.py:133-149).  The cells BEFORE the step are the step's onetime_info."""
-        from ..model.lstm_stem import rows_zfilter
+        """act() with the LSTM stem, for host and device observations alike through ONE call of sb200_ppo_act_rnn_f32:
+        z-filter -> per layer one LSTM step from each actor's cells, updated in place -> actor head -> sampling
+        (ppo_net.py:317-351, ppo_agent.py:133-149).  The cells BEFORE the step are the step's onetime_info.  Host input:
+        H2D of the observation (unless the wrapper already moved it), D2H of the results and one stream sync in that call."""
+        from ..model.lstm_stem import _sfx
         N, A, D = self.num_envs, self.action_dim, self.model.low_dim
         m, stem = self.model, self.model.rnn_stem
-        h, c = self._rnn_state()
+        self._rnn_state()
+        L, H = stem.layers, stem.H
         x = obs
         if isinstance(obs, dict):
             xs = [obs['low_dim'][k] for k in obs['low_dim']]
             x = xs[0] if len(xs) == 1 else (torch.cat(xs, -1) if isinstance(xs[0], torch.Tensor) else np.concatenate(xs, -1))
         host = not isinstance(x, torch.Tensor)
+        training = self.agent_mode == 'training'
+        a = _lib.PPOActRnn()
         if host:
-            if self._obs_pin is None:
-                self._obs_pin = torch.empty(N, D, dtype=torch.float32, pin_memory=True)
-            self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.float32).reshape(N, D)
-            self._obs_dev.copy_(self._obs_pin, non_blocking=True)
-            x = self._obs_dev
-        x = x.reshape(N, D)
-        self._h_before.copy_(h, non_blocking=True)
-        self._c_before.copy_(c, non_blocking=True)
-        rows_zfilter(x, D, x.stride(0), N, 1, D, m.z_stats, m.z_eps, self._xf)
-        # every layer steps from its own cells, which it updates in place
-        feat = stem.forward(self._xf, h, c, stem.H, N, 1, self._rnn_bufs, h_last=h, c_last=c)
-        ops.mlp_forward(m.actor, feat, out=self._mean)
+            obs_host, obs_dev = self._host_obs(np.asarray(x), D)
+            a.obs_host, a.obs, a.ld_obs = (obs_host.value if obs_host is not None else None), obs_dev.data_ptr(), D
+            if self._out_pin is None:
+                self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
+                                 torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
+            a.action_host, a.pd_host = self._out_pin[0].data_ptr(), self._out_pin[1].data_ptr()
+            if training:
+                if getattr(self, '_cells_pin', None) is None:
+                    self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
+                                       torch.empty(L, N, H, dtype=torch.float32, pin_memory=True))
+                a.h_before_host, a.c_before_host = self._cells_pin[0].data_ptr(), self._cells_pin[1].data_ptr()
+        else:
+            x = x.reshape(N, D)
+            a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
+        head = m.actor.desc()
+        ihs = [stem.ihs[k].desc(stem.seg('ih' + _sfx(k))) for k in range(L)]
+        a.head = C.pointer(head)
+        a.zf = ops.zfilter_desc(m.z_stats, m.z_eps)
+        for k in range(L):
+            a.ih[k] = C.pointer(ihs[k])
+            hh, lay = stem.seg('hh' + _sfx(k)), stem.hhs[k].layout[0]
+            a.whh[k], a.bhh[k] = hh.data_ptr() + 4 * lay['w'], hh.data_ptr() + 4 * lay['b']
+        a.layers, a.N, a.D, a.H = L, N, D, H
+        bufs = self._rnn_bufs
+        a.xf, a.ld_xf, a.pre_x = self._xf.data_ptr(), self._xf.stride(0), bufs['pre_x'].data_ptr()
+        a.h_out[0], a.ldh = bufs['h_out'].data_ptr(), bufs['h_out'].stride(0)
+        if L > 1:
+            a.h_out[1] = bufs['h_out1'].data_ptr()
+        a.h, a.c, a.h_before, a.c_before = self._hs.data_ptr(), self._cs.data_ptr(), self._hs_before.data_ptr(), self._cs_before.data_ptr()
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
         env = self.env
-        staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
+        staged = training and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
         counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
         eps_dev = None
         if eps is not None:
             eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-        if staged and counter is not self._counter and env.fuse_launches:
-            fifo_state, dest = env.slot_assignment_args()
-            check(_lib.lib().sb200_ppo_sample_assign_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos), _p(env.stage_act), _p(env.stage_pd),
-                env.n_step, _p(fifo_state), _p(dest), ops._stream()), 'sb200_ppo_sample_assign_f32')
-        else:
-            check(_lib.lib().sb200_ppo_sample_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
-                _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None,
-                env.n_step if staged else 1, ops._stream()), 'sb200_ppo_sample_f32')
+            a.eps = eps_dev.data_ptr()
+        a.mean, a.log_var, a.log_noise = self._mean.data_ptr(), m.log_var.data_ptr(), self._log_noise.data_ptr()
+        a.deterministic, a.seed, a.step_counter = int(det), self.seed, counter.data_ptr()
+        a.action, a.pd, a.n_step = self._action.data_ptr(), self._pd.data_ptr(), 1
+        if staged:
+            a.stage_pos, a.stage_act, a.stage_pd = env.stage_pos.data_ptr(), env.stage_act.data_ptr(), env.stage_pd.data_ptr()
+            a.n_step = env.n_step
+            if counter is not self._counter and env.fuse_launches:
+                fifo_state, dest = env.slot_assignment_args()
+                a.fifo_state, a.dest = fifo_state.data_ptr(), dest.data_ptr()
+        check(_lib.lib().sb200_ppo_act_rnn_f32(C.byref(a), ops._stream()), 'sb200_ppo_act_rnn_f32')
         if not staged and counter is self._counter:
             self._counter += 1
         if host:
-            torch.cuda.current_stream().synchronize()
-            action = self._action.cpu().numpy().astype(np.float64)
-            pd = self._pd.cpu().numpy()
-            onetime = [self._hs_before.cpu().numpy().transpose(1, 0, 2), self._cs_before.cpu().numpy().transpose(1, 0, 2)]   # [N, layers, H]
+            action = self._out_pin[0].numpy().astype(np.float64)   # the reference hands the env float64 (ppo_net.py:83)
+            pd = self._out_pin[1].numpy().copy()
+            onetime = None
+            if training:                                            # [N, layers, H]
+                onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
             if N == 1:
-                action, pd, onetime = action.reshape(-1), pd.reshape(-1), [onetime[0][0], onetime[1][0]]
+                action, pd = action.reshape(-1), pd.reshape(-1)
+                onetime = [onetime[0][0], onetime[1][0]] if onetime is not None else None
         else:
             action, pd = self._action, self._pd
             onetime = [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)]                          # [N, layers, H]
@@ -302,18 +309,7 @@ class PPOAgent(Agent):
         if self._out_pin is None:
             self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
                              torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
-        cached = env.cached_device_obs(x) if hasattr(env, 'cached_device_obs') else None
-        if cached is not None:
-            obs_host, obs_dev = None, cached                       # the wrapper already moved this observation
-        else:
-            src = x if (x.dtype == np.float32 and x.flags['C_CONTIGUOUS'] and x.flags['WRITEABLE'] and
-                        torch.from_numpy(x).is_pinned()) else None
-            if src is None:
-                if self._obs_pin is None:
-                    self._obs_pin = torch.empty(N, D, dtype=torch.float32, pin_memory=True)
-                self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.float32).reshape(N, D)
-                src = self._obs_pin.numpy()
-            obs_host, obs_dev = C.c_void_p(src.ctypes.data), self._obs_dev
+        obs_host, obs_dev = self._host_obs(x, D)
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
         staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
         counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
@@ -423,10 +419,8 @@ class PPOAgent(Agent):
         env = super().prepare_env_agent(env)
         if self.model.rnn_stem is not None:
             self._rnn_state()
-            lay = self._cell_layout
             w = ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config,
-                                                              obs_extra=lay.width - lay.obs_dim)
-            w.obs_augment = self._augment
+                                                              cells=(self._hs, self._cs))
             w.persistent_rollout = False
             return w
         return ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config)

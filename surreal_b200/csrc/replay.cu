@@ -95,7 +95,9 @@ struct UniformState {
     long long total_in;
 };
 
-__global__ void __launch_bounds__(1024) ssar_flags_kernel(const float* __restrict__ reward,
+// Rew: float for device envs, double for host envs, whose float64 rewards the reference sums as Python floats.
+template <typename Rew>
+__global__ void __launch_bounds__(1024) ssar_flags_kernel(const Rew* __restrict__ reward,
                                                           const float* __restrict__ done, int N, int n_step,
                                                           double gamma, int* __restrict__ dq_len,
                                                           double* __restrict__ dq_rew, int* __restrict__ dest,
@@ -349,11 +351,43 @@ extern "C" int sb200_ssar_step_f32(const float* obs, const float* action, const 
     SB200_REQUIRE(dest_scratch && emit_scratch && uniform_state && r_obs && r_obs_next && r_act && r_rew && r_done);
     SB200_REQUIRE(N >= 1 && n_step >= 1 && D >= 1 && A >= 1);
     cudaStream_t st = (cudaStream_t)stream;
-    ssar_flags_kernel<<<1, 1024, 0, st>>>(reward, done, N, n_step, gamma, dq_len, dq_rew, dest_scratch, emit_scratch,
-                                          (UniformState*)uniform_state, (unsigned long long*)step_counter);
+    ssar_flags_kernel<float><<<1, 1024, 0, st>>>(reward, done, N, n_step, gamma, dq_len, dq_rew, dest_scratch, emit_scratch,
+                                                 (UniformState*)uniform_state, (unsigned long long*)step_counter);
     ssar_commit_kernel<<<N, 128, 0, st>>>(obs, action, obs_next, done, N, n_step, D, A, dq_len, dq_obs, dq_act, dq_rew,
                                           dest_scratch, emit_scratch, r_obs, r_obs_next, r_act, r_rew, r_done);
     return sb200_launch_status(2);
+}
+
+extern "C" int sb200_ssar_step_host_f32(const float* obs_next_host, const float* obs_reset_host, const float* action_host,
+                                        const double* reward_host, const float* done_host, float* obs, float* obs_next_dev,
+                                        float* action_dev, double* reward_dev, float* done_dev, int N, int n_step,
+                                        double gamma, int D, int A, int* dq_len, float* dq_obs, float* dq_act,
+                                        double* dq_rew, int* dest_scratch, float* emit_scratch, void* uniform_state,
+                                        float* r_obs, float* r_obs_next, float* r_act, float* r_rew, float* r_done,
+                                        uint64_t* step_counter, void* stream) {
+    SB200_REQUIRE(obs_next_host && obs_reset_host && action_host && reward_host && done_host);
+    SB200_REQUIRE(obs && obs_next_dev && action_dev && reward_dev && done_dev && dq_len && dq_obs && dq_act && dq_rew);
+    SB200_REQUIRE(dest_scratch && emit_scratch && uniform_state && r_obs && r_obs_next && r_act && r_rew && r_done);
+    SB200_REQUIRE(N >= 1 && n_step >= 1 && D >= 1 && A >= 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t row_bytes = (size_t)N * D * sizeof(float);
+    SB200_CUDA(cudaMemcpyAsync(obs_next_dev, obs_next_host, row_bytes, cudaMemcpyHostToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(action_dev, action_host, (size_t)N * A * sizeof(float), cudaMemcpyHostToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(reward_dev, reward_host, (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(done_dev, done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
+    ssar_flags_kernel<double><<<1, 1024, 0, st>>>(reward_dev, done_dev, N, n_step, gamma, dq_len, dq_rew, dest_scratch,
+                                                  emit_scratch, (UniformState*)uniform_state,
+                                                  (unsigned long long*)step_counter);
+    ssar_commit_kernel<<<N, 128, 0, st>>>(obs, action_dev, obs_next_dev, done_dev, N, n_step, D, A, dq_len, dq_obs, dq_act,
+                                          dq_rew, dest_scratch, emit_scratch, r_obs, r_obs_next, r_act, r_rew, r_done);
+    const int rc = sb200_launch_status(2);
+    if (rc != SB200_OK) return rc;
+    // s_t of the next transition, after the commit has appended this one's
+    if (obs_reset_host != obs_next_host)
+        SB200_CUDA(cudaMemcpyAsync(obs, obs_reset_host, row_bytes, cudaMemcpyHostToDevice, st));
+    else
+        SB200_CUDA(cudaMemcpyAsync(obs, obs_next_dev, row_bytes, cudaMemcpyDeviceToDevice, st));
+    return SB200_OK;
 }
 
 // ---- CPython random.Random index stream (host) -------------------------------------------------

@@ -270,6 +270,47 @@ __global__ void __launch_bounds__(128) ppo_window_commit_kernel(const float* __r
                  stage_done, r_obs, r_act, r_pd, r_rew, r_done);
 }
 
+// Window commit of an RNN policy: the record row [obs (Do) | h_0 .. h_{L-1} | c_0 .. c_{L-1}] (utils.rnn_cell_layout) is
+// assembled in shared memory from the env's row and the agent's [L][N][H] cells, for the successor and the reset row alike,
+// then committed as any other row.
+__global__ void __launch_bounds__(128) ppo_window_commit_rnn_kernel(const float* __restrict__ obs_next,
+                                                                    const float* __restrict__ obs_reset,
+                                                                    const float* __restrict__ reward,
+                                                                    const float* __restrict__ done, int N, int n_step,
+                                                                    int stride, int Do, int L, int H,
+                                                                    const float* __restrict__ h,
+                                                                    const float* __restrict__ c, int A,
+                                                                    int* __restrict__ stage_pos,
+                                                                    float* __restrict__ stage_obs,
+                                                                    float* __restrict__ stage_act,
+                                                                    float* __restrict__ stage_pd,
+                                                                    float* __restrict__ stage_rew,
+                                                                    float* __restrict__ stage_done,
+                                                                    const int* __restrict__ dest,
+                                                                    float* __restrict__ r_obs, float* __restrict__ r_act,
+                                                                    float* __restrict__ r_pd, float* __restrict__ r_rew,
+                                                                    float* __restrict__ r_done) {
+    extern __shared__ float rows[];                // [2][D]: successor row, reset row
+    const int i = blockIdx.x;
+    const int LH = L * H, D = Do + 2 * LH;
+    float* s_next = rows;
+    float* s_reset = rows + D;
+    for (int d = threadIdx.x; d < D; d += blockDim.x) {
+        if (d < Do) {
+            s_next[d] = obs_next[(long long)i * Do + d];
+            s_reset[d] = obs_reset[(long long)i * Do + d];
+        } else {
+            const int e = d - Do, which = e / LH, r = e - which * LH, k = r / H, j = r - k * H;
+            const float v = (which == 0 ? h : c)[((long long)k * N + i) * H + j];
+            s_next[d] = v;
+            s_reset[d] = v;
+        }
+    }
+    __syncthreads();
+    commit_actor(true, i, threadIdx.x, blockDim.x, s_next, s_reset, reward[i], done[i], n_step, stride, D, A, stage_pos + i,
+                 dest[i], stage_obs, stage_act, stage_pd, stage_rew, stage_done, r_obs, r_act, r_pd, r_rew, r_done);
+}
+
 // Fused environment step + window commit for the device-resident synthetic env: the successor state never
 // leaves shared memory before it is staged.  One block per 4 actors, 64 threads per actor in the commit.
 __global__ void __launch_bounds__(RT) synth_env_window_step_kernel(
@@ -473,4 +514,131 @@ extern "C" int sb200_ppo_window_step_host_f32(const float* obs_next_host, const 
                                      reward_dev, done_dev, N, n_step, stride, D, A, stage_pos, stage_obs, stage_act,
                                      stage_pd, stage_rew, stage_done, dest_scratch, fifo_state, r_obs, r_act, r_pd, r_rew,
                                      r_done, step_counter, slots_assigned, stream);
+}
+
+extern "C" int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* obs_dev, int N, float* mean_dev,
+                                       const float* sigma, const double* sigma64, const float* unit_noise, int deterministic,
+                                       uint64_t seed, const uint64_t* step_counter, double theta, double dt,
+                                       double* ou_state, float* action_dev, float* action_host, void* stream) {
+    SB200_REQUIRE(net != nullptr && obs_dev != nullptr && mean_dev != nullptr && action_dev && action_host && N >= 1);
+    SB200_REQUIRE(ou_state != nullptr ? sigma64 != nullptr : sigma != nullptr);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int D = net->dims[0], A = net->dims[net->n_layers];
+    if (obs_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+    const sb200_zfilter nozf = {nullptr, 1e-5f};
+    const sb200_rows in = {obs_dev, nullptr, D, N, 0, nullptr, 0, nullptr, 0};
+    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
+    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
+    save[net->n_layers - 1] = mean_dev;
+    lds[net->n_layers - 1] = A;
+    int rc = sb200_mlp_forward_f32(net, &nozf, &in, save, lds, stream);
+    if (rc != SB200_OK) return rc;
+    if (ou_state != nullptr)
+        rc = sb200_ddpg_ou_noise_f32(mean_dev, A, sigma64, unit_noise, N, A, deterministic, seed, step_counter, theta, dt,
+                                     ou_state, action_dev, stream);
+    else
+        rc = sb200_ddpg_noise_f32(mean_dev, A, sigma, unit_noise, N, A, deterministic, seed, step_counter, action_dev, stream);
+    if (rc != SB200_OK) return rc;
+    SB200_CUDA(cudaMemcpyAsync(action_host, action_dev, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
+    SB200_CUDA(cudaStreamSynchronize(st));
+    return SB200_OK;
+}
+
+extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
+    SB200_REQUIRE(a != nullptr && a->head != nullptr && a->layers >= 1 && a->layers <= SB200_MAX_RNN_LAYERS);
+    SB200_REQUIRE(a->N >= 1 && a->D >= 1 && a->H >= 1 && a->ldh >= a->H && a->ld_obs >= a->D && a->ld_xf >= a->D);
+    SB200_REQUIRE(a->obs && a->xf && a->pre_x && a->h_out[0] && (a->layers == 1 || a->h_out[1]));
+    SB200_REQUIRE(a->h && a->c && a->h_before && a->c_before && a->mean && a->log_var && a->action && a->pd);
+    SB200_REQUIRE(a->obs_host == nullptr || a->ld_obs == a->D);
+    SB200_REQUIRE(a->action_host == nullptr || a->pd_host != nullptr);
+    SB200_REQUIRE((a->h_before_host == nullptr) == (a->c_before_host == nullptr));
+    for (int k = 0; k < a->layers; ++k) SB200_REQUIRE(a->ih[k] && a->whh[k] && a->bhh[k] && a->ih[k]->dims[1] == 4 * a->H);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int N = a->N, D = a->D, H = a->H, L = a->layers, A = a->head->dims[a->head->n_layers];
+    const size_t cells = (size_t)L * N * H * sizeof(float);
+    if (a->obs_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
+    int rc = sb200_rows_zfilter_f32(a->obs, D, a->ld_obs, N, 1, D, a->zf.stats, (double)a->zf.eps, a->xf, a->ld_xf, stream);
+    if (rc != SB200_OK) return rc;
+    const sb200_zfilter nozf = {nullptr, 1e-5f};
+    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
+    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
+    sb200_rows in = {a->xf, nullptr, a->ld_xf, N, 0, nullptr, 0, nullptr, 0};
+    for (int k = 0; k < L; ++k) {
+        save[0] = a->pre_x;
+        lds[0] = 4 * H;
+        rc = sb200_mlp_forward_f32(a->ih[k], &nozf, &in, save, lds, stream);
+        if (rc != SB200_OK) return rc;
+        float* ho = a->h_out[(L - 1 - k) & 1];
+        float* hk = a->h + (size_t)k * N * H;
+        float* ck = a->c + (size_t)k * N * H;
+        rc = sb200_lstm_forward_f32(a->pre_x, a->whh[k], a->bhh[k], hk, ck, H, N, 1, H, a->ldh, ho, nullptr, nullptr, nullptr,
+                                    hk, ck, stream);
+        if (rc != SB200_OK) return rc;
+        in.x = ho;
+        in.ldx = a->ldh;
+    }
+    save[0] = nullptr;
+    lds[0] = 0;
+    save[a->head->n_layers - 1] = a->mean;
+    lds[a->head->n_layers - 1] = A;
+    rc = sb200_mlp_forward_f32(a->head, &nozf, &in, save, lds, stream);
+    if (rc != SB200_OK) return rc;
+    if (a->fifo_state != nullptr)
+        rc = sb200_ppo_sample_assign_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed,
+                                         a->step_counter, a->action, a->pd, a->stage_pos, a->stage_act, a->stage_pd,
+                                         a->n_step, a->fifo_state, a->dest, stream);
+    else
+        rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed,
+                                  a->step_counter, a->action, a->pd, a->stage_pos, a->stage_act, a->stage_pd, a->n_step,
+                                  stream);
+    if (rc != SB200_OK || a->action_host == nullptr) return rc;
+    SB200_CUDA(cudaMemcpyAsync(a->action_host, a->action, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
+    SB200_CUDA(cudaMemcpyAsync(a->pd_host, a->pd, (size_t)N * 2 * A * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (a->h_before_host != nullptr) {
+        SB200_CUDA(cudaMemcpyAsync(a->h_before_host, a->h_before, cells, cudaMemcpyDeviceToHost, st));
+        SB200_CUDA(cudaMemcpyAsync(a->c_before_host, a->c_before, cells, cudaMemcpyDeviceToHost, st));
+    }
+    SB200_CUDA(cudaStreamSynchronize(st));
+    return SB200_OK;
+}
+
+extern "C" int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const float* obs_reset_host,
+                                             const float* reward_host, const float* done_host, float* obs_next,
+                                             float* obs_reset, float* reward, float* done, int N, int n_step, int stride,
+                                             int obs_dim, int layers, int H, const float* h, const float* c, int A,
+                                             int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
+                                             float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
+                                             float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
+                                             uint64_t* step_counter, int slots_assigned, void* stream) {
+    SB200_REQUIRE(obs_next && obs_reset && reward && done && h && c && stage_pos && stage_obs && stage_act && stage_pd);
+    SB200_REQUIRE(stage_rew && stage_done && dest_scratch && fifo_state && r_obs && r_act && r_pd && r_rew && r_done);
+    SB200_REQUIRE(N >= 1 && n_step >= 1 && stride >= 1 && obs_dim >= 1 && layers >= 1 && H >= 1 && A >= 1);
+    const bool host = obs_reset_host != nullptr;
+    SB200_REQUIRE(host ? (obs_next_host && reward_host && done_host) : (!obs_next_host && !reward_host && !done_host));
+    const int D = obs_dim + 2 * layers * H;
+    const size_t smem = (size_t)2 * D * sizeof(float);
+    SB200_REQUIRE(smem <= 48 * 1024);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float* next = obs_next;
+    if (host) {
+        const size_t row_bytes = (size_t)N * obs_dim * sizeof(float);
+        SB200_CUDA(cudaMemcpyAsync(obs_reset, obs_reset_host, row_bytes, cudaMemcpyHostToDevice, st));
+        if (obs_next_host != obs_reset_host)
+            SB200_CUDA(cudaMemcpyAsync(obs_next, obs_next_host, row_bytes, cudaMemcpyHostToDevice, st));
+        else
+            next = obs_reset;
+        SB200_CUDA(cudaMemcpyAsync(reward, reward_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(done, done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
+    }
+    if (!slots_assigned)
+        ppo_window_slots_kernel<<<1, 1024, 0, st>>>(N, n_step, stage_pos, dest_scratch, (FifoState*)fifo_state,
+                                                    (unsigned long long*)step_counter);
+    ppo_window_commit_rnn_kernel<<<N, 128, smem, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers, H, h,
+                                                       c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
+                                                       stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
+    return sb200_launch_status(slots_assigned ? 1 : 2);
 }

@@ -1,4 +1,4 @@
-"""Experience-sender wrappers for BATCHED device-resident envs (mirror of
+"""Experience-sender wrappers for BATCHED envs, device-resident or on the host (mirror of
 surreal/env/exp_sender_wrapper.py:72-112,153-264).
 
 The reference keeps one Python deque per actor process and ships finished windows / n-step transitions
@@ -34,10 +34,10 @@ class _WrapperBase:
         if self.replay is None:
             raise RuntimeError('no replay registered for this session: construct the Replay before the agent '
                                'wraps its env (the ZeroMQ collector address of the reference is gone)')
+        # D: floats per staged observation row = the env's obs_dim + obs_extra trailing floats (an RNN agent's LSTM cells,
+        # utils.record_obs_dim)
         self.N, self.D, self.A = env.N, env.D + int(obs_extra), env.A
-        # extra trailing floats per observation row, filled by ``obs_augment(rows [N, env.D]) -> [N, D]`` (an RNN agent appends
-        # its LSTM cells; utils.record_obs_dim)
-        self.obs_extra, self.obs_augment = int(obs_extra), None
+        self.obs_dim = env.D
         # a batched HOST env (numpy in / numpy out, attributes N, D, A) has no device: the staging lives with the replay
         self.device = env.device if hasattr(env, 'device') else self.replay.device
         self.host_env = not hasattr(env, 'device')
@@ -66,29 +66,24 @@ class _WrapperBase:
         dev.copy_(src, non_blocking=True)
         return dev
 
-    def _dev(self, name, shape):
+    def _dev(self, name, shape, dtype=torch.float32):
         dev = self._devs.get(name)
         if dev is None:
-            dev = self._devs[name] = torch.zeros(*shape, dtype=torch.float32, device=self.device)
+            dev = self._devs[name] = torch.zeros(*shape, dtype=dtype, device=self.device)
         return dev
 
-    def _pinned(self, name, arr, shape):
+    def _pinned(self, name, arr, shape, dtype=torch.float32):
         """Address (c_void_p) of ``arr`` if it already lives in pinned memory, else of a pinned staging copy."""
         import numpy as np
-        if isinstance(arr, np.ndarray) and arr.dtype == np.float32 and arr.flags['C_CONTIGUOUS'] and arr.flags['WRITEABLE'] \
+        npt = np.float64 if dtype == torch.float64 else np.float32
+        if isinstance(arr, np.ndarray) and arr.dtype == npt and arr.flags['C_CONTIGUOUS'] and arr.flags['WRITEABLE'] \
                 and torch.from_numpy(arr).is_pinned():
             return C.c_void_p(arr.ctypes.data)
         pin = self._pins.get(name)
         if pin is None:
-            pin = self._pins[name] = torch.empty(*shape, dtype=torch.float32, pin_memory=True)
-        pin.numpy()[...] = np.asarray(arr, dtype=np.float32).reshape(shape)
+            pin = self._pins[name] = torch.empty(*shape, dtype=dtype, pin_memory=True)
+        pin.numpy()[...] = np.asarray(arr, dtype=npt).reshape(shape)
         return C.c_void_p(pin.data_ptr())
-
-    def _aug(self, o):
-        return self.obs_augment(o, 0) if (self.obs_extra and self.obs_augment is not None) else o
-
-    def _aug_next(self, o):
-        return self.obs_augment(o, 1) if (self.obs_extra and self.obs_augment is not None) else o
 
     def cached_device_obs(self, obs_arr):
         """The device copy of the observation the last step() returned (the agent's next act() input), if
@@ -106,8 +101,12 @@ class _WrapperBase:
 class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
     """n_step windows with stride (exp_sender_wrapper.py:153-264) -> FIFOReplay ring."""
 
-    def __init__(self, env, learner_config, session_config, replay=None, obs_extra=0):
-        super().__init__(env, learner_config, session_config, replay, obs_extra=obs_extra)
+    def __init__(self, env, learner_config, session_config, replay=None, cells=None):
+        # RNN policy: the agent's (h, c) cells [layers, N, H], which every staged observation row carries behind the env's
+        # observation (utils.rnn_cell_layout), as they are when the row is staged
+        self.cells = cells
+        extra = 0 if cells is None else 2 * cells[0].shape[0] * cells[0].shape[2]
+        super().__init__(env, learner_config, session_config, replay, obs_extra=extra)
         self.n_step = self.learner_config.algo.n_step
         self.stride = self.learner_config.algo.stride
         if self.stride < 1:
@@ -129,12 +128,18 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         obs, info = self.env.reset()
         self.stage_pos.zero_()                                     # deque.clear() (exp_sender_wrapper.py:204-207)
         o = obs_flat(obs)
+        row0 = self.stage_obs[:, 0]
         if self.host_env:
-            d = self._h2d('obs', o, (self.N, self.D))
-            self.stage_obs[:, 0].copy_(d)
+            d = self._h2d('obs', o, (self.N, self.obs_dim))
+            row0[:, :self.obs_dim].copy_(d)
             self._last_obs_host, self._last_obs_dev = o, d
         else:
-            self.stage_obs[:, 0].copy_(self._aug(o))
+            row0[:, :self.obs_dim].copy_(o)
+        if self.cells is not None:                                 # the cells the agent acts from on this observation
+            h, c = self.cells
+            L, H = h.shape[0], h.shape[2]
+            row0[:, self.obs_dim:self.obs_dim + L * H].unflatten(1, (L, H)).copy_(h.transpose(0, 1))
+            row0[:, self.obs_dim + L * H:].unflatten(1, (L, H)).copy_(c.transpose(0, 1))
         return obs, info
 
     def rollout_outbox(self, T):
@@ -169,13 +174,14 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         a = action[0] if isinstance(action, tuple) else action
         r = self.replay
         ready, self._slots_ready = self._slots_ready, False
-        if ready and hasattr(self.env, 'step_and_commit_window') and not self.obs_extra:
+        if ready and hasattr(self.env, 'step_and_commit_window') and self.cells is None:
             return self.env.step_and_commit_window(a, self)        # env step + commit in ONE launch
         obs, reward, done, info = self.env.step(a)
         o = obs_flat(obs)
         on = obs_flat(info['obs_next']) if (isinstance(info, dict) and 'obs_next' in info) else o
-        if self.host_env and self.obs_extra:
-            raise NotImplementedError('RNN policy with a host env: stage the windows with replay.insert (onetime_infos) instead')
+        if self.cells is not None:
+            self._step_rnn(o, on, reward, done, ready)
+            return obs, reward, done, info
         if self.host_env:
             # host env: this step's successor observation / reward / done cross PCIe here (256 KB + 8 KB), issued with
             # the staging kernels from ONE C call; the device copy of the next observation is handed to the agent's
@@ -193,12 +199,6 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
                 'sb200_ppo_window_step_host_f32')
             self._last_obs_host, self._last_obs_dev = o, d_o
             return obs, reward, done, info
-        if self.obs_extra:
-            # both rows get the cells the agent holds NOW, i.e. before it acts on the next observation; `on` and `o` differ
-            # only where an episode ended
-            same = on is o
-            o = self._aug(o)
-            on = o if same else self._aug_next(on)
         check(_lib.lib().sb200_ppo_window_step_f32(
             _p(on), _p(o), _p(reward), _p(done), self.N, self.n_step,
             self.stride, self.D, self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act),
@@ -206,6 +206,30 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
             _p(r.r_act), _p(r.r_pd), _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), _st()),
             'sb200_ppo_window_step_f32')
         return obs, reward, done, info
+
+    def _step_rnn(self, o, on, reward, done, ready):
+        """Staging of an RNN policy's step in ONE C call (sb200_ppo_window_step_rnn_f32): both rows get the cells the agent
+        holds NOW, i.e. the ones it acts from on the next observation (`on` and `o` differ only where an episode ended).  A
+        host env's observation / successor / reward / done cross PCIe in that call, and the device copy of the next
+        observation is handed to the agent's next act() (cached_device_obs)."""
+        N, Do, r = self.N, self.obs_dim, self.replay
+        h, c = self.cells
+        if self.host_env:
+            h_o = self._pinned('obs', o, (N, Do))
+            h_on = h_o if on is o else self._pinned('obs_next', on, (N, Do))
+            h_r, h_d = self._pinned('rew', reward, (N,)), self._pinned('done', done, (N,))
+            d_o, d_on = self._dev('obs', (N, Do)), self._dev('obs_next', (N, Do))
+            d_r, d_d = self._dev('rew', (N,)), self._dev('done', (N,))
+        else:
+            h_o = h_on = h_r = h_d = None
+            d_o, d_on, d_r, d_d = o, on, reward, done
+        check(_lib.lib().sb200_ppo_window_step_rnn_f32(
+            h_on, h_o, h_r, h_d, _p(d_on), _p(d_o), _p(d_r), _p(d_d), N, self.n_step, self.stride, Do, h.shape[0], h.shape[2],
+            _p(h), _p(c), self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act), _p(self.stage_pd),
+            _p(self.stage_rew), _p(self.stage_done), _p(self._dest), _p(r.state), _p(r.r_obs), _p(r.r_act), _p(r.r_pd),
+            _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), _st()), 'sb200_ppo_window_step_rnn_f32')
+        if self.host_env:
+            self._last_obs_host, self._last_obs_dev = o, d_o
 
 
 class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
@@ -227,17 +251,45 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
     def reset(self):
         obs, info = self.env.reset()
         self.dq_len.zero_()
-        self._obs.copy_(obs['low_dim']['flat_inputs'])
+        if self.host_env:
+            import numpy as np
+            o = obs_flat(obs)
+            self._obs.copy_(torch.from_numpy(np.ascontiguousarray(o, dtype=np.float32)).view(self.N, self.D))
+            self._last_obs_host, self._last_obs_dev = o, self._obs
+        else:
+            self._obs.copy_(obs['low_dim']['flat_inputs'])
         return obs, info
 
     def step(self, action):
         obs, reward, done, info = self.env.step(action)
         r = self.replay
+        if self.host_env:
+            self._step_host(obs, action, reward, done, info)
+            return obs, reward, done, info
         check(_lib.lib().sb200_ssar_step_f32(
             _p(self._obs), _p(action), _p(info['obs_next']), _p(reward), _p(done), self.N, self.n_step,
             float(self.gamma), self.D, self.A, _p(self.dq_len), _p(self.dq_obs), _p(self.dq_act), _p(self.dq_rew),
             _p(self._dest), _p(self._emit), _p(r.state), _p(r.r_obs), _p(r.r_obs_next), _p(r.r_act), _p(r.r_rew),
-            _p(r.r_done), _p(self.env.step_counter), _st()), 'sb200_ssar_step_f32')
+            _p(r.r_done), _p(self.step_counter), _st()), 'sb200_ssar_step_f32')
         r.mark_device_inserts()
         self._obs.copy_(obs['low_dim']['flat_inputs'])             # s_t of the next transition (reset obs where done)
         return obs, reward, done, info
+
+    def _step_host(self, obs, action, reward, done, info):
+        """A host env's step in ONE C call (sb200_ssar_step_host_f32): successor, action, done and the float64 rewards
+        cross PCIe, the n-step sums stay float64 until emission, and s_t of the next transition is left in ``_obs`` --
+        the device copy the agent's next act() reuses (cached_device_obs)."""
+        N, D, A, r = self.N, self.D, self.A, self.replay
+        o = obs_flat(obs)
+        on = info['obs_next'] if (isinstance(info, dict) and 'obs_next' in info) else o
+        h_o = self._pinned('obs', o, (N, D))
+        h_on = h_o if on is o else self._pinned('obs_next', on, (N, D))
+        check(_lib.lib().sb200_ssar_step_host_f32(
+            h_on, h_o, self._pinned('act', action, (N, A)), self._pinned('rew', reward, (N,), torch.float64),
+            self._pinned('done', done, (N,)), _p(self._obs), _p(self._dev('obs_next', (N, D))), _p(self._dev('act', (N, A))),
+            _p(self._dev('rew', (N,), torch.float64)), _p(self._dev('done', (N,))), N, self.n_step, float(self.gamma), D, A,
+            _p(self.dq_len), _p(self.dq_obs), _p(self.dq_act), _p(self.dq_rew), _p(self._dest), _p(self._emit), _p(r.state),
+            _p(r.r_obs), _p(r.r_obs_next), _p(r.r_act), _p(r.r_rew), _p(r.r_done), _p(self.step_counter), _st()),
+            'sb200_ssar_step_host_f32')
+        r.mark_device_inserts()
+        self._last_obs_host, self._last_obs_dev = o, self._obs
