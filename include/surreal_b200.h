@@ -529,6 +529,20 @@ typedef struct {
     float* pd_host;
     float* h_before_host;               /* pinned; NULL: the cells stay on the device */
     float* c_before_host;
+    /* Optional CNN stem stage (pixel input, ppo_net.py:268-279): with frames != NULL layer 0 reads the stem's features
+     * instead of the z-filtered observations (obs and zf are not read):  [H2D frames_host -> frames unless NULL] ->
+     * conv_forward(1) of frames / 255 -> conv_forward(2) -> fc (Linear + ReLU) into xf [N][ld_xf], D = fc's output width.
+     * frames == NULL: no stem, the launches above unchanged.  3 kernels more while every forward stays below 2048 rows. */
+    const uint8_t* frames_host;         /* [N][frame_c][frame_h][frame_w] pinned, or NULL: frames already hold this step's */
+    uint8_t* frames;                    /* [N][frame_c][frame_h][frame_w] uint8 on the device, or NULL */
+    int frame_c, frame_h, frame_w;
+    const float* conv_w1;               /* conv1 k8 s4 -> 16 channels, kernel layout (csrc/stem.cu) */
+    const float* conv_b1;
+    const float* conv_w2;               /* conv2 k4 s2 -> 32 channels */
+    const float* conv_b2;
+    const sb200_mlp* fc;                /* the stem's Linear + ReLU: 32 * H2 * W2 -> D */
+    float* a1;                          /* [N][16][H1][W1] */
+    float* a2;                          /* [N][32 * H2 * W2] */
 } sb200_ppo_act_rnn;
 int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* args, void* stream);
 /*   ppo_window_step_rnn: ppo_window_step for an RNN policy, whose record rows are [obs (obs_dim) | h_0 .. h_{layers-1} |
@@ -536,14 +550,16 @@ int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* args, void* stream);
  *     from the env's [N][obs_dim] rows and the agent's [layers][N][H] cells h / c as they are now, i.e. the cells the
  *     agent acts from on the next observation.  With the host pointers non-NULL (all four) they are uploaded first into
  *     obs_next / obs_reset / reward / done, as ppo_window_step_host does (obs_next_host == obs_reset_host: one upload, into
- *     obs_reset).  Same kernels and launch count as ppo_window_step. */
+ *     obs_reset).  Same kernels and launch count as ppo_window_step.  Rows whose two copies exceed 48 KB of shared memory
+ *     (a pixel frame's words plus the cells) are committed by a kernel that reads the row words straight from obs / h / c
+ *     instead of staging them; force_wide = 1 takes that kernel for any row width (same bytes written). */
 int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const float* obs_reset_host, const float* reward_host,
                                   const float* done_host, float* obs_next, float* obs_reset, float* reward, float* done,
                                   int N, int n_step, int stride, int obs_dim, int layers, int H, const float* h,
                                   const float* c, int A, int* stage_pos, float* stage_obs, float* stage_act,
                                   float* stage_pd, float* stage_rew, float* stage_done, int* dest_scratch,
                                   void* fifo_state, float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                  uint64_t* step_counter, int slots_assigned, void* stream);
+                                  uint64_t* step_counter, int slots_assigned, int force_wide, void* stream);
 
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N
  * actors in ONE launch (a 4-CTA cluster owns 32 actors for the whole chunk; the policy weights stay resident in

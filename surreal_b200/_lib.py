@@ -62,7 +62,10 @@ class PPOActRnn(C.Structure):
                 ('action', C.c_void_p), ('pd', C.c_void_p), ('stage_pos', C.c_void_p), ('stage_act', C.c_void_p),
                 ('stage_pd', C.c_void_p), ('n_step', C.c_int), ('fifo_state', C.c_void_p), ('dest', C.c_void_p),
                 ('action_host', C.c_void_p), ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p),
-                ('c_before_host', C.c_void_p)]
+                ('c_before_host', C.c_void_p), ('frames_host', C.c_void_p), ('frames', C.c_void_p), ('frame_c', C.c_int),
+                ('frame_h', C.c_int), ('frame_w', C.c_int), ('conv_w1', C.c_void_p), ('conv_b1', C.c_void_p),
+                ('conv_w2', C.c_void_p), ('conv_b2', C.c_void_p), ('fc', C.POINTER(Mlp)), ('a1', C.c_void_p),
+                ('a2', C.c_void_p)]
 
 
 class Par(C.Structure):
@@ -140,7 +143,7 @@ def _declare(lib):
         'sb200_ddpg_act_host_f32': (I, [C.POINTER(Mlp), P, P, I, P, P, P, P, I, C.c_uint64, P, D, D, P, P, P, P]),
         'sb200_ppo_act_rnn_f32': (I, [C.POINTER(PPOActRnn), P]),
         'sb200_ppo_window_step_rnn_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P, P, P, P, P, P, P, P,
-                                              P, P, P, P, P, P, I, P]),
+                                              P, P, P, P, P, P, I, I, P]),
         'sb200_ppo_rollout_supported': (I, [C.POINTER(Mlp), I, I]),
         'sb200_ppo_rollout_scratch_ints': (S, [I, I, I]),
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),

@@ -69,10 +69,10 @@ class PPOAgent(Agent):
         """-> action (eval) or (action, [onetime_infos, [pd]]) in training, like ppo_agent.py:151-154.
         Device observations give device results; numpy in, numpy out."""
         N, A, D = self.num_envs, self.action_dim, self.model.low_dim
-        if self.model.cnn_stem is not None:
-            return self._act_pixel(obs, eps)
         if self.model.rnn_stem is not None:
             return self._act_rnn(obs, eps)
+        if self.model.cnn_stem is not None:
+            return self._act_pixel(obs, eps)
         x = obs
         if isinstance(obs, dict):
             xs = [obs['low_dim'][k] for k in obs['low_dim']]
@@ -156,6 +156,7 @@ class PPOAgent(Agent):
             self._hs, self._cs, self._hs_before, self._cs_before = z(L, N, H), z(L, N, H), z(L, N, H), z(L, N, H)
             self._h, self._c = self._hs.squeeze(0), self._cs.squeeze(0)
             self._h_before, self._c_before = self._hs_before.squeeze(0), self._cs_before.squeeze(0)
+            D = self.model.rnn_stem.D                             # the LSTM's input: observation or CNN feature width
             self._xf = z(N, ops._ru(D, 4))[:, :D]
             self._rnn_bufs = self.model.rnn_stem.buffers(N, 1, save=False)
         return self._h, self._c
@@ -164,22 +165,55 @@ class PPOAgent(Agent):
         """act() with the LSTM stem, for host and device observations alike through ONE call of sb200_ppo_act_rnn_f32:
         z-filter -> per layer one LSTM step from each actor's cells, updated in place -> actor head -> sampling
         (ppo_net.py:317-351, ppo_agent.py:133-149).  The cells BEFORE the step are the step's onetime_info.  Host input:
-        H2D of the observation (unless the wrapper already moved it), D2H of the results and one stream sync in that call."""
+        H2D of the observation (unless the wrapper already moved it), D2H of the results and one stream sync in that call.
+        Pixel input: uint8 frames [N, C, H, W] (device tensor or numpy) go through the CNN stem stage of the same call
+        instead of the z-filter."""
         from ..model.lstm_stem import _sfx
         N, A, D = self.num_envs, self.action_dim, self.model.low_dim
         m, stem = self.model, self.model.rnn_stem
         self._rnn_state()
         L, H = stem.layers, stem.H
+        cnn = m.cnn_stem
         x = obs
-        if isinstance(obs, dict):
+        if cnn is not None:
+            x = obs['pixel']['camera0'] if isinstance(obs, dict) else obs
+        elif isinstance(obs, dict):
             xs = [obs['low_dim'][k] for k in obs['low_dim']]
             x = xs[0] if len(xs) == 1 else (torch.cat(xs, -1) if isinstance(xs[0], torch.Tensor) else np.concatenate(xs, -1))
         host = not isinstance(x, torch.Tensor)
         training = self.agent_mode == 'training'
         a = _lib.PPOActRnn()
+        if cnn is not None:
+            # CNN stem stage of the same call: frames -> conv1 -> conv2 -> fc + ReLU -> the LSTM's input rows
+            D = cnn.d_out
+            if not host:
+                if x.dtype != torch.uint8 or x.numel() != N * cnn.C * cnn.H * cnn.W or not x.is_cuda:
+                    raise ValueError('pixel act() wants uint8 CUDA frames [%d, %d, %d, %d], got %s %s'
+                                     % (N, cnn.C, cnn.H, cnn.W, x.dtype, tuple(x.shape)))
+                x = x.contiguous()                               # held until the call below has been issued
+                a.frames = x.data_ptr()
+            else:
+                cached = self.env.cached_device_obs(x) if hasattr(self.env, 'cached_device_obs') else None
+                if cached is not None:                           # the wrapper already moved these frames (as words)
+                    a.frames = cached.data_ptr()
+                else:                                            # H2D inside the call, from pinned staging
+                    if self._obs_pin is None:
+                        self._obs_pin = torch.empty(N, cnn.C, cnn.H, cnn.W, dtype=torch.uint8, pin_memory=True)
+                        self._frames_dev = torch.empty(N, cnn.C, cnn.H, cnn.W, dtype=torch.uint8, device=self.device)
+                    self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.uint8).reshape(N, cnn.C, cnn.H, cnn.W)
+                    a.frames_host, a.frames = self._obs_pin.data_ptr(), self._frames_dev.data_ptr()
+            a.frame_c, a.frame_h, a.frame_w = cnn.C, cnn.H, cnn.W
+            a.conv_w1, a.conv_b1 = cnn.seg('w1').data_ptr(), cnn.seg('b1').data_ptr()
+            a.conv_w2, a.conv_b2 = cnn.seg('w2').data_ptr(), cnn.seg('b2').data_ptr()
+            fc = cnn.fc.desc()
+            a.fc = C.pointer(fc)
+            if getattr(self, '_stem_bufs', None) is None:
+                self._stem_bufs = cnn.buffers(N)
+            a.a1, a.a2 = self._stem_bufs['a1'].data_ptr(), self._stem_bufs['a2'].data_ptr()
         if host:
-            obs_host, obs_dev = self._host_obs(np.asarray(x), D)
-            a.obs_host, a.obs, a.ld_obs = (obs_host.value if obs_host is not None else None), obs_dev.data_ptr(), D
+            if cnn is None:
+                obs_host, obs_dev = self._host_obs(np.asarray(x), D)
+                a.obs_host, a.obs, a.ld_obs = (obs_host.value if obs_host is not None else None), obs_dev.data_ptr(), D
             if self._out_pin is None:
                 self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
                                  torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
@@ -189,7 +223,7 @@ class PPOAgent(Agent):
                     self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
                                        torch.empty(L, N, H, dtype=torch.float32, pin_memory=True))
                 a.h_before_host, a.c_before_host = self._cells_pin[0].data_ptr(), self._cells_pin[1].data_ptr()
-        else:
+        elif cnn is None:
             x = x.reshape(N, D)
             a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
         head = m.actor.desc()

@@ -311,6 +311,51 @@ __global__ void __launch_bounds__(128) ppo_window_commit_rnn_kernel(const float*
                  dest[i], stage_obs, stage_act, stage_pd, stage_rew, stage_done, r_obs, r_act, r_pd, r_rew, r_done);
 }
 
+// Record row [obs (Do) | h_0 .. h_{L-1} | c_0 .. c_{L-1}] of actor i read straight from the env's row and the agent's
+// [L][N][H] cells: the commit of rows too wide to stage in shared memory (a pixel frame plus the cells).
+struct CellRow {
+    const float* __restrict__ obs;      // the actor's Do observation words
+    const float* __restrict__ h;
+    const float* __restrict__ c;
+    int Do, LH, H, N, i;
+    __device__ __forceinline__ float operator[](int d) const {
+        if (d < Do) return obs[d];
+        int e = d - Do;
+        const float* cells = h;
+        if (e >= LH) {
+            e -= LH;
+            cells = c;
+        }
+        const int k = e / H;
+        return cells[((long long)k * N + i) * H + (e - k * H)];
+    }
+};
+
+__global__ void __launch_bounds__(128, 4) ppo_window_commit_rnn_wide_kernel(const float* __restrict__ obs_next,
+                                                                         const float* __restrict__ obs_reset,
+                                                                         const float* __restrict__ reward,
+                                                                         const float* __restrict__ done, int N, int n_step,
+                                                                         int stride, int Do, int L, int H,
+                                                                         const float* __restrict__ h,
+                                                                         const float* __restrict__ c, int A,
+                                                                         int* __restrict__ stage_pos,
+                                                                         float* __restrict__ stage_obs,
+                                                                         float* __restrict__ stage_act,
+                                                                         float* __restrict__ stage_pd,
+                                                                         float* __restrict__ stage_rew,
+                                                                         float* __restrict__ stage_done,
+                                                                         const int* __restrict__ dest,
+                                                                         float* __restrict__ r_obs, float* __restrict__ r_act,
+                                                                         float* __restrict__ r_pd, float* __restrict__ r_rew,
+                                                                         float* __restrict__ r_done) {
+    const int i = blockIdx.x;
+    const CellRow next = {obs_next + (long long)i * Do, h, c, Do, L * H, H, N, i};
+    const CellRow reset = {obs_reset + (long long)i * Do, h, c, Do, L * H, H, N, i};
+    commit_actor<BlockBarrier, CellRow>(true, i, threadIdx.x, blockDim.x, next, reset, reward[i], done[i], n_step, stride,
+                                        Do + 2 * L * H, A, stage_pos + i, dest[i], stage_obs, stage_act, stage_pd, stage_rew,
+                                        stage_done, r_obs, r_act, r_pd, r_rew, r_done);
+}
+
 // Fused environment step + window commit for the device-resident synthetic env: the successor state never
 // leaves shared memory before it is staged.  One block per 4 actors, 64 threads per actor in the commit.
 __global__ void __launch_bounds__(RT) synth_env_window_step_kernel(
@@ -547,8 +592,16 @@ extern "C" int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_ho
 
 extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
     SB200_REQUIRE(a != nullptr && a->head != nullptr && a->layers >= 1 && a->layers <= SB200_MAX_RNN_LAYERS);
-    SB200_REQUIRE(a->N >= 1 && a->D >= 1 && a->H >= 1 && a->ldh >= a->H && a->ld_obs >= a->D && a->ld_xf >= a->D);
-    SB200_REQUIRE(a->obs && a->xf && a->pre_x && a->h_out[0] && (a->layers == 1 || a->h_out[1]));
+    const bool stem = a->frames != nullptr;
+    SB200_REQUIRE(a->N >= 1 && a->D >= 1 && a->H >= 1 && a->ldh >= a->H && a->ld_xf >= a->D);
+    // stem geometry (k8 s4 then k4 s2), checked before anything is issued
+    const int H1 = (a->frame_h - 8) / 4 + 1, W1 = (a->frame_w - 8) / 4 + 1;
+    const int H2 = (H1 - 4) / 2 + 1, W2 = (W1 - 4) / 2 + 1;
+    SB200_REQUIRE(stem ? (a->fc && a->conv_w1 && a->conv_b1 && a->conv_w2 && a->conv_b2 && a->a1 && a->a2 &&
+                          a->obs_host == nullptr && a->frame_c >= 1 && a->frame_h >= 8 && a->frame_w >= 8 && H1 >= 4 &&
+                          W1 >= 4 && a->fc->n_layers == 1 && a->fc->dims[0] == 32 * H2 * W2 && a->fc->dims[1] == a->D)
+                       : (a->obs && a->ld_obs >= a->D && a->frames_host == nullptr));
+    SB200_REQUIRE(a->xf && a->pre_x && a->h_out[0] && (a->layers == 1 || a->h_out[1]));
     SB200_REQUIRE(a->h && a->c && a->h_before && a->c_before && a->mean && a->log_var && a->action && a->pd);
     SB200_REQUIRE(a->obs_host == nullptr || a->ld_obs == a->D);
     SB200_REQUIRE(a->action_host == nullptr || a->pd_host != nullptr);
@@ -557,15 +610,33 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const int N = a->N, D = a->D, H = a->H, L = a->layers, A = a->head->dims[a->head->n_layers];
     const size_t cells = (size_t)L * N * H * sizeof(float);
-    if (a->obs_host != nullptr)
-        SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
-    SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
-    int rc = sb200_rows_zfilter_f32(a->obs, D, a->ld_obs, N, 1, D, a->zf.stats, (double)a->zf.eps, a->xf, a->ld_xf, stream);
-    if (rc != SB200_OK) return rc;
     const sb200_zfilter nozf = {nullptr, 1e-5f};
     float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
     int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
+    int rc = SB200_OK;
+    if (stem) {
+        const size_t frame_bytes = (size_t)a->frame_c * a->frame_h * a->frame_w;
+        if (a->frames_host != nullptr)
+            SB200_CUDA(cudaMemcpyAsync(a->frames, a->frames_host, (size_t)N * frame_bytes, cudaMemcpyHostToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
+        rc = sb200_conv_forward_f32(1, a->frames, 1, N, a->frame_c, a->frame_h, a->frame_w, a->conv_w1, a->conv_b1,
+                                    1.0 / 255.0, a->a1, stream);
+        if (rc != SB200_OK) return rc;
+        rc = sb200_conv_forward_f32(2, a->a1, 0, N, 16, H1, W1, a->conv_w2, a->conv_b2, 1.0, a->a2, stream);
+        if (rc != SB200_OK) return rc;
+        const sb200_rows fin = {a->a2, nullptr, a->fc->dims[0], N, 0, nullptr, 0, nullptr, 0};
+        save[0] = a->xf;
+        lds[0] = a->ld_xf;
+        rc = sb200_mlp_forward_f32(a->fc, &nozf, &fin, save, lds, stream);
+    } else {
+        if (a->obs_host != nullptr)
+            SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
+        rc = sb200_rows_zfilter_f32(a->obs, D, a->ld_obs, N, 1, D, a->zf.stats, (double)a->zf.eps, a->xf, a->ld_xf, stream);
+    }
+    if (rc != SB200_OK) return rc;
     sb200_rows in = {a->xf, nullptr, a->ld_xf, N, 0, nullptr, 0, nullptr, 0};
     for (int k = 0; k < L; ++k) {
         save[0] = a->pre_x;
@@ -613,7 +684,7 @@ extern "C" int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const f
                                              int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
                                              float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
                                              float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                             uint64_t* step_counter, int slots_assigned, void* stream) {
+                                             uint64_t* step_counter, int slots_assigned, int force_wide, void* stream) {
     SB200_REQUIRE(obs_next && obs_reset && reward && done && h && c && stage_pos && stage_obs && stage_act && stage_pd);
     SB200_REQUIRE(stage_rew && stage_done && dest_scratch && fifo_state && r_obs && r_act && r_pd && r_rew && r_done);
     SB200_REQUIRE(N >= 1 && n_step >= 1 && stride >= 1 && obs_dim >= 1 && layers >= 1 && H >= 1 && A >= 1);
@@ -621,7 +692,7 @@ extern "C" int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const f
     SB200_REQUIRE(host ? (obs_next_host && reward_host && done_host) : (!obs_next_host && !reward_host && !done_host));
     const int D = obs_dim + 2 * layers * H;
     const size_t smem = (size_t)2 * D * sizeof(float);
-    SB200_REQUIRE(smem <= 48 * 1024);
+    const bool wide = smem > 48 * 1024 || force_wide;            // rows too wide to stage in shared memory
     cudaStream_t st = (cudaStream_t)stream;
     const float* next = obs_next;
     if (host) {
@@ -637,8 +708,13 @@ extern "C" int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const f
     if (!slots_assigned)
         ppo_window_slots_kernel<<<1, 1024, 0, st>>>(N, n_step, stage_pos, dest_scratch, (FifoState*)fifo_state,
                                                     (unsigned long long*)step_counter);
-    ppo_window_commit_rnn_kernel<<<N, 128, smem, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers, H, h,
-                                                       c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
-                                                       stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
+    if (wide)
+        ppo_window_commit_rnn_wide_kernel<<<N, 128, 0, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers,
+                                                             H, h, c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
+                                                             stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
+    else
+        ppo_window_commit_rnn_kernel<<<N, 128, smem, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers,
+                                                           H, h, c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
+                                                           stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
     return sb200_launch_status(slots_assigned ? 1 : 2);
 }

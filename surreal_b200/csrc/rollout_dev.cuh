@@ -111,9 +111,15 @@ struct BlockBarrier {
 struct WarpBarrier {
     __device__ __forceinline__ void operator()() const { __syncwarp(); }
 };
-template <class Barrier = BlockBarrier>
-__device__ void commit_actor(bool valid, int i, int g, int G, const float* __restrict__ next_row,
-                             const float* __restrict__ reset_row, float rew, float dn, int n_step, int stride, int D,
+// `next_row` / `reset_row` are read as next_row[d], d < D: float pointers by default, or -- given explicitly as Row -- a
+// type that assembles the row on the fly (rollout.cu's CellRow).
+template <class T>
+struct NoDeduce {
+    using type = T;
+};
+template <class Barrier = BlockBarrier, class Row = const float* __restrict__>
+__device__ void commit_actor(bool valid, int i, int g, int G, typename NoDeduce<Row>::type next_row,
+                             typename NoDeduce<Row>::type reset_row, float rew, float dn, int n_step, int stride, int D,
                              int A, int* __restrict__ pos, int slot, float* __restrict__ stage_obs,
                              float* __restrict__ stage_act, float* __restrict__ stage_pd,
                              float* __restrict__ stage_rew, float* __restrict__ stage_done,

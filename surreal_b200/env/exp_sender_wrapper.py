@@ -13,7 +13,7 @@ from .. import _lib
 from .._lib import check
 from ..distributed import LocalHub
 from ..session import ConfigError
-from ..utils import obs_flat
+from ..utils import obs_flat, obs_source
 
 
 def _p(t):
@@ -120,6 +120,7 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         self._slots_ready = False      # the agent's sampling kernel already assigned this step's replay slots
         self.fuse_launches = True      # sample+assign / env+commit: 3 launches per step instead of 5 (same results)
         self.persistent_rollout = True  # device env + supported policy: whole chunks in ONE launch (agent.rollout_chunk)
+        self.wide_commit = False       # RNN records: commit without shared-memory staging at any row width (same bytes)
         self._outbox = {}
         r = self.replay
         assert (r.n_step, r.D, r.A) == (n, D, A), 'replay record shape does not match the env / n_step'
@@ -132,7 +133,7 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         if self.host_env:
             d = self._h2d('obs', o, (self.N, self.obs_dim))
             row0[:, :self.obs_dim].copy_(d)
-            self._last_obs_host, self._last_obs_dev = o, d
+            self._last_obs_host, self._last_obs_dev = obs_source(obs), d
         else:
             row0[:, :self.obs_dim].copy_(o)
         if self.cells is not None:                                 # the cells the agent acts from on this observation
@@ -180,7 +181,7 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         o = obs_flat(obs)
         on = obs_flat(info['obs_next']) if (isinstance(info, dict) and 'obs_next' in info) else o
         if self.cells is not None:
-            self._step_rnn(o, on, reward, done, ready)
+            self._step_rnn(o, on, reward, done, ready, obs_source(obs))
             return obs, reward, done, info
         if self.host_env:
             # host env: this step's successor observation / reward / done cross PCIe here (256 KB + 8 KB), issued with
@@ -207,11 +208,12 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
             'sb200_ppo_window_step_f32')
         return obs, reward, done, info
 
-    def _step_rnn(self, o, on, reward, done, ready):
+    def _step_rnn(self, o, on, reward, done, ready, src):
         """Staging of an RNN policy's step in ONE C call (sb200_ppo_window_step_rnn_f32): both rows get the cells the agent
         holds NOW, i.e. the ones it acts from on the next observation (`on` and `o` differ only where an episode ended).  A
-        host env's observation / successor / reward / done cross PCIe in that call, and the device copy of the next
-        observation is handed to the agent's next act() (cached_device_obs)."""
+        host env's observation / successor / reward / done cross PCIe in that call (uint8 frames as their 32-bit words),
+        and the device copy of the next observation is handed to the agent's next act() (cached_device_obs, keyed by
+        ``src``, the array the env returned)."""
         N, Do, r = self.N, self.obs_dim, self.replay
         h, c = self.cells
         if self.host_env:
@@ -227,9 +229,10 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
             h_on, h_o, h_r, h_d, _p(d_on), _p(d_o), _p(d_r), _p(d_d), N, self.n_step, self.stride, Do, h.shape[0], h.shape[2],
             _p(h), _p(c), self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act), _p(self.stage_pd),
             _p(self.stage_rew), _p(self.stage_done), _p(self._dest), _p(r.state), _p(r.r_obs), _p(r.r_act), _p(r.r_pd),
-            _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), _st()), 'sb200_ppo_window_step_rnn_f32')
+            _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), int(self.wide_commit), _st()),
+            'sb200_ppo_window_step_rnn_f32')
         if self.host_env:
-            self._last_obs_host, self._last_obs_dev = o, d_o
+            self._last_obs_host, self._last_obs_dev = src, d_o
 
 
 class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):

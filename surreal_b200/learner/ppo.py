@@ -106,7 +106,8 @@ class PPOLearner(Learner):
         B, n, A = self.batch_size, self.n_step, self.action_dim
         self.pixel = self.model.cnn_stem is not None
         self.rnn = self.model.rnn_stem is not None
-        self.obs_dim = self.model.low_dim                         # width of the low-dim features themselves
+        # width of the observation itself in the records: the low-dim features, or the frame's 32-bit words
+        self.obs_dim = U.obs_packed_dim(self.obs_spec) if self.pixel else self.model.low_dim
         # width of one observation in the batch buffers: the low-dim features (+ the actor's LSTM cells h | c in RNN mode,
         # which ride in the observation rows of the HBM records -- the reference ships them as onetime_infos), or the uint8
         # frame as 32-bit words
@@ -131,16 +132,29 @@ class PPOLearner(Learner):
             from ..model.lstm_stem import RnnTrainer
             stem, E, Hh, od = self.model.rnn_stem, self.eff_len, self.model.rnn_stem.H, self.obs_dim
             self.actor_rnn, self.critic_rnn = RnnTrainer(stem, B, E), RnnTrainer(stem, B, E)
-            self._g_actor = torch.zeros(self.model.actor.size + stem.size, dtype=torch.float32, device=dev)
-            self._g_critic = torch.zeros(self.model.critic.size + stem.size, dtype=torch.float32, device=dev)
+            # one gradient buffer per optimiser: [head | CNN stem (pixel input) | LSTM stem]
+            ns = stem.size + (self.model.cnn_stem.size if self.pixel else 0)
+            self._g_actor = torch.zeros(self.model.actor.size + ns, dtype=torch.float32, device=dev)
+            self._g_critic = torch.zeros(self.model.critic.size + ns, dtype=torch.float32, device=dev)
             self.actor_optim.grad = self._g_actor[:self.model.actor.size]
             self.critic_optim.grad = self._g_critic[:self.model.critic.size]
             zz = lambda r, w: torch.zeros(r, ops._ru(w, 4), dtype=torch.float32, device=dev)[:, :w]  # noqa: E731
-            self._xf_all, self._xf_eff, self._xf_ref, self._xraw_eff = zz(B * (n + 1), od), zz(M, od), zz(M, od), zz(M, od)
+            # sequence-major rows: z-filtered observations, or -- pixel input -- dense frames (od words, a multiple of 4,
+            # so each buffer is a contiguous uint8 [rows, C, H, W] block the conv kernels read)
+            self._xf_all, self._xf_eff = zz(B * (n + 1), od), zz(M, od)
+            if not self.pixel:
+                self._xf_ref, self._xraw_eff = zz(M, od), zz(M, od)
             self._act_it, self._pd_it = torch.zeros(M, A, device=dev), torch.zeros(M, 2 * A, device=dev)
             self._rnn_all = stem.buffers(B, n + 1, save=False)
             self._rnn_ref = self.ref_target_model.rnn_stem.buffers(B, E, save=False)
-        if self.pixel:
+        if self.pixel and self.rnn:
+            # CNN stem in front of the LSTM stem: one StemTrainer per optimiser on the B*eff_len update frames
+            from ..model.cnn_stem import StemTrainer
+            stem = self.model.cnn_stem
+            self.actor_stem, self.critic_stem = StemTrainer(stem, M), StemTrainer(stem, M)
+            self._stem_all = stem.buffers(B * (n + 1))
+            self._ref_stem_bufs = self.ref_target_model.cnn_stem.buffers(M)
+        elif self.pixel:
             # the CNN stem is shared by actor and critic and trained by BOTH optimisers, each with its own Adam state
             # (ppo_net.py:202-224): one StemTrainer per optimiser, gradients of head + stem in one contiguous buffer
             from ..model.cnn_stem import StemTrainer
@@ -284,7 +298,12 @@ class PPOLearner(Learner):
         elif self.pixel:
             obs = None
             fo, fn = get('obs')['pixel']['camera0'], get('obs_next')['pixel']['camera0']
-            u8 = own['obs_full'].view(torch.uint8).view(B, n + 1, -1)
+            u8 = own['obs_full'].view(torch.uint8).view(B, n + 1, -1)[:, :, :4 * self.obs_dim]
+            if self.rnn:                          # onetime_infos = [h0, c0] [B, L, H] behind the first frame
+                hc, cl = get('onetime_infos'), self.cell_layout
+                LH = cl.layers * cl.hidden
+                cl.h(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[0]).reshape(B, LH), non_blocking=True)
+                cl.c(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[1]).reshape(B, LH), non_blocking=True)
             if isinstance(fo, torch.Tensor):
                 u8[:, :n].copy_(fo.reshape(B, n, -1), non_blocking=True)
                 u8[:, n:].copy_(fn.reshape(B, 1, -1), non_blocking=True)
@@ -341,7 +360,8 @@ class PPOLearner(Learner):
             # then the horizon-windowed GAE over eff_len positions (ppo.py:389-406)
             self._rnn_prepare()
             h0, c0, ld = self._cells()
-            h_all = m.rnn_stem.forward(self._xf_all, h0, c0, ld, B, n + 1, self._rnn_all)
+            x_all = m.cnn_stem.forward(self._frames(self._xf_all), self._stem_all) if self.pixel else self._xf_all
+            h_all = m.rnn_stem.forward(x_all, h0, c0, ld, B, n + 1, self._rnn_all)
             ops.mlp_forward(m.critic, h_all, out=self._values)
         elif self.pixel:
             # all B*(n+1) frames through the shared stem, then the critic head on the features (ppo.py:376-387, 5-D obs)
@@ -395,17 +415,41 @@ class PPOLearner(Learner):
     def _rnn_prepare(self):
         """Once per learn(): contiguous, z-filtered sequence rows -- all n+1 steps for the critic pass, the first eff_len
         for the updates (through the learner's AND the reference model's filter, ppo.py:507-539) -- and the step slices of
-        actions / behaviour policy the updates iterate on."""
+        actions / behaviour policy the updates iterate on.  Pixel input: the same two gathers, unfiltered, give the dense
+        uint8 frames of the CNN stem (a float load / store copies the bits of any word, denormal and NaN patterns too)."""
         from ..model.lstm_stem import rows_zfilter
         B, n, A, E, od, Dp = self.batch_size, self.n_step, self.action_dim, self.eff_len, self.obs_dim, self.low_dim
         m, ref = self.model, self.ref_target_model
         o = self._obs_full
         rows_zfilter(o, Dp, (n + 1) * Dp, B, n + 1, od, m.z_stats, m.z_eps, self._xf_all)
         rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, m.z_stats, m.z_eps, self._xf_eff)
-        rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, ref.z_stats, ref.z_eps, self._xf_ref)
-        rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, None, 0.0, self._xraw_eff)
+        if not self.pixel:
+            rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, ref.z_stats, ref.z_eps, self._xf_ref)
+            rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, None, 0.0, self._xraw_eff)
         rows_zfilter(self._actions, A, n * A, B, E, A, None, 0.0, self._act_it)
         rows_zfilter(self._pds, 2 * A, n * 2 * A, B, E, 2 * A, None, 0.0, self._pd_it)
+
+    def _frames(self, rows):
+        """The gathered frame rows [R, od] as the uint8 [R, C, H, W] frames the CNN stem reads."""
+        return rows.view(torch.uint8).view(rows.shape[0], *stem_shape(self.model.cnn_stem))
+
+    def _rnn_forward(self, rnn_tr, stem_tr):
+        """Training forward of one optimiser through its stem trainers on the eff_len update steps: the LSTM's top-layer
+        output [B*eff_len, H], the CNN stem in front of it with pixel input."""
+        x = stem_tr.forward(self._frames(self._xf_eff)) if self.pixel else self._xf_eff
+        return rnn_tr.forward(x, *self._cells())
+
+    def _rnn_backward(self, head_tr, rnn_tr, stem_tr, grad, norm_out, stop=None):
+        """BPTT of the LSTM stem from the head's input gradient, then -- pixel input -- the CNN stem's backward from the
+        LSTM's input gradient masked by relu'(features), and ONE joint step over [head | CNN | LSTM]."""
+        from ..model.cnn_stem import joint_step
+        rnn_tr.backward(head_tr.dx0)
+        if self.pixel:
+            rnn_tr.backward_input(stem_tr.d_fc, stem_tr.bufs['feat'])
+            stem_tr.backward(stem_tr.d_fc)
+            joint_step(head_tr, [stem_tr, rnn_tr], grad, norm_out=norm_out, stop_flag=stop)
+        else:
+            joint_step(head_tr, rnn_tr, grad, norm_out=norm_out, stop_flag=stop)
 
     # -- live kernel timing for bench.py's roofline (CUDA events on the launching stream) ---------------
     def _prof_begin(self):
@@ -441,7 +485,7 @@ class PPOLearner(Learner):
         M = self._rows
         acts, lda, pds, ldp = (self._act_it, A, self._pd_it, 2 * A) if self.rnn else (self._actions, n * A, self._pds, n * 2 * A)
         if self.rnn:
-            mean = tr.forward(self.actor_rnn.forward(self._xf_eff, *self._cells())) if fresh else tr.out
+            mean = tr.forward(self._rnn_forward(self.actor_rnn, getattr(self, 'actor_stem', None))) if fresh else tr.out
         elif self.pixel:
             mean = tr.forward(self.actor_stem.forward(self._frames0)) if fresh else tr.out
         else:
@@ -458,10 +502,9 @@ class PPOLearner(Learner):
                                           _ptr(stop), st), 'sb200_ppo_policy_loss_f32')
         tr.backward()
         if self.rnn:
-            from ..model.cnn_stem import joint_step
-            self.actor_rnn.backward(tr.dx0)
-            joint_step(tr, self.actor_rnn, self._g_actor, norm_out=self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop_flag=stop)
-            self._cur_mean = tr.forward(self.actor_rnn.forward(self._xf_eff, *self._cells()))
+            stem_tr = getattr(self, 'actor_stem', None)
+            self._rnn_backward(tr, self.actor_rnn, stem_tr, self._g_actor, self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop)
+            self._cur_mean = tr.forward(self._rnn_forward(self.actor_rnn, stem_tr))
         elif self.pixel:
             from ..model.cnn_stem import joint_step
             self.actor_stem.backward(tr.dx0)
@@ -539,7 +582,7 @@ class PPOLearner(Learner):
         B, n, D = self.batch_size, self.n_step, self.low_dim
         m, tr, st = self.model, self.critic_optim, ops._stream()
         if self.rnn:
-            v = tr.forward(self.critic_rnn.forward(self._xf_eff, *self._cells()))
+            v = tr.forward(self._rnn_forward(self.critic_rnn, getattr(self, 'critic_stem', None)))
         elif self.pixel:
             v = tr.forward(self.critic_stem.forward(self._frames0))
         else:
@@ -548,9 +591,8 @@ class PPOLearner(Learner):
                                      _ptr(self._stats), _ptr(self._loss_ws_v), st), 'sb200_value_loss_f32')
         tr.backward()
         if self.rnn:
-            from ..model.cnn_stem import joint_step
-            self.critic_rnn.backward(tr.dx0)
-            joint_step(tr, self.critic_rnn, self._g_critic, norm_out=self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
+            self._rnn_backward(tr, self.critic_rnn, getattr(self, 'critic_stem', None), self._g_critic,
+                               self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
         elif self.pixel:
             from ..model.cnn_stem import joint_step
             self.critic_stem.backward(tr.dx0)
@@ -563,7 +605,8 @@ class PPOLearner(Learner):
         ref = self.ref_target_model
         self._gae_and_return()
         if self.rnn:
-            h_ref = ref.rnn_stem.forward(self._xf_ref, *self._cells(), B, self.eff_len, self._rnn_ref)
+            x_ref = ref.cnn_stem.forward(self._frames(self._xf_eff), self._ref_stem_bufs) if self.pixel else self._xf_ref
+            h_ref = ref.rnn_stem.forward(x_ref, *self._cells(), B, self.eff_len, self._rnn_ref)
             ops.mlp_forward(ref.actor, h_ref, out=self._ref_mean)
         elif self.pixel:
             # step-0 frames of every window, contiguous (ppo.py:527-537), then the reference policy on them
@@ -817,7 +860,9 @@ class PPOLearner(Learner):
         ck = self.session_config.checkpoint.learner
         if 'include_optimizer' in ck and ck.include_optimizer:
             attrs += ['actor_optim', 'critic_optim', 'adapt_state']
-            if self.rnn:                                          # each optimiser's Adam moments over the shared LSTM stem
+            if self.pixel:                                        # each optimiser's Adam moments over the shared CNN stem
+                attrs += ['actor_stem', 'critic_stem']
+            if self.rnn:                                          # ... and over the shared LSTM stem
                 attrs += ['actor_rnn', 'critic_rnn']
         return attrs
 

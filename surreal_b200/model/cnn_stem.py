@@ -156,27 +156,34 @@ class StemTrainer:
         self.exp_avg_sq.copy_(torch.as_tensor(sd['exp_avg_sq']).to(self.stem.device))
 
 
-def joint_step(head, stem_tr, grad, norm_out=None, stop_flag=None):
-    """One optimiser step over a head network (ops.MlpTrainer) AND the shared stem: the reference clips the global norm of
-    head + stem parameters together (get_actor_params / get_critic_params, ppo_net.py:202-224; ppo.py:244-246,349-351)
-    and steps ONE Adam over both.  ``grad`` = [head gradient | stem gradient] is one contiguous buffer so that the norm
-    (and a data-parallel all-reduce) sees everything at once; head.ws carries the shared step count / norm."""
+def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None):
+    """One optimiser step over a head network (ops.MlpTrainer) AND the shared stems: the reference clips the global norm
+    of head + stem parameters together (get_actor_params / get_critic_params chain actor, cnn_stem and rnn_stem,
+    ppo_net.py:202-224; ppo.py:244-246,349-351) and steps ONE Adam over all of them.  ``stem_trs`` is one stem trainer
+    (StemTrainer / lstm_stem.RnnTrainer) or a list of them; ``grad`` = [head gradient | stem gradients in that order] is
+    one contiguous buffer so that the norm (and a data-parallel all-reduce) sees everything at once; head.ws carries the
+    shared step count / norm."""
     L, st = _lib.lib(), ops._stream()
-    nh, ns = head.net.size, stem_tr.stem.size
-    gh, gs = grad[:nh], grad[nh:nh + ns]
+    trs = stem_trs if isinstance(stem_trs, (list, tuple)) else [stem_trs]
+    nh = head.net.size
+    segs, o = [(head.net.params, grad[:nh], head.exp_avg, head.exp_avg_sq, nh, norm_out)], nh
     sf = C.c_void_p(stop_flag.data_ptr()) if stop_flag is not None else None
-    check(L.sb200_grad_reduce_norm_f32(_p(head.slabs), nh, head.splits, _p(gh), nh, 1.0, 0, _p(head.ws), sf, st),
+    check(L.sb200_grad_reduce_norm_f32(_p(head.slabs), nh, head.splits, _p(grad[:nh]), nh, 1.0, 0, _p(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(head)')
-    check(L.sb200_grad_reduce_norm_f32(_p(stem_tr.slabs), ns, stem_tr.splits, _p(gs), ns, 1.0, 0, _p(head.ws), sf, st),
-          'sb200_grad_reduce_norm_f32(stem)')
+    for tr in trs:
+        ns = tr.stem.size
+        gs = grad[o:o + ns]
+        check(L.sb200_grad_reduce_norm_f32(_p(tr.slabs), ns, tr.splits, _p(gs), ns, 1.0, 0, _p(head.ws), sf, st),
+              'sb200_grad_reduce_norm_f32(stem)')
+        segs.append((tr.stem.params, gs, tr.exp_avg, tr.exp_avg_sq, ns, None))
+        o += ns
     dp = getattr(head, 'dp', None)
     scale = 1.0
     if dp is not None:
         dp.sum_(grad)
         scale = 1.0 / dp.world
-    check(L.sb200_grad_reduce_norm_f32(_p(grad), nh + ns, 1, _p(grad), nh + ns, scale, 1, _p(head.ws), sf, st),
+    check(L.sb200_grad_reduce_norm_f32(_p(grad), o, 1, _p(grad), o, scale, 1, _p(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(joint norm)')
-    for params, g, m, v, n, no in ((head.net.params, gh, head.exp_avg, head.exp_avg_sq, nh, norm_out),
-                                   (stem_tr.stem.params, gs, stem_tr.exp_avg, stem_tr.exp_avg_sq, ns, None)):
+    for params, g, m, v, n, no in segs:
         check(L.sb200_clip_adam_f32(_p(params), _p(g), _p(m), _p(v), n, _p(head.lr), 0.9, 0.999, 1e-8, head.weight_decay,
                                     head.clip_mode, head.clip_value, _p(head.ws), _p(no), sf, st), 'sb200_clip_adam_f32')

@@ -180,6 +180,16 @@ class RnnTrainer:
                 check(L_.sb200_linear_bwd_dx_f32(_p(dpre), G, C.c_void_p(ih.params.data_ptr() + 4 * lay_i['w']), lay_i['ldw'], None, 0,
                                                  _p(dh), dh.stride(0), R, G, s.H, st), 'sb200_linear_bwd_dx_f32(lstm layer input)')
 
+    def backward_input(self, dx, x_act):
+        """After ``backward``: the gradient w.r.t. layer 0's input, dpre_0 . W_ih_0, masked by relu'(x_act) -- i.e. w.r.t.
+        the pre-activation of a ReLU layer in front of the stem whose output ``x_act`` [B*L, D] the stem read (the CNN
+        stem's features) -- into ``dx`` [B*L, >= D]."""
+        s, R, G = self.stem, self.B * self.L, 4 * self.stem.H
+        ih, lay = s.ihs[0], s.ihs[0].layout[0]
+        check(_lib.lib().sb200_linear_bwd_dx_f32(_p(self.dpres[0]), G, C.c_void_p(ih.params.data_ptr() + 4 * lay['w']), lay['ldw'],
+                                                 _p(x_act), x_act.stride(0), _p(dx), dx.stride(0), R, G, s.D, ops._stream()),
+              'sb200_linear_bwd_dx_f32(lstm stem input)')
+
     def state_dict(self):
         return {'exp_avg': self.exp_avg.detach().clone(), 'exp_avg_sq': self.exp_avg_sq.detach().clone()}
 

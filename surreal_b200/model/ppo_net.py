@@ -26,7 +26,8 @@ def _default_linear_init(dims, seed_gen=None):
 
 class PPOModel:
     """Same constructor keywords as the reference's PPOModel (ppo_net.py:110-118).  The LSTM stem (rnn_layer layers) is
-    model/lstm_stem.py; the CNN stem (pixel input) is model/cnn_stem.py."""
+    model/lstm_stem.py; the CNN stem (pixel input) is model/cnn_stem.py.  With both, frames run through the CNN stem,
+    its features through the LSTM stem, and the heads read the LSTM's output."""
 
     def __init__(self, obs_spec, action_dim, model_config, use_cuda=True, init_log_sig=0, use_z_filter=False,
                  if_pixel_input=False, rnn_config=None, device=None):
@@ -52,9 +53,8 @@ class PPOModel:
             self.cnn_stem = CNNStem(obs_spec['pixel']['camera0'], model_config.cnn_feature_dim, self.device)
         in_dim = self.low_dim + (model_config.cnn_feature_dim if if_pixel_input else 0)
         if self.if_rnn:
-            # optional LSTM stem feature extractor (ppo_net.py:143-152), shared by actor and critic
-            if if_pixel_input:
-                raise NotImplementedError('CNN + LSTM stems together (pixel input with if_rnn_policy) are not built')
+            # optional LSTM stem feature extractor (ppo_net.py:143-152), shared by actor and critic; with pixel input it
+            # reads the CNN stem's features (the two stems in series, ppo_net.py:268-279)
             from .lstm_stem import LSTMStem
             if int(rnn_config.rnn_layer) < 1:
                 from ..session import ConfigError

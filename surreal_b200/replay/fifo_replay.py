@@ -142,17 +142,17 @@ class FIFOReplay(Replay):
         if self.check_underflow and int(self._status.item()) != 0:      # host sync; the engine polls
             raise IndexError('pop from a FIFO replay holding fewer than %d windows' % batch_size)   # len() instead
         obs_full = out['obs_full']
-        if self.pixel_shape is not None:
-            fr = obs_full.view(torch.uint8).view(batch_size, n + 1, *self.pixel_shape)
-            return {'obs': {'pixel': {'camera0': fr[:, :n]}}, 'obs_next': {'pixel': {'camera0': fr[:, n:]}},
-                    'obs_full': obs_full, 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'],
-                    'persistent_infos': [out['pd']], 'onetime_infos': None}
         od = self.obs_dim
         onetime = None
         cl = self.cells
         if cl is not None:         # RNN policy: the LSTM cells of the window's first step ride behind the observation
             onetime = [cl.h(obs_full[:, 0]).unflatten(1, (cl.layers, cl.hidden)),
                        cl.c(obs_full[:, 0]).unflatten(1, (cl.layers, cl.hidden))]       # [B, L, H] views
+        if self.pixel_shape is not None:
+            fr = obs_full.view(torch.uint8).view(batch_size, n + 1, 4 * D)[:, :, :4 * od].unflatten(2, self.pixel_shape)
+            return {'obs': {'pixel': {'camera0': fr[:, :n]}}, 'obs_next': {'pixel': {'camera0': fr[:, n:]}},
+                    'obs_full': obs_full, 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'],
+                    'persistent_infos': [out['pd']], 'onetime_infos': onetime}
         return {'obs': {'low_dim': {'flat_inputs': obs_full[:, :n, :od]}},
                 'obs_next': {'low_dim': {'flat_inputs': obs_full[:, n:, :od]}},
                 'obs_full': obs_full, 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'],

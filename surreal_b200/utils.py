@@ -166,8 +166,19 @@ def obs_flat(obs):
         if 'low_dim' in obs and len(obs['low_dim']) > 0:
             return obs['low_dim']['flat_inputs'] if 'flat_inputs' in obs['low_dim'] else next(iter(obs['low_dim'].values()))
         fr = obs['pixel']['camera0']
+        if not isinstance(fr, torch.Tensor):                      # a host env's numpy frames
+            import numpy as np
+            return np.ascontiguousarray(fr, dtype=np.uint8).reshape(fr.shape[0], -1).view(np.float32)
         return fr.reshape(fr.shape[0], -1).view(torch.float32)
     return obs
+
+
+def obs_source(obs):
+    """The array an env returned for ``obs``: the frames of a pixel observation, else obs_flat(obs) itself -- what an agent
+    passes to the window wrapper's cached_device_obs."""
+    if isinstance(obs, dict) and 'pixel' in obs and len(obs['pixel']) > 0 and not obs.get('low_dim'):
+        return obs['pixel']['camera0']
+    return obs_flat(obs)
 
 
 class CellLayout(collections.namedtuple('CellLayout', 'layers hidden obs_dim')):
