@@ -482,6 +482,43 @@ int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* 
                             uint64_t seed, const uint64_t* step_counter, double theta, double dt, double* ou_state,
                             float* action_dev, float* action_host, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * DDPG parameter-space exploration noise (surreal/agent/param_noise.py:9-74, ddpg_agent.py:136-153,174-175): every
+ * actor acts with its own perturbed copy of the policy.  Images are [N][actor_stride] floats, each in the layout of
+ * the actor's flat buffer (FlatNet), actor_stride = flat size rounded up to 32 floats (128 B); padding stays zero.
+ * Adaptive mode keeps a device act counter (AdaptiveNormalParameterNoise.i) and per-actor distances dist[N]. */
+typedef struct {
+    uint64_t acts;          /* acts since the last apply (param_noise.py:38,47,60) */
+    uint32_t ticket;        /* last-CTA ticket of the launches below; 0 between launches */
+    uint32_t pad;
+} sb200_param_noise_state;
+/* param_noise_apply: NormalParameterNoise.apply / AdaptiveNormalParameterNoise.apply (param_noise.py:14-24,49-71) on the
+ *   unperturbed flat actor `net`: image_k = fl32((double)W + sigma[k] * z), z ~ N(0,1) in float64, from `unit_noise`
+ *   ([N][actor_stride] float64, tests) or Philox4x32-10 + double Box-Muller keyed by (seed, fetch_index, actor, offset).
+ *   When `state` != NULL (adaptive) the same launch first updates sigma[k] in float64 from dist[k] / state->acts (float32)
+ *   against target_stddev, skipped when acts == 0, then resets acts to 0.  No host synchronisation. */
+int sb200_ddpg_param_noise_apply_f32(const sb200_mlp* net, int N, float* images, int64_t actor_stride, double* sigma,
+                                     const double* unit_noise, uint64_t seed, uint64_t fetch_index, const float* dist,
+                                     sb200_param_noise_state* state, double alpha, double target_stddev, void* stream);
+/* Per-actor forward (ddpg_agent.py:173, csrc/mlp_fwd_per_actor.cu): out[k] = net_k(x[k]) where net_k is `net` (the
+ *   descriptor of image 0) shifted by k * actor_stride floats (0: every row uses the same weights).  fp32, fixed-order
+ *   sums: bit-identical from run to run.  When `state` != NULL the launch counts one act (state->acts += 1), and when also
+ *   `shared` != NULL (the unperturbed actor, same layout) and state->acts % dist_interval == 0 on entry it writes
+ *   dist[k] = |pi_shared(x[k]) - pi_k(x[k])|_2 (compute_action_distance, param_noise.py:42-47).  The counter is read on
+ *   the device, so the call can be captured in a graph.  No aux input; SB200_ERR_UNSUPPORTED above 48 KB of shared memory. */
+int sb200_mlp_forward_per_actor_f32(const sb200_mlp* net, int64_t actor_stride, const float* x, int64_t ldx, int N,
+                                    float* out, int64_t ld_out, const sb200_mlp* shared, float* dist, int dist_interval,
+                                    sb200_param_noise_state* state, void* stream);
+/* ddpg_act_host_per_actor: sb200_ddpg_act_host_f32 (DDPGAgent.act on host observations, ddpg_agent.py:155-184) with the
+ *   per-actor forward in place of the shared one: [H2D obs] -> per-actor forward -> ddpg_noise / ddpg_ou_noise -> D2H
+ *   action -> ONE stream synchronisation.  2 kernels. */
+int sb200_ddpg_act_host_per_actor_f32(const sb200_mlp* net, int64_t actor_stride, const sb200_mlp* shared, float* dist,
+                                      int dist_interval, sb200_param_noise_state* state, const float* obs_host,
+                                      float* obs_dev, int N, float* mean_dev, const float* sigma, const double* sigma64,
+                                      const float* unit_noise, int deterministic, uint64_t seed,
+                                      const uint64_t* step_counter, double theta, double dt, double* ou_state,
+                                      float* action_dev, float* action_host, void* stream);
+
 /* RNN-mode PPOAgent.act (ppo_net.py:317-351, ppo_agent.py:133-149) for host or device observations, one call:
  *   [H2D obs_host -> obs unless obs_host is NULL] -> h, c copied to h_before, c_before (the step's onetime_infos) ->
  *   rows_zfilter -> per layer k: input projection (mlp_forward of ih[k] into pre_x) and lstm_forward from layer k's cells,

@@ -141,6 +141,10 @@ def _declare(lib):
         'sb200_ppo_window_step_host_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P,
                                                P, I, P]),
         'sb200_ddpg_act_host_f32': (I, [C.POINTER(Mlp), P, P, I, P, P, P, P, I, C.c_uint64, P, D, D, P, P, P, P]),
+        'sb200_ddpg_param_noise_apply_f32': (I, [C.POINTER(Mlp), I, P, L, P, P, C.c_uint64, C.c_uint64, P, P, D, D, P]),
+        'sb200_mlp_forward_per_actor_f32': (I, [C.POINTER(Mlp), L, P, L, I, P, L, C.POINTER(Mlp), P, I, P, P]),
+        'sb200_ddpg_act_host_per_actor_f32': (I, [C.POINTER(Mlp), L, C.POINTER(Mlp), P, I, P, P, P, I, P, P, P, P, I,
+                                                  C.c_uint64, P, D, D, P, P, P, P]),
         'sb200_ppo_act_rnn_f32': (I, [C.POINTER(PPOActRnn), P]),
         'sb200_ppo_window_step_rnn_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P, P, P, P, P, P, P, P,
                                               P, P, P, P, P, P, I, I, P]),

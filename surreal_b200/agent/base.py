@@ -225,7 +225,8 @@ class Agent(metaclass=U.AutoInitializeMeta):
         params, info = self._ps_client.fetch_parameter_with_info()
         if params:
             params = self.on_parameter_fetched(params, info)
-            self._module_dict.load(params)
+            if params is not None:             # None: the hook has loaded the parameters itself
+                self._module_dict.load(params)
 
     def fetch_parameter_info(self):
         return self._ps_client.fetch_info()
