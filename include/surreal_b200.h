@@ -60,6 +60,13 @@ typedef struct {
     int ldw[SB200_MAX_LAYERS];
     int aux_layer;                      /* -1: none */
     int aux_dim;
+    /* LayerNorm after layer l's activation (ActorNetworkX / CriticNetworkX with use_layernorm, builders.py:42-48,64-77):
+     * y = (h - mean) * rsqrt(var + ln_eps) * ln_g[l] + ln_b[l] over the dims[l+1] columns of a row, biased variance
+     * (torch.nn.LayerNorm).  ln_g[l] = ln_b[l] = NULL: none (a zero-initialised descriptor has no LayerNorm).  Hidden
+     * layers only.  Only the entries that say so implement it; every other entry rejects such a descriptor. */
+    const float* ln_g[SB200_MAX_LAYERS];    /* [ldw_l] gain */
+    const float* ln_b[SB200_MAX_LAYERS];    /* [ldw_l] bias */
+    float ln_eps;
 } sb200_mlp;
 
 /* ZFilter (surreal/model/z_filter.py:59-79): stats = running_sum[D] | running_sumsq[D] | count[1]. */
@@ -81,6 +88,11 @@ typedef struct {
     int64_t aux_ld;
     float* save_x;                      /* optional: receives the z-filtered input rows [rows][ld_save_x] */
     int64_t ld_save_x;
+    /* optional, layers with LayerNorm: ln_save[l] receives the LayerNorm output [rows][ld_ln_save[l]] (the next layer's
+     * input; save[l] then holds the activation BEFORE the LayerNorm), ln_stats[l] the per-row (mean, rstd) [rows][2] */
+    float* ln_save[SB200_MAX_LAYERS];
+    int64_t ld_ln_save[SB200_MAX_LAYERS];
+    float* ln_stats[SB200_MAX_LAYERS];
 } sb200_rows;
 
 /* Fused forward of a whole MLP on row tiles (z-filter -> Linear/act x n_layers): activations stay in
@@ -273,6 +285,16 @@ int sb200_linear_bwd_dx_f32(const float* dY, int64_t ldy, const float* W, int ld
 int sb200_linear_bwd_dw_f32(const float* X, int64_t ldx, const float* dY, int64_t ldy, float* dW_slabs,
                             float* db_slabs, int64_t slab_stride, int splits, int ldw, int M, int K, int N,
                             void* stream);
+/* Backward of a LayerNorm that follows an activation (csrc/layernorm.cu).  dY [M][ldy]: gradient w.r.t. the LayerNorm
+ * output (sb200_linear_bwd_dx_f32 of the next layer with x_act = NULL); h [M][ldh]: the saved activation before the
+ * LayerNorm; stats [M][2]: the forward's (mean, rstd); g [N]: the gain.  With x^ = (h - mean) * rstd:
+ *   dX = rstd * (g*dY - mean(g*dY) - x^ * mean(g*dY*x^)), times relu'(h) when relu != 0  ->  dX [M][lddx]
+ *   dg_slabs + z*slab_stride / db_slabs + z*slab_stride  <-  sum over split z's rows of dY*x^ / dY (splits slabs of N
+ *   floats, rows split as sb200_linear_bwd_dw_f32 does; reduce with sb200_grad_reduce_norm_f32).
+ * dg_slabs = db_slabs = NULL: no parameter gradient (the slabs are not touched). */
+int sb200_layernorm_bwd_f32(const float* dY, int64_t ldy, const float* h, int64_t ldh, const float* stats,
+                            const float* g, int M, int N, int relu, float* dX, int64_t lddx, float* dg_slabs,
+                            float* db_slabs, int64_t slab_stride, int splits, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Windowed GAE + n-step return (surreal/learner/ppo.py:372-374,387-418).

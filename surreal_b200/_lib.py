@@ -26,7 +26,10 @@ class Mlp(C.Structure):
                 ('b', C.c_void_p * MAX_LAYERS),
                 ('ldw', C.c_int * MAX_LAYERS),
                 ('aux_layer', C.c_int),
-                ('aux_dim', C.c_int)]
+                ('aux_dim', C.c_int),
+                ('ln_g', C.c_void_p * MAX_LAYERS),
+                ('ln_b', C.c_void_p * MAX_LAYERS),
+                ('ln_eps', C.c_float)]
 
 
 class PPORollout(C.Structure):
@@ -91,7 +94,9 @@ class Epochs(C.Structure):
 class Rows(C.Structure):
     _fields_ = [('x', C.c_void_p), ('x_next', C.c_void_p), ('ldx', C.c_int64), ('rows', C.c_int64),
                 ('win_n', C.c_int), ('aux', C.c_void_p), ('aux_ld', C.c_int64),
-                ('save_x', C.c_void_p), ('ld_save_x', C.c_int64)]
+                ('save_x', C.c_void_p), ('ld_save_x', C.c_int64),
+                ('ln_save', C.c_void_p * MAX_LAYERS), ('ld_ln_save', C.c_int64 * MAX_LAYERS),
+                ('ln_stats', C.c_void_p * MAX_LAYERS)]
 
 
 _lib = None
@@ -155,6 +160,7 @@ def _declare(lib):
         'sb200_ppo_rollout_commit_f32': (I, [C.POINTER(PPORollout), P, P, P, P, P, P, P, P, P]),
         'sb200_linear_bwd_dx_f32': (I, [P, L, P, I, P, L, P, L, I, I, I, P]),
         'sb200_linear_bwd_dw_f32': (I, [P, L, P, L, P, P, L, I, I, I, I, I, P]),
+        'sb200_layernorm_bwd_f32': (I, [P, L, P, L, P, P, I, I, I, P, L, P, P, L, I, P]),
         'sb200_make_pd_f32': (I, [P, L, P, P, I, I, P, L, P]),
         'sb200_zfilter_update_f32': (I, [P, L, L, I, P, P]),
         'sb200_reward_filter_f32': (I, [P, L, D, D, P, P, P]),

@@ -41,6 +41,13 @@ static inline int sb200_launch_status(int kernels = 1) {
         }                                                                               \
     } while (0)
 
+// Does the descriptor carry a LayerNorm (sb200_mlp.ln_g / ln_b)?  Entries that do not implement it reject such nets.
+static inline bool sb200_mlp_has_ln(const sb200_mlp* net) {
+    for (int l = 0; l < SB200_MAX_LAYERS; ++l)
+        if (net->ln_g[l] != nullptr || net->ln_b[l] != nullptr) return true;
+    return false;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -1141,7 +1141,7 @@ bool e2_plan(const sb200_epochs* const* a, int n_jobs, Plan* pl) {
     int blocks = 0;
     for (int j = 0; j < n_jobs; ++j) {
         const sb200_mlp* net = a[j]->net;
-        if (!e2_net_ok(net)) return false;
+        if (!e2_net_ok(net) || sb200_mlp_has_ln(net)) return false;
         ld_xs = std::max(ld_xs, ru4(net->dims[0]));
         ld_h1 = std::max(ld_h1, ru4(net->dims[1]));
         ld_h2 = std::max(ld_h2, ru4(net->dims[2]));

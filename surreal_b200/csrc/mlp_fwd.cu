@@ -43,6 +43,12 @@ struct FwdParams {
     long long ld_save[SB200_MAX_LAYERS];
     int ldh;
     int scratch_floats;
+    const float* ln_g[SB200_MAX_LAYERS];     // LayerNorm after layer l (sb200_mlp.ln_g / ln_b), nullptr: none
+    const float* ln_b[SB200_MAX_LAYERS];
+    float ln_eps;
+    float* ln_save[SB200_MAX_LAYERS];        // sb200_rows.ln_save / ln_stats
+    long long ld_ln_save[SB200_MAX_LAYERS];
+    float* ln_stats[SB200_MAX_LAYERS];
 };
 
 __host__ __device__ inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
@@ -51,6 +57,43 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     if (act == SB200_ACT_RELU) return fmaxf(v, 0.0f);
     if (act == SB200_ACT_TANH) return tanhf(v);
     return v;
+}
+
+// LayerNorm epilogue of layer l on the tile's `rows` activation rows H[m][0, N) in shared memory, in place, a warp per
+// row: two-pass mean / biased variance (exact for all-zero rows: y == b), y = fma((h - mean) * rstd, g, b).  Runs after
+// the layer's barrier and before the next layer reads H; columns >= N are not touched.  Not inlined: the GEMM loops
+// around it keep their register allocation.
+__device__ __noinline__ void ln_epilogue(const FwdParams& p, int l, float* H, int ldh, int rows, long long row0) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int N = p.dims[l + 1];
+    const float* __restrict__ g = p.ln_g[l];
+    const float* __restrict__ b = p.ln_b[l];
+    float* sv = p.ln_save[l];
+    float* st = p.ln_stats[l];
+    const long long lds = p.ld_ln_save[l];
+    for (int m = warp; m < rows; m += SB200_THREADS / 32) {
+        float* hr = H + m * ldh;
+        float s = 0.0f;
+        for (int j = lane; j < N; j += 32) s += hr[j];
+        const float mean = warp_sum(s) / (float)N;
+        float q = 0.0f;
+        for (int j = lane; j < N; j += 32) {
+            const float d = hr[j] - mean;
+            q = fmaf(d, d, q);
+        }
+        const float rstd = 1.0f / sqrtf(warp_sum(q) / (float)N + p.ln_eps);
+        const long long r = row0 + m;
+        const bool keep = r < p.rows;
+        for (int j = lane; j < N; j += 32) {
+            const float y = fmaf((hr[j] - mean) * rstd, __ldg(g + j), __ldg(b + j));
+            hr[j] = y;
+            if (sv != nullptr && keep) sv[r * lds + j] = y;
+        }
+        if (st != nullptr && keep && lane == 0) {
+            st[2 * r] = mean;
+            st[2 * r + 1] = rstd;
+        }
+    }
 }
 
 template <int TM, int BK>
@@ -271,6 +314,7 @@ __global__ void __launch_bounds__(SB200_THREADS, (TM <= 4 && BK == 16) ? 2 : 1) 
         }
         __syncthreads();
         if (!last) {
+            if (p.ln_g[l] != nullptr) ln_epilogue(p, l, Hout, ldh, BM, row0);
             // columns [N, N+aux) <- aux input of the next layer; [.., pad16) <- 0
             const int auxd = (p.aux_layer == l + 1) ? p.aux_dim : 0;
             const int wp = round_up(N + auxd, BK);
@@ -467,6 +511,7 @@ __global__ void __launch_bounds__(SB200_THREADS, 2) mlp_fwd_skinny_kernel(const 
         }
         __syncthreads();
         if (!last) {
+            if (p.ln_g[l] != nullptr) ln_epilogue(p, l, Hout, ldh, SK_R, row0);
             const int auxd = (p.aux_layer == l + 1) ? p.aux_dim : 0;
             const int wp2 = round_up(N + auxd, SK_U * SK_D);
             const int span = wp2 - N;
@@ -569,8 +614,16 @@ static int fill_fwd_params(const sb200_mlp* net, const sb200_zfilter* zf, const 
         p.ldw[l] = on ? net->ldw[l] : 0;
         p.save[l] = (on && save != nullptr) ? save[l] : nullptr;
         p.ld_save[l] = (on && save != nullptr && ld_save != nullptr) ? ld_save[l] : 0;
+        p.ln_g[l] = on ? net->ln_g[l] : nullptr;
+        p.ln_b[l] = on ? net->ln_b[l] : nullptr;
+        p.ln_save[l] = p.ln_g[l] != nullptr ? in->ln_save[l] : nullptr;
+        p.ld_ln_save[l] = p.ln_g[l] != nullptr ? in->ld_ln_save[l] : 0;
+        p.ln_stats[l] = p.ln_g[l] != nullptr ? in->ln_stats[l] : nullptr;
         if (on) {
             SB200_REQUIRE(p.W[l] != nullptr && p.b[l] != nullptr);
+            SB200_REQUIRE((p.ln_g[l] == nullptr) == (p.ln_b[l] == nullptr));
+            SB200_REQUIRE(p.ln_g[l] == nullptr || (l + 1 < net->n_layers && net->ln_eps > 0.0f));
+            SB200_REQUIRE(p.ln_save[l] == nullptr || p.ld_ln_save[l] >= p.dims[l + 1]);
             SB200_REQUIRE(p.dims[l + 1] >= 1 && p.ldw[l] >= p.dims[l + 1] && p.ldw[l] % 4 == 0);
             SB200_REQUIRE((((uintptr_t)p.W[l]) & 15) == 0);
             SB200_REQUIRE(p.save[l] == nullptr || p.ld_save[l] >= p.dims[l + 1]);
@@ -578,6 +631,8 @@ static int fill_fwd_params(const sb200_mlp* net, const sb200_zfilter* zf, const 
             if (w > maxw) maxw = w;
         }
     }
+    for (int l = net->n_layers; l < SB200_MAX_LAYERS; ++l) SB200_REQUIRE(net->ln_g[l] == nullptr && net->ln_b[l] == nullptr);
+    p.ln_eps = net->ln_eps;
     *maxw_out = maxw;
     return SB200_OK;
 }
@@ -592,6 +647,7 @@ static long long pack_layer_floats(const sb200_mlp* net, int l) {
 // Shared-memory plan of mlp_fwd_pk_kernel (floats); false when the architecture does not fit one SM.
 static bool pack_plan(const sb200_mlp* net, bool zf, PkParams* pp, size_t* smem_bytes) {
     if (net == nullptr || net->n_layers < 1 || net->n_layers > SB200_MAX_LAYERS) return false;
+    if (sb200_mlp_has_ln(net)) return false;          // no LayerNorm epilogue in mlp_fwd_pk_kernel
     for (int l = 0; l + 1 < net->n_layers; ++l)
         if (net->dims[l + 1] <= 32) return false;        // wide layers first, a narrow layer only as the last one
     long long off = 0;

@@ -221,6 +221,7 @@ __global__ void __launch_bounds__(SB200_THREADS, (MT <= 2) ? 2 : 1) mlp_fwd_mma_
         }
         __syncthreads();
         if (!last) {
+            if (p.ln_g[l] != nullptr) ln_epilogue(p, l, Hout, ldh, BM, row0);
             const int auxd = (p.aux_layer == l + 1) ? p.aux_dim : 0;
             const int wp2 = round_up(N + auxd, 8);
             const int span = wp2 - N;

@@ -26,6 +26,9 @@ struct PaLayout {
     int ldw[SB200_MAX_LAYERS];
     long long w[SB200_MAX_LAYERS];   // offsets in floats from the image base
     long long b[SB200_MAX_LAYERS];
+    long long g[SB200_MAX_LAYERS];   // LayerNorm gain / bias after layer l, -1: none
+    long long beta[SB200_MAX_LAYERS];
+    float ln_eps;
 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -67,6 +70,32 @@ __device__ __forceinline__ void layer_row(const float* __restrict__ W, const flo
     __syncthreads();
 }
 
+// LayerNorm of one row h[0:N) in place (g / b point into the row's image).  Warp 0 reduces in a fixed order (lanes
+// stride the row, then a butterfly), two passes, biased variance; an all-zero row gives exactly b.
+__device__ __forceinline__ void layernorm_row(const float* __restrict__ g, const float* __restrict__ b, int N, float eps,
+                                              float* h, float* part) {
+    if (threadIdx.x < 32) {
+        const int lane = threadIdx.x;
+        float s = 0.0f;
+        for (int j = lane; j < N; j += 32) s = __fadd_rn(s, h[j]);
+        const float mean = __fdiv_rn(warp_sum(s), (float)N);
+        float q = 0.0f;
+        for (int j = lane; j < N; j += 32) {
+            const float d = __fsub_rn(h[j], mean);
+            q = fmaf(d, d, q);
+        }
+        const float var = __fdiv_rn(warp_sum(q), (float)N);
+        if (lane == 0) {
+            part[0] = mean;
+            part[1] = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(var, eps)));
+        }
+    }
+    __syncthreads();
+    const float mean = part[0], rstd = part[1];
+    for (int j = threadIdx.x; j < N; j += PT) h[j] = fmaf(__fmul_rn(__fsub_rn(h[j], mean), rstd), __ldg(g + j), __ldg(b + j));
+    __syncthreads();
+}
+
 // Whole network on one row; returns the shared-memory buffer that holds the output.
 __device__ __forceinline__ float* net_row(const PaLayout& P, const float* __restrict__ base, float* h0, float* h1,
                                           float* part) {
@@ -74,6 +103,7 @@ __device__ __forceinline__ float* net_row(const PaLayout& P, const float* __rest
     float* out = h1;
     for (int l = 0; l < P.L; ++l) {
         layer_row(base + P.w[l], base + P.b[l], P.dims[l], P.dims[l + 1], P.ldw[l], P.act[l], in, out, part);
+        if (P.g[l] >= 0) layernorm_row(base + P.g[l], base + P.beta[l], P.dims[l + 1], P.ln_eps, out, part);
         float* t = in;
         in = out;
         out = t;
@@ -153,11 +183,19 @@ extern "C" int sb200_mlp_forward_per_actor_f32(const sb200_mlp* net, int64_t act
         P.w[l] = (long long)(net->W[l] - base);
         P.b[l] = (long long)(net->b[l] - base);
         SB200_REQUIRE(P.w[l] % 4 == 0 && P.b[l] >= 0);
+        SB200_REQUIRE((net->ln_g[l] == nullptr) == (net->ln_b[l] == nullptr));
+        SB200_REQUIRE(net->ln_g[l] == nullptr || (l + 1 < net->n_layers && net->ln_eps > 0.0f));
+        P.g[l] = net->ln_g[l] != nullptr ? (long long)(net->ln_g[l] - base) : -1;
+        P.beta[l] = net->ln_b[l] != nullptr ? (long long)(net->ln_b[l] - base) : -1;
+        SB200_REQUIRE(net->ln_g[l] == nullptr || (P.g[l] >= 0 && P.beta[l] >= 0));
         if (shared != nullptr)     // the unperturbed net must have the image's layout
             SB200_REQUIRE(shared->n_layers == net->n_layers && shared->W[l] - shared->W[0] == P.w[l] &&
                           shared->b[l] - shared->W[0] == P.b[l] && shared->ldw[l] == net->ldw[l] &&
-                          shared->dims[l + 1] == net->dims[l + 1]);
+                          shared->dims[l + 1] == net->dims[l + 1] &&
+                          (shared->ln_g[l] == nullptr ? -1 : shared->ln_g[l] - shared->W[0]) == P.g[l] &&
+                          (shared->ln_b[l] == nullptr ? -1 : shared->ln_b[l] - shared->W[0]) == P.beta[l]);
     }
+    P.ln_eps = net->ln_eps;
     SB200_REQUIRE(((uintptr_t)base & 15u) == 0 && (shared == nullptr || ((uintptr_t)shared->W[0] & 15u) == 0));
     int part = 0, wpad = 0;
     const size_t smem = per_actor_smem_bytes(net, &part, &wpad);

@@ -334,7 +334,7 @@ int sb200_mlp_tc5_init() {
 }
 
 static bool tc5_net_ok(const sb200_mlp* net) {
-    if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0) return false;
+    if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0 || sb200_mlp_has_ln(net)) return false;
     const int K0 = net->dims[0], N1 = net->dims[1], N2 = net->dims[2], NO = net->dims[3];
     if (K0 % KC != 0 || K0 < KC || K0 > MAX_K0) return false;
     if (N1 % KC != 0 || N1 < KC || N1 > MAXN) return false;

@@ -18,13 +18,17 @@ struct PnLayout {
     int N[SB200_MAX_LAYERS];
     int ldw[SB200_MAX_LAYERS];
     long long w[SB200_MAX_LAYERS], wend[SB200_MAX_LAYERS], b[SB200_MAX_LAYERS];
+    long long g[SB200_MAX_LAYERS], beta[SB200_MAX_LAYERS];    // LayerNorm gain / bias segments, -1: none
 };
 
-// Is flat offset p a parameter (true) or a padding column / the tail up to actor_stride (false)?
+// Is flat offset p a parameter (true) or a padding column / the tail up to actor_stride (false)?  LayerNorm gains and
+// biases are parameters too: the reference perturbs every entry of the state dict (param_noise.py:14-23,61-69).
 __device__ __forceinline__ bool is_param(const PnLayout& P, long long p) {
     for (int l = 0; l < P.L; ++l) {
         if (p >= P.w[l] && p < P.wend[l]) return (int)((p - P.w[l]) % P.ldw[l]) < P.N[l];
         if (p >= P.b[l] && p < P.b[l] + P.ldw[l]) return (int)(p - P.b[l]) < P.N[l];
+        if (P.g[l] >= 0 && p >= P.g[l] && p < P.g[l] + P.ldw[l]) return (int)(p - P.g[l]) < P.N[l];
+        if (P.beta[l] >= 0 && p >= P.beta[l] && p < P.beta[l] + P.ldw[l]) return (int)(p - P.beta[l]) < P.N[l];
     }
     return false;
 }
@@ -107,6 +111,11 @@ extern "C" int sb200_ddpg_param_noise_apply_f32(const sb200_mlp* net, int N, flo
         P.wend[l] = P.w[l] + (long long)net->dims[l] * net->ldw[l];
         P.b[l] = (long long)(net->b[l] - base);
         SB200_REQUIRE(P.w[l] >= 0 && P.b[l] >= 0 && P.wend[l] <= actor_stride && P.b[l] + net->ldw[l] <= actor_stride);
+        SB200_REQUIRE((net->ln_g[l] == nullptr) == (net->ln_b[l] == nullptr));
+        P.g[l] = net->ln_g[l] != nullptr ? (long long)(net->ln_g[l] - base) : -1;
+        P.beta[l] = net->ln_b[l] != nullptr ? (long long)(net->ln_b[l] - base) : -1;
+        SB200_REQUIRE(net->ln_g[l] == nullptr || (P.g[l] >= 0 && P.beta[l] >= 0 && P.g[l] + net->ldw[l] <= actor_stride &&
+                                                  P.beta[l] + net->ldw[l] <= actor_stride));
     }
     const dim3 grid((unsigned)((actor_stride + 4 * NT - 1) / (4 * NT)), (unsigned)N);
     param_noise_apply_kernel<<<grid, NT, 0, (cudaStream_t)stream>>>(

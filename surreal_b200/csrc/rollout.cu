@@ -509,7 +509,7 @@ extern "C" int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter*
     const int D = net->dims[0], A = net->dims[net->n_layers];
     if (obs_host != nullptr)
         SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    sb200_rows in;
+    sb200_rows in = {};
     in.x = obs_dev;
     in.x_next = nullptr;
     in.ldx = D;
@@ -607,6 +607,10 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
     SB200_REQUIRE(a->action_host == nullptr || a->pd_host != nullptr);
     SB200_REQUIRE((a->h_before_host == nullptr) == (a->c_before_host == nullptr));
     for (int k = 0; k < a->layers; ++k) SB200_REQUIRE(a->ih[k] && a->whh[k] && a->bhh[k] && a->ih[k]->dims[1] == 4 * a->H);
+    // no LayerNorm in the recurrent policy's head, input projections or CNN stem
+    if (sb200_mlp_has_ln(a->head) || (stem && sb200_mlp_has_ln(a->fc))) return SB200_ERR_UNSUPPORTED;
+    for (int k = 0; k < a->layers; ++k)
+        if (sb200_mlp_has_ln(a->ih[k])) return SB200_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
     const int N = a->N, D = a->D, H = a->H, L = a->layers, A = a->head->dims[a->head->n_layers];
     const size_t cells = (size_t)L * N * H * sizeof(float);

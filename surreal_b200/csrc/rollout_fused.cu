@@ -1658,7 +1658,7 @@ __global__ void __launch_bounds__(256) ppo_rollout_copy_kernel(const int* __rest
 // and the per-group tiles and state twice, `gstride` floats apart.  At the configs[1] shape [64, 256, 256, 8]:
 // G = 1 204 512 B, G = 2 219 552 B.
 bool rf_plan(const sb200_mlp* net, int D, int A, int G, RfParams* p, size_t* smem_bytes) {
-    if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0) return false;
+    if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0 || sb200_mlp_has_ln(net)) return false;
     const int H1 = net->dims[1], H2 = net->dims[2];
     if (net->dims[0] != D || net->dims[3] != A) return false;
     if (D % 4 != 0 || D > 128 || A < 1 || A > 32 || H1 % 16 != 0 || H2 % 16 != 0) return false;

@@ -11,6 +11,9 @@ import torch
 from . import _lib
 from ._lib import Mlp, ZFilter, Rows, ACT_NONE, ACT_RELU, ACT_TANH, MAX_LAYERS, check  # noqa: F401
 
+# torch.nn.LayerNorm's default eps: the reference's torchx LayerNorm(1) is nn.LayerNorm over the last dimension
+LAYERNORM_EPS = 1e-5
+
 
 def _ru(v, m):
     return (v + m - 1) // m * m
@@ -36,28 +39,43 @@ class FlatNet:
     (W[l] = [in_l][ldw_l], the transpose of torch.nn.Linear.weight; ldw = out rounded up to 4;
     padding stays zero).  Gradients / Adam moments use buffers of the same layout, so optimiser and
     NCCL all-reduce are single flat kernels / one collective.  ``extra`` trailing floats hold
-    non-layer parameters (PPO's log_var, builders.py:112)."""
+    non-layer parameters (PPO's log_var, builders.py:112).
 
-    def __init__(self, dims, acts, device, aux_layer=-1, aux_dim=0, extra=0):
+    ``layernorm``: every hidden layer is followed by a LayerNorm (builders.py:42-48,64-77); its gain and bias sit right
+    after that layer's bias, [ldw] each like a bias, so the flat order is the reference's state-dict order and flat
+    passes (Adam, clipping, target updates, parameter noise) cover them unchanged.  Gain 1, bias 0 at construction."""
+
+    def __init__(self, dims, acts, device, aux_layer=-1, aux_dim=0, extra=0, layernorm=False):
         assert 1 <= len(dims) - 1 <= MAX_LAYERS and len(acts) == len(dims) - 1
         self.dims = list(dims)
         self.acts = list(acts)
         self.aux_layer, self.aux_dim = aux_layer, (aux_dim if aux_layer >= 0 else 0)
         self.n_layers = len(dims) - 1
+        self.layernorm = bool(layernorm)
         self.layout = []
         off = 0
         for l in range(self.n_layers):
             K = dims[l] + (self.aux_dim if aux_layer == l else 0)
             N = dims[l + 1]
             ldw = _ru(N, 4)
-            self.layout.append(dict(w=off, b=off + K * ldw, K=K, N=N, ldw=ldw))
+            lay = dict(w=off, b=off + K * ldw, K=K, N=N, ldw=ldw, g=None, beta=None)
             off += K * ldw + ldw
+            if self.layernorm and l + 1 < self.n_layers:
+                lay['g'], lay['beta'] = off, off + ldw
+                off += 2 * ldw
+            self.layout.append(lay)
         self.extra = extra
         self.extra_off = off
         off += _ru(extra, 4)
         self.size = off
         self.device = torch.device(device)
         self.params = torch.zeros(off, dtype=torch.float32, device=self.device)
+        for l in self.ln_layers():
+            self.ln_g(l)[:self.layout[l]['N']] = 1.0
+
+    def ln_layers(self):
+        """Indices of the layers followed by a LayerNorm."""
+        return [l for l, lay in enumerate(self.layout) if lay['g'] is not None]
 
     # -- views -----------------------------------------------------------------------------------
     def W(self, l, buf=None):
@@ -69,6 +87,25 @@ class FlatNet:
         lay = self.layout[l]
         buf = self.params if buf is None else buf
         return buf[lay['b']:lay['b'] + lay['ldw']]
+
+    def ln_g(self, l, buf=None):
+        lay = self.layout[l]
+        buf = self.params if buf is None else buf
+        return buf[lay['g']:lay['g'] + lay['ldw']]
+
+    def ln_b(self, l, buf=None):
+        lay = self.layout[l]
+        buf = self.params if buf is None else buf
+        return buf[lay['beta']:lay['beta'] + lay['ldw']]
+
+    def set_ln(self, l, gain, bias):
+        N = self.layout[l]['N']
+        self.ln_g(l)[:N] = torch.as_tensor(gain, dtype=torch.float32).to(self.device)
+        self.ln_b(l)[:N] = torch.as_tensor(bias, dtype=torch.float32).to(self.device)
+
+    def get_ln(self, l, buf=None):
+        N = self.layout[l]['N']
+        return self.ln_g(l, buf)[:N].clone(), self.ln_b(l, buf)[:N].clone()
 
     def extra_view(self, buf=None):
         buf = self.params if buf is None else buf
@@ -92,7 +129,7 @@ class FlatNet:
         return self
 
     def clone_like(self):
-        n = FlatNet(self.dims, self.acts, self.device, self.aux_layer, self.aux_dim, self.extra)
+        n = FlatNet(self.dims, self.acts, self.device, self.aux_layer, self.aux_dim, self.extra, self.layernorm)
         n.params.copy_(self.params)
         return n
 
@@ -109,8 +146,12 @@ class FlatNet:
             m.W[l] = base + 4 * lay['w']
             m.b[l] = base + 4 * lay['b']
             m.ldw[l] = lay['ldw']
+            if lay['g'] is not None:
+                m.ln_g[l] = base + 4 * lay['g']
+                m.ln_b[l] = base + 4 * lay['beta']
         m.aux_layer = self.aux_layer
         m.aux_dim = self.aux_dim
+        m.ln_eps = LAYERNORM_EPS if self.layernorm else 0.0
         return m
 
 
@@ -227,13 +268,16 @@ def mlp_forward_dual(net, x, zf_stats=None, zf_eps=1e-5, out=None, frac=None):
 
 
 def mlp_forward(net, x, zf_stats=None, zf_eps=1e-5, x_next=None, win_n=0, aux=None, save_all=False,
-                params=None, out=None, rows=None, ldx=None, saves=None, save_x=None, variant=0):
+                params=None, out=None, rows=None, ldx=None, saves=None, save_x=None, variant=0, ln_saves=None,
+                ln_stats=None):
     """Run the fused forward.
 
     ``x``: [rows, D] (any row stride via ``ldx``), or [B, n, D] with ``x_next`` [B, 1, D] and win_n=n for
     the virtual cat of ppo.py:376-383.  Returns the network output [rows, out_dim]; with ``save_all`` a
     list of every layer's post-activation output.  ``saves``: optional explicit list of per-layer output
-    buffers ([rows, ld] each, or None) -- used by MlpTrainer; ``save_x`` receives the z-filtered input."""
+    buffers ([rows, ld] each, or None) -- used by MlpTrainer; ``save_x`` receives the z-filtered input.
+    With LayerNorm layers, ``saves`` receive the activation before the LayerNorm, ``ln_saves`` / ``ln_stats``
+    (per-layer lists) the LayerNorm output and the per-row (mean, rstd) [rows, 2]."""
     L = _lib.lib()
     assert x.is_cuda and x.dtype == torch.float32
     D = net.dims[0]
@@ -262,6 +306,13 @@ def mlp_forward(net, x, zf_stats=None, zf_eps=1e-5, x_next=None, win_n=0, aux=No
         r.save_x, r.ld_save_x = save_x.data_ptr(), save_x.stride(0)
     else:
         r.save_x, r.ld_save_x = None, 0
+    for l in range(net.n_layers):
+        t = ln_saves[l] if ln_saves is not None else None
+        if t is not None:
+            r.ln_save[l], r.ld_ln_save[l] = t.data_ptr(), t.stride(0)
+        t = ln_stats[l] if ln_stats is not None else None
+        if t is not None:
+            r.ln_stats[l] = t.data_ptr()
     outs = []
     if saves is None:
         saves = [None] * net.n_layers
@@ -315,6 +366,12 @@ class MlpTrainer:
         self._side = None
         if net.aux_layer >= 0 and net.aux_dim % 4 != 0:       # pre-allocated: nothing may allocate during graph capture
             self._aux_pad = z(M, _ru(net.aux_dim, 4))
+        # LayerNorm layers: h[l] holds the activation before the LayerNorm, ln_out[l] its output (the next layer's input),
+        # ln_stats[l] the per-row (mean, rstd), dln[l] the gradient w.r.t. the LayerNorm output
+        lnl = net.ln_layers()
+        self.ln_out = [z(M, _ru(n, 4)) if l in lnl else None for l, n in enumerate(net.dims[1:])]
+        self.ln_stats = [z(M, 2) if l in lnl else None for l in range(net.n_layers)]
+        self.dln = [z(M, _ru(n, 4)) if l in lnl else None for l, n in enumerate(net.dims[1:])]
 
     @property
     def out(self):
@@ -330,8 +387,30 @@ class MlpTrainer:
             aux = self._aux_pad
         self.aux = aux
         mlp_forward(self.net, x, zf_stats=zf_stats, zf_eps=zf_eps, aux=aux, rows=rows, ldx=ldx,
-                    saves=self.h, save_x=self.x_in)
+                    saves=self.h, save_x=self.x_in, ln_saves=self.ln_out, ln_stats=self.ln_stats)
         return self.out
+
+    def _input_grad(self, l, param_grad):
+        """d[l-1] from d[l]: layer l's dX GEMM times relu'(h[l-1]), or, when layer l-1 has a LayerNorm, the dX GEMM into
+        dln[l-1] and the LayerNorm backward (which adds the gain / bias gradients to the slabs when ``param_grad``)."""
+        L, net, M = _lib.lib(), self.net, self.M
+        lay, prev = net.layout[l], net.layout[l - 1]
+        dY, h, dX = self.d[l], self.h[l - 1], self.d[l - 1]
+        w = C.c_void_p(net.params.data_ptr() + 4 * lay['w'])
+        if prev['g'] is None:
+            check(L.sb200_linear_bwd_dx_f32(_ptr(dY), dY.stride(0), w, lay['ldw'], _ptr(h), h.stride(0), _ptr(dX),
+                                            dX.stride(0), M, lay['N'], net.dims[l], _stream()), 'sb200_linear_bwd_dx_f32')
+            return
+        dln = self.dln[l - 1]
+        check(L.sb200_linear_bwd_dx_f32(_ptr(dY), dY.stride(0), w, lay['ldw'], None, 0, _ptr(dln), dln.stride(0), M,
+                                        lay['N'], net.dims[l], _stream()), 'sb200_linear_bwd_dx_f32')
+        base = self.slabs.data_ptr()
+        dg = C.c_void_p(base + 4 * prev['g']) if param_grad else None
+        db = C.c_void_p(base + 4 * prev['beta']) if param_grad else None
+        check(L.sb200_layernorm_bwd_f32(_ptr(dln), dln.stride(0), _ptr(h), h.stride(0), _ptr(self.ln_stats[l - 1]),
+                                        C.c_void_p(net.params.data_ptr() + 4 * prev['g']), M, prev['N'],
+                                        int(net.acts[l - 1] == ACT_RELU), _ptr(dX), dX.stride(0), dg, db, net.size,
+                                        self.splits, _stream()), 'sb200_layernorm_bwd_f32')
 
     def backward(self, need_dx0=False):
         """self.d[-1] must hold dL/d(pre-activation of the last layer).
@@ -351,7 +430,7 @@ class MlpTrainer:
         def dw_layer(l, st):
             lay = net.layout[l]
             K0, N, ldw = net.dims[l], lay['N'], lay['ldw']
-            X = self.x_in if l == 0 else self.h[l - 1]
+            X = self.x_in if l == 0 else (self.h[l - 1] if self.ln_out[l - 1] is None else self.ln_out[l - 1])
             dY = self.d[l]
             check(L.sb200_linear_bwd_dw_f32(_ptr(X), X.stride(0), _ptr(dY), dY.stride(0),
                                             C.c_void_p(base + 4 * lay['w']), C.c_void_p(base + 4 * lay['b']),
@@ -363,17 +442,10 @@ class MlpTrainer:
                                                 self.splits, ldw, M, net.aux_dim, N, st), 'sb200_linear_bwd_dw_f32(aux)')
 
         for l in reversed(range(net.n_layers)):
-            lay = net.layout[l]
-            K0, N, ldw = net.dims[l], lay['N'], lay['ldw']
-            dY = self.d[l]
             if side is not None:
                 side.wait_stream(main)                  # dY_l is ready on the main stream
             if l > 0:                                   # critical path first
-                Xa = self.h[l - 1]
-                dX = self.d[l - 1]
-                check(L.sb200_linear_bwd_dx_f32(_ptr(dY), dY.stride(0), C.c_void_p(net.params.data_ptr() + 4 * lay['w']),
-                                                ldw, _ptr(Xa), Xa.stride(0), _ptr(dX), dX.stride(0), M, N, K0, _stream()),
-                      'sb200_linear_bwd_dx_f32')
+                self._input_grad(l, True)
             if side is not None:
                 with torch.cuda.stream(side):
                     dw_layer(l, _stream())
@@ -390,13 +462,8 @@ class MlpTrainer:
     def backward_inputs(self, stop_layer=1):
         """Only the dX chain from the last layer down to ``stop_layer`` (fills self.d[stop_layer-1 ...]); no weight
         gradients -- the DDPG actor loss back-propagates THROUGH the critic without updating it."""
-        L, net, M = _lib.lib(), self.net, self.M
-        for l in reversed(range(stop_layer + 1, net.n_layers)):
-            lay = net.layout[l]
-            dY, Xa, dX = self.d[l], self.h[l - 1], self.d[l - 1]
-            check(L.sb200_linear_bwd_dx_f32(_ptr(dY), dY.stride(0), C.c_void_p(net.params.data_ptr() + 4 * lay['w']),
-                                            lay['ldw'], _ptr(Xa), Xa.stride(0), _ptr(dX), dX.stride(0), M, lay['N'],
-                                            net.dims[l], _stream()), 'sb200_linear_bwd_dx_f32')
+        for l in reversed(range(stop_layer + 1, self.net.n_layers)):
+            self._input_grad(l, False)
 
     def grad_wrt_aux(self, l, out):
         """d loss / d aux input of layer l (the DDPG actor gradient dQ/da, ddpg.py:324-330)."""
