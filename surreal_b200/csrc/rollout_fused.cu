@@ -4,13 +4,14 @@
 // every launch re-fetches the policy weights from L2 (a chain of dependent round trips) and pays
 // launch + drain, 128 steps x 3 launches per rollout for a fraction of that in arithmetic.  Actors are
 // independent of one another, so the loop over time can move INSIDE the kernel:
-//   * a thread-block cluster of 4 CTAs owns 32 actors for the whole chunk;
+//   * a thread-block cluster of 4 CTAs owns a group of 32 actors (G = 2: two groups) for the whole chunk;
 //   * each CTA keeps a QUARTER of every hidden layer's weights resident in shared memory for all T steps (fetched
-//     once with cp.async) and computes that quarter of the layer's columns for the cluster's 32 rows (fp32 FFMA,
-//     thread = 1 row x 4 columns); layer outputs are exchanged through distributed shared memory (16-byte
-//     st.shared::cluster pushes into all four copies) with one cluster barrier per layer;
-//   * each CTA then finishes ITS 8 actors: head, sampling, environment step, window staging -- one warp per actor,
-//     observations / env state never leave shared memory between steps;
+//     once with cp.async); its 8 layer warps compute that quarter of the layer's columns for the group's 32 rows
+//     (fp32 FFMA in register tiles) and push the result into the peers' shared memory with st.async, which counts
+//     the bytes on the receiver's mbarrier: no cluster barrier inside the loop over steps;
+//   * each CTA then finishes ITS 8 actors of the group: head, sampling, environment step, window staging -- one warp
+//     per actor, observations / env state never leave shared memory between steps; the other 8 warps do the
+//     action-independent half of the env step while the layers run;
 //   * finished windows go to a per-actor outbox with their completion step; sb200_ppo_rollout_commit_f32 assigns
 //     FIFO slots in the reference's (step, actor) arrival order afterwards and copies them into the replay ring.
 // Sampling and environment arithmetic (and their Philox keys) are those of rollout.cu, so both paths draw the
@@ -20,7 +21,6 @@
 
 #include <algorithm>
 #include <mutex>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "rollout_dev.cuh"
@@ -110,8 +110,7 @@ struct RfParams {
     int oHs;                        // two groups per cluster: head slice sums [16][8][ldw[2]]
     int gstride;                    // two groups per cluster: floats between group 0's and group 1's X0 .. Pre
     int ldx0, ldh1, ldh2;
-    int l1_direct;                  // v2: reduction-free first layer (rf2_layer1)
-    int head_mode;                  // v2: 1 = k-sliced head over all owned actors, 0 = two warps per actor
+    int head_mode;                  // G = 1: 1 = k-sliced head over all owned actors, 0 = two warps per actor
 };
 
 __device__ __forceinline__ float rf_act(float v, int act) {
@@ -126,395 +125,19 @@ __device__ __forceinline__ unsigned rf_mapa(unsigned addr, unsigned rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
     return r;
 }
-__device__ __forceinline__ void rf_st_cluster_v4(unsigned addr, const float4& v) {
-    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                 : "memory");
-}
 
-// One hidden layer for the cluster's 32 rows, this CTA's Nc columns: out[row][col0 + c] = act(x[row] . Ws[:, c] + b).
-// Xin [32][ldin] and Ws [K][Nc] live in shared memory; K % 4 == 0.
-//   Thread tile 4 rows x 4 columns (16 accumulators): with the first version's 1 x 4 tile every 16 FFMA needed 5
-//   LDS.128 and the layer was bound by shared-memory bandwidth (ncu: mio_throttle + short_scoreboard, 60 % of the
-//   kernel); 4 x 4 needs 8 LDS.128 per 64 FFMA.  The 512 threads form 4 groups of 128 that split K; the partial
-//   tiles are summed in a fixed order (deterministic) through `Part` [4][32][Nc].
-//   ALL_ROWS: the result is stored in every CTA's copy of Hout [32][ldout] (input of the next hidden layer);
-//   otherwise each row goes only to the CTA that owns the actor, into its Hout [8][ldout] (input of the head).
-template <bool ALL_ROWS>
-__device__ __forceinline__ void rf_layer(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
-                                         int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
-                                         int ldout, int col0, float* __restrict__ Part, unsigned smem_base,
-                                         unsigned crank, int rf_t, int rf_id) {
-    const int tid = threadIdx.x;
-    const int q = tid >> 7, t128 = tid & 127, ty = t128 >> 4, tx = t128 & 15;
-    const int kq = (((K >> 2) + 3) >> 2) << 2;               // k span of one group (multiple of 4)
-    const int k_lo = q * kq, k_hi = min(K, k_lo + kq);
-    const int nq = Nc >> 2;
-    for (int c4 = tx; c4 < nq; c4 += 16) {
-        const float* xr = Xin + (ty * 4) * ldin;
-        const float* wp = Ws + c4 * 4;
-        float acc[4][4];
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) acc[r][c] = 0.0f;
-#pragma unroll 2
-        for (int k = k_lo; k < k_hi; k += 4) {
-            float4 a[4];
-#pragma unroll
-            for (int r = 0; r < 4; ++r) a[r] = *reinterpret_cast<const float4*>(xr + r * ldin + k);
-            const float4 w0 = *reinterpret_cast<const float4*>(wp + (k + 0) * Nc);
-            const float4 w1 = *reinterpret_cast<const float4*>(wp + (k + 1) * Nc);
-            const float4 w2 = *reinterpret_cast<const float4*>(wp + (k + 2) * Nc);
-            const float4 w3 = *reinterpret_cast<const float4*>(wp + (k + 3) * Nc);
-#pragma unroll
-            for (int r = 0; r < 4; ++r) {
-                acc[r][0] = fmaf(a[r].x, w0.x, acc[r][0]); acc[r][1] = fmaf(a[r].x, w0.y, acc[r][1]);
-                acc[r][2] = fmaf(a[r].x, w0.z, acc[r][2]); acc[r][3] = fmaf(a[r].x, w0.w, acc[r][3]);
-                acc[r][0] = fmaf(a[r].y, w1.x, acc[r][0]); acc[r][1] = fmaf(a[r].y, w1.y, acc[r][1]);
-                acc[r][2] = fmaf(a[r].y, w1.z, acc[r][2]); acc[r][3] = fmaf(a[r].y, w1.w, acc[r][3]);
-                acc[r][0] = fmaf(a[r].z, w2.x, acc[r][0]); acc[r][1] = fmaf(a[r].z, w2.y, acc[r][1]);
-                acc[r][2] = fmaf(a[r].z, w2.z, acc[r][2]); acc[r][3] = fmaf(a[r].z, w2.w, acc[r][3]);
-                acc[r][0] = fmaf(a[r].w, w3.x, acc[r][0]); acc[r][1] = fmaf(a[r].w, w3.y, acc[r][1]);
-                acc[r][2] = fmaf(a[r].w, w3.z, acc[r][2]); acc[r][3] = fmaf(a[r].w, w3.w, acc[r][3]);
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-            *reinterpret_cast<float4*>(Part + ((q * RF_ROWS + ty * 4 + r) * Nc + c4 * 4)) =
-                make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
-    }
-    RF_STAMP(rf_id, 0);
-    __syncthreads();
-    RF_STAMP(rf_id + 1, 0);
-    for (int idx = tid; idx < RF_ROWS * nq; idx += RF_THREADS) {
-        const int row = idx / nq, c4 = idx - row * nq;
-        const float* pp = Part + row * Nc + c4 * 4;
-        const float4 p0 = *reinterpret_cast<const float4*>(pp);
-        const float4 p1 = *reinterpret_cast<const float4*>(pp + RF_ROWS * Nc);
-        const float4 p2 = *reinterpret_cast<const float4*>(pp + 2 * RF_ROWS * Nc);
-        const float4 p3 = *reinterpret_cast<const float4*>(pp + 3 * RF_ROWS * Nc);
-        const float4 bv = *reinterpret_cast<const float4*>(bias_s + c4 * 4);
-        float4 o;
-        o.x = rf_act(((p0.x + p1.x) + (p2.x + p3.x)) + bv.x, act);
-        o.y = rf_act(((p0.y + p1.y) + (p2.y + p3.y)) + bv.y, act);
-        o.z = rf_act(((p0.z + p1.z) + (p2.z + p3.z)) + bv.z, act);
-        o.w = rf_act(((p0.w + p1.w) + (p2.w + p3.w)) + bv.w, act);
-        if (ALL_ROWS) {
-            float* qd = Hout + row * ldout + col0 + c4 * 4;
-            *reinterpret_cast<float4*>(qd) = o;
-            const unsigned off = rf_smem_u32(qd) - smem_base;
-#pragma unroll
-            for (int c = 1; c < RF_CS; ++c) rf_st_cluster_v4(rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS) + off, o);
-        } else {
-            const unsigned owner = (unsigned)(row / RF_OWN);
-            float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
-            if (owner == crank) *reinterpret_cast<float4*>(qd) = o;
-            else rf_st_cluster_v4(rf_mapa(smem_base, owner) + (rf_smem_u32(qd) - smem_base), o);
-        }
-    }
-}
-
-__global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
-    ppo_rollout_kernel(const __grid_constant__ RfParams p) {
-    cg::cluster_group cluster = cg::this_cluster();
-    const unsigned crank = cluster.block_rank();
-    extern __shared__ __align__(16) float smem[];
-    const unsigned smem_base = rf_smem_u32(smem);
-    unsigned peer_base[RF_CS - 1];
-#pragma unroll
-    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
-    __shared__ int s_pos[RF_OWN], s_ep[RF_OWN], s_cnt[RF_OWN];
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
-    const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
-    const int ldwh = p.ldw[2];
-    float* W1s = smem + p.oW1;          // [D][Nc1]
-    float* W2s = smem + p.oW2;          // [H1][Nc2]
-    float* Whs = smem + p.oWh;          // [H2][ldwh]
-    float* B1s = smem + p.oB;           // [Nc1] | [Nc2] | [ldwh]
-    float* B2s = B1s + Nc1;
-    float* Bhs = B2s + Nc2;
-    float* X0 = smem + p.oX0;           // [32][ldx0]  z-filtered observations of the cluster's actors
-    float* Hb1 = smem + p.oH1;          // [32][ldh1]
-    float* Hb2 = smem + p.oH2;          // [8][ldh2]   last hidden layer, owned actors only
-    float* Part = smem + p.oPart;       // [4][32][max(Nc1, Nc2)] k-split partial tiles
-    float* Zm = smem + p.oZf;           // [D] mean | [D] std
-    float* Zs = Zm + D;
-    float* EWs = smem + p.oEnv;         // [D][D] | [A][D]   (k-major)
-    float* EWa = EWs + D * D;
-    float* S = smem + p.oS;             // [8][D]   env state of the owned actors (what they observe next)
-    float* Nx = smem + p.oNext;         // [8][D]   true successor of the step
-    float* Ac = smem + p.oAct;          // [8][A]   sampled actions | means | std | N(0,1) draws
-    float* Mu = Ac + RF_OWN * A;
-    float* Sd = Mu + RF_OWN * A;
-    float* Zn = Sd + RF_OWN * A;
-    float* Eacc = smem + p.oPre;        // [8][D] Ws.s | [8][D] env noise | [8][D] reset draws | [16] |s|^2, reward noise
-    float* Egx = Eacc + RF_OWN * D;
-    float* Erz = Egx + RF_OWN * D;
-    float* Eq = Erz + RF_OWN * D;
-    const long long row0 = (long long)(blockIdx.x / RF_CS) * RF_ROWS;
-
-    // ---- one-time loads: weight slices, biases, env matrices (cp.async burst), z-filter columns, actor state
-    for (int f = tid; f < D * (Nc1 >> 2); f += RF_THREADS) {
-        const int k = f / (Nc1 >> 2), q = f - k * (Nc1 >> 2);
-        cp_async16(W1s + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
-    }
-    for (int f = tid; f < H1 * (Nc2 >> 2); f += RF_THREADS) {
-        const int k = f / (Nc2 >> 2), q = f - k * (Nc2 >> 2);
-        cp_async16(W2s + k * Nc2 + q * 4, p.W[1] + (long long)k * p.ldw[1] + crank * Nc2 + q * 4, 16);
-    }
-    for (int f = tid; f < (H2 * ldwh) >> 2; f += RF_THREADS) cp_async16(Whs + f * 4, p.W[2] + f * 4, 16);
-    for (int f = tid; f < (D * D) >> 2; f += RF_THREADS) cp_async16(EWs + f * 4, p.WsT + f * 4, 16);
-    for (int f = tid; f < (A * D) >> 2; f += RF_THREADS) cp_async16(EWa + f * 4, p.WaT + f * 4, 16);
-    cp_async_commit();
-    for (int n = tid; n < Nc1; n += RF_THREADS) B1s[n] = p.b[0][crank * Nc1 + n];
-    for (int n = tid; n < Nc2; n += RF_THREADS) B2s[n] = p.b[1][crank * Nc2 + n];
-    for (int n = tid; n < ldwh; n += RF_THREADS) Bhs[n] = (n < A) ? p.b[2][n] : 0.0f;
-    if (p.zf != nullptr) {
-        const float cnt = p.zf[2 * D];
-        for (int k = tid; k < D; k += RF_THREADS) {
-            const float mean = p.zf[k] / cnt;
-            const float var = p.zf[D + k] / cnt - mean * mean;
-            Zm[k] = mean;
-            Zs[k] = fmaxf(sqrtf(var), p.zf_eps);
-        }
-    }
-    if (tid < RF_OWN) {
-        const long long i = row0 + crank * RF_OWN + tid;
-        s_pos[tid] = (i < p.N) ? p.stage_pos[i] : 0;
-        s_ep[tid] = (i < p.N) ? p.ep_step[i] : 0;
-        s_cnt[tid] = 0;
-    }
-    __syncthreads();
-    for (int idx = tid; idx < RF_ROWS * D; idx += RF_THREADS) {       // all 32 rows: every CTA needs the full input
-        const int m = idx / D, k = idx - m * D;
-        const long long i = row0 + m;
-        float v = (i < p.N) ? p.state[i * D + k] : 0.0f;
-        const int own = m - (int)crank * RF_OWN;
-        if (own >= 0 && own < RF_OWN) S[own * D + k] = v;
-        if (p.zf != nullptr) v = fminf(fmaxf((v - Zm[k]) / Zs[k], -5.0f), 5.0f);
-        X0[m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
-    }
-    const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
-    cp_async_wait<0>();
-    cluster.sync();                                   // weights landed; every peer is running (DSMEM is live)
-
-    const int own = warp;                             // warps 0..7: one owned actor each
-    const bool owner = own < RF_OWN;
-    const int m_own = (int)crank * RF_OWN + own;
-    const long long i_own = row0 + m_own;
-    const bool valid = owner && (i_own < p.N);
-    const float sc = (valid && p.log_noise != nullptr) ? expf(p.log_noise[i_own]) : 1.0f;
-    if (owner && lane < A) Sd[own * A + lane] = __fmul_rn(expf(p.log_var[lane]), sc);     // constant over the chunk
-    __syncthreads();
-
-    for (int t = 0; t < p.T; ++t) {
-        const unsigned long long ctr = ctr0 + (unsigned long long)t;
-        const bool final_step = (t == p.T - 1);
-        const int rf_t = t;
-        RF_STAMP(0, 0);
-        rf_layer<true>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, Part, smem_base, crank, rf_t, 1);
-        RF_STAMP(3, 0);
-        cluster.sync();
-        RF_STAMP(4, 0);
-        rf_layer<false>(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5);
-        RF_STAMP(7, 0);
-        cluster.sync();
-        RF_STAMP(8, 0);
-        RF_STAMP(16, 256);
-
-        float rew = 0.0f, dn = 0.0f;
-        int slot = SLOT_NONE;
-        // ---- phase 1, two halves of the CTA in parallel.  Owner warps 0..7: the head.  Helper warps 8..15 (one per
-        // owned actor): everything of the step that does not depend on the action -- the exploration draws, Ws.s, the
-        // env noise, |s|^2 -- so that the serial chain after the head is a handful of instructions.
-        if (owner) {
-            const float* hrow = Hb2 + own * p.ldh2;
-            for (int n8 = 0; n8 < A; n8 += 8) {
-                float s8[8];
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) s8[jj] = 0.0f;
-                const bool second = (n8 + 4 < ldwh);
-                for (int k = lane; k < H2; k += 32) {
-                    const float hv = hrow[k];
-                    const float* wr = Whs + k * ldwh + n8;
-                    const float4 w0 = *reinterpret_cast<const float4*>(wr);
-                    s8[0] = fmaf(hv, w0.x, s8[0]); s8[1] = fmaf(hv, w0.y, s8[1]);
-                    s8[2] = fmaf(hv, w0.z, s8[2]); s8[3] = fmaf(hv, w0.w, s8[3]);
-                    if (second) {
-                        const float4 w1 = *reinterpret_cast<const float4*>(wr + 4);
-                        s8[4] = fmaf(hv, w1.x, s8[4]); s8[5] = fmaf(hv, w1.y, s8[5]);
-                        s8[6] = fmaf(hv, w1.z, s8[6]); s8[7] = fmaf(hv, w1.w, s8[7]);
-                    }
-                }
-                float mine = 0.0f;
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) {
-                    const float tt = warp_sum(s8[jj]);
-                    if (lane == jj) mine = tt;
-                }
-                const int j = n8 + lane;
-                if (lane < 8 && j < A) Mu[own * A + j] = rf_act(mine + Bhs[j], p.act[2]);
-            }
-        } else {
-            const int h = warp - RF_OWN;                       // helper of owned actor h
-            const long long ih = row0 + (int)crank * RF_OWN + h;
-            const float* sh = S + h * D;
-            float q = 0.0f;
-            for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
-            q = warp_sum(q);
-            const bool h_done = (p.max_steps > 0) && (s_ep[h] + 1 >= p.max_steps);
-            for (int d = lane; d < D; d += 32) {
-                float acc = 0.0f;                              // WsT is [k][d]: conflict-free across lanes
-#pragma unroll 8
-                for (int k = 0; k < D; ++k) acc = fmaf(EWs[k * D + d], sh[k], acc);
-                const Philox4 r = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr,
-                                                ((unsigned long long)ih << 20) | (unsigned long long)d);
-                const float2 gz = box_muller(r.x, r.y);
-                Eacc[h * D + d] = acc;
-                Egx[h * D + d] = gz.x;
-                Erz[h * D + d] = h_done ? box_muller(r.z, r.w).x : 0.0f;
-                if (d == 0) {
-                    Eq[2 * h] = q;
-                    Eq[2 * h + 1] = gz.y;
-                }
-            }
-            if (!p.deterministic && lane < A) {                // PPOAgent.act's N(0,1) draws: keys of sample_one()
-                const int j = lane;
-                const Philox4 r = philox4x32_10(p.agent_seed, ctr, ((unsigned long long)ih << 16) | (unsigned long long)(j >> 2));
-                const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
-                const int c = j & 3;
-                Zn[h * A + j] = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
-            }
-        }
-        RF_STAMP(9, 0);
-        RF_STAMP(17, 256);
-        __syncthreads();
-        RF_STAMP(10, 0);
-        // ---- phase 2 (owner warps): action, env step, bookkeeping -- same arithmetic, operand order and Philox keys as
-        // sample_one() / synth_env_block() of rollout.cu
-        if (owner) {
-            const int pos = s_pos[own];
-            if (lane < A) {
-                const int j = lane;
-                const float mu = Mu[own * A + j];
-                const float sd = Sd[own * A + j];
-                float a = mu;
-                if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
-                a = fminf(fmaxf(a, -1.0f), 1.0f);
-                Ac[own * A + j] = a;
-                if (valid) {
-                    p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
-                    p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + j] = mu;
-                    p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + A + j] = sd;
-                    if (final_step) {
-                        p.action[i_own * A + j] = a;
-                        p.pd[i_own * 2 * A + j] = mu;
-                        p.pd[i_own * 2 * A + A + j] = sd;
-                    }
-                }
-            }
-            __syncwarp();
-            float* sown = S + own * D;
-            const int ep = s_ep[own] + 1;
-            const bool is_done = (p.max_steps > 0) && (ep >= p.max_steps);
-            dn = is_done ? 1.0f : 0.0f;
-            rew = -Eq[2 * own] / (float)D + 0.1f * Eq[2 * own + 1];
-            for (int d = lane; d < D; d += 32) {
-                float acc = Eacc[own * D + d];
-#pragma unroll 4
-                for (int k = 0; k < A; ++k) acc = fmaf(EWa[k * D + d], Ac[own * A + k], acc);
-                const float nxt = tanhf(acc) + 0.01f * Egx[own * D + d];
-                Nx[own * D + d] = nxt;
-                sown[d] = is_done ? Erz[own * D + d] : nxt;
-                if (valid && final_step) p.obs_next[i_own * D + d] = nxt;
-            }
-            if (lane == 0) {
-                s_ep[own] = is_done ? 0 : ep;
-                if (valid && final_step) {
-                    p.reward[i_own] = rew;
-                    p.done[i_own] = dn;
-                }
-                if (valid && pos + 1 == p.n_step) {            // this step completes a window -> next outbox entry
-                    const int w = s_cnt[own];
-                    if (w < p.Wout) {
-                        slot = (int)(i_own * p.Wout + w);
-                        p.ev_step[slot] = t;
-                        s_cnt[own] = w + 1;
-                    } else {
-                        slot = SLOT_DROPPED;
-                    }
-                }
-            }
-            slot = __shfl_sync(0xffffffffu, slot, 0);
-            __syncwarp();
-        }
-        RF_STAMP(11, 0);
-        // ---- window staging (block-wide barriers inside: every warp calls; only owners do work)
-        commit_actor(valid, (int)i_own, lane, 32, Nx + (owner ? own : 0) * D, S + (owner ? own : 0) * D, rew, dn, p.n_step,
-                     p.stride, D, A, s_pos + (owner ? own : 0), slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew,
-                     p.stage_done, p.o_obs, p.o_act, p.o_pd, p.o_rew, p.o_done);
-        RF_STAMP(12, 0);
-        // ---- next observation -> z-filter -> every CTA's input tile
-        if (owner) {
-            const int q4 = lane;                            // D / 4 <= 32 float4 per row
-            if (q4 < (D >> 2)) {
-                float4 v = *reinterpret_cast<const float4*>(S + own * D + q4 * 4);
-                if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (p.zf != nullptr) {
-                    const float4 zm = *reinterpret_cast<const float4*>(Zm + q4 * 4);
-                    const float4 zs = *reinterpret_cast<const float4*>(Zs + q4 * 4);
-                    v.x = fminf(fmaxf((v.x - zm.x) / zs.x, -5.0f), 5.0f);
-                    v.y = fminf(fmaxf((v.y - zm.y) / zs.y, -5.0f), 5.0f);
-                    v.z = fminf(fmaxf((v.z - zm.z) / zs.z, -5.0f), 5.0f);
-                    v.w = fminf(fmaxf((v.w - zm.w) / zs.w, -5.0f), 5.0f);
-                    if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-                float* qx = X0 + m_own * p.ldx0 + q4 * 4;
-                *reinterpret_cast<float4*>(qx) = v;
-                const unsigned off = rf_smem_u32(qx) - smem_base;
-#pragma unroll
-                for (int c = 0; c < RF_CS - 1; ++c) rf_st_cluster_v4(peer_base[c] + off, v);
-            }
-        }
-        RF_STAMP(13, 0);
-        cluster.sync();
-        RF_STAMP(14, 0);
-    }
-
-    // ---- write the per-actor control state back
-    if (valid) {
-        for (int d = lane; d < D; d += 32) p.state[i_own * D + d] = S[own * D + d];
-        if (lane == 0) {
-            p.stage_pos[i_own] = s_pos[own];
-            p.ep_step[i_own] = s_ep[own];
-            p.ev_count[i_own] = s_cnt[own];
-        }
-    }
-}
-
-
-// =====================================================================================================================
-// v2 of the persistent rollout kernel: same cluster / resident-weight / DSMEM structure, same arithmetic for sampling and
-// the environment, two changes of schedule that the clock64 trace of v1 asked for (tools/rollout_trace.py):
-//   * WARP SPECIALISATION.  In v1 the action-independent half of the env step (Philox + Box-Muller draws, Ws.s, |s|^2:
-//     ~6.8 K cycles on 8 helper warps) sat on the serial chain behind the layers.  Now warps 0..7 ("math warps") run
-//     the two hidden layers while warps 8..15 ("env warps") do that work for the SAME step concurrently -- it depends
-//     only on the state at the top of the step.  The env warps arrive at cluster barrier 1 before they start
-//     (barrier.cluster.arrive / .wait are split-phase), so they never hold the math warps up.
-//   * 8 x 4 REGISTER TILES in the layers (was 4 x 4): 12 LDS.128 per 128 FMA instead of 8 per 64 -- the layer loop was
-//     bound by shared-memory loads, not by FFMA issue.  A warp = 16 column quads x 2 k-halves over ONE 8-row group, so
-//     the activation loads are warp-wide broadcasts.
-//   * the head runs on all 16 warps (2 per owned actor, k halves) with a 9-shuffle transposing reduction.
+// Schedule of a step.  Warps 0..7 run the hidden layers; warps 8..15 meanwhile do the part of the env step that does
+// not depend on the action (Philox + Box-Muller draws, Ws.s, |s|^2): it needs only the state at the top of the step, so
+// it stays off the serial chain behind the layers.  Where a layer's k split goes through shared memory its register
+// tiles are 8 rows x 4 columns: 12 LDS.128 per 128 FMA instead of 8 per 64 with 4 x 4 tiles -- the layer loop is bound
+// by shared-memory loads, not by FFMA issue.  A warp = 16 column quads x 2 k-halves over ONE 8-row group, so the
+// activation loads are warp-wide broadcasts.  Named barrier 1 joins the 256 threads of the layer warps.
 __device__ __forceinline__ void rf_bar_math() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-__device__ __forceinline__ void rf_cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void rf_cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
-// ---- mbarrier-signalled DSMEM hand-off (the ASYNC variant of the v2 kernel).  barrier.cluster.arrive.release compiles to
-// MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR in front of the barrier (the kernel's global stores of the step must drain to L2
-// first) and the wait to a CCTL.IVALL: three times per env step.  st.async carries the data AND the completion count to
-// the consumer's mbarrier, so the producer needs no fence and the consumer polls its own shared memory.
+// ---- mbarrier-signalled DSMEM hand-offs.  A cluster barrier would cost more: barrier.cluster.arrive.release compiles
+// to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR in front of the barrier (the kernel's global stores of the step must drain to
+// L2 first) and the wait to a CCTL.IVALL.  st.async carries the data AND the completion count to the consumer's
+// mbarrier, so the producer needs no fence and the consumer polls its own shared memory.
 __device__ __forceinline__ void rf_mbar_init(unsigned long long* bar, unsigned count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rf_smem_u32(bar)), "r"(count) : "memory");
 }
@@ -561,9 +184,9 @@ __device__ __forceinline__ float rf_reduce8(const float (&s)[8], int lane) {
     return v;
 }
 
-// One hidden layer on the 8 math warps (tid 0..255): warp = (row group rg = warp & 3: rows 8rg..8rg+7, k quarter pair),
-// lane = (column quad, k half) -> 4-way k split, partial tiles summed in a fixed order through Part [4][32][Nc].
-template <bool ALL_ROWS, bool ASYNC>
+// Last hidden layer (G = 1) on the 8 math warps (tid 0..255): warp = (row group rg = warp & 3: rows 8rg..8rg+7, k quarter
+// pair), lane = (column quad, k half) -> 4-way k split, partial tiles summed in a fixed order through Part [4][32][Nc].
+// Each row goes only to the CTA that owns its actor, into its Hout [8][ldout] (input of the head).
 __device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
                                           int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
                                           int ldout, int col0, float* __restrict__ Part, unsigned smem_base,
@@ -623,26 +246,13 @@ __device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldi
         o.y = rf_act(((p0.y + p1.y) + (p2.y + p3.y)) + bv.y, act);
         o.z = rf_act(((p0.z + p1.z) + (p2.z + p3.z)) + bv.z, act);
         o.w = rf_act(((p0.w + p1.w) + (p2.w + p3.w)) + bv.w, act);
-        if (ALL_ROWS) {
-            float* qd = Hout + row * ldout + col0 + c4 * 4;
+        const unsigned owner = (unsigned)(row / RF_OWN);
+        float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
+        if (owner == crank) {
             *reinterpret_cast<float4*>(qd) = o;
-            const unsigned off = rf_smem_u32(qd) - smem_base;
-#pragma unroll
-            for (int c = 1; c < RF_CS; ++c) {
-                const unsigned pb = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
-                if (ASYNC) rf_st_async_v4(pb + off, o, pb + bar_off);
-                else rf_st_cluster_v4(pb + off, o);
-            }
         } else {
-            const unsigned owner = (unsigned)(row / RF_OWN);
-            float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
-            if (owner == crank) {
-                *reinterpret_cast<float4*>(qd) = o;
-            } else {
-                const unsigned pb = rf_mapa(smem_base, owner);
-                if (ASYNC) rf_st_async_v4(pb + (rf_smem_u32(qd) - smem_base), o, pb + bar_off);
-                else rf_st_cluster_v4(pb + (rf_smem_u32(qd) - smem_base), o);
-            }
+            const unsigned pb = rf_mapa(smem_base, owner);
+            rf_st_async_v4(pb + (rf_smem_u32(qd) - smem_base), o, pb + bar_off);
         }
     }
 }
@@ -651,10 +261,9 @@ __device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldi
 // rf2_layer spent more on partial tiles, the barrier and the second pass (1.5 K cycles) than on its 4 k quads of FMAs.
 // Here warp w owns rows 4w..4w+3, lane = (column quad, k half); the two k halves of a lane pair are summed by shuffle
 // (each lane keeps two of the four rows) and the epilogue stores / pushes straight from registers.
-template <bool ASYNC>
 __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws, int Nc,
                                            const float* __restrict__ bias_s, int act, float* __restrict__ Hout, int ldout,
-                                           int col0, unsigned smem_base, unsigned crank, unsigned bar_off, int rf_t) {
+                                           int col0, unsigned smem_base, unsigned crank, unsigned bar_off) {
     const int tid = (int)RF_TID, warp = tid >> 5, lane = tid & 31;
     const int cg0 = lane & 15, kh = lane >> 4;
     const bool up = kh != 0;
@@ -710,22 +319,17 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
                 *reinterpret_cast<float4*>(qd) = o;
                 const unsigned off = rf_smem_u32(qd) - smem_base;
 #pragma unroll
-                for (int c = 0; c < RF_CS - 1; ++c) {
-                    if (ASYNC) rf_st_async_v4(pb[c] + off, o, pb[c] + bar_off);
-                    else rf_st_cluster_v4(pb[c] + off, o);
-                }
+                for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(pb[c] + off, o, pb[c] + bar_off);
             }
         }
     }
-    RF_STAMP(1, 0);
-    RF_STAMP(2, 0);
 }
 
-// Last hidden layer on the 8 math warps WITHOUT the shared-memory reduction of rf2_layer<false, true>, with the same
+// Last hidden layer on the 8 math warps WITHOUT the shared-memory reduction of rf2_layer, with the same
 // result bit for bit: the same four k quarters, each accumulated in the same order by one lane, meet through two rounds of
 // shuffles as ((p0 + p1) + (p2 + p3)) + bias (fp32 addition is commutative, so which lane of a pair adds does not
 // matter).  Warp = (row group rg = warp & 3: rows 8rg..8rg+7, column half ch = warp >> 2), lane = (column quad cq = lane & 7,
-// k quarter ks = lane >> 3).  Each row goes to the CTA that owns its actor, as in rf2_layer<false, .>.
+// k quarter ks = lane >> 3).  Each row goes to the CTA that owns its actor, as in rf2_layer.
 __device__ __forceinline__ void rf2_layer2_direct(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
                                                   int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
                                                   int ldout, int col0, unsigned smem_base, unsigned crank, unsigned bar_off) {
@@ -809,7 +413,7 @@ __device__ __forceinline__ void rf_bar_arrive(int id, int n) { asm volatile("bar
 // Warps 8..15 ("tail warps", warp 8 + a for owned actor a of each group) take the whole tail of a group -- the
 // action-independent env precompute, head, sampling, env step, window staging, the push of the next input rows -- while
 // the layer warps compute the other group.  Arithmetic, operand order and Philox keys are those of the G = 1 schedule
-// (head_mode 1, reduction-free layer 1, rf2_layer2_direct = rf2_layer<false> bit for bit), so both give the same results.
+// (head_mode 1, rf2_layer2_direct = rf2_layer bit for bit), so both give the same results.
 //
 // Hand-offs, per group g (each group has its own tiles, state and three mbarriers):
 //   layer -> peers: H1 rows (all 32) and H2 rows (owners' only) by st.async, counted on the receiver's h1[g] / h2[g];
@@ -927,7 +531,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
     if (layer) {
         for (int t = 0; t < p.T; ++t) {
             const bool final_step = (t == p.T - 1);
-            const int rf_t = t;
+            [[maybe_unused]] const int rf_t = t;      // read by RF_STAMP only
             RF_STAMP(0, 0);
             for (int g = 0; g < G; ++g) {
                 float* X0 = smem + p.oX0 + g * gs;
@@ -942,8 +546,8 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                     rf_mbar_arm(&s_bar[g][1], tx_h2);
                     if (!final_step) rf_mbar_arm(&s_bar[g][2], tx_x0);
                 }
-                rf2_layer1<true>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank,
-                                 rf_smem_u32(&s_bar[g][0]) - smem_base, rf_t);
+                rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank,
+                           rf_smem_u32(&s_bar[g][0]) - smem_base);
                 rf_bar_math();
                 rf_mbar_wait(&s_bar[g][0], (unsigned)t & 1u);
                 RF_STAMP(3 + 2 * g, 0);
@@ -957,7 +561,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
         for (int t = 0; t < p.T; ++t) {
             const unsigned long long ctr = ctr0 + (unsigned long long)t;
             const bool final_step = (t == p.T - 1);
-            const int rf_t = t;
+            [[maybe_unused]] const int rf_t = t;      // read by RF_STAMP only
             for (int g = 0; g < G; ++g) {
                 float* X0 = smem + p.oX0 + g * gs;
                 float* Hb2 = smem + p.oH2 + g * gs;
@@ -1176,10 +780,9 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
     }
 }
 
-template <bool ASYNC, int G>
+template <int G>
 __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     ppo_rollout2_kernel(const __grid_constant__ RfParams p) {
-    static_assert(G == 1 || (G == 2 && ASYNC), "two groups per cluster use the mbarrier hand-offs");
     RF_CTA_STAMP(1);
     if constexpr (G == 2) {
         rf2_two_groups(p);
@@ -1194,7 +797,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
 #pragma unroll
     for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
     __shared__ int s_pos[RF_OWN], s_ep[RF_OWN], s_cnt[RF_OWN];
-    __shared__ __align__(8) unsigned long long s_bar[3];      // ASYNC: hidden layer 1 | last hidden layer rows | next input tile
+    __shared__ __align__(8) unsigned long long s_bar[3];      // hidden layer 1 | last hidden layer rows | next input tile
 
     // (tried: the two roles on swapped warp halves, in case the scheduler's preference for one end of the warp index range
     // starved the layers -- no difference in clock64 traces)
@@ -1219,7 +822,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     float* S = smem + p.oS;
     float* Nx = smem + p.oNext;
     float* Ac = smem + p.oAct;
-    float* Sd = Ac + 2 * RF_OWN * A;     // (slot 1 = Mu of v1: unused here)
+    float* Sd = Ac + 2 * RF_OWN * A;     // (slot 1 unused, see rf_plan)
     float* Zn = Sd + RF_OWN * A;
     float* Hp = Zn + RF_OWN * A;         // [2][8][A] head partial sums of the two k halves
     float* Eacc = smem + p.oPre;
@@ -1228,7 +831,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     float* Eq = Erz + RF_OWN * D;
     const long long row0 = (long long)(blockIdx.x / RF_CS) * RF_ROWS;
 
-    // ---- one-time loads (as v1)
+    // ---- one-time loads: weight slices, biases, env matrices (cp.async burst), z-filter columns, actor state
     for (int f = tid; f < D * (Nc1 >> 2); f += RF_THREADS) {
         const int k = f / (Nc1 >> 2), q = f - k * (Nc1 >> 2);
         cp_async16(W1s + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
@@ -1270,7 +873,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
         X0[m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
     }
     const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
-    if (ASYNC && tid == 0) {
+    if (tid == 0) {
         for (int i = 0; i < 3; ++i) rf_mbar_init(&s_bar[i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -1299,43 +902,28 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
         const bool final_step = (t == p.T - 1);
         const int rf_t = t;
         RF_STAMP(0, 0);
-        if (ASYNC && tid == 0) {                              // arm this step's phases (the previous ones were consumed)
+        if (tid == 0) {                                       // arm this step's phases (the previous ones were consumed)
             rf_mbar_arm(&s_bar[0], tx_h1);
             rf_mbar_arm(&s_bar[1], tx_h2);
         }
         if (math) {
-            if (ASYNC && t > 0) {                             // the input tile: own rows (math warps wrote them) + the peers' rows
+            if (t > 0) {                                      // the input tile: own rows (math warps wrote them) + the peers' rows
                 rf_bar_math();
                 rf_mbar_wait(&s_bar[2], (unsigned)(t - 1) & 1u);
             }
             RF_STAMP(18, 0);
-            if (ASYNC && tid == 0 && !final_step) rf_mbar_arm(&s_bar[2], tx_x0);     // next tile's phase: only now is the previous one complete
-            if (p.l1_direct)                                   // 8 math warps x 4 rows: the reduction-free form
-                rf2_layer1<ASYNC>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank, bar_off_h1, rf_t);
-            else
-                rf2_layer<true, ASYNC>(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, Part, smem_base, crank, rf_t, 1,
-                                       bar_off_h1);
+            if (tid == 0 && !final_step) rf_mbar_arm(&s_bar[2], tx_x0);     // next tile's phase: only now is the previous one complete
+            rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank, bar_off_h1);
             RF_STAMP(3, 0);
-            if (ASYNC) {
-                rf_bar_math();
-                rf_mbar_wait(&s_bar[0], (unsigned)t & 1u);
-            } else {
-                rf_cluster_arrive();
-                rf_cluster_wait();
-            }
+            rf_bar_math();
+            rf_mbar_wait(&s_bar[0], (unsigned)t & 1u);
             RF_STAMP(4, 0);
-            rf2_layer<false, ASYNC>(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5,
-                                    bar_off_h2);
+            rf2_layer(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5,
+                      bar_off_h2);
             RF_STAMP(7, 0);
-            if (!ASYNC) {
-                rf_cluster_arrive();
-                rf_cluster_wait();
-            }
-            RF_STAMP(8, 0);
         } else {
             // ---- env warp h: everything of this step that does not depend on the action (arithmetic and Philox keys of
             // sample_one() / synth_env_block() in rollout.cu), concurrently with the layers
-            if (!ASYNC) rf_cluster_arrive();                  // barrier 1: nothing to publish
             RF_STAMP(16, 256);
             const int h = own;
             const long long ih = row0 + (int)crank * RF_OWN + h;
@@ -1367,16 +955,9 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 Zn[h * A + j] = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
             }
             RF_STAMP(17, 256);
-            if (!ASYNC) {
-                rf_cluster_wait();
-                rf_cluster_arrive();
-                rf_cluster_wait();
-            }
         }
-        if (ASYNC) {                                          // last hidden layer: own columns (block barrier) + the peers' columns
-            __syncthreads();
-            rf_mbar_wait(&s_bar[1], (unsigned)t & 1u);
-        }
+        __syncthreads();                                      // last hidden layer: own columns (block barrier) + the peers' columns
+        rf_mbar_wait(&s_bar[1], (unsigned)t & 1u);
         // ---- head.  p.head_mode 1: warp w takes the k slice [w H2/16, (w+1) H2/16) for ALL 8 owned actors (lane = actor x 4 k
         // sub-lanes), so the head weights are read from shared memory once per step instead of once per actor (the 2 x 8 KB
         // per actor were 1 K cycles of the shared-memory pipe); the 16 slice sums meet in the (idle) Part buffer.
@@ -1541,22 +1122,15 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 float* qx = X0 + m_own * p.ldx0 + q4 * 4;
                 *reinterpret_cast<float4*>(qx) = v;
                 const unsigned off = rf_smem_u32(qx) - smem_base;
-                if (ASYNC) {
-                    if (!final_step) {
+                if (!final_step) {
 #pragma unroll
-                        for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off_x0);
-                    }
-                } else {
-#pragma unroll
-                    for (int c = 0; c < RF_CS - 1; ++c) rf_st_cluster_v4(peer_base[c] + off, v);
+                    for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off_x0);
                 }
             }
         }
         RF_STAMP(13, 0);
-        if (!ASYNC) cluster.sync();
-        RF_STAMP(14, 0);
     }
-    if (ASYNC) cluster.sync();                                // nobody leaves while a peer may still address its shared memory
+    cluster.sync();                                           // nobody leaves while a peer may still address its shared memory
 
     if (valid) {
         for (int d = lane; d < D; d += 32) p.state[i_own * D + d] = S[own * D + d];
@@ -1652,7 +1226,7 @@ __global__ void __launch_bounds__(256) ppo_rollout_copy_kernel(const int* __rest
     copy_floats(r_done + (long long)slot * n_step, o_done + e * n_step, n_step, g, G);
 }
 
-// Shared-memory plan of ppo_rollout2_kernel<., G>.  G = 1: weights, the cluster's activation tiles, the k-split partial
+// Shared-memory plan of ppo_rollout2_kernel<G>.  G = 1: weights, the cluster's activation tiles, the k-split partial
 // tiles (Part), the env matrices and the owned actors' state.  G = 2: no Part (both layers are reduction-free), the env
 // matrices stay in global memory (read through L1 by the tail warps, off the layers' path), a 4 KB head slice buffer,
 // and the per-group tiles and state twice, `gstride` floats apart.  At the configs[1] shape [64, 256, 256, 8]:
@@ -1669,6 +1243,8 @@ bool rf_plan(const sb200_mlp* net, int D, int A, int G, RfParams* p, size_t* sme
     const int oB = take(Nc1 + Nc2 + ldwh);
     const int ldx0 = D + 4, ldh1 = H1 + 4, ldh2 = H2 + 4;
     int oX0, oH1, oH2, oPart = -1, oZf, oEnv = -1, oS, oNext, oAct, oPre, oHs = -1, gstride = 0;
+    // Act: actions | unused | std | N(0,1) draws | two head halves; the unused slot stays so that the plan, and with it the
+    // supported envelope and the one- / two-group choice, does not move
     if (G == 1) {
         oX0 = take(RF_ROWS * ldx0); oH1 = take(RF_ROWS * ldh1); oH2 = take(RF_OWN * ldh2);
         oPart = take(4LL * RF_ROWS * (Nc1 > Nc2 ? Nc1 : Nc2));
@@ -1712,12 +1288,12 @@ cudaError_t rf_query_clusters(size_t smem, int* n) {
     cfg.numAttrs = 1;
     // without the opt-in to > 48 KB of dynamic shared memory the answer is 0 clusters (and it is cached): set it here too,
     // so that a query made before sb200_init() is right
-    const cudaError_t e = cudaFuncSetAttribute(ppo_rollout2_kernel<true, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    const cudaError_t e = cudaFuncSetAttribute(ppo_rollout2_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
     if (e != cudaSuccess) return e;
-    return cudaOccupancyMaxActiveClusters(n, ppo_rollout2_kernel<true, G>, &cfg);
+    return cudaOccupancyMaxActiveClusters(n, ppo_rollout2_kernel<G>, &cfg);
 }
 
-// How many 4-CTA clusters of ppo_rollout2_kernel<true, G> with `smem` dynamic bytes the current device runs at once.
+// How many 4-CTA clusters of ppo_rollout2_kernel<G> with `smem` dynamic bytes the current device runs at once.
 // A cluster must sit inside one GPC, and an H100's GPCs have uneven SM counts, so this is below SMs / 4 (30 on an H100
 // SXM with 132 SMs at the configs[1] plan).  Queried once per (device, G, bytes).
 int rf_max_clusters(int G, size_t smem, int* n_out) {
@@ -1740,42 +1316,30 @@ int rf_max_clusters(int G, size_t smem, int* n_out) {
     return SB200_OK;
 }
 
-// Launch shape of a chunk: kernel variant, groups per cluster, CTAs, and whether they are all resident at once.
+// Launch shape of a chunk: groups per cluster, CTAs, and whether they are all resident at once.
 struct RfShape {
-    bool v2, async;
     int groups;
     long long ctas;
-    bool one_wave;                    // known to run in one wave (false also when residency was not queried)
+    bool one_wave;                    // known to run in one wave
 };
 
-// `p` / `smem` hold the G = 1 plan of rf_plan on entry; on return the plan of the chosen shape (l1_direct and head_mode set).
+// `p` / `smem` hold the G = 1 plan of rf_plan on entry; on return the plan of the chosen shape (head_mode set).
 int rf_shape(const sb200_ppo_rollout* a, RfParams* p, size_t* smem, RfShape* sh) {
     const long long clusters = ((long long)a->N + RF_ROWS - 1) / RF_ROWS;
-    // v2 (warp-specialised env warps, 8x4 register tiles) is the default; SB200_RF_V2=0 selects the v1 kernel
-    static const int v2 = [] { const char* e = getenv("SB200_RF_V2"); return e ? atoi(e) : 1; }();
-    static const int l1_direct = [] { const char* e = getenv("SB200_RF_L1DIRECT"); return e ? atoi(e) : 1; }();
-    p->l1_direct = (l1_direct && RF_ROWS == 4 * RF_OWN) ? 1 : 0;
-    static const int head_mode = [] { const char* e = getenv("SB200_RF_HEAD"); return e ? atoi(e) : 1; }();
-    // the slice sums need 16 warps x 8 actors x ldw[2] floats of the Part buffer (4 x 32 x max(Nc1, Nc2))
-    p->head_mode = (head_mode == 1 && 16 * RF_OWN * a->net->ldw[2] <= 4 * RF_ROWS * std::max(a->net->dims[1], a->net->dims[2]) / RF_CS) ? 1 : 0;
-    // default: mbarrier-signalled st.async hand-offs instead of the three cluster barriers per step (1.47 -> 1.38 ms per
-    // 128-step chunk of 1024 actors, same results bit for bit); SB200_RF_ASYNC=0 selects the barrier.cluster variant
-    static const int rf_async = [] { const char* e = getenv("SB200_RF_ASYNC"); return e ? atoi(e) : 1; }();
-    const bool async = v2 && rf_async && a->D % 4 == 0 && (3u * RF_ROWS * (unsigned)(a->net->dims[1] / RF_CS) * 4u) < (1u << 20);
+    // head_mode 1 when the slice sums fit: 16 warps x 8 actors x ldw[2] floats of the Part buffer (4 x 32 x max(Nc1, Nc2))
+    p->head_mode = (16 * RF_OWN * a->net->ldw[2] <= 4 * RF_ROWS * std::max(a->net->dims[1], a->net->dims[2]) / RF_CS) ? 1 : 0;
     // Two groups of 32 actors per cluster when the device cannot hold all ceil(N / 32) one-group clusters at once (the
     // clusters that do not fit run as a whole further wave of the chunk) AND two groups at least halve the number of
     // waves: a two-group step does both groups' work, 1.74x the time of a one-group step at the configs[1] shape on an
     // H100 (38 K vs 22 K cycles), so fewer waves pay only when they are at most half as many (1024 actors: 2 -> 1
     // wave; 4096 actors: 5 -> 3 waves would be slower).  Same results as one group: same arithmetic (head_mode 1,
-    // reduction-free layer 1, rf2_layer2_direct).
+    // rf2_layer2_direct).
     int groups = 1, fit1 = 0, fit2 = 0;
-    if (async) {
-        const int rc = rf_max_clusters(1, *smem, &fit1);
-        if (rc != SB200_OK) return rc;
-    }
+    const int rc1 = rf_max_clusters(1, *smem, &fit1);
+    if (rc1 != SB200_OK) return rc1;
     RfParams p2 = *p;
     size_t smem2 = 0;
-    if (async && p->l1_direct && p->head_mode == 1 && rf_plan(a->net, a->D, a->A, 2, &p2, &smem2)) {
+    if (p->head_mode == 1 && rf_plan(a->net, a->D, a->A, 2, &p2, &smem2)) {
         const int rc = rf_max_clusters(2, smem2, &fit2);
         if (rc != SB200_OK) return rc;
         if (fit1 >= 1 && fit2 >= 1 && clusters > fit1) {
@@ -1788,21 +1352,17 @@ int rf_shape(const sb200_ppo_rollout* a, RfParams* p, size_t* smem, RfShape* sh)
         }
     }
     const long long launched = (clusters + groups - 1) / groups;
-    sh->v2 = v2 != 0;
-    sh->async = async;
     sh->groups = groups;
     sh->ctas = launched * RF_CS;
-    sh->one_wave = async && launched <= (groups == 2 ? fit2 : fit1);
+    sh->one_wave = launched <= (groups == 2 ? fit2 : fit1);
     return SB200_OK;
 }
 
 }  // namespace
 
 int sb200_rollout_fused_init() {
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
-    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    SB200_CUDA(cudaFuncSetAttribute(ppo_rollout2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
     return SB200_OK;
 }
 
@@ -1818,7 +1378,7 @@ extern "C" int sb200_debug_rf_trace(long long* host_out) {
 }
 
 // per-CTA [smid, entry ns, exit ns] of the last persistent launch (RF_TR_CTAS rows); info = {grid CTAs, dynamic shared
-// bytes, groups per cluster G, cudaOccupancyMaxActiveClusters of ppo_rollout2_kernel<true, G> at that configuration}
+// bytes, groups per cluster G, cudaOccupancyMaxActiveClusters of ppo_rollout2_kernel<G> at that configuration}
 extern "C" int sb200_debug_rf_ctas(long long* host_out, long long* info) {
     SB200_CUDA(cudaDeviceSynchronize());
     SB200_CUDA(cudaMemcpyFromSymbol(host_out, g_rf_cta, sizeof(g_rf_cta)));
@@ -1899,17 +1459,14 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     const int rc = rf_shape(a, &p, &smem, &sh);
     if (rc != SB200_OK) return rc;
     const int groups = sh.groups;
-    const bool async = sh.async, v2 = sh.v2;
     const long long ctas = sh.ctas;
 #ifdef RF_TRACE
     g_rf_last_grid = (unsigned)ctas;
     g_rf_last_smem = smem;
     g_rf_last_groups = groups;
 #endif
-    if (groups == 2) ppo_rollout2_kernel<true, 2><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else if (async) ppo_rollout2_kernel<true, 1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else if (v2) ppo_rollout2_kernel<false, 1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
-    else ppo_rollout_kernel<<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    if (groups == 2) ppo_rollout2_kernel<2><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
+    else ppo_rollout2_kernel<1><<<(unsigned)ctas, RF_THREADS, smem, (cudaStream_t)stream>>>(p);
     return sb200_launch_status();
 }
 
