@@ -106,7 +106,7 @@ int sb200_mlp_forward_f32(const sb200_mlp* net, const sb200_zfilter* zf, const s
  * 32 rows, 2 = fp32 FFMA tiles of 32 rows (both <= 128 registers per thread, 2 CTAs/SM).  Variant 1 is what large
  * batches get by default (631 us on the 132 096-row critic pass).  Launching 1 and 2 on two streams over the two
  * halves of a batch -- tensor pipe and FMA pipe at once -- was measured SLOWER (700-760 us): both kernels are bound
- * by instruction issue, not by their math pipes; it stays available as an experiment (SB200_DUAL_CRITIC=1). */
+ * by instruction issue, not by their math pipes; it stays available as an experiment (ops.mlp_forward_dual). */
 int sb200_mlp_forward_variant_f32(const sb200_mlp* net, const sb200_zfilter* zf, const sb200_rows* in,
                                   float* const* save, const int64_t* ld_save, int variant, void* stream);
 /* Small-batch inference on PRE-PACKED weights (the actors' per-step policy forward, ppo_agent.py:138-141 /

@@ -68,7 +68,7 @@ class PPOAgent(Agent):
     def act(self, obs, eps=None):
         """-> action (eval) or (action, [onetime_infos, [pd]]) in training, like ppo_agent.py:151-154.
         Device observations give device results; numpy in, numpy out."""
-        N, A, D = self.num_envs, self.action_dim, self.model.low_dim
+        N, D = self.num_envs, self.model.low_dim
         if self.model.rnn_stem is not None:
             return self._act_rnn(obs, eps)
         if self.model.cnn_stem is not None:
@@ -103,8 +103,20 @@ class PPOAgent(Agent):
             ops.mlp_forward_packed(self._packed, x, zf_stats=m.z_stats, zf_eps=m.z_eps, out=self._mean)
         else:
             ops.mlp_forward(m.actor, x, zf_stats=m.z_stats, zf_eps=m.z_eps, out=self._mean)
+        self._sample(eps)
+        return self._host_result(True, self._unbatched(obs), []) if host else self._result(self._action, self._pd, [])
+
+    def _unbatched(self, obs):
+        """One actor's observation without the batch dimension (numpy in: its results lose theirs too)."""
+        return self.num_envs == 1 and np.asarray(obs['low_dim'][next(iter(obs['low_dim']))] if isinstance(obs, dict)
+                                                 else obs).ndim == 1
+
+    def _sample(self, eps):
+        """The sampling kernel on self._mean: each actor's exploration scale, N(mean, std), clip, behaviour policy -- and,
+        in training behind the window wrapper, this step's staging (+ its replay-slot assignment when the wrapper fuses
+        launches) -- then the step counter."""
+        N, A, m, env = self.num_envs, self.action_dim, self.model, self.env
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        env = self.env
         staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
         counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
         eps_dev = None
@@ -123,26 +135,41 @@ class PPOAgent(Agent):
                 _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
                 _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None,
                 env.n_step if staged else 1, ops._stream()), 'sb200_ppo_sample_f32')
+        self._count_step(staged, counter)
+
+    def _count_step(self, staged, counter):
+        """Advance the agent's own step counter (the seed of the sampling noise); the wrapper's advances on the device."""
         if not staged and counter is self._counter:
             self._counter += 1
-        if host:
-            if self._out_pin is None:
-                self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
-                                 torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
-            self._out_pin[0].copy_(self._action, non_blocking=True)
-            self._out_pin[1].copy_(self._pd, non_blocking=True)
-            torch.cuda.current_stream().synchronize()              # one sync for both D2H copies
-            action = self._out_pin[0].numpy().astype(np.float64)   # the reference hands the env float64 (ppo_net.py:83)
-            pd = self._out_pin[1].numpy().copy()
-            if N == 1 and np.asarray(obs['low_dim'][next(iter(obs['low_dim']))] if isinstance(obs, dict) else obs).ndim == 1:
-                action, pd = action.reshape(-1), pd.reshape(-1)
-        else:
-            action, pd = self._action, self._pd
+
+    def _pinned_out(self):
+        if self._out_pin is None:
+            N, A = self.num_envs, self.action_dim
+            self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
+                             torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
+        return self._out_pin
+
+    def _host_result(self, d2h, single, onetime):
+        """act()'s numpy result from the pinned outputs: with ``d2h`` the D2H copies of action / pd and one sync for both
+        (else the C call has done them); float64 actions, as the reference hands the env (ppo_net.py:83); ``single``: one
+        actor's unbatched observation gives unbatched results."""
+        out = self._pinned_out()
+        if d2h:
+            out[0].copy_(self._action, non_blocking=True)
+            out[1].copy_(self._pd, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        action, pd = out[0].numpy().astype(np.float64), out[1].numpy().copy()
+        if single:
+            action, pd = action.reshape(-1), pd.reshape(-1)
+        return self._result(action, pd, onetime)
+
+    def _result(self, action, pd, onetime):
+        """-> action (eval) or (action, [onetime_infos, [pd]]) in training (ppo_agent.py:151-154)."""
         if self.agent_mode != 'training':
             return action
         if self.env_config.sleep_time:
             time.sleep(self.env_config.sleep_time)
-        return action, [[], [pd]]
+        return action, [onetime, [pd]]
 
     # -- RNN policy (the reference's default PPO config) ------------------------------------------------------------
     def _rnn_state(self):
@@ -214,10 +241,8 @@ class PPOAgent(Agent):
             if cnn is None:
                 obs_host, obs_dev = self._host_obs(np.asarray(x), D)
                 a.obs_host, a.obs, a.ld_obs = (obs_host.value if obs_host is not None else None), obs_dev.data_ptr(), D
-            if self._out_pin is None:
-                self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
-                                 torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
-            a.action_host, a.pd_host = self._out_pin[0].data_ptr(), self._out_pin[1].data_ptr()
+            out = self._pinned_out()
+            a.action_host, a.pd_host = out[0].data_ptr(), out[1].data_ptr()
             if training:
                 if getattr(self, '_cells_pin', None) is None:
                     self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
@@ -259,30 +284,20 @@ class PPOAgent(Agent):
                 fifo_state, dest = env.slot_assignment_args()
                 a.fifo_state, a.dest = fifo_state.data_ptr(), dest.data_ptr()
         check(_lib.lib().sb200_ppo_act_rnn_f32(C.byref(a), ops._stream()), 'sb200_ppo_act_rnn_f32')
-        if not staged and counter is self._counter:
-            self._counter += 1
-        if host:
-            action = self._out_pin[0].numpy().astype(np.float64)   # the reference hands the env float64 (ppo_net.py:83)
-            pd = self._out_pin[1].numpy().copy()
-            onetime = None
-            if training:                                            # [N, layers, H]
-                onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
+        self._count_step(staged, counter)
+        if not host:
+            return self._result(self._action, self._pd, [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)])
+        onetime = None
+        if training:                                                # [N, layers, H]
+            onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
             if N == 1:
-                action, pd = action.reshape(-1), pd.reshape(-1)
-                onetime = [onetime[0][0], onetime[1][0]] if onetime is not None else None
-        else:
-            action, pd = self._action, self._pd
-            onetime = [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)]                          # [N, layers, H]
-        if self.agent_mode != 'training':
-            return action
-        if self.env_config.sleep_time:
-            time.sleep(self.env_config.sleep_time)
-        return action, [onetime, [pd]]
+                onetime = [onetime[0][0], onetime[1][0]]
+        return self._host_result(False, N == 1, onetime)
 
     def _act_pixel(self, obs, eps=None):
         """act() on uint8 frames [N, C, H, W] (device tensor or numpy): CNN stem -> actor head -> sampling kernel
         (ppo_net.py:268-273,368-375; ppo_agent.py:138-149)."""
-        N, A = self.num_envs, self.action_dim
+        N = self.num_envs
         m, stem = self.model, self.model.cnn_stem
         fr = obs['pixel']['camera0'] if isinstance(obs, dict) else obs
         host = not isinstance(fr, torch.Tensor)
@@ -298,51 +313,15 @@ class PPOAgent(Agent):
             self._stem_bufs = stem.buffers(N)
         feat = stem.forward(fr, self._stem_bufs)
         ops.mlp_forward(m.actor, feat, out=self._mean)
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        env = self.env
-        staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        eps_dev = None
-        if eps is not None:
-            eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-        if staged and counter is not self._counter and env.fuse_launches:
-            fifo_state, dest = env.slot_assignment_args()
-            check(_lib.lib().sb200_ppo_sample_assign_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos), _p(env.stage_act), _p(env.stage_pd),
-                env.n_step, _p(fifo_state), _p(dest), ops._stream()), 'sb200_ppo_sample_assign_f32')
-        else:
-            check(_lib.lib().sb200_ppo_sample_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
-                _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None,
-                env.n_step if staged else 1, ops._stream()), 'sb200_ppo_sample_f32')
-        if not staged and counter is self._counter:
-            self._counter += 1
-        if host:
-            if self._out_pin is None:
-                self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
-                                 torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
-            self._out_pin[0].copy_(self._action, non_blocking=True)
-            self._out_pin[1].copy_(self._pd, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-            action, pd = self._out_pin[0].numpy().astype(np.float64), self._out_pin[1].numpy().copy()
-        else:
-            action, pd = self._action, self._pd
-        if self.agent_mode != 'training':
-            return action
-        if self.env_config.sleep_time:
-            time.sleep(self.env_config.sleep_time)
-        return action, [[], [pd]]
+        self._sample(eps)
+        return self._host_result(True, False, []) if host else self._result(self._action, self._pd, [])
 
     def _act_host(self, obs, x):
         """act() for a HOST observation batch through sb200_ppo_act_host_f32 (H2D -> forward -> sample -> D2H -> sync
         issued back to back from C): numpy in, numpy out, same results as the generic path."""
-        N, A, D = self.num_envs, self.action_dim, self.model.low_dim
+        N, D = self.num_envs, self.model.low_dim
         m, env = self.model, self.env
-        if self._out_pin is None:
-            self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
-                             torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
+        out = self._pinned_out()
         obs_host, obs_dev = self._host_obs(x, D)
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
         staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
@@ -356,20 +335,10 @@ class PPOAgent(Agent):
             C.byref(d), C.byref(zf), obs_host, _p(obs_dev), N, _p(self._mean), _p(m.log_var), _p(self._log_noise),
             int(det), self.seed, _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
             _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None, env.n_step if staged else 1,
-            _p(fifo_state), _p(dest), C.c_void_p(self._out_pin[0].data_ptr()), C.c_void_p(self._out_pin[1].data_ptr()),
+            _p(fifo_state), _p(dest), C.c_void_p(out[0].data_ptr()), C.c_void_p(out[1].data_ptr()),
             ops._stream()), 'sb200_ppo_act_host_f32')
-        if not staged and counter is self._counter:
-            self._counter += 1
-        action = self._out_pin[0].numpy().astype(np.float64)       # the reference hands the env float64 (ppo_net.py:83)
-        pd = self._out_pin[1].numpy().copy()
-        o0 = obs['low_dim'][next(iter(obs['low_dim']))] if isinstance(obs, dict) else obs
-        if N == 1 and np.asarray(o0).ndim == 1:
-            action, pd = action.reshape(-1), pd.reshape(-1)
-        if self.agent_mode != 'training':
-            return action
-        if self.env_config.sleep_time:
-            time.sleep(self.env_config.sleep_time)
-        return action, [[], [pd]]
+        self._count_step(staged, counter)
+        return self._host_result(False, self._unbatched(obs), [])
 
     def rollout_chunk_supported(self):
         """True when ``steps`` consecutive act -> env.step -> staging iterations can run as the persistent rollout

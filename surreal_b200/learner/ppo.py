@@ -15,7 +15,9 @@ import torch
 from .. import _lib, ops
 from .. import utils as U
 from .._lib import check
+from ..model.lstm_stem import rows_zfilter
 from ..model.ppo_net import PPOModel, DiagGauss
+from ..model.stem_chain import ChainTrainer, StemChain
 from ..session import ConfigError
 from .aggregator import MultistepAggregatorWithInfo
 from .base import Learner
@@ -27,10 +29,6 @@ S = dict(SURR=0, LOSS=1, ENTROPY=2, KL_PRE=3, KL_POST=4, GN_ACTOR=5, VAL_LOSS=6,
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def stem_shape(stem):
-    return (stem.C, stem.H, stem.W)
 
 
 class PPOLearner(Learner):
@@ -107,18 +105,26 @@ class PPOLearner(Learner):
         self.pixel = self.model.cnn_stem is not None
         self.rnn = self.model.rnn_stem is not None
         # width of the observation itself in the records: the low-dim features, or the frame's 32-bit words
-        self.obs_dim = U.obs_packed_dim(self.obs_spec) if self.pixel else self.model.low_dim
+        self.obs_dim = U.obs_packed_dim(self.obs_spec)
         # width of one observation in the batch buffers: the low-dim features (+ the actor's LSTM cells h | c in RNN mode,
         # which ride in the observation rows of the HBM records -- the reference ships them as onetime_infos), or the uint8
         # frame as 32-bit words
         D = U.record_obs_dim(lc, self.env_config)
         self.low_dim = D
-        self.cell_layout = U.rnn_cell_layout(lc, self.env_config) if self.rnn else None
+        self.cell_layout = U.rnn_cell_layout(lc, self.env_config)
         self.eff_len = (n - self.horizon + 1) if self.rnn else 1
         M = B * self.eff_len                                      # rows the heads train on (ppo.py:518-537)
         self._rows = M
         dev = self.device
-        ig = 'linear' if self.rnn else self.pixel
+        f = lambda *sh: torch.zeros(*sh, dtype=torch.float32, device=dev)  # noqa: E731
+        # own batch buffers (host-batch path); a device batch from the HBM replay is used in place instead
+        self._own = dict(obs_full=f(B, n + 1, D), actions=f(B, n, A), pds=f(B, n, 2 * A), rewards=f(B, n),
+                         dones=f(B, n))
+        self._obs_full, self._actions, self._pds = self._own['obs_full'], self._own['actions'], self._own['pds']
+        self._rewards, self._dones = self._own['rewards'], self._own['dones']
+        # the stems between the records and the heads (None: MLP mode), with one trainer per optimiser
+        self.chain = StemChain(self.model, self.ref_target_model, self._obs_full, self.eff_len) if self.model.stems else None
+        ig = self.chain.input_grad if self.chain is not None else False
         self.actor_optim = ops.MlpTrainer(self.model.actor, M, self.lr_actor,
                                           clip_mode=1 if self.clip_actor_gradient else 0,
                                           clip_value=self.actor_gradient_clip_value,
@@ -127,46 +133,22 @@ class PPOLearner(Learner):
                                            clip_mode=1 if self.clip_critic_gradient else 0,
                                            clip_value=self.critic_gradient_clip_value,
                                            weight_decay=net.critic_regularization, input_grad=ig)
+        self._actor_chain = self._critic_chain = None
+        if self.chain is not None:
+            self._actor_chain = ChainTrainer(self.chain, self.actor_optim)
+            self._critic_chain = ChainTrainer(self.chain, self.critic_optim)
+            # [head | CNN | LSTM] gradient of each optimiser; each optimiser's Adam state over the stems is checkpointed
+            # under these names
+            self._g_actor, self._g_critic = self._actor_chain.grad, self._critic_chain.grad
+            self.actor_stem, self.critic_stem = self._actor_chain.cnn, self._critic_chain.cnn
+            self.actor_rnn, self.critic_rnn = self._actor_chain.rnn, self._critic_chain.rnn
+        # actions / behaviour policy of the update rows: step 0 of every window read in place, or the first eff_len steps
+        # of every window gathered contiguous in RNN mode
+        self._upd = (self._actions, n * A, self._pds, n * 2 * A)
         if self.rnn:
-            # the LSTM stem is shared by actor and critic and trained by BOTH optimisers (ppo_net.py:202-224)
-            from ..model.lstm_stem import RnnTrainer
-            stem, E, Hh, od = self.model.rnn_stem, self.eff_len, self.model.rnn_stem.H, self.obs_dim
-            self.actor_rnn, self.critic_rnn = RnnTrainer(stem, B, E), RnnTrainer(stem, B, E)
-            # one gradient buffer per optimiser: [head | CNN stem (pixel input) | LSTM stem]
-            ns = stem.size + (self.model.cnn_stem.size if self.pixel else 0)
-            self._g_actor = torch.zeros(self.model.actor.size + ns, dtype=torch.float32, device=dev)
-            self._g_critic = torch.zeros(self.model.critic.size + ns, dtype=torch.float32, device=dev)
-            self.actor_optim.grad = self._g_actor[:self.model.actor.size]
-            self.critic_optim.grad = self._g_critic[:self.model.critic.size]
-            zz = lambda r, w: torch.zeros(r, ops._ru(w, 4), dtype=torch.float32, device=dev)[:, :w]  # noqa: E731
-            # sequence-major rows: z-filtered observations, or -- pixel input -- dense frames (od words, a multiple of 4,
-            # so each buffer is a contiguous uint8 [rows, C, H, W] block the conv kernels read)
-            self._xf_all, self._xf_eff = zz(B * (n + 1), od), zz(M, od)
-            if not self.pixel:
-                self._xf_ref, self._xraw_eff = zz(M, od), zz(M, od)
-            self._act_it, self._pd_it = torch.zeros(M, A, device=dev), torch.zeros(M, 2 * A, device=dev)
-            self._rnn_all = stem.buffers(B, n + 1, save=False)
-            self._rnn_ref = self.ref_target_model.rnn_stem.buffers(B, E, save=False)
-        if self.pixel and self.rnn:
-            # CNN stem in front of the LSTM stem: one StemTrainer per optimiser on the B*eff_len update frames
-            from ..model.cnn_stem import StemTrainer
-            stem = self.model.cnn_stem
-            self.actor_stem, self.critic_stem = StemTrainer(stem, M), StemTrainer(stem, M)
-            self._stem_all = stem.buffers(B * (n + 1))
-            self._ref_stem_bufs = self.ref_target_model.cnn_stem.buffers(M)
-        elif self.pixel:
-            # the CNN stem is shared by actor and critic and trained by BOTH optimisers, each with its own Adam state
-            # (ppo_net.py:202-224): one StemTrainer per optimiser, gradients of head + stem in one contiguous buffer
-            from ..model.cnn_stem import StemTrainer
-            stem = self.model.cnn_stem
-            self.actor_stem, self.critic_stem = StemTrainer(stem, B), StemTrainer(stem, B)
-            self._g_actor = torch.zeros(self.model.actor.size + stem.size, dtype=torch.float32, device=dev)
-            self._g_critic = torch.zeros(self.model.critic.size + stem.size, dtype=torch.float32, device=dev)
-            self.actor_optim.grad = self._g_actor[:self.model.actor.size]
-            self.critic_optim.grad = self._g_critic[:self.model.critic.size]
-            self._frames0 = torch.zeros(B, *stem_shape(stem), dtype=torch.uint8, device=dev)
-            self._stem_all = None                                 # activation buffers of the B*(n+1)-frame critic pass
-            self._ref_stem_bufs = self.ref_target_model.cnn_stem.buffers(B)
+            self._act_it, self._pd_it = f(M, A), f(M, 2 * A)
+            self._upd = (self._act_it, A, self._pd_it, 2 * A)
+            self._xraw_eff = f(M, ops._ru(self.obs_dim, 4))[:, :self.obs_dim] if self.use_z_filter else None
 
         # learning-rate schedule (ppo.py:121-125,171-178)
         an = net.anneal
@@ -181,12 +163,6 @@ class PPOLearner(Learner):
         self.cells = None
 
         # ---- device state of one learn(): allocated once, reused (graph-friendly, no allocator traffic)
-        f = lambda *sh: torch.zeros(*sh, dtype=torch.float32, device=dev)  # noqa: E731
-        # own batch buffers (host-batch path); a device batch from the HBM replay is used in place instead
-        self._own = dict(obs_full=f(B, n + 1, D), actions=f(B, n, A), pds=f(B, n, 2 * A), rewards=f(B, n),
-                         dones=f(B, n))
-        self._obs_full, self._actions, self._pds = self._own['obs_full'], self._own['actions'], self._own['pds']
-        self._rewards, self._dones = self._own['rewards'], self._own['dones']
         self._rewards_f = f(B, n) if self.use_r_filter else None
         self._values = f(B * (n + 1), 1)
         self._adv, self._ret = f(B, self.eff_len), f(B, self.eff_len)
@@ -204,11 +180,8 @@ class PPOLearner(Learner):
         self._pin = {}
         self._gae_ws = torch.zeros(int(L.sb200_gae_workspace_bytes(B, n, n)), dtype=torch.uint8, device=dev)
         self.use_cuda_graph = ops.graphs_enabled()
-        # policy || value epochs as concurrent graph branches -- not in pixel mode, where both optimisers update the SHARED stem
-        self.parallel_branches = os.environ.get("SB200_PPO_FORK", "1") != "0" and not self.pixel and not self.rnn
-        # tensor pipe || FMA pipe critic pass: measured SLOWER (701-757 us) than the 2-CTA/SM tensor-core tiles alone
-        # (631 us) -- both kernels are issue-bound, they do not add up -- so it stays an experiment
-        self.dual_critic = os.environ.get("SB200_DUAL_CRITIC", "0") == "1"
+        # policy || value epochs as concurrent graph branches -- not with stems, which both optimisers update
+        self.parallel_branches = os.environ.get("SB200_PPO_FORK", "1") != "0" and self.chain is None
         self._graph = ops.GraphRunner()
         self._graph_head = ops.GraphRunner()
         self.before_epochs_hook = None                    # see _optimize
@@ -219,7 +192,7 @@ class PPOLearner(Learner):
         self.dp_v = None
         # all epochs of BOTH optimisers as ONE persistent kernel (csrc/epoch2.cu) instead of ~10 launches per epoch;
         # SB200_EPOCH_KERNEL=0 selects the launch chain (always the path of the pixel / RNN stems)
-        self.use_epoch_kernel = os.environ.get('SB200_EPOCH_KERNEL', '2') != '0' and not self.pixel and not self.rnn
+        self.use_epoch_kernel = os.environ.get('SB200_EPOCH_KERNEL', '2') != '0' and self.chain is None
         self._ek = None
         self.epoch_kernel_gen = 2 if self.use_epoch_kernel else 0
         self.epoch_history = []
@@ -262,6 +235,19 @@ class PPOLearner(Learner):
         return isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() \
             and tuple(t.shape) == tuple(shape)
 
+    def _put_cells(self, row0, get):
+        """RNN mode: onetime_infos = [h0, c0] [B, layers, H], the cells of every window's first step, into the cell
+        columns of the records' row 0 ``row0`` (device rows, or numpy rows of the pinned staging)."""
+        cl = self.cell_layout
+        if cl is None:
+            return
+        hc, shape = get('onetime_infos'), (self.batch_size, cl.layers * cl.hidden)
+        for dst, src in ((cl.h(row0), hc[0]), (cl.c(row0), hc[1])):
+            if isinstance(dst, np.ndarray):
+                dst[...] = np.asarray(src, dtype=np.float32).reshape(shape)
+            else:
+                dst.copy_(torch.as_tensor(src).reshape(shape), non_blocking=True)
+
     def _preprocess_batch_ppo(self, batch):
         """ppo.py:420-484: everything becomes fp32 on the device.  The learner's working layout is
         obs_full [B, n+1, D] (row n = obs_next), i.e. the reference's cat([obs, obs_next], 1) (ppo.py:380)
@@ -290,20 +276,15 @@ class PPOLearner(Learner):
         self._obs_full, self._actions, self._pds = own['obs_full'], own['actions'], own['pds']
         self._rewards, self._dones = own['rewards'], own['dones']
         nbytes = 0
+        od = self.obs_dim
         if isinstance(full, torch.Tensor) and not full.is_cuda and tuple(full.shape) == (B, n + 1, D):
             # host batch already in the working layout (ideally pinned): one DMA, no staging copy
             own['obs_full'].copy_(full, non_blocking=True)
             nbytes += own['obs_full'].numel() * 4
-            obs = None
         elif self.pixel:
-            obs = None
             fo, fn = get('obs')['pixel']['camera0'], get('obs_next')['pixel']['camera0']
-            u8 = own['obs_full'].view(torch.uint8).view(B, n + 1, -1)[:, :, :4 * self.obs_dim]
-            if self.rnn:                          # onetime_infos = [h0, c0] [B, L, H] behind the first frame
-                hc, cl = get('onetime_infos'), self.cell_layout
-                LH = cl.layers * cl.hidden
-                cl.h(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[0]).reshape(B, LH), non_blocking=True)
-                cl.c(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[1]).reshape(B, LH), non_blocking=True)
+            u8 = own['obs_full'].view(torch.uint8).view(B, n + 1, -1)[:, :, :4 * od]
+            self._put_cells(own['obs_full'][:, 0], get)
             if isinstance(fo, torch.Tensor):
                 u8[:, :n].copy_(fo.reshape(B, n, -1), non_blocking=True)
                 u8[:, n:].copy_(fn.reshape(B, 1, -1), non_blocking=True)
@@ -317,30 +298,19 @@ class PPOLearner(Learner):
                 nbytes += u8.numel()
         else:
             obs, obs_next = self._low_dim(get('obs')), self._low_dim(get('obs_next'))
-        od = self.obs_dim
-        if obs is None:
-            pass
-        elif isinstance(obs, torch.Tensor):
-            own['obs_full'][:, :n, :od].copy_(obs.reshape(B, n, od), non_blocking=True)
-            own['obs_full'][:, n:, :od].copy_(obs_next.reshape(B, 1, od), non_blocking=True)
-            if self.rnn:                          # onetime_infos = [h0, c0] [B, L, H] of the window's first step
-                hc, cl = get('onetime_infos'), self.cell_layout
-                LH = cl.layers * cl.hidden
-                cl.h(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[0]).reshape(B, LH), non_blocking=True)
-                cl.c(own['obs_full'][:, 0]).copy_(torch.as_tensor(hc[1]).reshape(B, LH), non_blocking=True)
-        else:
-            if 'obs_full' not in self._pin:
-                self._pin['obs_full'] = torch.zeros(B, n + 1, D, dtype=torch.float32).pin_memory()
-            pf = self._pin['obs_full'].numpy()
-            pf[:, :n, :od] = np.asarray(obs).reshape(B, n, od)
-            pf[:, n:, :od] = np.asarray(obs_next).reshape(B, 1, od)
-            if self.rnn:
-                hc, cl = get('onetime_infos'), self.cell_layout
-                LH = cl.layers * cl.hidden
-                cl.h(pf[:, 0])[...] = np.asarray(hc[0], dtype=np.float32).reshape(B, LH)
-                cl.c(pf[:, 0])[...] = np.asarray(hc[1], dtype=np.float32).reshape(B, LH)
-            own['obs_full'].copy_(self._pin['obs_full'], non_blocking=True)
-            nbytes += own['obs_full'].numel() * 4
+            if isinstance(obs, torch.Tensor):
+                own['obs_full'][:, :n, :od].copy_(obs.reshape(B, n, od), non_blocking=True)
+                own['obs_full'][:, n:, :od].copy_(obs_next.reshape(B, 1, od), non_blocking=True)
+                self._put_cells(own['obs_full'][:, 0], get)
+            else:
+                if 'obs_full' not in self._pin:
+                    self._pin['obs_full'] = torch.zeros(B, n + 1, D, dtype=torch.float32).pin_memory()
+                pf = self._pin['obs_full'].numpy()
+                pf[:, :n, :od] = np.asarray(obs).reshape(B, n, od)
+                pf[:, n:, :od] = np.asarray(obs_next).reshape(B, 1, od)
+                self._put_cells(pf[:, 0], get)
+                own['obs_full'].copy_(self._pin['obs_full'], non_blocking=True)
+                nbytes += own['obs_full'].numel() * 4
         nbytes += self._h2d('actions', get('actions'), own['actions'])
         nbytes += self._h2d('rewards', get('rewards'), own['rewards'])
         nbytes += self._h2d('dones', get('dones'), own['dones'])
@@ -350,39 +320,26 @@ class PPOLearner(Learner):
 
     # ------------------------------------------------------------------------------------------------
     def _gae_and_return(self):
-        """ppo.py:355-418 (MLP branch): critic over all B*(n+1) rows without materialising the cat, then GAE."""
-        B, n = self.batch_size, self.n_step
+        """ppo.py:355-418: critic over all B*(n+1) rows without materialising the cat, then GAE (horizon-windowed over
+        eff_len positions in RNN mode, ppo.py:389-406)."""
+        B, n, A = self.batch_size, self.n_step, self.action_dim
         m = self.model
         ev = self._prof_begin()
         rows = B * (n + 1)
-        if self.rnn:
-            # the critic over the whole [B, n+1] sequence through the LSTM from the window's initial cells (ppo.py:376-387),
-            # then the horizon-windowed GAE over eff_len positions (ppo.py:389-406)
-            self._rnn_prepare()
-            h0, c0, ld = self._cells()
-            x_all = m.cnn_stem.forward(self._frames(self._xf_all), self._stem_all) if self.pixel else self._xf_all
-            h_all = m.rnn_stem.forward(x_all, h0, c0, ld, B, n + 1, self._rnn_all)
-            ops.mlp_forward(m.critic, h_all, out=self._values)
-        elif self.pixel:
-            # all B*(n+1) frames through the shared stem, then the critic head on the features (ppo.py:376-387, 5-D obs)
-            stem = m.cnn_stem
-            if self._stem_all is None:
-                self._stem_all = stem.buffers(rows)
-            frames = self._obs_full.view(torch.uint8).view(rows, *stem_shape(stem))
-            feat = stem.forward(frames, self._stem_all)
-            if rows >= self.tc5_min_rows and self._tc5.supported(rows):
-                self._tc5(feat, self._values.view(rows, 1))
-            else:
-                ops.mlp_forward(m.critic, feat, out=self._values)
-        elif rows >= self.tc5_min_rows and self._tc5.supported(rows):
+        x, zf = self._obs_full.view(rows, -1), m.z_stats                # MLP: the head z-filters the records in place
+        if self.chain is not None:
+            # the stems' input rows of this batch, then all B*(n+1) rows through the stems, the LSTM from the window's
+            # initial cells (ppo.py:376-387)
+            self.chain.gather()
+            if self.rnn:
+                rows_zfilter(self._actions, A, n * A, B, self.eff_len, A, None, 0.0, self._act_it)
+                rows_zfilter(self._pds, 2 * A, n * 2 * A, B, self.eff_len, 2 * A, None, 0.0, self._pd_it)
+            x, zf = self.chain.critic_features(self._cells()), None
+        if m.rnn_stem is None and rows >= self.tc5_min_rows and self._tc5.supported(rows):
             # Hopper path: wgmma tiles, accumulators in registers, weights streamed by the TMA engine
-            self._tc5(self._obs_full.view(rows, -1), self._values.view(rows, 1), zf_stats=m.z_stats, zf_eps=m.z_eps)
-        elif self.dual_critic and rows >= 32768:
-            ops.mlp_forward_dual(m.critic, self._obs_full.view(rows, -1), zf_stats=m.z_stats, zf_eps=m.z_eps,
-                                 out=self._values.view(rows, 1))
+            self._tc5(x, self._values.view(rows, 1), zf_stats=zf, zf_eps=m.z_eps)
         else:
-            ops.mlp_forward(m.critic, self._obs_full.view(rows, -1), zf_stats=m.z_stats, zf_eps=m.z_eps,
-                            out=self._values)
+            ops.mlp_forward(m.critic, x, zf_stats=zf, zf_eps=m.z_eps, out=self._values)
         self._prof_end('critic_pass', ev)
         rewards, scale = self._rewards, self.reward_scale
         if self.use_r_filter:
@@ -404,52 +361,32 @@ class PPOLearner(Learner):
         self._prof_end('gae', ev)
         return self._adv, self._ret
 
-    # -- RNN mode helpers ---------------------------------------------------------------------------------
     def _cells(self):
-        """(h0, c0, ld): per layer, the LSTM cells at the first step of every window; they ride in row 0 of the observation
-        records (utils.rnn_cell_layout; the reference ships them as onetime_infos, ppo_agent.py:133-137, ppo.py:507-510)."""
+        """(h0, c0, ld) in RNN mode, else None: per layer, the LSTM cells at the first step of every window; they ride in
+        row 0 of the observation records (utils.rnn_cell_layout; the reference ships them as onetime_infos,
+        ppo_agent.py:133-137, ppo.py:507-510)."""
         cl, row0 = self.cell_layout, self._obs_full[:, 0]
+        if cl is None:
+            return None
         return ([cl.h(row0, k) for k in range(cl.layers)], [cl.c(row0, k) for k in range(cl.layers)],
                 self._obs_full.stride(0))
 
-    def _rnn_prepare(self):
-        """Once per learn(): contiguous, z-filtered sequence rows -- all n+1 steps for the critic pass, the first eff_len
-        for the updates (through the learner's AND the reference model's filter, ppo.py:507-539) -- and the step slices of
-        actions / behaviour policy the updates iterate on.  Pixel input: the same two gathers, unfiltered, give the dense
-        uint8 frames of the CNN stem (a float load / store copies the bits of any word, denormal and NaN patterns too)."""
-        from ..model.lstm_stem import rows_zfilter
-        B, n, A, E, od, Dp = self.batch_size, self.n_step, self.action_dim, self.eff_len, self.obs_dim, self.low_dim
-        m, ref = self.model, self.ref_target_model
-        o = self._obs_full
-        rows_zfilter(o, Dp, (n + 1) * Dp, B, n + 1, od, m.z_stats, m.z_eps, self._xf_all)
-        rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, m.z_stats, m.z_eps, self._xf_eff)
-        if not self.pixel:
-            rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, ref.z_stats, ref.z_eps, self._xf_ref)
-            rows_zfilter(o, Dp, (n + 1) * Dp, B, E, od, None, 0.0, self._xraw_eff)
-        rows_zfilter(self._actions, A, n * A, B, E, A, None, 0.0, self._act_it)
-        rows_zfilter(self._pds, 2 * A, n * 2 * A, B, E, 2 * A, None, 0.0, self._pd_it)
+    def _head_forward(self, tr, chain_tr):
+        """One optimiser's head on the update rows: through its stems, or -- MLP mode -- straight from the records, step 0
+        of every window z-filtered inside the head."""
+        if chain_tr is not None:
+            return tr.forward(chain_tr.forward(self._cells()))
+        m = self.model
+        return tr.forward(self._obs_full, zf_stats=m.z_stats, zf_eps=m.z_eps, rows=self.batch_size,
+                          ldx=(self.n_step + 1) * self.low_dim)
 
-    def _frames(self, rows):
-        """The gathered frame rows [R, od] as the uint8 [R, C, H, W] frames the CNN stem reads."""
-        return rows.view(torch.uint8).view(rows.shape[0], *stem_shape(self.model.cnn_stem))
-
-    def _rnn_forward(self, rnn_tr, stem_tr):
-        """Training forward of one optimiser through its stem trainers on the eff_len update steps: the LSTM's top-layer
-        output [B*eff_len, H], the CNN stem in front of it with pixel input."""
-        x = stem_tr.forward(self._frames(self._xf_eff)) if self.pixel else self._xf_eff
-        return rnn_tr.forward(x, *self._cells())
-
-    def _rnn_backward(self, head_tr, rnn_tr, stem_tr, grad, norm_out, stop=None):
-        """BPTT of the LSTM stem from the head's input gradient, then -- pixel input -- the CNN stem's backward from the
-        LSTM's input gradient masked by relu'(features), and ONE joint step over [head | CNN | LSTM]."""
-        from ..model.cnn_stem import joint_step
-        rnn_tr.backward(head_tr.dx0)
-        if self.pixel:
-            rnn_tr.backward_input(stem_tr.d_fc, stem_tr.bufs['feat'])
-            stem_tr.backward(stem_tr.d_fc)
-            joint_step(head_tr, [stem_tr, rnn_tr], grad, norm_out=norm_out, stop_flag=stop)
+    @staticmethod
+    def _step(tr, chain_tr, norm_out, stop=None):
+        """The optimiser step after the head's backward: head alone, or head + stems as one joint step."""
+        if chain_tr is not None:
+            chain_tr.step(norm_out, stop)
         else:
-            joint_step(head_tr, rnn_tr, grad, norm_out=norm_out, stop_flag=stop)
+            tr.step(norm_out=norm_out, stop_flag=stop)
 
     # -- live kernel timing for bench.py's roofline (CUDA events on the launching stream) ---------------
     def _prof_begin(self):
@@ -480,17 +417,10 @@ class PPOLearner(Learner):
         inputs and parameters as the NEXT epoch's training forward, so it is done once, with saved activations:
         ``fresh=False`` reuses it."""
         L = _lib.lib()
-        B, n, A, D = self.batch_size, self.n_step, self.action_dim, self.low_dim
+        A, M = self.action_dim, self._rows
         m, tr, st = self.model, self.actor_optim, ops._stream()
-        M = self._rows
-        acts, lda, pds, ldp = (self._act_it, A, self._pd_it, 2 * A) if self.rnn else (self._actions, n * A, self._pds, n * 2 * A)
-        if self.rnn:
-            mean = tr.forward(self._rnn_forward(self.actor_rnn, getattr(self, 'actor_stem', None))) if fresh else tr.out
-        elif self.pixel:
-            mean = tr.forward(self.actor_stem.forward(self._frames0)) if fresh else tr.out
-        else:
-            mean = tr.forward(self._obs_full, zf_stats=m.z_stats, zf_eps=m.z_eps, rows=B, ldx=(n + 1) * D) if fresh \
-                else tr.out
+        acts, lda, pds, ldp = self._upd
+        mean = self._head_forward(tr, self._actor_chain) if fresh else tr.out
         mode = 0 if self.ppo_mode == 'clip' else 1
         if mode == 1:
             self._kl(mean, S['KL_PRE'], 0.0, stop)
@@ -501,19 +431,9 @@ class PPOLearner(Learner):
                                           tr.d[-1].stride(0), _ptr(dlog_var), _ptr(self._stats), _ptr(self._loss_ws),
                                           _ptr(stop), st), 'sb200_ppo_policy_loss_f32')
         tr.backward()
-        if self.rnn:
-            stem_tr = getattr(self, 'actor_stem', None)
-            self._rnn_backward(tr, self.actor_rnn, stem_tr, self._g_actor, self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop)
-            self._cur_mean = tr.forward(self._rnn_forward(self.actor_rnn, stem_tr))
-        elif self.pixel:
-            from ..model.cnn_stem import joint_step
-            self.actor_stem.backward(tr.dx0)
-            joint_step(tr, self.actor_stem, self._g_actor, norm_out=self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop_flag=stop)
-            self._cur_mean = tr.forward(self.actor_stem.forward(self._frames0))
-        else:
-            tr.step(norm_out=self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop_flag=stop)
-            # post-step KL(ref || current) (ppo.py:553-556)
-            self._cur_mean = tr.forward(self._obs_full, zf_stats=m.z_stats, zf_eps=m.z_eps, rows=B, ldx=(n + 1) * D)
+        self._step(tr, self._actor_chain, self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop)
+        # post-step KL(ref || current) (ppo.py:553-556)
+        self._cur_mean = self._head_forward(tr, self._actor_chain)
         self._kl(self._cur_mean, S['KL_POST'], 4.0 * self.kl_target, self._stop)
 
     def _kl(self, mean, slot, threshold, stop):
@@ -539,7 +459,7 @@ class PPOLearner(Learner):
             raise NotImplementedError('reward filter + data parallel')
         if self.rnn:
             raise NotImplementedError('RNN mode + data parallel')
-        stem_n = self.model.cnn_stem.size if self.pixel else 0
+        stem_n = self.chain.size if self.chain is not None else 0
         peer_floats = max(self.model.actor.size, self.model.critic.size) + stem_n + 64
         self.dp = LearnerDP(group, peer_floats=peer_floats)
         # the value branch gets its OWN communicator: with the policy || value fork both branches issue collectives
@@ -579,40 +499,20 @@ class PPOLearner(Learner):
 
     def _value_epoch(self):
         L = _lib.lib()
-        B, n, D = self.batch_size, self.n_step, self.low_dim
-        m, tr, st = self.model, self.critic_optim, ops._stream()
-        if self.rnn:
-            v = tr.forward(self._rnn_forward(self.critic_rnn, getattr(self, 'critic_stem', None)))
-        elif self.pixel:
-            v = tr.forward(self.critic_stem.forward(self._frames0))
-        else:
-            v = tr.forward(self._obs_full, zf_stats=m.z_stats, zf_eps=m.z_eps, rows=B, ldx=(n + 1) * D)
+        tr, st = self.critic_optim, ops._stream()
+        v = self._head_forward(tr, self._critic_chain)
         check(L.sb200_value_loss_f32(_ptr(v), v.stride(0), _ptr(self._ret), self._rows, _ptr(tr.d[-1]), tr.d[-1].stride(0),
                                      _ptr(self._stats), _ptr(self._loss_ws_v), st), 'sb200_value_loss_f32')
         tr.backward()
-        if self.rnn:
-            self._rnn_backward(tr, self.critic_rnn, getattr(self, 'critic_stem', None), self._g_critic,
-                               self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
-        elif self.pixel:
-            from ..model.cnn_stem import joint_step
-            self.critic_stem.backward(tr.dx0)
-            joint_step(tr, self.critic_stem, self._g_critic, norm_out=self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
-        else:
-            tr.step(norm_out=self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
+        self._step(tr, self._critic_chain, self._stats[S['GN_CRITIC']:S['GN_CRITIC'] + 1])
 
     def _optimize_head(self):
         B, n, A, D = self.batch_size, self.n_step, self.action_dim, self.low_dim
         ref = self.ref_target_model
         self._gae_and_return()
-        if self.rnn:
-            x_ref = ref.cnn_stem.forward(self._frames(self._xf_eff), self._ref_stem_bufs) if self.pixel else self._xf_ref
-            h_ref = ref.rnn_stem.forward(x_ref, *self._cells(), B, self.eff_len, self._rnn_ref)
-            ops.mlp_forward(ref.actor, h_ref, out=self._ref_mean)
-        elif self.pixel:
-            # step-0 frames of every window, contiguous (ppo.py:527-537), then the reference policy on them
-            fr = self._obs_full.view(torch.uint8).view(B, n + 1, -1)
-            self._frames0.view(B, -1).copy_(fr[:, 0])
-            ops.mlp_forward(ref.actor, ref.cnn_stem.forward(self._frames0, self._ref_stem_bufs), out=self._ref_mean)
+        # the reference policy on the update rows (ppo.py:527-537)
+        if self.chain is not None:
+            ops.mlp_forward(ref.actor, self.chain.ref_features(self._cells()), out=self._ref_mean)
         else:
             ops.mlp_forward(ref.actor, self._obs_full, zf_stats=ref.z_stats, zf_eps=ref.z_eps, rows=B, ldx=(n + 1) * D,
                             out=self._ref_mean)
@@ -627,7 +527,7 @@ class PPOLearner(Learner):
         if not value_done:
             for _ in range(self.epoch_baseline):
                 self._value_epoch()
-        acts, lda, pds, ldp = (self._act_it, A, self._pd_it, 2 * A) if self.rnn else (self._actions, n * A, self._pds, n * 2 * A)
+        acts, lda, pds, ldp = self._upd
         check(L.sb200_ppo_final_stats_f32(_ptr(self._cur_mean), self._cur_mean.stride(0), _ptr(m.log_var),
                                           _ptr(acts), lda, _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, self._rows, A,
                                           _ptr(self._stats), _ptr(self._loss_ws), st), 'sb200_ppo_final_stats_f32')
@@ -635,6 +535,7 @@ class PPOLearner(Learner):
             # the rows the updates trained on (step 0 of every window; the first eff_len steps in RNN mode), AFTER the
             # updates (ppo.py:578)
             if self.rnn:
+                rows_zfilter(self._obs_full, D, (n + 1) * D, B, self.eff_len, self.obs_dim, None, 0.0, self._xraw_eff)
                 ops.zfilter_update(self._xraw_eff, self._rows, self.obs_dim, self._xraw_eff.stride(0), m.z_stats)
             elif self.dp is None:
                 ops.zfilter_update(self._obs_full, B, D, (n + 1) * D, m.z_stats)
@@ -860,10 +761,8 @@ class PPOLearner(Learner):
         ck = self.session_config.checkpoint.learner
         if 'include_optimizer' in ck and ck.include_optimizer:
             attrs += ['actor_optim', 'critic_optim', 'adapt_state']
-            if self.pixel:                                        # each optimiser's Adam moments over the shared CNN stem
-                attrs += ['actor_stem', 'critic_stem']
-            if self.rnn:                                          # ... and over the shared LSTM stem
-                attrs += ['actor_rnn', 'critic_rnn']
+            # each optimiser's Adam moments over the shared CNN and LSTM stems
+            attrs += [a for a in ('actor_stem', 'critic_stem', 'actor_rnn', 'critic_rnn') if getattr(self, a, None) is not None]
         return attrs
 
     @property

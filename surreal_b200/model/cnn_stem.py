@@ -159,18 +159,17 @@ class StemTrainer:
 def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None):
     """One optimiser step over a head network (ops.MlpTrainer) AND the shared stems: the reference clips the global norm
     of head + stem parameters together (get_actor_params / get_critic_params chain actor, cnn_stem and rnn_stem,
-    ppo_net.py:202-224; ppo.py:244-246,349-351) and steps ONE Adam over all of them.  ``stem_trs`` is one stem trainer
-    (StemTrainer / lstm_stem.RnnTrainer) or a list of them; ``grad`` = [head gradient | stem gradients in that order] is
+    ppo_net.py:202-224; ppo.py:244-246,349-351) and steps ONE Adam over all of them.  ``stem_trs`` is the list of stem
+    trainers (StemTrainer / lstm_stem.RnnTrainer); ``grad`` = [head gradient | stem gradients in that order] is
     one contiguous buffer so that the norm (and a data-parallel all-reduce) sees everything at once; head.ws carries the
     shared step count / norm."""
     L, st = _lib.lib(), ops._stream()
-    trs = stem_trs if isinstance(stem_trs, (list, tuple)) else [stem_trs]
     nh = head.net.size
     segs, o = [(head.net.params, grad[:nh], head.exp_avg, head.exp_avg_sq, nh, norm_out)], nh
     sf = C.c_void_p(stop_flag.data_ptr()) if stop_flag is not None else None
     check(L.sb200_grad_reduce_norm_f32(_p(head.slabs), nh, head.splits, _p(grad[:nh]), nh, 1.0, 0, _p(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(head)')
-    for tr in trs:
+    for tr in stem_trs:
         ns = tr.stem.size
         gs = grad[o:o + ns]
         check(L.sb200_grad_reduce_norm_f32(_p(tr.slabs), ns, tr.splits, _p(gs), ns, 1.0, 0, _p(head.ws), sf, st),

@@ -61,6 +61,8 @@ class PPOModel:
                 raise ConfigError('algo.rnn.rnn_layer must be at least 1, got %d' % int(rnn_config.rnn_layer))
             self.rnn_stem = LSTMStem(in_dim, rnn_config.rnn_hidden, self.device, layers=rnn_config.rnn_layer)
             in_dim = rnn_config.rnn_hidden
+        # the stems between an observation and the heads, in order: [], [cnn], [lstm] or [cnn, lstm]
+        self.stems = [s for s in (self.cnn_stem, self.rnn_stem) if s is not None]
         D, A = in_dim, action_dim
         ah, ch = list(model_config.actor_fc_hidden_sizes), list(model_config.critic_fc_hidden_sizes)
         R, T, N = ops.ACT_RELU, ops.ACT_TANH, ops.ACT_NONE
@@ -170,8 +172,14 @@ class PPOModel:
             self._stem_bufs, self._stem_bufs_rows = self.cnn_stem.buffers(rows), rows
         return self.cnn_stem.forward(fr, self._stem_bufs)
 
+    def _no_rnn(self):
+        if self.rnn_stem is not None:
+            raise NotImplementedError('PPOModel.forward_actor / forward_critic run feed-forward models only; an RNN policy '
+                                      'acts through PPOAgent.act and trains through PPOLearner')
+
     def forward_actor(self, obs, cells=None, out_pd=None):
         """-> [rows, 2A] = cat(mean, std) (builders.py:114-132)."""
+        self._no_rnn()
         if self.cnn_stem is not None:
             x2 = self._features(obs)
             mean = ops.mlp_forward(self.actor, x2)
@@ -188,6 +196,7 @@ class PPOModel:
         return pd
 
     def forward_critic(self, obs, cells=None):
+        self._no_rnn()
         if self.cnn_stem is not None:
             return ops.mlp_forward(self.critic, self._features(obs))
         x = self._flat(obs)

@@ -280,6 +280,22 @@ def test_ppo_agent_act_rnn_matches_reference(golden):
         np.testing.assert_allclose(a, g['actions'][i], rtol=0, atol=5e-6)
 
 
+@pytest.mark.parametrize('D', [5, 40])
+def test_ppo_model_forward_refuses_rnn(D):
+    """PPOModel.forward_actor / forward_critic have no cells to run an LSTM stem from: an RNN model raises instead of
+    applying the heads to raw observations, whether the observation is narrower than rnn_hidden (16) or not."""
+    from surreal_b200.model.ppo_net import PPOModel
+    cfg = dict(D=D, A=3, actor_h=[32, 24], critic_h=[28, 20], n_step=4, B=4, mode='clip', lr=1e-4, exp_interval=64, horizon=2,
+               rnn_hidden=16, rnn_layer=1)
+    lc, ec, sc = _rnn_cfg(cfg)
+    m = PPOModel(ec.obs_spec, 3, lc.model, use_z_filter=lc.algo.use_z_filter, rnn_config=lc.algo.rnn, device=DEV)
+    obs = torch.randn(8, D, device=DEV)
+    with pytest.raises(NotImplementedError):
+        m.forward_actor(obs)
+    with pytest.raises(NotImplementedError):
+        m.forward_critic(obs)
+
+
 ACT_BAR = 2e-6        # one step from the agent's own cells: pd, action and the new cells, max |err|; measured 2.6e-7
 DRIFT_BAR = 1.5e-6    # free-running float64 trajectory against the agent's cells over 40 steps, max |err|; measured 1.6e-7
 
