@@ -47,7 +47,7 @@ def box_muller(a, b):
 
 def agent_eps(agent_seed, step, actor_ids, A):
     """N(0,1) draws of PPOAgent.act at global step `step` for actors `actor_ids` -> [len(ids), A] float32
-    (rollout.cu: sample_one -- key = agent seed, counter = (step, actor << 16 | j // 4))."""
+    (common.cuh: action_noise4 -- key = agent seed, counter = (step, actor << 16 | j // 4))."""
     ids = np.asarray(actor_ids, dtype=np.uint64)[:, None]
     grp = np.arange((A + 3) // 4, dtype=np.uint64)[None, :]
     x, y, z, w = philox4x32_10(np.uint64(agent_seed), np.uint64(step), (ids << np.uint64(16)) | grp)

@@ -102,6 +102,36 @@ __device__ __forceinline__ float4 ld_stream4(const float* p) {   // read-once da
     return r;
 }
 
+__device__ __forceinline__ float apply_act(float v, int act) {
+    if (act == SB200_ACT_RELU) return fmaxf(v, 0.0f);
+    if (act == SB200_ACT_TANH) return tanhf(v);
+    return v;
+}
+
+// 3xTF32 split: x = hi + lo with hi = tf32(x), lo = tf32(x - hi); a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (fp32 accumulate)
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
+    const float r = x - __uint_as_float(hi);
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
+}
+
+// shared-memory address of a generic pointer into shared memory, and (distributed shared memory) the address of CTA
+// `rank`'s copy of a local shared-memory location
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+
+// mbarrier in shared memory: initialise with an arrival count; arrive once and expect `bytes` of transactions this phase
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+
 // Philox4x32-10 counter-based generator (Salmon et al. 2011), written from the published round
 // function; one call yields 4 x 32 random bits for (key, counter).
 struct Philox4 { unsigned int x, y, z, w; };
@@ -129,4 +159,26 @@ __device__ __forceinline__ float2 box_muller(unsigned int a, unsigned int b) {
     float s, c;
     sincosf(6.283185307179586f * u2, &s, &c);
     return make_float2(rad * c, rad * s);
+}
+
+// Action-noise stream (PPO sampling, DDPG Gaussian / OU exploration and target smoothing): the N(0,1) draws of action
+// dims [4 quad, 4 quad + 4) of batch row `row` at step counter `ctr`, keyed by (seed, ctr, row << 16 | quad).
+__device__ __forceinline__ float4 action_noise4(unsigned long long seed, unsigned long long ctr, unsigned long long row,
+                                                int quad) {
+    const Philox4 r = philox4x32_10(seed, ctr, (row << 16) | (unsigned long long)quad);
+    const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
+    return make_float4(a.x, a.y, b.x, b.y);
+}
+// the draw of action dim j alone
+__device__ __forceinline__ float action_noise1(unsigned long long seed, unsigned long long ctr, unsigned long long row, int j) {
+    const float4 z = action_noise4(seed, ctr, row, j >> 2);
+    const int c = j & 3;
+    return (c == 0) ? z.x : (c == 1) ? z.y : (c == 2) ? z.z : z.w;
+}
+
+// Env-noise stream of the synthetic environment: the random words of feature d of actor `actor` at step counter `ctr`.
+// box_muller(.x, .y) is the transition noise (its .y the reward noise at d == 0), box_muller(.z, .w).x the reset state.
+__device__ __forceinline__ Philox4 env_noise(unsigned long long env_seed, unsigned long long ctr, unsigned long long actor,
+                                             int d) {
+    return philox4x32_10(env_seed ^ 0x5851F42D4C957F2Dull, ctr, (actor << 20) | (unsigned long long)d);
 }

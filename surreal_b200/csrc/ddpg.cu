@@ -170,10 +170,7 @@ __global__ void __launch_bounds__(256) ddpg_smooth_action_kernel(const float* __
         e = unit_noise[idx];
     } else {
         const unsigned long long ctr = (step_ctr != nullptr) ? *step_ctr : 0ull;
-        const Philox4 r = philox4x32_10(seed, ctr, ((unsigned long long)b << 16) | (unsigned long long)(j >> 2));
-        const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
-        const int c = j & 3;
-        e = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
+        e = action_noise1(seed, ctr, b, j);
     }
     const float nz = fminf(fmaxf(__fmul_rn(e, policy_noise), -noise_clip), noise_clip);
     out[(long long)b * ldo + j] = fminf(fmaxf(__fadd_rn(pi[(long long)b * ldp + j], nz), -1.0f), 1.0f);

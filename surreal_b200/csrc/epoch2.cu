@@ -21,7 +21,7 @@
 //   P4  clip by global norm + Adam (torch's arithmetic, optim_dev.cuh), W2^T refresh    -> barrier
 // Everything is deterministic (static work assignment, fixed-order sums).  Buffers rewritten by other CTAs between
 // barriers are read with ld.global.cg only.  Data-parallel exchanges (KL scalar, flat gradients) happen inside the
-// kernel over NVLink peer memory with the protocol of peer_allreduce.cu.
+// kernel over NVLink peer memory with the protocol of peer_allreduce.cu (peer_dev.cuh).
 #include <math.h>
 #include <stddef.h>
 
@@ -30,10 +30,12 @@
 #include "common.cuh"
 #include "gemm_tiles.cuh"
 #include "optim_dev.cuh"
+#include "peer_dev.cuh"
 #include "ppo_loss_dev.cuh"
 
 namespace {
 
+using namespace peer_dev;
 using optim_dev::OptWs;
 
 constexpr int E2T = 512;              // threads per CTA (16 warps: the phases are latency-bound, 8 warps hid too little)
@@ -42,49 +44,6 @@ constexpr int RB = 16;                // rows per block
 constexpr int E2_MAX_OUT = 32;
 constexpr int E2_SLOTS = 4 + E2_MAX_OUT;
 constexpr int E2_MAX_G = 192;
-
-// ---- peer exchange (same layout as peer_allreduce.cu)
-constexpr int PAR_MAX_WORLD = 8;
-constexpr int PAR_MAX_CTAS = 16;
-struct ParHeader {
-    unsigned int flags[PAR_MAX_WORLD * PAR_MAX_CTAS];
-    unsigned int counter;
-    unsigned int ticket;
-    unsigned int pad[2];
-    double partial[PAR_MAX_CTAS];
-};
-struct ParCtx {
-    void* peers[PAR_MAX_WORLD];
-    int world;
-    int rank;
-    long long max_floats;
-};
-__device__ __forceinline__ float* slot_of(void* base, long long max_floats, unsigned int parity) {
-    return reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(base) + sizeof(ParHeader)) + (size_t)parity * (size_t)max_floats;
-}
-__device__ __forceinline__ void st_release_sys(unsigned int* p, unsigned int v) {
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned int ld_acquire_sys(const unsigned int* p) {
-    unsigned int v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ float ld_sys1(const float* p) {
-    float r;
-    asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(r) : "l"(p) : "memory");
-    return r;
-}
-__device__ __forceinline__ float4 ld_sys4(const float* p) {
-    float4 r;
-    asm volatile("ld.relaxed.sys.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
-    return r;
-}
-__device__ __forceinline__ double ld_sys_f64(const double* p) {
-    double r;
-    asm volatile("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(r) : "l"(p) : "memory");
-    return r;
-}
 
 struct Job {                          // one optimiser
     float* params;
@@ -124,7 +83,7 @@ struct Job {                          // one optimiser
     int n_rb;                         // row blocks
     int s;                            // row splits of the weight-gradient phase (slabs used)
     int rps;                          // rows per split
-    ParCtx par;
+    sb200_par par;                    // world 1 (and no peers) when the job does not exchange
 };
 
 struct E2Params {
@@ -148,7 +107,7 @@ __device__ __forceinline__ double peer_sum_slice(const Job& p, long long lo, lon
     double sq = 0.0;
     const float* slot[W];
 #pragma unroll
-    for (int q = 0; q < W; ++q) slot[q] = slot_of(p.par.peers[min(q, p.par.world - 1)], p.par.max_floats, parity);
+    for (int q = 0; q < W; ++q) slot[q] = slot_of(p.par, min(q, p.par.world - 1), parity);
     for (long long base = lo + (long long)threadIdx.x * 4; base < hi; base += (long long)E2T * 4 * CH) {
         float4 v[CH][W];
 #pragma unroll
@@ -769,7 +728,7 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
         const Job& p = P.job[j];
         step0[j] = p.opt->step;
         if (p.stop != nullptr && *p.stop) left[j] = true;      // raised only behind a barrier every CTA has passed: uniform
-        if (p.par.world > 1) par_k[j] = reinterpret_cast<ParHeader*>(p.par.peers[p.par.rank])->counter;
+        if (p.par.world > 1) par_k[j] = header_of(p.par, p.par.rank)->counter;
         const int last = (p.mode != 2) ? p.epochs : p.epochs - 1;
         e_max = max(e_max, last);
     }
@@ -830,25 +789,19 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
                 klm[j] = (double)(float)(acc * (1.0 / (double)p.M));           // .mean() in fp32 (kl_kernel)
             }
             if (p.par.world > 1) {                                             // average the scalar over ranks (CTA 0)
-                ParHeader* par_me = reinterpret_cast<ParHeader*>(p.par.peers[p.par.rank]);
+                ParHeader* par_me = header_of(p.par, p.par.rank);
                 if (c == 0) {
                     const unsigned int k = par_k[j] + 1u;
-                    double* mine = reinterpret_cast<double*>(slot_of(p.par.peers[p.par.rank], p.par.max_floats, k & 1u));
+                    double* mine = reinterpret_cast<double*>(slot_of(p.par, p.par.rank, k & 1u));
                     if (tid == 0) {
                         *mine = klm[j];
                         __threadfence_system();
                     }
-                    __syncthreads();
-                    if (tid < p.par.world && tid != p.par.rank) {
-                        st_release_sys(&reinterpret_cast<ParHeader*>(p.par.peers[tid])->flags[p.par.rank * PAR_MAX_CTAS], k);
-                        const unsigned int* f = &par_me->flags[tid * PAR_MAX_CTAS];
-                        while ((int)(ld_acquire_sys(f) - k) < 0) { }
-                    }
-                    __syncthreads();
+                    publish_and_wait(p.par, par_me, 0, k);
                     if (tid == 0) {
                         double a = 0.0;
                         for (int q = 0; q < p.par.world; ++q)
-                            a += ld_sys_f64(reinterpret_cast<const double*>(slot_of(p.par.peers[q], p.par.max_floats, k & 1u)));
+                            a += ld_sys_f64(reinterpret_cast<const double*>(slot_of(p.par, q, k & 1u)));
                         *p.kl_global = (double)(float)(a * (1.0 / (double)p.par.world));
                     }
                 }
@@ -1014,30 +967,24 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
                     par_k[j] += 1u;
                     const int cl = c - j * PG;                                 // this job's slice owners: CTAs [j PG, (j+1) PG)
                     if (cl < 0 || cl >= PG) continue;                          // block-uniform
-                    ParHeader* par_me = reinterpret_cast<ParHeader*>(p.par.peers[p.par.rank]);
+                    ParHeader* par_me = header_of(p.par, p.par.rank);
                     double sq = 0.0;
                     long long per = (p.n_params + PG - 1) / PG;
                     per = (per + 3) & ~3ll;
                     const long long lo = (long long)cl * per;
                     const long long hi = (lo + per < p.n_params) ? lo + per : p.n_params;
-                    float* mine = slot_of(p.par.peers[p.par.rank], p.par.max_floats, k & 1u);
+                    float* mine = slot_of(p.par, p.par.rank, k & 1u);
                     for (long long i = lo + (long long)tid * 4; i < hi; i += (long long)E2T * 4)
                         *reinterpret_cast<float4*>(mine + i) = gt::ldcg4(p.grad + i);
                     __threadfence_system();
-                    __syncthreads();
-                    if (tid < p.par.world && tid != p.par.rank) {
-                        st_release_sys(&reinterpret_cast<ParHeader*>(p.par.peers[tid])->flags[p.par.rank * PAR_MAX_CTAS + cl], k);
-                        const unsigned int* f = &par_me->flags[tid * PAR_MAX_CTAS + cl];
-                        while ((int)(ld_acquire_sys(f) - k) < 0) { }
-                    }
-                    __syncthreads();
+                    publish_and_wait(p.par, par_me, cl, k);
                     const float scale = 1.0f / (float)p.par.world;
                     if ((p.par.max_floats & 3) == 0) {
                         sq = peer_sum_slice<PAR_MAX_WORLD, 1>(p, lo, hi, k & 1u, scale);      // one path for every world size
                     } else {
                         for (long long i = lo + tid; i < hi; i += E2T) {
                             float a = 0.f;
-                            for (int q = 0; q < p.par.world; ++q) a += ld_sys1(slot_of(p.par.peers[q], p.par.max_floats, k & 1u) + i);
+                            for (int q = 0; q < p.par.world; ++q) a += ld_sys1(slot_of(p.par, q, k & 1u) + i);
                             a = __fmul_rn(a, scale);
                             p.grad[i] = a;
                             sq += (double)a * (double)a;
@@ -1101,7 +1048,7 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
     }
     if (c == 0 && tid == 0)
         for (int j = 0; j < NJ; ++j)
-            if (P.job[j].par.world > 1) reinterpret_cast<ParHeader*>(P.job[j].par.peers[P.job[j].par.rank])->counter = par_k[j];
+            if (P.job[j].par.world > 1) header_of(P.job[j].par, P.job[j].par.rank)->counter = par_k[j];
 }
 
 bool e2_net_ok(const sb200_mlp* net) {
@@ -1257,16 +1204,11 @@ int e2_fill_job(const sb200_epochs* a, Job* p, unsigned char* ws, const WsLayout
         SB200_REQUIRE(a->lda >= p->NO && a->ldb >= 2 * p->NO && a->ldr >= 2 * p->NO);
         SB200_REQUIRE(a->extra_off >= 0 && a->extra_off + p->NO <= a->n_params);
     }
-    for (int q = 0; q < PAR_MAX_WORLD; ++q) p->par.peers[q] = nullptr;
-    p->par.world = 1; p->par.rank = 0; p->par.max_floats = 0;
+    p->par = sb200_par{};
+    p->par.world = 1;
     if (a->par != nullptr && a->par->world > 1) {
-        SB200_REQUIRE(a->par->world <= PAR_MAX_WORLD && a->par->rank >= 0 && a->par->rank < a->par->world);
-        SB200_REQUIRE(a->n_params <= a->par->max_floats);
-        for (int q = 0; q < a->par->world; ++q) {
-            SB200_REQUIRE(a->par->peers[q] != nullptr);
-            p->par.peers[q] = a->par->peers[q];
-        }
-        p->par.world = a->par->world; p->par.rank = a->par->rank; p->par.max_floats = a->par->max_floats;
+        if (const int e = sb200_par_check(a->par, a->n_params)) return e;
+        p->par = *a->par;
     }
     return SB200_OK;
 }

@@ -53,12 +53,6 @@ struct FwdParams {
 
 __host__ __device__ inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
-__device__ __forceinline__ float apply_act(float v, int act) {
-    if (act == SB200_ACT_RELU) return fmaxf(v, 0.0f);
-    if (act == SB200_ACT_TANH) return tanhf(v);
-    return v;
-}
-
 // LayerNorm epilogue of layer l on the tile's `rows` activation rows H[m][0, N) in shared memory, in place, a warp per
 // row: two-pass mean / biased variance (exact for all-zero rows: y == b), y = fma((h - mean) * rstd, g, b).  Runs after
 // the layer's barrier and before the next layer reads H; columns >= N are not touched.  Not inlined: the GEMM loops

@@ -1,7 +1,7 @@
 // Tensor-core variant of the fused MLP forward: warp-level mma.sync m16n8k8 TF32 with the 3xTF32
 // error-compensated split (x = hi + lo, hi = tf32(x), lo = tf32(x - hi);  A.B ~= A_lo.B_hi + A_hi.B_lo + A_hi.B_hi,
 // fp32 accumulate), which restores fp32-level accuracy (~1e-6 relative) -- plain TF32 (~1e-3) would miss the 1e-5
-// parity bar.  Included by mlp_fwd.cu (shares FwdParams / apply_act / round_up).
+// parity bar.  Included by mlp_fwd.cu (shares FwdParams / round_up).
 //
 // Why mma.sync and not wgmma here: these are skinny problems.  One env step of all actors is 1024 rows, a learner
 // minibatch 1024-4096 rows; a wgmma tile is 64 rows per warpgroup fed through an mbarrier pipeline, which would leave
@@ -18,12 +18,6 @@
 namespace {
 
 constexpr int MMA_D = 3;     // register stages of B fragments in flight (8 k-rows each)
-
-__device__ __forceinline__ void split_tf32(float x, unsigned& hi, unsigned& lo) {
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
-    const float r = x - __uint_as_float(hi);
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
-}
 
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const unsigned (&a)[4], unsigned b0, unsigned b1) {
     asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"

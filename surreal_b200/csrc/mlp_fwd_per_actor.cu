@@ -31,12 +31,6 @@ struct PaLayout {
     float ln_eps;
 };
 
-__device__ __forceinline__ float apply_act(float v, int act) {
-    if (act == SB200_ACT_RELU) return fmaxf(v, 0.0f);
-    if (act == SB200_ACT_TANH) return tanhf(v);
-    return v;
-}
-
 // One Linear + activation of one row: hout[0:N) = act(hin[0:K) @ W + b).  W / b point into the row's image.
 __device__ __forceinline__ void layer_row(const float* __restrict__ W, const float* __restrict__ b, int K, int N,
                                           int ldw, int act, const float* hin, float* hout, float* part) {

@@ -46,13 +46,7 @@ __device__ __forceinline__ void mma_tf32u(float (&d)[4], const uint4& a, unsigne
                  : "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b0), "r"(b1));
 }
 
-// distributed shared memory: address of CTA `rank`'s copy of a local shared-memory location, and a store to it
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned mapa_u32(unsigned addr, unsigned rank) {
-    unsigned r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
+// distributed shared memory: a store to a cluster address (mapa_u32)
 __device__ __forceinline__ void st_cluster_v4(unsigned addr, const float4& v) {
     asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
                  : "memory");

@@ -7,19 +7,13 @@
 // fp32 results agree with the reference to rounding.  The step counter lives on the device so that the
 // whole update can be replayed from a CUDA graph.
 #include "common.cuh"
+#include "optim_dev.cuh"
 
 namespace {
 
-constexpr int OT = 256;
-constexpr int MAX_BLOCKS = 1024;
+using optim_dev::OptWs;
 
-struct OptWs {
-    unsigned int counter;
-    int step;
-    float total_norm;
-    float pad;
-    double partial[MAX_BLOCKS];
-};
+constexpr int OT = 256;
 
 __global__ void __launch_bounds__(OT) grad_reduce_norm_kernel(const float* __restrict__ slabs, long long slab_stride,
                                                               int splits, float* __restrict__ grad, long long n,
@@ -37,14 +31,8 @@ __global__ void __launch_bounds__(OT) grad_reduce_norm_kernel(const float* __res
     }
     const double t = block_sum(sq, sh);
     if (threadIdx.x == 0) ws->partial[blockIdx.x] = t;
-    if (last_block_ticket(&ws->counter, gridDim.x)) {
-        if (threadIdx.x == 0) {
-            double acc = 0.0;
-            for (unsigned int k = 0; k < gridDim.x; ++k) acc += ws->partial[k];
-            ws->total_norm = (float)sqrt(acc);
-            if (bump_step) ws->step += 1;
-        }
-    }
+    if (last_block_ticket(&ws->counter, gridDim.x) && threadIdx.x == 0)
+        optim_dev::finish_norm(ws, ws->partial, gridDim.x, bump_step);
 }
 
 __global__ void __launch_bounds__(OT) clip_adam_kernel(float* __restrict__ p, const float* __restrict__ grad,
@@ -54,30 +42,12 @@ __global__ void __launch_bounds__(OT) clip_adam_kernel(float* __restrict__ p, co
                                                        double clip_value, const OptWs* __restrict__ ws,
                                                        float* __restrict__ norm_out, const int* __restrict__ stop) {
     if (stop != nullptr && *stop) return;
-    const int t = ws->step;
-    const double bc1 = 1.0 - pow(beta1, (double)t);
-    const double bc2 = 1.0 - pow(beta2, (double)t);
-    const float neg_step = (float)(-(lr_ptr[0] / bc1));
-    const float bc2_sqrt = (float)sqrt(bc2);
-    const float w1 = (float)(1.0 - beta1), b2 = (float)beta2, a2 = (float)(1.0 - beta2), epsf = (float)eps;
-    float coef = 1.0f;
-    if (clip_mode == 1) {
-        const float c = (float)clip_value / (ws->total_norm + 1e-6f);      // clip_grad_norm_
-        coef = fminf(c, 1.0f);
-    }
+    const optim_dev::AdamCoef c = optim_dev::adam_coef(ws->step, lr_ptr[0], beta1, beta2, eps, weight_decay, clip_mode,
+                                                       clip_value, ws->total_norm);
     if (norm_out != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *norm_out = ws->total_norm;
-    const float cv = (float)clip_value, wd = (float)weight_decay;
     for (long long i = (long long)blockIdx.x * OT + threadIdx.x; i < n; i += (long long)gridDim.x * OT) {
-        float g = grad[i];
-        if (clip_mode == 1) g = __fmul_rn(g, coef);
-        else if (clip_mode == 2) g = fminf(fmaxf(g, -cv), cv);
-        float pi = p[i];
-        if (wd != 0.0f) g = __fadd_rn(g, __fmul_rn(wd, pi));
-        float mi = m[i], vi = v[i];
-        mi = fmaf(w1, __fsub_rn(g, mi), mi);                                  // exp_avg.lerp_(grad, 1-beta1)
-        vi = __fadd_rn(__fmul_rn(vi, b2), __fmul_rn(__fmul_rn(a2, g), g));   // mul_(beta2).addcmul_(g, g, 1-beta2)
-        const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vi), bc2_sqrt), epsf);
-        pi = __fadd_rn(pi, __fdiv_rn(__fmul_rn(neg_step, mi), denom));      // addcdiv_(exp_avg, denom, -step_size)
+        float pi = p[i], mi = m[i], vi = v[i];
+        optim_dev::adam_apply(c, grad[i], pi, mi, vi);
         p[i] = pi;
         m[i] = mi;
         v[i] = vi;

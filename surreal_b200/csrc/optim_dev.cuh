@@ -7,13 +7,22 @@ namespace optim_dev {
 
 constexpr int MAX_BLOCKS = 1024;
 
-struct OptWs {
+struct OptWs {                           // sb200_optim_workspace_bytes() bytes
     unsigned int counter;
     int step;
     float total_norm;
     float pad;
     double partial[MAX_BLOCKS];
 };
+
+// The single thread that finishes a squared-norm reduction: total_norm = sqrt(sum of the n partials in order), and the
+// step bump of the Adam update that follows.
+__device__ __forceinline__ void finish_norm(OptWs* ws, const double* partial, unsigned int n, int bump_step) {
+    double acc = 0.0;
+    for (unsigned int k = 0; k < n; ++k) acc += partial[k];
+    ws->total_norm = (float)sqrt(acc);
+    if (bump_step) ws->step += 1;
+}
 
 struct AdamCoef {
     float neg_step, bc2_sqrt, w1, b2, a2, eps, coef, cv, wd;

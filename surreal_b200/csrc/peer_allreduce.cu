@@ -16,62 +16,20 @@
 // peer reads instead of an NCCL launch + ring/tree protocol (~30-40 us on this box for messages this small).
 // The call counter lives in device memory, so the launch can be captured in a CUDA graph and replayed.
 #include "common.cuh"
+#include "optim_dev.cuh"
+#include "peer_dev.cuh"
 #include <string.h>
 
 namespace {
 
-constexpr int PAR_MAX_WORLD = 8;
-constexpr int PAR_MAX_CTAS = 16;
+using namespace peer_dev;
+
 constexpr int PAR_T = 256;
 
-struct ParHeader {                       // at the start of every rank's symmetric buffer
-    unsigned int flags[PAR_MAX_WORLD * PAR_MAX_CTAS];   // flags[p * PAR_MAX_CTAS + b]: last call whose slice b rank p published
-    unsigned int counter;                // calls completed by THIS rank
-    unsigned int ticket;
-    unsigned int pad[2];
-    double partial[PAR_MAX_CTAS];
-};
-
-struct ParCtx {                          // mirrors sb200_par (include/surreal_b200.h)
-    void* peers[PAR_MAX_WORLD];
-    int world;
-    int rank;
-    long long max_floats;
-};
-
-struct OptWsView {                       // first fields of optim.cu's OptWs
-    unsigned int counter;
-    int step;
-    float total_norm;
-    float pad;
-};
-
-__device__ __forceinline__ float* slot_of(void* base, long long max_floats, unsigned int parity) {
-    return reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(base) + sizeof(ParHeader)) + (size_t)parity * (size_t)max_floats;
-}
-__device__ __forceinline__ void st_release_sys(unsigned int* p, unsigned int v) {
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned int ld_acquire_sys(const unsigned int* p) {
-    unsigned int v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ float4 ld_sys4(const float* p) {
-    float4 r;
-    asm volatile("ld.relaxed.sys.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p) : "memory");
-    return r;
-}
-__device__ __forceinline__ float ld_sys1(const float* p) {
-    float r;
-    asm volatile("ld.relaxed.sys.global.f32 %0, [%1];" : "=f"(r) : "l"(p) : "memory");
-    return r;
-}
-
-__global__ void __launch_bounds__(PAR_T) par_allreduce_kernel(const __grid_constant__ ParCtx c, const float* __restrict__ x,
+__global__ void __launch_bounds__(PAR_T) par_allreduce_kernel(const __grid_constant__ sb200_par c, const float* __restrict__ x,
                                                               float* __restrict__ out, long long n, float scale, int bump_step,
-                                                              OptWsView* ws, const int* __restrict__ stop) {
-    ParHeader* me = reinterpret_cast<ParHeader*>(c.peers[c.rank]);
+                                                              optim_dev::OptWs* ws, const int* __restrict__ stop) {
+    ParHeader* me = header_of(c, c.rank);
     __shared__ double sh[32];
     const int b = blockIdx.x, G = gridDim.x, tid = threadIdx.x;
     // NOTE: the exchange itself is unconditional (every rank must take part in every call); `stop` only gates the norm /
@@ -82,7 +40,7 @@ __global__ void __launch_bounds__(PAR_T) par_allreduce_kernel(const __grid_const
     per = (per + 3) & ~3ll;                                   // 16-byte aligned slices
     const long long lo = (long long)b * per;
     const long long hi = (lo + per < n) ? lo + per : n;
-    float* mine = slot_of(c.peers[c.rank], c.max_floats, parity);
+    float* mine = slot_of(c, c.rank, parity);
     const bool vec = ((((uintptr_t)x) | ((uintptr_t)out)) & 15) == 0;
     // 1. local slice -> own slot
     if (vec) {
@@ -94,20 +52,13 @@ __global__ void __launch_bounds__(PAR_T) par_allreduce_kernel(const __grid_const
         for (long long i = lo + tid; i < hi; i += PAR_T) mine[i] = x[i];
     }
     __threadfence_system();
-    __syncthreads();
     // 2. publish, 3. wait
-    if (tid < c.world && tid != c.rank)
-        st_release_sys(&reinterpret_cast<ParHeader*>(c.peers[tid])->flags[c.rank * PAR_MAX_CTAS + b], k);
-    if (tid < c.world && tid != c.rank) {
-        const unsigned int* f = &me->flags[tid * PAR_MAX_CTAS + b];
-        while ((int)(ld_acquire_sys(f) - k) < 0) { }
-    }
-    __syncthreads();
+    publish_and_wait(c, me, b, k);
     // 4. sum in rank order
     double sq = 0.0;
     const float* slots[PAR_MAX_WORLD];
 #pragma unroll
-    for (int p = 0; p < PAR_MAX_WORLD; ++p) slots[p] = (p < c.world) ? slot_of(c.peers[p], c.max_floats, parity) : nullptr;
+    for (int p = 0; p < PAR_MAX_WORLD; ++p) slots[p] = (p < c.world) ? slot_of(c, p, parity) : nullptr;
     if (vec) {
         for (long long i = lo + 4 * tid; i + 3 < hi; i += 4 * PAR_T) {
             float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -144,42 +95,25 @@ __global__ void __launch_bounds__(PAR_T) par_allreduce_kernel(const __grid_const
     if (last_block_ticket(&me->ticket, G)) {
         if (tid == 0) {
             me->counter = k;                                   // this rank has completed call k
-            if (ws != nullptr && !(stop != nullptr && *stop)) {
-                double acc = 0.0;
-                for (int q = 0; q < G; ++q) acc += me->partial[q];
-                ws->total_norm = (float)sqrt(acc);
-                if (bump_step) ws->step += 1;
-            }
+            if (ws != nullptr && !(stop != nullptr && *stop)) optim_dev::finish_norm(ws, me->partial, G, bump_step);
         }
     }
 }
 
 // float64 variant for the scalar exchanges (KL, advantage moments): a handful of elements, one CTA, same protocol
-__global__ void __launch_bounds__(64) par_allreduce_f64_kernel(const __grid_constant__ ParCtx c, const double* __restrict__ x,
+__global__ void __launch_bounds__(64) par_allreduce_f64_kernel(const __grid_constant__ sb200_par c, const double* __restrict__ x,
                                                                double* __restrict__ out, int n, double scale) {
-    ParHeader* me = reinterpret_cast<ParHeader*>(c.peers[c.rank]);
+    ParHeader* me = header_of(c, c.rank);
     const int tid = threadIdx.x;
     const unsigned int k = me->counter + 1u;
     const unsigned int parity = k & 1u;
-    double* mine = reinterpret_cast<double*>(slot_of(c.peers[c.rank], c.max_floats, parity));
+    double* mine = reinterpret_cast<double*>(slot_of(c, c.rank, parity));
     for (int i = tid; i < n; i += 64) mine[i] = x[i];
     __threadfence_system();
-    __syncthreads();
-    if (tid < c.world && tid != c.rank)
-        st_release_sys(&reinterpret_cast<ParHeader*>(c.peers[tid])->flags[c.rank * PAR_MAX_CTAS], k);
-    if (tid < c.world && tid != c.rank) {
-        const unsigned int* f = &me->flags[tid * PAR_MAX_CTAS];
-        while ((int)(ld_acquire_sys(f) - k) < 0) { }
-    }
-    __syncthreads();
+    publish_and_wait(c, me, 0, k);
     for (int i = tid; i < n; i += 64) {
         double a = 0.0;
-        for (int p = 0; p < c.world; ++p) {
-            const double* s = reinterpret_cast<const double*>(slot_of(c.peers[p], c.max_floats, parity)) + i;
-            double v;
-            asm volatile("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(v) : "l"(s) : "memory");
-            a += v;
-        }
+        for (int p = 0; p < c.world; ++p) a += ld_sys_f64(reinterpret_cast<const double*>(slot_of(c, p, parity)) + i);
         out[i] = a * scale;
     }
     __syncthreads();
@@ -225,26 +159,19 @@ extern "C" int sb200_par_close(void* ptr, int own) {
 // bookkeeping of sb200_grad_reduce_norm_f32 on the result (opt_workspace may be NULL).
 extern "C" int sb200_par_allreduce_f32(const sb200_par* ctx, const float* x, float* out, int64_t n, double scale, int bump_step,
                                        void* opt_workspace, const int* stop_flag, void* stream) {
-    SB200_REQUIRE(ctx && x && out && n >= 1 && ctx->world >= 1 && ctx->world <= PAR_MAX_WORLD && ctx->rank >= 0 && ctx->rank < ctx->world);
-    SB200_REQUIRE(n <= ctx->max_floats);
-    ParCtx c;
-    for (int p = 0; p < PAR_MAX_WORLD; ++p) c.peers[p] = (p < ctx->world) ? ctx->peers[p] : nullptr;
-    c.world = ctx->world; c.rank = ctx->rank; c.max_floats = ctx->max_floats;
-    for (int p = 0; p < ctx->world; ++p) SB200_REQUIRE(c.peers[p] != nullptr);
+    SB200_REQUIRE(x && out && n >= 1);
+    if (const int e = sb200_par_check(ctx, n)) return e;
     int G = (int)((n + 16383) / 16384);                        // ~64 KB of fp32 per CTA
     if (G < 1) G = 1;
     if (G > PAR_MAX_CTAS) G = PAR_MAX_CTAS;
-    par_allreduce_kernel<<<G, PAR_T, 0, (cudaStream_t)stream>>>(c, x, out, n, (float)scale, bump_step, (OptWsView*)opt_workspace, stop_flag);
+    par_allreduce_kernel<<<G, PAR_T, 0, (cudaStream_t)stream>>>(*ctx, x, out, n, (float)scale, bump_step,
+                                                                (optim_dev::OptWs*)opt_workspace, stop_flag);
     return sb200_launch_status();
 }
 
 extern "C" int sb200_par_allreduce_f64(const sb200_par* ctx, const double* x, double* out, int n, double scale, void* stream) {
-    SB200_REQUIRE(ctx && x && out && n >= 1 && ctx->world >= 1 && ctx->world <= PAR_MAX_WORLD && ctx->rank >= 0 && ctx->rank < ctx->world);
-    SB200_REQUIRE(2ll * n <= ctx->max_floats);
-    ParCtx c;
-    for (int p = 0; p < PAR_MAX_WORLD; ++p) c.peers[p] = (p < ctx->world) ? ctx->peers[p] : nullptr;
-    c.world = ctx->world; c.rank = ctx->rank; c.max_floats = ctx->max_floats;
-    for (int p = 0; p < ctx->world; ++p) SB200_REQUIRE(c.peers[p] != nullptr);
-    par_allreduce_f64_kernel<<<1, 64, 0, (cudaStream_t)stream>>>(c, x, out, n, scale);
+    SB200_REQUIRE(x && out && n >= 1);
+    if (const int e = sb200_par_check(ctx, 2ll * n)) return e;
+    par_allreduce_f64_kernel<<<1, 64, 0, (cudaStream_t)stream>>>(*ctx, x, out, n, scale);
     return sb200_launch_status();
 }

@@ -30,9 +30,8 @@ __device__ __forceinline__ void sample_one(const float* __restrict__ mean, long 
     const int p = (stage_pos != nullptr) ? stage_pos[i] : 0;
     float z[4] = {0.f, 0.f, 0.f, 0.f};
     if (!deterministic && eps == nullptr) {
-        const Philox4 r = philox4x32_10(seed, ctr, ((unsigned long long)i << 16) | (unsigned long long)(j0 >> 2));
-        const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
-        z[0] = a.x; z[1] = a.y; z[2] = b.x; z[3] = b.y;
+        const float4 n = action_noise4(seed, ctr, i, j0 >> 2);
+        z[0] = n.x; z[1] = n.y; z[2] = n.z; z[3] = n.w;
     }
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -97,9 +96,8 @@ __global__ void __launch_bounds__(RT) ddpg_noise_kernel(const float* __restrict_
     for (int j0 = 0; j0 < A; j0 += 4) {
         float z[4] = {0.f, 0.f, 0.f, 0.f};
         if (!deterministic && unit_noise == nullptr) {
-            const Philox4 r = philox4x32_10(seed, ctr, ((unsigned long long)i << 16) | (unsigned long long)(j0 >> 2));
-            const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
-            z[0] = a.x; z[1] = a.y; z[2] = b.x; z[3] = b.y;
+            const float4 n = action_noise4(seed, ctr, i, j0 >> 2);
+            z[0] = n.x; z[1] = n.y; z[2] = n.z; z[3] = n.w;
         }
         for (int c = 0; c < 4 && j0 + c < A; ++c) {
             const int j = j0 + c;
@@ -133,10 +131,7 @@ __global__ void __launch_bounds__(RT) ddpg_ou_noise_kernel(const float* __restri
             e = (double)unit_noise[idx];
         } else {
             const unsigned long long ctr = (step_ctr != nullptr) ? *step_ctr : 0ull;
-            const Philox4 r = philox4x32_10(seed, ctr, ((unsigned long long)i << 16) | (unsigned long long)(j >> 2));
-            const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
-            const int c = j & 3;
-            e = (double)((c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y);
+            e = (double)action_noise1(seed, ctr, i, j);
         }
         const double xp = ou_state[idx];
         const double drift = __dmul_rn(__dmul_rn(theta, 0.0 - xp), dt);
@@ -197,7 +192,7 @@ __device__ void synth_env_block(float* __restrict__ state, const float* __restri
         for (int k = 0; k < D; ++k) acc = fmaf(__ldg(Ws + (long long)k * D + d), s_s[q * D + k], acc);
 #pragma unroll 4
         for (int k = 0; k < A; ++k) acc = fmaf(__ldg(Wa + (long long)k * D + d), s_a[q * A + k], acc);
-        const Philox4 r = philox4x32_10(seed ^ 0x5851F42D4C957F2Dull, ctr, ((unsigned long long)i << 20) | (unsigned long long)d);
+        const Philox4 r = env_noise(seed, ctr, i, d);
         const float2 g = box_muller(r.x, r.y);
         const float nxt = tanhf(acc) + 0.01f * g.x;
         const int t = ep_step[i] + 1;

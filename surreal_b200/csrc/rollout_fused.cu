@@ -14,9 +14,9 @@
 //     action-independent half of the env step while the layers run;
 //   * finished windows go to a per-actor outbox with their completion step; sb200_ppo_rollout_commit_f32 assigns
 //     FIFO slots in the reference's (step, actor) arrival order afterwards and copies them into the replay ring.
-// Sampling and environment arithmetic (and their Philox keys) are those of rollout.cu, so both paths draw the
-// same noise; the policy forward is fp32 FFMA (the per-step path uses 3xTF32 tensor-core products; both are
-// fp32-accurate, they differ by rounding order only).
+// Sampling and environment arithmetic are those of rollout.cu, and both paths draw their noise from common.cuh
+// (action_noise1, env_noise), so they draw the same noise; the policy forward is fp32 FFMA (the per-step path uses
+// 3xTF32 tensor-core products; both are fp32-accurate, they differ by rounding order only).
 #include <cooperative_groups.h>
 
 #include <algorithm>
@@ -113,19 +113,6 @@ struct RfParams {
     int head_mode;                  // G = 1: 1 = k-sliced head over all owned actors, 0 = two warps per actor
 };
 
-__device__ __forceinline__ float rf_act(float v, int act) {
-    if (act == SB200_ACT_RELU) return fmaxf(v, 0.0f);
-    if (act == SB200_ACT_TANH) return tanhf(v);
-    return v;
-}
-
-__device__ __forceinline__ unsigned rf_smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned rf_mapa(unsigned addr, unsigned rank) {
-    unsigned r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-
 // Schedule of a step.  Warps 0..7 run the hidden layers; warps 8..15 meanwhile do the part of the env step that does
 // not depend on the action (Philox + Box-Muller draws, Ws.s, |s|^2): it needs only the state at the top of the step, so
 // it stays off the serial chain behind the layers.  Where a layer's k split goes through shared memory its register
@@ -138,16 +125,10 @@ __device__ __forceinline__ void rf_bar_math() { asm volatile("bar.sync 1, 256;" 
 // to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR in front of the barrier (the kernel's global stores of the step must drain to
 // L2 first) and the wait to a CCTL.IVALL.  st.async carries the data AND the completion count to the consumer's
 // mbarrier, so the producer needs no fence and the consumer polls its own shared memory.
-__device__ __forceinline__ void rf_mbar_init(unsigned long long* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rf_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void rf_mbar_arm(unsigned long long* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rf_smem_u32(bar)), "r"(bytes) : "memory");
-}
-// spin until the phase with this parity has completed; a transaction count that can never be met would hang the GPU, so
-// the spin is bounded (~1 s) and traps instead
-__device__ __forceinline__ void rf_mbar_wait(unsigned long long* bar, unsigned parity) {
-    const unsigned a = rf_smem_u32(bar);
+// Spin until the phase with this parity has completed; a transaction count that can never be met would hang the GPU, so
+// the spin is bounded (~1 s) and traps instead.
+__device__ __forceinline__ void rf_mbar_wait(uint64_t* bar, unsigned parity) {
+    const unsigned a = smem_u32(bar);
     for (unsigned spin = 0;; ++spin) {
         unsigned ok;
         asm volatile(
@@ -242,17 +223,17 @@ __device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldi
         const float4 p3 = *reinterpret_cast<const float4*>(pp + 3 * RF_ROWS * Nc);
         const float4 bv = *reinterpret_cast<const float4*>(bias_s + c4 * 4);
         float4 o;
-        o.x = rf_act(((p0.x + p1.x) + (p2.x + p3.x)) + bv.x, act);
-        o.y = rf_act(((p0.y + p1.y) + (p2.y + p3.y)) + bv.y, act);
-        o.z = rf_act(((p0.z + p1.z) + (p2.z + p3.z)) + bv.z, act);
-        o.w = rf_act(((p0.w + p1.w) + (p2.w + p3.w)) + bv.w, act);
+        o.x = apply_act(((p0.x + p1.x) + (p2.x + p3.x)) + bv.x, act);
+        o.y = apply_act(((p0.y + p1.y) + (p2.y + p3.y)) + bv.y, act);
+        o.z = apply_act(((p0.z + p1.z) + (p2.z + p3.z)) + bv.z, act);
+        o.w = apply_act(((p0.w + p1.w) + (p2.w + p3.w)) + bv.w, act);
         const unsigned owner = (unsigned)(row / RF_OWN);
         float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
         if (owner == crank) {
             *reinterpret_cast<float4*>(qd) = o;
         } else {
-            const unsigned pb = rf_mapa(smem_base, owner);
-            rf_st_async_v4(pb + (rf_smem_u32(qd) - smem_base), o, pb + bar_off);
+            const unsigned pb = mapa_u32(smem_base, owner);
+            rf_st_async_v4(pb + (smem_u32(qd) - smem_base), o, pb + bar_off);
         }
     }
 }
@@ -273,7 +254,7 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
     const float* xr = Xin + (warp * 4) * ldin;
     unsigned pb[RF_CS - 1];
 #pragma unroll
-    for (int c = 1; c < RF_CS; ++c) pb[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
+    for (int c = 1; c < RF_CS; ++c) pb[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
     for (int c4 = cg0; c4 < ((nq + 15) & ~15); c4 += 16) {    // uniform trip count: the shuffles need the whole warp
         const bool on = c4 < nq;
         const float* wp = Ws + (on ? c4 : 0) * 4;
@@ -309,15 +290,15 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
             const float2 s0 = up ? acc[r][0] : acc[r + 2][0], s1 = up ? acc[r][1] : acc[r + 2][1];
             const float2 m0 = up ? acc[r + 2][0] : acc[r][0], m1 = up ? acc[r + 2][1] : acc[r][1];
             float4 o;
-            o.x = rf_act((m0.x + __shfl_xor_sync(0xffffffffu, s0.x, 16)) + bv.x, act);
-            o.y = rf_act((m0.y + __shfl_xor_sync(0xffffffffu, s0.y, 16)) + bv.y, act);
-            o.z = rf_act((m1.x + __shfl_xor_sync(0xffffffffu, s1.x, 16)) + bv.z, act);
-            o.w = rf_act((m1.y + __shfl_xor_sync(0xffffffffu, s1.y, 16)) + bv.w, act);
+            o.x = apply_act((m0.x + __shfl_xor_sync(0xffffffffu, s0.x, 16)) + bv.x, act);
+            o.y = apply_act((m0.y + __shfl_xor_sync(0xffffffffu, s0.y, 16)) + bv.y, act);
+            o.z = apply_act((m1.x + __shfl_xor_sync(0xffffffffu, s1.x, 16)) + bv.z, act);
+            o.w = apply_act((m1.y + __shfl_xor_sync(0xffffffffu, s1.y, 16)) + bv.w, act);
             if (on) {
                 const int row = warp * 4 + (up ? 2 : 0) + r;
                 float* qd = Hout + row * ldout + col0 + c4 * 4;
                 *reinterpret_cast<float4*>(qd) = o;
-                const unsigned off = rf_smem_u32(qd) - smem_base;
+                const unsigned off = smem_u32(qd) - smem_base;
 #pragma unroll
                 for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(pb[c] + off, o, pb[c] + bar_off);
             }
@@ -387,18 +368,18 @@ __device__ __forceinline__ void rf2_layer2_direct(const float* __restrict__ Xin,
             const float2 snd0 = u4 ? s[r][0] : s[r + 2][0], kp0 = u4 ? s[r + 2][0] : s[r][0];
             const float2 snd1 = u4 ? s[r][1] : s[r + 2][1], kp1 = u4 ? s[r + 2][1] : s[r][1];
             float4 o;
-            o.x = rf_act((kp0.x + __shfl_xor_sync(0xffffffffu, snd0.x, 16)) + bv.x, act);
-            o.y = rf_act((kp0.y + __shfl_xor_sync(0xffffffffu, snd0.y, 16)) + bv.y, act);
-            o.z = rf_act((kp1.x + __shfl_xor_sync(0xffffffffu, snd1.x, 16)) + bv.z, act);
-            o.w = rf_act((kp1.y + __shfl_xor_sync(0xffffffffu, snd1.y, 16)) + bv.w, act);
+            o.x = apply_act((kp0.x + __shfl_xor_sync(0xffffffffu, snd0.x, 16)) + bv.x, act);
+            o.y = apply_act((kp0.y + __shfl_xor_sync(0xffffffffu, snd0.y, 16)) + bv.y, act);
+            o.z = apply_act((kp1.x + __shfl_xor_sync(0xffffffffu, snd1.x, 16)) + bv.z, act);
+            o.w = apply_act((kp1.y + __shfl_xor_sync(0xffffffffu, snd1.y, 16)) + bv.w, act);
             if (on) {
                 const int row = rg * 8 + (u3 ? 4 : 0) + (u4 ? 2 : 0) + r;
                 const unsigned owner = (unsigned)(row / RF_OWN);
                 float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
                 if (owner == crank) *reinterpret_cast<float4*>(qd) = o;
                 else {
-                    const unsigned pb = rf_mapa(smem_base, owner);
-                    rf_st_async_v4(pb + (rf_smem_u32(qd) - smem_base), o, pb + bar_off);
+                    const unsigned pb = mapa_u32(smem_base, owner);
+                    rf_st_async_v4(pb + (smem_u32(qd) - smem_base), o, pb + bar_off);
                 }
             }
         }
@@ -442,12 +423,12 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
     cg::cluster_group cluster = cg::this_cluster();
     const unsigned crank = cluster.block_rank();
     extern __shared__ __align__(16) float smem[];
-    const unsigned smem_base = rf_smem_u32(smem);
+    const unsigned smem_base = smem_u32(smem);
     unsigned peer_base[RF_CS - 1];
 #pragma unroll
-    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
+    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
     __shared__ int s_pos[G][RF_OWN], s_ep[G][RF_OWN], s_cnt[G][RF_OWN];
-    __shared__ __align__(8) unsigned long long s_bar[G][3];   // per group: hidden layer 1 | last hidden layer rows | next input tile
+    __shared__ __align__(8) uint64_t s_bar[G][3];   // per group: hidden layer 1 | last hidden layer rows | next input tile
 
     const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
     const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
@@ -511,7 +492,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
     const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
     if (tid == 0) {
         for (int g = 0; g < G; ++g)
-            for (int i = 0; i < 3; ++i) rf_mbar_init(&s_bar[g][i], 1);
+            for (int i = 0; i < 3; ++i) mbar_init(&s_bar[g][i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // bytes a CTA receives from its three peers per step and group (as G = 1)
@@ -542,17 +523,17 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                     rf_mbar_wait(&s_bar[g][2], (unsigned)(t - 1) & 1u);
                 }
                 if (tid == 0) {
-                    rf_mbar_arm(&s_bar[g][0], tx_h1);
-                    rf_mbar_arm(&s_bar[g][1], tx_h2);
-                    if (!final_step) rf_mbar_arm(&s_bar[g][2], tx_x0);
+                    mbar_arrive_expect_tx(&s_bar[g][0], tx_h1);
+                    mbar_arrive_expect_tx(&s_bar[g][1], tx_h2);
+                    if (!final_step) mbar_arrive_expect_tx(&s_bar[g][2], tx_x0);
                 }
                 rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank,
-                           rf_smem_u32(&s_bar[g][0]) - smem_base);
+                           smem_u32(&s_bar[g][0]) - smem_base);
                 rf_bar_math();
                 rf_mbar_wait(&s_bar[g][0], (unsigned)t & 1u);
                 RF_STAMP(3 + 2 * g, 0);
                 rf2_layer2_direct(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, smem_base, crank,
-                                  rf_smem_u32(&s_bar[g][1]) - smem_base);
+                                  smem_u32(&s_bar[g][1]) - smem_base);
                 RF_STAMP(4 + 2 * g, 0);
                 rf_bar_arrive(2 + g, 2 * 256);
             }
@@ -602,9 +583,8 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                             acc0 = fmaf(w2.x, s4.z, acc0); acc1 = fmaf(w2.y, s4.z, acc1);
                             acc0 = fmaf(w3.x, s4.w, acc0); acc1 = fmaf(w3.y, s4.w, acc1);
                         }
-                        const unsigned long long key = ((unsigned long long)i_own << 20) | (unsigned long long)d;
-                        const Philox4 r0 = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr, key);
-                        const Philox4 r1 = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr, key + 1);
+                        const Philox4 r0 = env_noise(p.env_seed, ctr, i_own, d);
+                        const Philox4 r1 = env_noise(p.env_seed, ctr, i_own, d + 1);
                         const float2 gz0 = box_muller(r0.x, r0.y), gz1 = box_muller(r1.x, r1.y);
                         *reinterpret_cast<float2*>(Eacc + own * D + d) = make_float2(acc0, acc1);
                         *reinterpret_cast<float2*>(Egx + own * D + d) = make_float2(gz0.x, gz1.x);
@@ -615,13 +595,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                             Eq[2 * own + 1] = gz0.y;
                         }
                     }
-                    if (!p.deterministic && lane < A) {
-                        const int j = lane;
-                        const Philox4 r = philox4x32_10(p.agent_seed, ctr, ((unsigned long long)i_own << 16) | (unsigned long long)(j >> 2));
-                        const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
-                        const int c = j & 3;
-                        Zn[own * A + j] = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
-                    }
+                    if (!p.deterministic && lane < A) Zn[own * A + lane] = action_noise1(p.agent_seed, ctr, i_own, lane);
                 }
                 rf_bar_sync(2 + g, 2 * 256);                   // own rows of the last hidden layer, then the peers' rows
                 rf_mbar_wait(&s_bar[g][1], (unsigned)t & 1u);
@@ -681,7 +655,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                         float pre = 0.0f;
 #pragma unroll 4
                         for (int w = 0; w < RF_THREADS / 32; ++w) pre += Hs[(w * RF_OWN + own) * ldwh + j];
-                        const float mu = rf_act(pre + Bhs[j], p.act[2]);
+                        const float mu = apply_act(pre + Bhs[j], p.act[2]);
                         const float sd = Sd[own * A + j];
                         float a = mu;
                         if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
@@ -753,8 +727,8 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                         }
                         float* qx = X0 + m_own * p.ldx0 + q4 * 4;
                         *reinterpret_cast<float4*>(qx) = v;
-                        const unsigned off = rf_smem_u32(qx) - smem_base;
-                        const unsigned bar_off = rf_smem_u32(&s_bar[g][2]) - smem_base;
+                        const unsigned off = smem_u32(qx) - smem_base;
+                        const unsigned bar_off = smem_u32(&s_bar[g][2]) - smem_base;
 #pragma unroll
                         for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off);
                     }
@@ -792,12 +766,12 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     cg::cluster_group cluster = cg::this_cluster();
     const unsigned crank = cluster.block_rank();
     extern __shared__ __align__(16) float smem[];
-    const unsigned smem_base = rf_smem_u32(smem);
+    const unsigned smem_base = smem_u32(smem);
     unsigned peer_base[RF_CS - 1];
 #pragma unroll
-    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = rf_mapa(smem_base, (crank + (unsigned)c) % RF_CS);
+    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
     __shared__ int s_pos[RF_OWN], s_ep[RF_OWN], s_cnt[RF_OWN];
-    __shared__ __align__(8) unsigned long long s_bar[3];      // hidden layer 1 | last hidden layer rows | next input tile
+    __shared__ __align__(8) uint64_t s_bar[3];      // hidden layer 1 | last hidden layer rows | next input tile
 
     // (tried: the two roles on swapped warp halves, in case the scheduler's preference for one end of the warp index range
     // starved the layers -- no difference in clock64 traces)
@@ -874,11 +848,11 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     }
     const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
     if (tid == 0) {
-        for (int i = 0; i < 3; ++i) rf_mbar_init(&s_bar[i], 1);
+        for (int i = 0; i < 3; ++i) mbar_init(&s_bar[i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    const unsigned bar_off_h1 = rf_smem_u32(&s_bar[0]) - smem_base, bar_off_h2 = rf_smem_u32(&s_bar[1]) - smem_base;
-    const unsigned bar_off_x0 = rf_smem_u32(&s_bar[2]) - smem_base;
+    const unsigned bar_off_h1 = smem_u32(&s_bar[0]) - smem_base, bar_off_h2 = smem_u32(&s_bar[1]) - smem_base;
+    const unsigned bar_off_x0 = smem_u32(&s_bar[2]) - smem_base;
     // bytes a CTA receives from its three peers per step: their column quarters of hidden layer 1 for all 32 rows, their
     // column quarters of the last hidden layer for the 8 owned rows, their 8 rows of the next input tile
     const unsigned tx_h1 = 3u * RF_ROWS * Nc1 * 4u, tx_h2 = 3u * RF_OWN * Nc2 * 4u, tx_x0 = 3u * RF_OWN * D * 4u;
@@ -903,8 +877,8 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
         const int rf_t = t;
         RF_STAMP(0, 0);
         if (tid == 0) {                                       // arm this step's phases (the previous ones were consumed)
-            rf_mbar_arm(&s_bar[0], tx_h1);
-            rf_mbar_arm(&s_bar[1], tx_h2);
+            mbar_arrive_expect_tx(&s_bar[0], tx_h1);
+            mbar_arrive_expect_tx(&s_bar[1], tx_h2);
         }
         if (math) {
             if (t > 0) {                                      // the input tile: own rows (math warps wrote them) + the peers' rows
@@ -912,7 +886,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 rf_mbar_wait(&s_bar[2], (unsigned)(t - 1) & 1u);
             }
             RF_STAMP(18, 0);
-            if (tid == 0 && !final_step) rf_mbar_arm(&s_bar[2], tx_x0);     // next tile's phase: only now is the previous one complete
+            if (tid == 0 && !final_step) mbar_arrive_expect_tx(&s_bar[2], tx_x0);     // next tile's phase: only now is the previous one complete
             rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank, bar_off_h1);
             RF_STAMP(3, 0);
             rf_bar_math();
@@ -922,8 +896,8 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                       bar_off_h2);
             RF_STAMP(7, 0);
         } else {
-            // ---- env warp h: everything of this step that does not depend on the action (arithmetic and Philox keys of
-            // sample_one() / synth_env_block() in rollout.cu), concurrently with the layers
+            // ---- env warp h: everything of this step that does not depend on the action (the arithmetic of sample_one() /
+            // synth_env_block() in rollout.cu), concurrently with the layers
             RF_STAMP(16, 256);
             const int h = own;
             const long long ih = row0 + (int)crank * RF_OWN + h;
@@ -936,8 +910,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 float acc = 0.0f;
 #pragma unroll 8
                 for (int k = 0; k < D; ++k) acc = fmaf(EWs[k * D + d], sh[k], acc);
-                const Philox4 r = philox4x32_10(p.env_seed ^ 0x5851F42D4C957F2Dull, ctr,
-                                                ((unsigned long long)ih << 20) | (unsigned long long)d);
+                const Philox4 r = env_noise(p.env_seed, ctr, ih, d);
                 const float2 gz = box_muller(r.x, r.y);
                 Eacc[h * D + d] = acc;
                 Egx[h * D + d] = gz.x;
@@ -947,13 +920,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                     Eq[2 * h + 1] = gz.y;
                 }
             }
-            if (!p.deterministic && lane < A) {
-                const int j = lane;
-                const Philox4 r = philox4x32_10(p.agent_seed, ctr, ((unsigned long long)ih << 16) | (unsigned long long)(j >> 2));
-                const float2 z01 = box_muller(r.x, r.y), z23 = box_muller(r.z, r.w);
-                const int c = j & 3;
-                Zn[h * A + j] = (c == 0) ? z01.x : (c == 1) ? z01.y : (c == 2) ? z23.x : z23.y;
-            }
+            if (!p.deterministic && lane < A) Zn[h * A + lane] = action_noise1(p.agent_seed, ctr, ih, lane);
             RF_STAMP(17, 256);
         }
         __syncthreads();                                      // last hidden layer: own columns (block barrier) + the peers' columns
@@ -1046,7 +1013,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                     pre = Hp[own * A + j] + Hp[(RF_OWN + own) * A + j];
                 }
                 RF_STAMP(19, 0);
-                const float mu = rf_act(pre + Bhs[j], p.act[2]);
+                const float mu = apply_act(pre + Bhs[j], p.act[2]);
                 const float sd = Sd[own * A + j];
                 float a = mu;
                 if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
@@ -1121,7 +1088,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 }
                 float* qx = X0 + m_own * p.ldx0 + q4 * 4;
                 *reinterpret_cast<float4*>(qx) = v;
-                const unsigned off = rf_smem_u32(qx) - smem_base;
+                const unsigned off = smem_u32(qx) - smem_base;
                 if (!final_step) {
 #pragma unroll
                     for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off_x0);

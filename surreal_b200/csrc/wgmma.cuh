@@ -1,26 +1,18 @@
 // Hopper (sm_90a) building blocks of the wgmma kernels of this library: mbarrier, bulk-copy TMA, the wgmma shared-memory
 // descriptor and the m64n128k8 tf32 wgmma with its A operand in registers.  Everything is inline PTX; there is no CUTLASS
-// dependency.  The descriptor bit layout follows the PTX ISA's "matrix descriptor" table for wgmma.
+// dependency.  The descriptor bit layout follows the PTX ISA's "matrix descriptor" table for wgmma.  mbar_init,
+// mbar_arrive_expect_tx, smem_u32 and split_tf32 are shared with the other kernels and live in common.cuh.
 #pragma once
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "common.cuh"
 
 namespace wg {
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 // ---- mbarrier ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
 __device__ __forceinline__ void mbar_init_fence() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t a = smem_u32(bar);
@@ -100,13 +92,6 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32_rs(float (&d)[64], uint32_t
           "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(desc_b), "r"(accumulate)
         : "memory");
-}
-
-// 3xTF32 split: x = hi + lo with hi = tf32(x), lo = tf32(x - hi); a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi (fp32 accumulate)
-__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
-    const float r = x - __uint_as_float(hi);
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
 }
 
 }  // namespace wg
