@@ -433,26 +433,65 @@ int sb200_tanh_bwd_f32(const float* dout, int64_t ldo, const float* out, int64_t
                        float* dpre, int64_t ldd, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Experience staging of PPO: ExpSenderWrapperMultiStepMovingWindowWithInfo._step (exp_sender_wrapper.py:209-228) for N
+ * actors + FIFOReplay.insert (fifo_replay.py:27,34-35).  Every entry that stages a step takes this one descriptor of the
+ * buffers involved (all device memory, allocated once by the caller).
+ *   Per actor a window deque in HBM: stage_pos [N] = items it holds, stage_obs [N][n+1][D], stage_act [N][n][A],
+ *   stage_pd [N][n][2A], stage_rew / stage_done [N][n].  A window is complete at n items; completed windows are copied
+ *   into FIFO slots in (step, actor) order, drop-oldest at capacity; then `stride` items are popped; done clears the deque.
+ *   Record layout, in the deques and in the ring alike (n = n_step; r_*: C records, one array per field):
+ *     obs [n+1][D] (row n = obs_next) | act [n][A] | pd [n][2A] (mean | std) | rew [n] | done [n]
+ *   D = floats per observation row of a record (an RNN policy's rows also carry its cells, see sb200_window_rows).
+ *   dest [N]: the current step's slot of each actor's window (slot | -1 not complete | -2 complete but dropped).
+ *   fifo_state: sb200_fifo_state_bytes() bytes {int head,count,capacity,dropped; int64 total_in,total_out}.
+ *   step_counter: the Philox step counter; the step's slot assignment advances it by one. */
+typedef struct {
+    int N, n_step, stride, D, A;
+    int* stage_pos;
+    float *stage_obs, *stage_act, *stage_pd, *stage_rew, *stage_done;
+    int* dest;
+    void* fifo_state;
+    float *r_obs, *r_act, *r_pd, *r_rew, *r_done;
+    uint64_t* step_counter;
+} sb200_windows;
+/* The rows one env step hands the window staging.  obs_next: each actor's true successor; obs_reset: what it observes
+ * next (the reset observation where done); [N][obs_dim] each; reward / done [N].
+ *   *_host: pinned host copies, all four or none.  With them the call first uploads them into the device rows
+ *     (obs_next_host == obs_reset_host: one upload, into obs_reset, which then serves as both).
+ *   layers > 0: an RNN policy, whose record rows are [obs (obs_dim) | h_0 .. h_{layers-1} | c_0 .. c_{layers-1}]
+ *     (D = obs_dim + 2 * layers * H).  The successor row and the reset row are assembled from the env's rows and the
+ *     agent's [layers][N][H] cells h / c as they are now, i.e. the cells it acts from on the next observation.  Rows whose
+ *     two copies exceed 48 KB of shared memory (a pixel frame's words plus the cells) are committed by a kernel that reads
+ *     the row words straight from the rows and cells instead of staging them; force_wide = 1 takes that kernel for any
+ *     row width (same bytes written).  layers = 0: D = obs_dim, no cells.
+ *   slots_assigned: sb200_ppo_sample_f32 (assign_slots = 1) has already assigned this step's slots. */
+typedef struct {
+    float *obs_next, *obs_reset, *reward, *done;
+    const float *obs_next_host, *obs_reset_host, *reward_host, *done_host;
+    int obs_dim;
+    int layers, H;
+    const float *h, *c;
+    int slots_assigned, force_wide;
+} sb200_window_rows;
+/* ppo_window_step: [H2D of the host rows] -> slot assignment of the windows this step completes (unless slots_assigned;
+ * advances fifo_state and *step_counter) -> commit of the step into the deques and of the completed windows into the
+ * ring.  1 or 2 kernels. */
+int sb200_ppo_window_step_f32(const sb200_windows* windows, const sb200_window_rows* rows, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Batched actors (one call serves all N co-located actors of a step).
  *   ppo_sample: PPOAgent.act after the network (surreal/agent/ppo_agent.py:138-149): pd = [mean | exp(log_var)*
  *     exp(log_noise_i)], action = clip(eps*std+mean, -1, 1).  eps [N,A] injected N(0,1) draws or NULL for
- *     Philox4x32-10 keyed by (seed, *step_counter, actor).  When stage_act != NULL the step's action / pd rows
- *     are also written to the window staging area at stage_pos[i] (see ppo_window_step).
+ *     Philox4x32-10 keyed by (seed, *step_counter, actor).  With `stage` (sb200_windows; NULL: not staged) the step's
+ *     action / pd rows are also written to each actor's window deque.  assign_slots = 1 (needs `stage`, and
+ *     step_counter == stage->step_counter) fuses the slot assignment of the windows this step completes (it depends only
+ *     on the deque lengths, so it can precede the env step): the same launch writes stage->dest, advances fifo_state and
+ *     *step_counter (+1, after every block has drawn with the old value).  Follow with ppo_window_step
+ *     (slots_assigned = 1) or synth_env_window_step.
  *   ddpg_noise: DDPGAgent.act after the network (ddpg_agent.py:176-183): clip -> + sigma_i*N(0,1) -> clip. */
 int sb200_ppo_sample_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
-                         const float* eps, int N, int A, int deterministic, uint64_t seed,
-                         const uint64_t* step_counter, float* action, float* pd, const int* stage_pos,
-                         float* stage_act, float* stage_pd, int n_step, void* stream);
-/*   ppo_sample_assign: ppo_sample fused with the slot assignment of ppo_window_step for the windows this step
- *     completes (it depends only on the deque lengths, so it can precede the env step): writes dest[N]
- *     (slot | -1 not complete | -2 complete but dropped), advances fifo_state and *step_counter (+1, after every
- *     block has drawn with the old value).  Follow with ppo_window_step(slots_assigned=1) or
- *     synth_env_window_step. */
-int sb200_ppo_sample_assign_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
-                                const float* eps, int N, int A, int deterministic, uint64_t seed,
-                                uint64_t* step_counter, float* action, float* pd, const int* stage_pos,
-                                float* stage_act, float* stage_pd, int n_step, void* fifo_state, int* dest,
-                                void* stream);
+                         const float* eps, int N, int A, int deterministic, uint64_t seed, uint64_t* step_counter,
+                         float* action, float* pd, const sb200_windows* stage, int assign_slots, void* stream);
 int sb200_ddpg_noise_f32(const float* mean, int64_t ldm, const float* sigma, const float* unit_noise, int N,
                          int A, int deterministic, uint64_t seed, const uint64_t* step_counter,
                          float* action, void* stream);
@@ -470,32 +509,22 @@ int sb200_synth_env_step_f32(float* state, const float* action, const float* Ws,
                              int D, int A, int max_steps, int* ep_step, uint64_t seed,
                              const uint64_t* step_counter, float* obs_next, float* reward, float* done,
                              void* stream);
-/* synth_env_step fused with the commit half of ppo_window_step (dest from ppo_sample_assign): the successor
- * state is staged straight from shared memory.  One launch per rollout step instead of three. */
+/* synth_env_step fused with the commit half of ppo_window_step (`windows`, whose dest ppo_sample has assigned): the
+ * successor state is staged straight from shared memory.  One launch per rollout step instead of three. */
 int sb200_synth_env_window_step_f32(float* state, const float* action, const float* Ws, const float* Wa, int N,
                                     int D, int A, int max_steps, int* ep_step, uint64_t seed,
                                     const uint64_t* step_counter, float* obs_next, float* reward, float* done,
-                                    int n_step, int stride, int* stage_pos, float* stage_obs, float* stage_act,
-                                    float* stage_pd, float* stage_rew, float* stage_done, const int* dest,
-                                    float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                    void* stream);
+                                    const sb200_windows* windows, void* stream);
 
-/* Host-env fast path (one C call per agent.act() / ExpSender-wrapper step when the environment lives on the host):
- *   ppo_act_host: [H2D obs_host -> obs_dev unless obs_host is NULL] -> policy forward -> ppo_sample (ppo_sample_assign
- *     when fifo_state != NULL) -> D2H action / pd -> ONE stream synchronisation.  Host pointers must be pinned.
- *   ppo_window_step_host: H2D of the step's successor / next observation, reward and done, then ppo_window_step. */
+/* Host-env fast path (one C call per agent.act() / ExpSender-wrapper step when the environment lives on the host; the
+ * wrapper's step is sb200_ppo_window_step_f32 with host rows):
+ *   ppo_act_host: [H2D obs_host -> obs_dev unless obs_host is NULL] -> policy forward -> ppo_sample (with `stage` and
+ *     assign_slots) -> D2H action / pd -> ONE stream synchronisation.  Host pointers must be pinned. */
 int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter* zf, const float* obs_host, float* obs_dev, int N,
                            float* mean_dev, const float* log_var, const float* log_noise, int deterministic,
                            uint64_t seed, uint64_t* step_counter, float* action_dev, float* pd_dev,
-                           const int* stage_pos, float* stage_act, float* stage_pd, int n_step, void* fifo_state,
-                           int* dest, float* action_host, float* pd_host, void* stream);
-int sb200_ppo_window_step_host_f32(const float* obs_next_host, const float* obs_reset_host, const float* reward_host,
-                                   const float* done_host, float* obs_next_dev, float* obs_reset_dev,
-                                   float* reward_dev, float* done_dev, int N, int n_step, int stride, int D, int A,
-                                   int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
-                                   float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
-                                   float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                   uint64_t* step_counter, int slots_assigned, void* stream);
+                           const sb200_windows* stage, int assign_slots, float* action_host, float* pd_host,
+                           void* stream);
 /*   ddpg_act_host: DDPGAgent.act on a host observation batch: [H2D obs_host -> obs_dev unless obs_host is NULL] -> actor
  *     forward -> ddpg_ou_noise (when ou_state != NULL, with sigma64) or ddpg_noise (with sigma) -> D2H action -> ONE stream
  *     synchronisation.  unit_noise: injected N(0,1) draws [N][A] or NULL (Philox).  2 kernels below 2048 actors. */
@@ -544,7 +573,7 @@ int sb200_ddpg_act_host_per_actor_f32(const sb200_mlp* net, int64_t actor_stride
 /* RNN-mode PPOAgent.act (ppo_net.py:317-351, ppo_agent.py:133-149) for host or device observations, one call:
  *   [H2D obs_host -> obs unless obs_host is NULL] -> h, c copied to h_before, c_before (the step's onetime_infos) ->
  *   rows_zfilter -> per layer k: input projection (mlp_forward of ih[k] into pre_x) and lstm_forward from layer k's cells,
- *   updated in place -> head forward -> ppo_sample (ppo_sample_assign when fifo_state != NULL) -> [when action_host is not
+ *   updated in place -> head forward -> ppo_sample (with `stage` and assign_slots) -> [when action_host is not
  *   NULL: D2H action / pd, and h_before / c_before when h_before_host is not NULL, then ONE stream synchronisation].
  *   Cells are [layers][N][H] (h_before_host / c_before_host receive that layout).  Layer k writes h_out[(layers-1-k) % 2].
  *   Kernels: 2 * layers + 3 while every forward stays below 2048 rows (one kernel each).  With the host pointers NULL no
@@ -578,12 +607,8 @@ typedef struct {
     uint64_t* step_counter;
     float* action;
     float* pd;
-    const int* stage_pos;               /* window staging rows of this step (NULL: not staged), see ppo_sample */
-    float* stage_act;
-    float* stage_pd;
-    int n_step;
-    void* fifo_state;                   /* non-NULL: ppo_sample_assign with dest */
-    int* dest;
+    const sb200_windows* stage;         /* window staging of this step (NULL: not staged), see ppo_sample */
+    int assign_slots;
     float* action_host;                 /* pinned; NULL: no D2H and no synchronisation */
     float* pd_host;
     float* h_before_host;               /* pinned; NULL: the cells stay on the device */
@@ -604,31 +629,18 @@ typedef struct {
     float* a2;                          /* [N][32 * H2 * W2] */
 } sb200_ppo_act_rnn;
 int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* args, void* stream);
-/*   ppo_window_step_rnn: ppo_window_step for an RNN policy, whose record rows are [obs (obs_dim) | h_0 .. h_{layers-1} |
- *     c_0 .. c_{layers-1}] (D = obs_dim + 2 * layers * H).  The commit kernel assembles the successor row and the reset row
- *     from the env's [N][obs_dim] rows and the agent's [layers][N][H] cells h / c as they are now, i.e. the cells the
- *     agent acts from on the next observation.  With the host pointers non-NULL (all four) they are uploaded first into
- *     obs_next / obs_reset / reward / done, as ppo_window_step_host does (obs_next_host == obs_reset_host: one upload, into
- *     obs_reset).  Same kernels and launch count as ppo_window_step.  Rows whose two copies exceed 48 KB of shared memory
- *     (a pixel frame's words plus the cells) are committed by a kernel that reads the row words straight from obs / h / c
- *     instead of staging them; force_wide = 1 takes that kernel for any row width (same bytes written). */
-int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const float* obs_reset_host, const float* reward_host,
-                                  const float* done_host, float* obs_next, float* obs_reset, float* reward, float* done,
-                                  int N, int n_step, int stride, int obs_dim, int layers, int H, const float* h,
-                                  const float* c, int A, int* stage_pos, float* stage_obs, float* stage_act,
-                                  float* stage_pd, float* stage_rew, float* stage_done, int* dest_scratch,
-                                  void* fifo_state, float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                  uint64_t* step_counter, int slots_assigned, int force_wide, void* stream);
 
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N
  * actors in ONE launch (a 4-CTA cluster owns 32 actors for the whole chunk; the policy weights stay resident in
- * shared memory, layer outputs cross CTAs through distributed shared memory).  Replaces T x (ppo_sample_assign +
- * synth_env_window_step + the policy forward), i.e. the actor main loop of surreal/agent/base.py:224-271 for a
- * device-resident env.  Same sampling / env arithmetic and Philox keys as the per-step entries.
- *   Completed windows are written to a per-actor OUTBOX (o_*: [N*W] records in the replay's record layout,
+ * shared memory, layer outputs cross CTAs through distributed shared memory).  Replaces T x (ppo_sample with
+ * assign_slots + synth_env_window_step + the policy forward), i.e. the actor main loop of surreal/agent/base.py:224-271
+ * for a device-resident env.  Same sampling / env arithmetic and Philox keys as the per-step entries.
+ *   The kernel stages into the window deques of `windows` (whose N / D / A must match) and reads its step counter.
+ *   Completed windows are written to a per-actor OUTBOX (o_*: [N*W] records in the record layout of sb200_windows,
  *   ev_step [N*W] = chunk-relative completion step, ev_count [N]); W >= T / stride + 2.
  *   rollout_commit then assigns FIFO slots in the reference's (step, actor) arrival order, copies the windows into
- *   the replay ring, advances fifo_state and *step_counter (+T).  scratch: sb200_ppo_rollout_scratch_ints() ints.
+ *   the ring of `windows`, advances its fifo_state and *step_counter (+T).  scratch: sb200_ppo_rollout_scratch_ints()
+ *   ints.
  *   rollout_supported: 1 when `net` (2 hidden layers whose widths are multiples of 16, head <= 32, D % 4 == 0,
  *   D <= 128) fits the shared-memory plan; otherwise use the per-step entries. */
 typedef struct {
@@ -650,12 +662,7 @@ typedef struct {
     float* obs_next;
     float* reward;
     float* done;
-    int* stage_pos;                     /* window staging, see ppo_window_step */
-    float* stage_obs;
-    float* stage_act;
-    float* stage_pd;
-    float* stage_rew;
-    float* stage_done;
+    const sb200_windows* windows;       /* window staging and FIFO ring (not read by rollout_footprint) */
     float* o_obs;                       /* outbox */
     float* o_act;
     float* o_pd;
@@ -664,8 +671,7 @@ typedef struct {
     int* ev_step;
     int* ev_count;
     int W;
-    int N, D, A, n_step, stride, T;
-    const uint64_t* step_counter;       /* read only; rollout_commit advances it */
+    int N, D, A, T;
 } sb200_ppo_rollout;
 int sb200_ppo_rollout_supported(const sb200_mlp* net, int D, int A);
 size_t sb200_ppo_rollout_scratch_ints(int N, int W, int T);
@@ -673,28 +679,14 @@ int sb200_ppo_rollout_f32(const sb200_ppo_rollout* args, void* stream);
 /* SMs that sb200_ppo_rollout_f32 with these net / N / D / A holds for the whole chunk when all its CTAs are resident at
  * once (one wave, one CTA per SM) -> *sms; 0 when the chunk runs in several waves or residency is not known. */
 int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* args, int* sms);
-int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, void* fifo_state, float* r_obs,
-                                 float* r_act, float* r_pd, float* r_rew, float* r_done, uint64_t* step_counter,
-                                 void* stream);
+int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Experience staging + HBM replay.
- *   ppo_window_step: ExpSenderWrapperMultiStepMovingWindowWithInfo._step (exp_sender_wrapper.py:209-228) for N
- *     actors + FIFOReplay.insert (fifo_replay.py:27,34-35): per-actor deque in HBM (stage_*: obs [N][n+1][D],
- *     act [N][n][A], pd [N][n][2A], rew/done [N][n], pos [N]); completed windows are copied into FIFO slots in
- *     (step, actor) order, drop-oldest at capacity; `stride` items are popped; done clears the deque.
- *     Replay storage r_*: obs [C][n+1][D] (row n = obs_next), act [C][n][A], pd [C][n][2A], rew/done [C][n].
- *   fifo_state: sb200_fifo_state_bytes() bytes {int head,count,capacity,dropped; int64 total_in,total_out}.
+ * HBM replay (the PPO window staging that fills the FIFO ring is sb200_windows above).
  *   fifo_pop: FIFOReplay.sample (fifo_replay.py:37-39): slot ids of the `batch` oldest windows; *status = 1
  *     if fewer are queued.   fifo_push: host-side Replay.insert() of k windows -> their slot ids.
  *   replay_gather: out[b] = src[idx[b]] for records of record_floats floats (idx32 or idx64 non-NULL). */
 size_t sb200_fifo_state_bytes(void);
-int sb200_ppo_window_step_f32(const float* obs_next, const float* obs_reset, const float* reward,
-                              const float* done, int N, int n_step, int stride, int D, int A,
-                              int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
-                              float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
-                              float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                              uint64_t* step_counter, int slots_assigned, void* stream);
 int sb200_fifo_pop(void* fifo_state, int batch, int* idx, int* status, void* stream);
 int sb200_fifo_push(void* fifo_state, int k, int* slots, void* stream);
 int sb200_replay_gather_f32(const float* src, int64_t record_floats, const int* idx32, const int64_t* idx64,
@@ -703,25 +695,38 @@ int sb200_replay_gather_f32(const float* src, int64_t record_floats, const int* 
  * outs[f][b] = srcs[f][idx[b]].  Replaces the per-key np.stack loops of aggregator.py:52-103,151-205. */
 int sb200_replay_gather_multi_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
                                   int nfields, const int* idx32, const int64_t* idx64, int batch, void* stream);
-/*   ssar_step: ExpSenderWrapperSSARNStepBootstrap._step (exp_sender_wrapper.py:96-112) for N actors +
- *     UniformReplay.insert (uniform_replay.py:36-41): k-th insert -> slot k % capacity, actor order.
- *     uniform_state: sb200_uniform_state_bytes() bytes {int64 next_idx,size,capacity,total_in}. */
+/* Experience staging of DDPG: ExpSenderWrapperSSARNStepBootstrap._step (exp_sender_wrapper.py:96-112) for N actors +
+ * UniformReplay.insert (uniform_replay.py:36-41): k-th insert -> slot k % capacity, actor order.  One descriptor of the
+ * buffers involved (device memory, allocated once by the caller), taken whole by both ssar_step entries.
+ *   Per actor a deque of < n_step pending transitions: dq_len [N], dq_obs [N][n][D], dq_act [N][n][A], dq_rew [N][n]
+ *   (float64 running n-step sums).  dest / emit [N]: the current step's ring slot and float32 reward of each actor's
+ *   emitted record.  Ring r_*: obs / obs_next [C][D], act [C][A], rew / done [C].
+ *   uniform_state: sb200_uniform_state_bytes() bytes {int64 next_idx,size,capacity,total_in}.
+ *   step_counter: the Philox step counter, advanced by one per step. */
+typedef struct {
+    int N, n_step;
+    double gamma;
+    int D, A;
+    int* dq_len;
+    float *dq_obs, *dq_act;
+    double* dq_rew;
+    int* dest;
+    float* emit;
+    void* uniform_state;
+    float *r_obs, *r_obs_next, *r_act, *r_rew, *r_done;
+    uint64_t* step_counter;
+} sb200_ssar;
 size_t sb200_uniform_state_bytes(void);
-int sb200_ssar_step_f32(const float* obs, const float* action, const float* obs_next, const float* reward,
-                        const float* done, int N, int n_step, double gamma, int D, int A, int* dq_len,
-                        float* dq_obs, float* dq_act, double* dq_rew, int* dest_scratch, float* emit_scratch,
-                        void* uniform_state, float* r_obs, float* r_obs_next, float* r_act, float* r_rew,
-                        float* r_done, uint64_t* step_counter, void* stream);
+/*   ssar_step: one step of a device env: s_t = obs [N][D], a_t = action [N][A], obs_next / reward / done. */
+int sb200_ssar_step_f32(const sb200_ssar* ssar, const float* obs, const float* action, const float* obs_next,
+                        const float* reward, const float* done, void* stream);
 /*   ssar_step_host: ssar_step for a host env, one call: H2D of obs_next, action, done and the rewards AS FLOAT64 (the
  *     reference sums Python floats; the record's reward is rounded to float32 once, at emission), then the ssar_step
  *     kernels, then obs <- the reset observation (obs_reset_host, or obs_next when obs_reset_host == obs_next_host).
  *     obs [N][D] holds s_t on entry and the next s_t on return.  Host pointers must be pinned. */
-int sb200_ssar_step_host_f32(const float* obs_next_host, const float* obs_reset_host, const float* action_host,
-                             const double* reward_host, const float* done_host, float* obs, float* obs_next_dev,
-                             float* action_dev, double* reward_dev, float* done_dev, int N, int n_step, double gamma,
-                             int D, int A, int* dq_len, float* dq_obs, float* dq_act, double* dq_rew, int* dest_scratch,
-                             float* emit_scratch, void* uniform_state, float* r_obs, float* r_obs_next, float* r_act,
-                             float* r_rew, float* r_done, uint64_t* step_counter, void* stream);
+int sb200_ssar_step_host_f32(const sb200_ssar* ssar, const float* obs_next_host, const float* obs_reset_host,
+                             const float* action_host, const double* reward_host, const float* done_host, float* obs,
+                             float* obs_next_dev, float* action_dev, double* reward_dev, float* done_dev, void* stream);
 /* CPython random.Random-compatible MT19937 on the HOST (uniform_replay.py:43-45 draws
  * random.randint(0, len-1) per sample; SURVEY Appendix A.6).  state_h: sb200_mt19937_state_bytes() bytes. */
 size_t sb200_mt19937_state_bytes(void);

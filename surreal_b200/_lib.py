@@ -32,18 +32,42 @@ class Mlp(C.Structure):
                 ('ln_eps', C.c_float)]
 
 
+class Windows(C.Structure):
+    """sb200_windows (include/surreal_b200.h): the PPO window deques of N actors and the FIFO ring they commit into."""
+    _fields_ = [('N', C.c_int), ('n_step', C.c_int), ('stride', C.c_int), ('D', C.c_int), ('A', C.c_int),
+                ('stage_pos', C.c_void_p), ('stage_obs', C.c_void_p), ('stage_act', C.c_void_p), ('stage_pd', C.c_void_p),
+                ('stage_rew', C.c_void_p), ('stage_done', C.c_void_p), ('dest', C.c_void_p), ('fifo_state', C.c_void_p),
+                ('r_obs', C.c_void_p), ('r_act', C.c_void_p), ('r_pd', C.c_void_p), ('r_rew', C.c_void_p),
+                ('r_done', C.c_void_p), ('step_counter', C.c_void_p)]
+
+
+class WindowRows(C.Structure):
+    """sb200_window_rows (include/surreal_b200.h): the rows one env step hands the window staging."""
+    _fields_ = [('obs_next', C.c_void_p), ('obs_reset', C.c_void_p), ('reward', C.c_void_p), ('done', C.c_void_p),
+                ('obs_next_host', C.c_void_p), ('obs_reset_host', C.c_void_p), ('reward_host', C.c_void_p),
+                ('done_host', C.c_void_p), ('obs_dim', C.c_int), ('layers', C.c_int), ('H', C.c_int), ('h', C.c_void_p),
+                ('c', C.c_void_p), ('slots_assigned', C.c_int), ('force_wide', C.c_int)]
+
+
+class Ssar(C.Structure):
+    """sb200_ssar (include/surreal_b200.h): the DDPG n-step deques of N actors and the uniform ring they emit into."""
+    _fields_ = [('N', C.c_int), ('n_step', C.c_int), ('gamma', C.c_double), ('D', C.c_int), ('A', C.c_int),
+                ('dq_len', C.c_void_p), ('dq_obs', C.c_void_p), ('dq_act', C.c_void_p), ('dq_rew', C.c_void_p),
+                ('dest', C.c_void_p), ('emit', C.c_void_p), ('uniform_state', C.c_void_p), ('r_obs', C.c_void_p),
+                ('r_obs_next', C.c_void_p), ('r_act', C.c_void_p), ('r_rew', C.c_void_p), ('r_done', C.c_void_p),
+                ('step_counter', C.c_void_p)]
+
+
 class PPORollout(C.Structure):
     """sb200_ppo_rollout (include/surreal_b200.h)."""
     _fields_ = [('net', C.POINTER(Mlp)), ('zf_stats', C.c_void_p), ('zf_eps', C.c_float), ('log_var', C.c_void_p),
                 ('log_noise', C.c_void_p), ('agent_seed', C.c_uint64), ('deterministic', C.c_int),
                 ('state', C.c_void_p), ('WsT', C.c_void_p), ('WaT', C.c_void_p), ('ep_step', C.c_void_p),
                 ('max_steps', C.c_int), ('env_seed', C.c_uint64), ('action', C.c_void_p), ('pd', C.c_void_p),
-                ('obs_next', C.c_void_p), ('reward', C.c_void_p), ('done', C.c_void_p), ('stage_pos', C.c_void_p),
-                ('stage_obs', C.c_void_p), ('stage_act', C.c_void_p), ('stage_pd', C.c_void_p),
-                ('stage_rew', C.c_void_p), ('stage_done', C.c_void_p), ('o_obs', C.c_void_p), ('o_act', C.c_void_p),
-                ('o_pd', C.c_void_p), ('o_rew', C.c_void_p), ('o_done', C.c_void_p), ('ev_step', C.c_void_p),
-                ('ev_count', C.c_void_p), ('W', C.c_int), ('N', C.c_int), ('D', C.c_int), ('A', C.c_int),
-                ('n_step', C.c_int), ('stride', C.c_int), ('T', C.c_int), ('step_counter', C.c_void_p)]
+                ('obs_next', C.c_void_p), ('reward', C.c_void_p), ('done', C.c_void_p), ('windows', C.POINTER(Windows)),
+                ('o_obs', C.c_void_p), ('o_act', C.c_void_p), ('o_pd', C.c_void_p), ('o_rew', C.c_void_p),
+                ('o_done', C.c_void_p), ('ev_step', C.c_void_p), ('ev_count', C.c_void_p), ('W', C.c_int), ('N', C.c_int),
+                ('D', C.c_int), ('A', C.c_int), ('T', C.c_int)]
 
 
 MAX_RNN_LAYERS = 8
@@ -62,8 +86,7 @@ class PPOActRnn(C.Structure):
                 ('h_out', C.c_void_p * 2), ('ldh', C.c_int), ('h', C.c_void_p), ('c', C.c_void_p), ('h_before', C.c_void_p),
                 ('c_before', C.c_void_p), ('mean', C.c_void_p), ('log_var', C.c_void_p), ('log_noise', C.c_void_p),
                 ('eps', C.c_void_p), ('deterministic', C.c_int), ('seed', C.c_uint64), ('step_counter', C.c_void_p),
-                ('action', C.c_void_p), ('pd', C.c_void_p), ('stage_pos', C.c_void_p), ('stage_act', C.c_void_p),
-                ('stage_pd', C.c_void_p), ('n_step', C.c_int), ('fifo_state', C.c_void_p), ('dest', C.c_void_p),
+                ('action', C.c_void_p), ('pd', C.c_void_p), ('stage', C.POINTER(Windows)), ('assign_slots', C.c_int),
                 ('action_host', C.c_void_p), ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p),
                 ('c_before_host', C.c_void_p), ('frames_host', C.c_void_p), ('frames', C.c_void_p), ('frame_c', C.c_int),
                 ('frame_h', C.c_int), ('frame_w', C.c_int), ('conv_w1', C.c_void_p), ('conv_b1', C.c_void_p),
@@ -141,23 +164,19 @@ def _declare(lib):
         'sb200_mlp_pack_floats': (S, [C.POINTER(Mlp)]),
         'sb200_mlp_pack_tf32': (I, [C.POINTER(Mlp), P, P]),
         'sb200_mlp_forward_packed_f32': (I, [C.POINTER(Mlp), P, C.POINTER(ZFilter), C.POINTER(Rows), P, L, P]),
-        'sb200_ppo_act_host_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), P, P, I, P, P, P, I, C.c_uint64, P, P, P, P, P, P,
-                                       I, P, P, P, P, P]),
-        'sb200_ppo_window_step_host_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P,
-                                               P, I, P]),
+        'sb200_ppo_act_host_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), P, P, I, P, P, P, I, C.c_uint64, P, P, P,
+                                       C.POINTER(Windows), I, P, P, P]),
         'sb200_ddpg_act_host_f32': (I, [C.POINTER(Mlp), P, P, I, P, P, P, P, I, C.c_uint64, P, D, D, P, P, P, P]),
         'sb200_ddpg_param_noise_apply_f32': (I, [C.POINTER(Mlp), I, P, L, P, P, C.c_uint64, C.c_uint64, P, P, D, D, P]),
         'sb200_mlp_forward_per_actor_f32': (I, [C.POINTER(Mlp), L, P, L, I, P, L, C.POINTER(Mlp), P, I, P, P]),
         'sb200_ddpg_act_host_per_actor_f32': (I, [C.POINTER(Mlp), L, C.POINTER(Mlp), P, I, P, P, P, I, P, P, P, P, I,
                                                   C.c_uint64, P, D, D, P, P, P, P]),
         'sb200_ppo_act_rnn_f32': (I, [C.POINTER(PPOActRnn), P]),
-        'sb200_ppo_window_step_rnn_f32': (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, I, P, P, I, P, P, P, P, P, P, P, P,
-                                              P, P, P, P, P, P, I, I, P]),
         'sb200_ppo_rollout_supported': (I, [C.POINTER(Mlp), I, I]),
         'sb200_ppo_rollout_scratch_ints': (S, [I, I, I]),
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),
         'sb200_ppo_rollout_footprint': (I, [C.POINTER(PPORollout), C.POINTER(C.c_int)]),
-        'sb200_ppo_rollout_commit_f32': (I, [C.POINTER(PPORollout), P, P, P, P, P, P, P, P, P]),
+        'sb200_ppo_rollout_commit_f32': (I, [C.POINTER(PPORollout), P, P]),
         'sb200_linear_bwd_dx_f32': (I, [P, L, P, I, P, L, P, L, I, I, I, P]),
         'sb200_linear_bwd_dw_f32': (I, [P, L, P, L, P, P, L, I, I, I, I, I, P]),
         'sb200_layernorm_bwd_f32': (I, [P, L, P, L, P, P, I, I, I, P, L, P, P, L, I, P]),
@@ -175,25 +194,22 @@ def _declare(lib):
         'sb200_add_f32': (I, [P, P, L, P]),
         'sb200_value_loss_f32': (I, [P, L, P, I, P, L, P, P, P]),
         'sb200_ppo_final_stats_f32': (I, [P, L, P, P, L, P, L, P, L, I, I, P, P, P]),
-        'sb200_ppo_sample_f32': (I, [P, L, P, P, P, I, I, I, C.c_uint64, P, P, P, P, P, P, I, P]),
+        'sb200_ppo_sample_f32': (I, [P, L, P, P, P, I, I, I, C.c_uint64, P, P, P, C.POINTER(Windows), I, P]),
         'sb200_ddpg_noise_f32': (I, [P, L, P, P, I, I, I, C.c_uint64, P, P, P]),
         'sb200_ddpg_target2_f32': (I, [P, P, L, P, L, P, P, L, I, I, D, P, P, P, P]),
         'sb200_ddpg_smooth_action_f32': (I, [P, L, P, I, I, D, D, C.c_uint64, P, P, L, P]),
         'sb200_ddpg_ou_noise_f32': (I, [P, L, P, P, I, I, I, C.c_uint64, P, D, D, P, P, P]),
         'sb200_synth_env_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, P]),
         'sb200_fifo_state_bytes': (S, []),
-        'sb200_ppo_window_step_f32': (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I, P]),
-        'sb200_ppo_sample_assign_f32': (I, [P, L, P, P, P, I, I, I, C.c_uint64, P, P, P, P, P, P, I, P, P, P]),
-        'sb200_synth_env_window_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, I, I,
-                                                P, P, P, P, P, P, P, P, P, P, P, P, P]),
+        'sb200_ppo_window_step_f32': (I, [C.POINTER(Windows), C.POINTER(WindowRows), P]),
+        'sb200_synth_env_window_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, C.POINTER(Windows), P]),
         'sb200_fifo_pop': (I, [P, I, P, P, P]),
         'sb200_fifo_push': (I, [P, I, P, P]),
         'sb200_replay_gather_f32': (I, [P, L, P, P, I, P, P]),
         'sb200_replay_gather_multi_f32': (I, [P, P, P, I, P, P, I, P]),
         'sb200_uniform_state_bytes': (S, []),
-        'sb200_ssar_step_f32': (I, [P, P, P, P, P, I, I, D, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P]),
-        'sb200_ssar_step_host_f32': (I, [P, P, P, P, P, P, P, P, P, P, I, I, D, I, I, P, P, P, P, P, P, P, P, P, P, P, P,
-                                         P, P]),
+        'sb200_ssar_step_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P]),
+        'sb200_ssar_step_host_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P, P, P, P, P, P]),
         'sb200_mt19937_state_bytes': (S, []),
         'sb200_mt19937_seed_h': (I, [P, P, I]),
         'sb200_mt19937_set_state_h': (I, [P, P, I]),

@@ -122,20 +122,20 @@ class PPOAgent(Agent):
         eps_dev = None
         if eps is not None:
             eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-        if staged and counter is not self._counter and env.fuse_launches:
-            # sampling + this step's replay-slot assignment + step-counter advance in one launch
-            fifo_state, dest = env.slot_assignment_args()
-            check(_lib.lib().sb200_ppo_sample_assign_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos), _p(env.stage_act), _p(env.stage_pd),
-                env.n_step, _p(fifo_state), _p(dest), ops._stream()), 'sb200_ppo_sample_assign_f32')
-        else:
-            check(_lib.lib().sb200_ppo_sample_f32(
-                _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed,
-                _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
-                _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None,
-                env.n_step if staged else 1, ops._stream()), 'sb200_ppo_sample_f32')
+        assign = self._assign_slots(staged, counter)
+        check(_lib.lib().sb200_ppo_sample_f32(
+            _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed, _p(counter),
+            _p(self._action), _p(self._pd), C.byref(env.windows) if staged else None, int(assign), ops._stream()),
+            'sb200_ppo_sample_f32')
         self._count_step(staged, counter)
+
+    def _assign_slots(self, staged, counter):
+        """Whether this step's sampling launch also assigns the step's replay slots and advances the wrapper's step
+        counter (the wrapper's step() then skips its own assignment pass)."""
+        assign = staged and counter is not self._counter and self.env.fuse_launches
+        if assign:
+            self.env.mark_slots_assigned()
+        return assign
 
     def _count_step(self, staged, counter):
         """Advance the agent's own step counter (the seed of the sampling noise); the wrapper's advances on the device."""
@@ -276,13 +276,10 @@ class PPOAgent(Agent):
             a.eps = eps_dev.data_ptr()
         a.mean, a.log_var, a.log_noise = self._mean.data_ptr(), m.log_var.data_ptr(), self._log_noise.data_ptr()
         a.deterministic, a.seed, a.step_counter = int(det), self.seed, counter.data_ptr()
-        a.action, a.pd, a.n_step = self._action.data_ptr(), self._pd.data_ptr(), 1
+        a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
         if staged:
-            a.stage_pos, a.stage_act, a.stage_pd = env.stage_pos.data_ptr(), env.stage_act.data_ptr(), env.stage_pd.data_ptr()
-            a.n_step = env.n_step
-            if counter is not self._counter and env.fuse_launches:
-                fifo_state, dest = env.slot_assignment_args()
-                a.fifo_state, a.dest = fifo_state.data_ptr(), dest.data_ptr()
+            a.stage = C.pointer(env.windows)
+        a.assign_slots = self._assign_slots(staged, counter)
         check(_lib.lib().sb200_ppo_act_rnn_f32(C.byref(a), ops._stream()), 'sb200_ppo_act_rnn_f32')
         self._count_step(staged, counter)
         if not host:
@@ -326,17 +323,14 @@ class PPOAgent(Agent):
         det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
         staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
         counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        fifo_state = dest = None
-        if staged and counter is not self._counter and env.fuse_launches:
-            fifo_state, dest = env.slot_assignment_args()
+        assign = self._assign_slots(staged, counter)
         d = m.actor.desc()
         zf = ops.zfilter_desc(m.z_stats, m.z_eps)
         check(_lib.lib().sb200_ppo_act_host_f32(
             C.byref(d), C.byref(zf), obs_host, _p(obs_dev), N, _p(self._mean), _p(m.log_var), _p(self._log_noise),
-            int(det), self.seed, _p(counter), _p(self._action), _p(self._pd), _p(env.stage_pos) if staged else None,
-            _p(env.stage_act) if staged else None, _p(env.stage_pd) if staged else None, env.n_step if staged else 1,
-            _p(fifo_state), _p(dest), C.c_void_p(out[0].data_ptr()), C.c_void_p(out[1].data_ptr()),
-            ops._stream()), 'sb200_ppo_act_host_f32')
+            int(det), self.seed, _p(counter), _p(self._action), _p(self._pd), C.byref(env.windows) if staged else None,
+            int(assign), C.c_void_p(out[0].data_ptr()), C.c_void_p(out[1].data_ptr()), ops._stream()),
+            'sb200_ppo_act_host_f32')
         self._count_step(staged, counter)
         return self._host_result(False, self._unbatched(obs), [])
 
@@ -376,7 +370,7 @@ class PPOAgent(Agent):
     def rollout_chunk(self, steps):
         """``steps`` iterations of the actor loop (agent/base.py:244-262) in one launch + the ordered commit pass."""
         w = self.env
-        e, r, m = w.env, w.replay, self.model
+        e, m = w.env, self.model
         ob = w.rollout_outbox(steps)
         if ob is None:
             return False
@@ -391,19 +385,14 @@ class PPOAgent(Agent):
         a.max_steps, a.env_seed = e.max_steps, e.seed + 7
         a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
         a.obs_next, a.reward, a.done = e.obs_next.data_ptr(), e.reward.data_ptr(), e.done.data_ptr()
-        a.stage_pos, a.stage_obs, a.stage_act = w.stage_pos.data_ptr(), w.stage_obs.data_ptr(), w.stage_act.data_ptr()
-        a.stage_pd, a.stage_rew, a.stage_done = w.stage_pd.data_ptr(), w.stage_rew.data_ptr(), w.stage_done.data_ptr()
+        a.windows = C.pointer(w.windows)           # its step counter is the env's: the wrapper shares it
         a.o_obs, a.o_act, a.o_pd = ob['o_obs'].data_ptr(), ob['o_act'].data_ptr(), ob['o_pd'].data_ptr()
         a.o_rew, a.o_done = ob['o_rew'].data_ptr(), ob['o_done'].data_ptr()
         a.ev_step, a.ev_count, a.W = ob['ev_step'].data_ptr(), ob['ev_count'].data_ptr(), ob['W']
-        a.N, a.D, a.A = self.num_envs, m.low_dim, self.action_dim
-        a.n_step, a.stride, a.T = w.n_step, w.stride, int(steps)
-        a.step_counter = e.step_counter.data_ptr()
+        a.N, a.D, a.A, a.T = self.num_envs, m.low_dim, self.action_dim, int(steps)
         L, st = _lib.lib(), ops._stream()
         check(L.sb200_ppo_rollout_f32(C.byref(a), st), 'sb200_ppo_rollout_f32')
-        check(L.sb200_ppo_rollout_commit_f32(C.byref(a), _p(ob['scratch']), _p(r.state), _p(r.r_obs), _p(r.r_act),
-                                             _p(r.r_pd), _p(r.r_rew), _p(r.r_done), _p(e.step_counter), st),
-              'sb200_ppo_rollout_commit_f32')
+        check(L.sb200_ppo_rollout_commit_f32(C.byref(a), _p(ob['scratch']), st), 'sb200_ppo_rollout_commit_f32')
         return True
 
     def module_dict(self):

@@ -3,7 +3,7 @@
 
 unsigned long long g_sb200_launches = 0;
 
-extern "C" int sb200_version(void) { return 100; }
+extern "C" int sb200_version(void) { return 101; }
 
 extern "C" uint64_t sb200_launch_counter(int reset) {
     const unsigned long long v = g_sb200_launches;

@@ -342,45 +342,46 @@ extern "C" int sb200_replay_gather_multi_f32(const float* const* srcs, float* co
 
 extern "C" size_t sb200_uniform_state_bytes(void) { return sizeof(UniformState); }
 
-extern "C" int sb200_ssar_step_f32(const float* obs, const float* action, const float* obs_next, const float* reward,
-                                   const float* done, int N, int n_step, double gamma, int D, int A, int* dq_len,
-                                   float* dq_obs, float* dq_act, double* dq_rew, int* dest_scratch, float* emit_scratch,
-                                   void* uniform_state, float* r_obs, float* r_obs_next, float* r_act, float* r_rew,
-                                   float* r_done, uint64_t* step_counter, void* stream) {
-    SB200_REQUIRE(obs && action && obs_next && reward && done && dq_len && dq_obs && dq_act && dq_rew);
-    SB200_REQUIRE(dest_scratch && emit_scratch && uniform_state && r_obs && r_obs_next && r_act && r_rew && r_done);
-    SB200_REQUIRE(N >= 1 && n_step >= 1 && D >= 1 && A >= 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    ssar_flags_kernel<float><<<1, 1024, 0, st>>>(reward, done, N, n_step, gamma, dq_len, dq_rew, dest_scratch, emit_scratch,
-                                                 (UniformState*)uniform_state, (unsigned long long*)step_counter);
-    ssar_commit_kernel<<<N, 128, 0, st>>>(obs, action, obs_next, done, N, n_step, D, A, dq_len, dq_obs, dq_act, dq_rew,
-                                          dest_scratch, emit_scratch, r_obs, r_obs_next, r_act, r_rew, r_done);
+// Host check of an SSAR staging descriptor: every buffer present and the shape sane (step_counter may be NULL).
+static bool ssar_ok(const sb200_ssar* s) {
+    return s != nullptr && s->N >= 1 && s->n_step >= 1 && s->D >= 1 && s->A >= 1 && s->dq_len && s->dq_obs && s->dq_act &&
+           s->dq_rew && s->dest && s->emit && s->uniform_state && s->r_obs && s->r_obs_next && s->r_act && s->r_rew &&
+           s->r_done;
+}
+
+// The two kernels of one SSAR step; Rew: float for device envs, double for host envs.
+template <typename Rew>
+static int ssar_launch(const sb200_ssar* s, const float* obs, const float* action, const float* obs_next, const Rew* reward,
+                       const float* done, cudaStream_t st) {
+    ssar_flags_kernel<Rew><<<1, 1024, 0, st>>>(reward, done, s->N, s->n_step, s->gamma, s->dq_len, s->dq_rew, s->dest,
+                                               s->emit, (UniformState*)s->uniform_state,
+                                               (unsigned long long*)s->step_counter);
+    ssar_commit_kernel<<<s->N, 128, 0, st>>>(obs, action, obs_next, done, s->N, s->n_step, s->D, s->A, s->dq_len, s->dq_obs,
+                                             s->dq_act, s->dq_rew, s->dest, s->emit, s->r_obs, s->r_obs_next, s->r_act,
+                                             s->r_rew, s->r_done);
     return sb200_launch_status(2);
 }
 
-extern "C" int sb200_ssar_step_host_f32(const float* obs_next_host, const float* obs_reset_host, const float* action_host,
-                                        const double* reward_host, const float* done_host, float* obs, float* obs_next_dev,
-                                        float* action_dev, double* reward_dev, float* done_dev, int N, int n_step,
-                                        double gamma, int D, int A, int* dq_len, float* dq_obs, float* dq_act,
-                                        double* dq_rew, int* dest_scratch, float* emit_scratch, void* uniform_state,
-                                        float* r_obs, float* r_obs_next, float* r_act, float* r_rew, float* r_done,
-                                        uint64_t* step_counter, void* stream) {
-    SB200_REQUIRE(obs_next_host && obs_reset_host && action_host && reward_host && done_host);
-    SB200_REQUIRE(obs && obs_next_dev && action_dev && reward_dev && done_dev && dq_len && dq_obs && dq_act && dq_rew);
-    SB200_REQUIRE(dest_scratch && emit_scratch && uniform_state && r_obs && r_obs_next && r_act && r_rew && r_done);
-    SB200_REQUIRE(N >= 1 && n_step >= 1 && D >= 1 && A >= 1);
+extern "C" int sb200_ssar_step_f32(const sb200_ssar* s, const float* obs, const float* action, const float* obs_next,
+                                   const float* reward, const float* done, void* stream) {
+    SB200_REQUIRE(ssar_ok(s) && obs && action && obs_next && reward && done);
+    return ssar_launch(s, obs, action, obs_next, reward, done, (cudaStream_t)stream);
+}
+
+extern "C" int sb200_ssar_step_host_f32(const sb200_ssar* s, const float* obs_next_host, const float* obs_reset_host,
+                                        const float* action_host, const double* reward_host, const float* done_host,
+                                        float* obs, float* obs_next_dev, float* action_dev, double* reward_dev,
+                                        float* done_dev, void* stream) {
+    SB200_REQUIRE(ssar_ok(s) && obs_next_host && obs_reset_host && action_host && reward_host && done_host);
+    SB200_REQUIRE(obs && obs_next_dev && action_dev && reward_dev && done_dev);
+    const int N = s->N;
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t row_bytes = (size_t)N * D * sizeof(float);
+    const size_t row_bytes = (size_t)N * s->D * sizeof(float);
     SB200_CUDA(cudaMemcpyAsync(obs_next_dev, obs_next_host, row_bytes, cudaMemcpyHostToDevice, st));
-    SB200_CUDA(cudaMemcpyAsync(action_dev, action_host, (size_t)N * A * sizeof(float), cudaMemcpyHostToDevice, st));
+    SB200_CUDA(cudaMemcpyAsync(action_dev, action_host, (size_t)N * s->A * sizeof(float), cudaMemcpyHostToDevice, st));
     SB200_CUDA(cudaMemcpyAsync(reward_dev, reward_host, (size_t)N * sizeof(double), cudaMemcpyHostToDevice, st));
     SB200_CUDA(cudaMemcpyAsync(done_dev, done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-    ssar_flags_kernel<double><<<1, 1024, 0, st>>>(reward_dev, done_dev, N, n_step, gamma, dq_len, dq_rew, dest_scratch,
-                                                  emit_scratch, (UniformState*)uniform_state,
-                                                  (unsigned long long*)step_counter);
-    ssar_commit_kernel<<<N, 128, 0, st>>>(obs, action_dev, obs_next_dev, done_dev, N, n_step, D, A, dq_len, dq_obs, dq_act,
-                                          dq_rew, dest_scratch, emit_scratch, r_obs, r_obs_next, r_act, r_rew, r_done);
-    const int rc = sb200_launch_status(2);
+    const int rc = ssar_launch(s, obs, action_dev, obs_next_dev, reward_dev, done_dev, st);
     if (rc != SB200_OK) return rc;
     // s_t of the next transition, after the commit has appended this one's
     if (obs_reset_host != obs_next_host)

@@ -384,29 +384,18 @@ __global__ void __launch_bounds__(RT) synth_env_window_step_kernel(
 }  // namespace
 
 extern "C" int sb200_ppo_sample_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
-                                    const float* eps, int N, int A, int deterministic, uint64_t seed,
-                                    const uint64_t* step_counter, float* action, float* pd, const int* stage_pos,
-                                    float* stage_act, float* stage_pd, int n_step, void* stream) {
+                                    const float* eps, int N, int A, int deterministic, uint64_t seed, uint64_t* step_counter,
+                                    float* action, float* pd, const sb200_windows* stage, int assign_slots, void* stream) {
     SB200_REQUIRE(mean && log_var && action && pd && N >= 1 && A >= 1 && ldm >= A);
-    SB200_REQUIRE(stage_act == nullptr || (stage_pos != nullptr && stage_pd != nullptr && n_step >= 1));
+    SB200_REQUIRE(stage == nullptr || (windows_ok(stage) && stage->N == N && stage->A == A));
+    // the fused slot assignment advances the staging's step counter, which must be the one the draws are keyed by
+    SB200_REQUIRE(!assign_slots || (stage != nullptr && step_counter != nullptr && step_counter == stage->step_counter));
     ppo_sample_kernel<<<(N * ((A + 3) / 4) + RT - 1) / RT, RT, 0, (cudaStream_t)stream>>>(
         mean, ldm, log_var, log_noise, eps, N, A, deterministic, (unsigned long long)seed,
-        (const unsigned long long*)step_counter, action, pd, stage_pos, stage_act, stage_pd, n_step, nullptr, nullptr,
-        nullptr);
-    return sb200_launch_status();
-}
-
-extern "C" int sb200_ppo_sample_assign_f32(const float* mean, int64_t ldm, const float* log_var,
-                                           const float* log_noise, const float* eps, int N, int A, int deterministic,
-                                           uint64_t seed, uint64_t* step_counter, float* action, float* pd,
-                                           const int* stage_pos, float* stage_act, float* stage_pd, int n_step,
-                                           void* fifo_state, int* dest, void* stream) {
-    SB200_REQUIRE(mean && log_var && action && pd && N >= 1 && A >= 1 && ldm >= A);
-    SB200_REQUIRE(stage_pos && stage_act && stage_pd && n_step >= 1 && fifo_state && dest && step_counter);
-    ppo_sample_kernel<<<(N * ((A + 3) / 4) + RT - 1) / RT, RT, 0, (cudaStream_t)stream>>>(
-        mean, ldm, log_var, log_noise, eps, N, A, deterministic, (unsigned long long)seed,
-        (const unsigned long long*)step_counter, action, pd, stage_pos, stage_act, stage_pd, n_step,
-        (FifoState*)fifo_state, dest, (unsigned long long*)step_counter);
+        (const unsigned long long*)step_counter, action, pd, stage ? stage->stage_pos : nullptr,
+        stage ? stage->stage_act : nullptr, stage ? stage->stage_pd : nullptr, stage ? stage->n_step : 1,
+        assign_slots ? (FifoState*)stage->fifo_state : nullptr, assign_slots ? stage->dest : nullptr,
+        assign_slots ? (unsigned long long*)step_counter : nullptr);
     return sb200_launch_status();
 }
 
@@ -450,41 +439,58 @@ static bool env_smem_ok(int D, int A, bool fused) {
 extern "C" int sb200_synth_env_window_step_f32(float* state, const float* action, const float* Ws, const float* Wa,
                                                int N, int D, int A, int max_steps, int* ep_step, uint64_t seed,
                                                const uint64_t* step_counter, float* obs_next, float* reward,
-                                               float* done, int n_step, int stride, int* stage_pos, float* stage_obs,
-                                               float* stage_act, float* stage_pd, float* stage_rew, float* stage_done,
-                                               const int* dest, float* r_obs, float* r_act, float* r_pd, float* r_rew,
-                                               float* r_done, void* stream) {
-    SB200_REQUIRE(state && action && Ws && Wa && ep_step && obs_next && reward && done);
-    SB200_REQUIRE(stage_pos && stage_obs && stage_act && stage_pd && stage_rew && stage_done && dest);
-    SB200_REQUIRE(r_obs && r_act && r_pd && r_rew && r_done);
-    SB200_REQUIRE(N >= 1 && D >= 1 && A >= 1 && n_step >= 1 && stride >= 1 && env_smem_ok(D, A, true));
+                                               float* done, const sb200_windows* w, void* stream) {
+    SB200_REQUIRE(state && action && Ws && Wa && ep_step && obs_next && reward && done && windows_ok(w));
+    SB200_REQUIRE(w->N == N && w->D == D && w->A == A && env_smem_ok(D, A, true));
     const size_t smem = (size_t)(4 * (D + A) + 8 * D) * sizeof(float);
     synth_env_window_step_kernel<<<(N + 3) / 4, RT, smem, (cudaStream_t)stream>>>(
         state, action, Ws, Wa, N, D, A, max_steps, ep_step, (unsigned long long)seed,
-        (const unsigned long long*)step_counter, obs_next, reward, done, n_step, stride, stage_pos, stage_obs, stage_act,
-        stage_pd, stage_rew, stage_done, dest, r_obs, r_act, r_pd, r_rew, r_done);
+        (const unsigned long long*)step_counter, obs_next, reward, done, w->n_step, w->stride, w->stage_pos, w->stage_obs,
+        w->stage_act, w->stage_pd, w->stage_rew, w->stage_done, w->dest, w->r_obs, w->r_act, w->r_pd, w->r_rew, w->r_done);
     return sb200_launch_status();
 }
 
 extern "C" size_t sb200_fifo_state_bytes(void) { return sizeof(FifoState); }
 
-extern "C" int sb200_ppo_window_step_f32(const float* obs_next, const float* obs_reset, const float* reward,
-                                         const float* done, int N, int n_step, int stride, int D, int A,
-                                         int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
-                                         float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
-                                         float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                         uint64_t* step_counter, int slots_assigned, void* stream) {
-    SB200_REQUIRE(obs_next && obs_reset && reward && done && stage_pos && stage_obs && stage_act && stage_pd);
-    SB200_REQUIRE(stage_rew && stage_done && dest_scratch && fifo_state && r_obs && r_act && r_pd && r_rew && r_done);
-    SB200_REQUIRE(N >= 1 && n_step >= 1 && stride >= 1 && D >= 1 && A >= 1);
+extern "C" int sb200_ppo_window_step_f32(const sb200_windows* w, const sb200_window_rows* r, void* stream) {
+    SB200_REQUIRE(windows_ok(w) && r != nullptr && r->obs_next && r->obs_reset && r->reward && r->done);
+    SB200_REQUIRE(r->obs_dim >= 1 && r->layers >= 0 && (r->layers == 0 || (r->H >= 1 && r->h && r->c)));
+    SB200_REQUIRE(w->D == r->obs_dim + 2 * r->layers * r->H);
+    const bool host = r->obs_reset_host != nullptr;
+    SB200_REQUIRE(host ? (r->obs_next_host && r->reward_host && r->done_host)
+                       : (!r->obs_next_host && !r->reward_host && !r->done_host));
+    const int N = w->N, n = w->n_step, L = r->layers, H = r->H, Do = r->obs_dim;
     cudaStream_t st = (cudaStream_t)stream;
-    if (!slots_assigned)
-        ppo_window_slots_kernel<<<1, 1024, 0, st>>>(N, n_step, stage_pos, dest_scratch, (FifoState*)fifo_state,
-                                                    (unsigned long long*)step_counter);
-    ppo_window_commit_kernel<<<N, 128, 0, st>>>(obs_next, obs_reset, reward, done, N, n_step, stride, D, A, stage_pos,
-                                                stage_obs, stage_act, stage_pd, stage_rew, stage_done, dest_scratch,
-                                                r_obs, r_act, r_pd, r_rew, r_done);
-    return sb200_launch_status(slots_assigned ? 1 : 2);
+    const float* next = r->obs_next;
+    if (host) {
+        const size_t row_bytes = (size_t)N * Do * sizeof(float);
+        SB200_CUDA(cudaMemcpyAsync(r->obs_reset, r->obs_reset_host, row_bytes, cudaMemcpyHostToDevice, st));
+        if (r->obs_next_host != r->obs_reset_host)
+            SB200_CUDA(cudaMemcpyAsync(r->obs_next, r->obs_next_host, row_bytes, cudaMemcpyHostToDevice, st));
+        else
+            next = r->obs_reset;
+        SB200_CUDA(cudaMemcpyAsync(r->reward, r->reward_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
+        SB200_CUDA(cudaMemcpyAsync(r->done, r->done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
+    }
+    if (!r->slots_assigned)
+        ppo_window_slots_kernel<<<1, 1024, 0, st>>>(N, n, w->stage_pos, w->dest, (FifoState*)w->fifo_state,
+                                                    (unsigned long long*)w->step_counter);
+    const size_t smem = (size_t)2 * w->D * sizeof(float);
+    if (L == 0)
+        ppo_window_commit_kernel<<<N, 128, 0, st>>>(next, r->obs_reset, r->reward, r->done, N, n, w->stride, w->D, w->A,
+                                                    w->stage_pos, w->stage_obs, w->stage_act, w->stage_pd, w->stage_rew,
+                                                    w->stage_done, w->dest, w->r_obs, w->r_act, w->r_pd, w->r_rew, w->r_done);
+    else if (smem > 48 * 1024 || r->force_wide)             // rows too wide to stage in shared memory
+        ppo_window_commit_rnn_wide_kernel<<<N, 128, 0, st>>>(next, r->obs_reset, r->reward, r->done, N, n, w->stride, Do, L,
+                                                             H, r->h, r->c, w->A, w->stage_pos, w->stage_obs, w->stage_act,
+                                                             w->stage_pd, w->stage_rew, w->stage_done, w->dest, w->r_obs,
+                                                             w->r_act, w->r_pd, w->r_rew, w->r_done);
+    else
+        ppo_window_commit_rnn_kernel<<<N, 128, smem, st>>>(next, r->obs_reset, r->reward, r->done, N, n, w->stride, Do, L, H,
+                                                           r->h, r->c, w->A, w->stage_pos, w->stage_obs, w->stage_act,
+                                                           w->stage_pd, w->stage_rew, w->stage_done, w->dest, w->r_obs,
+                                                           w->r_act, w->r_pd, w->r_rew, w->r_done);
+    return sb200_launch_status(r->slots_assigned ? 1 : 2);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -495,9 +501,9 @@ extern "C" int sb200_ppo_window_step_f32(const float* obs_next, const float* obs
 extern "C" int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter* zf, const float* obs_host,
                                       float* obs_dev, int N, float* mean_dev, const float* log_var,
                                       const float* log_noise, int deterministic, uint64_t seed,
-                                      uint64_t* step_counter, float* action_dev, float* pd_dev, const int* stage_pos,
-                                      float* stage_act, float* stage_pd, int n_step, void* fifo_state, int* dest,
-                                      float* action_host, float* pd_host, void* stream) {
+                                      uint64_t* step_counter, float* action_dev, float* pd_dev,
+                                      const sb200_windows* stage, int assign_slots, float* action_host, float* pd_host,
+                                      void* stream) {
     SB200_REQUIRE(net != nullptr && obs_dev != nullptr && mean_dev != nullptr && N >= 1);
     SB200_REQUIRE(action_dev && pd_dev && action_host && pd_host && step_counter);
     cudaStream_t st = (cudaStream_t)stream;
@@ -520,40 +526,13 @@ extern "C" int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter*
     lds[net->n_layers - 1] = A;
     int rc = sb200_mlp_forward_f32(net, zf, &in, save, lds, stream);
     if (rc != SB200_OK) return rc;
-    if (fifo_state != nullptr)
-        rc = sb200_ppo_sample_assign_f32(mean_dev, A, log_var, log_noise, nullptr, N, A, deterministic, seed, step_counter,
-                                         action_dev, pd_dev, stage_pos, stage_act, stage_pd, n_step, fifo_state, dest,
-                                         stream);
-    else
-        rc = sb200_ppo_sample_f32(mean_dev, A, log_var, log_noise, nullptr, N, A, deterministic, seed, step_counter,
-                                  action_dev, pd_dev, stage_pos, stage_act, stage_pd, n_step, stream);
+    rc = sb200_ppo_sample_f32(mean_dev, A, log_var, log_noise, nullptr, N, A, deterministic, seed, step_counter, action_dev,
+                              pd_dev, stage, assign_slots, stream);
     if (rc != SB200_OK) return rc;
     SB200_CUDA(cudaMemcpyAsync(action_host, action_dev, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaMemcpyAsync(pd_host, pd_dev, (size_t)N * 2 * A * sizeof(float), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaStreamSynchronize(st));
     return SB200_OK;
-}
-
-extern "C" int sb200_ppo_window_step_host_f32(const float* obs_next_host, const float* obs_reset_host,
-                                              const float* reward_host, const float* done_host, float* obs_next_dev,
-                                              float* obs_reset_dev, float* reward_dev, float* done_dev, int N,
-                                              int n_step, int stride, int D, int A, int* stage_pos, float* stage_obs,
-                                              float* stage_act, float* stage_pd, float* stage_rew, float* stage_done,
-                                              int* dest_scratch, void* fifo_state, float* r_obs, float* r_act,
-                                              float* r_pd, float* r_rew, float* r_done, uint64_t* step_counter,
-                                              int slots_assigned, void* stream) {
-    SB200_REQUIRE(obs_next_host && obs_reset_host && reward_host && done_host);
-    SB200_REQUIRE(obs_next_dev && obs_reset_dev && reward_dev && done_dev && N >= 1 && D >= 1);
-    cudaStream_t st = (cudaStream_t)stream;
-    SB200_CUDA(cudaMemcpyAsync(obs_reset_dev, obs_reset_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    if (obs_next_host != obs_reset_host)
-        SB200_CUDA(cudaMemcpyAsync(obs_next_dev, obs_next_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    SB200_CUDA(cudaMemcpyAsync(reward_dev, reward_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-    SB200_CUDA(cudaMemcpyAsync(done_dev, done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-    return sb200_ppo_window_step_f32((obs_next_host != obs_reset_host) ? obs_next_dev : obs_reset_dev, obs_reset_dev,
-                                     reward_dev, done_dev, N, n_step, stride, D, A, stage_pos, stage_obs, stage_act,
-                                     stage_pd, stage_rew, stage_done, dest_scratch, fifo_state, r_obs, r_act, r_pd, r_rew,
-                                     r_done, step_counter, slots_assigned, stream);
 }
 
 extern "C" int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* obs_dev, int N, float* mean_dev,
@@ -657,14 +636,8 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
     lds[a->head->n_layers - 1] = A;
     rc = sb200_mlp_forward_f32(a->head, &nozf, &in, save, lds, stream);
     if (rc != SB200_OK) return rc;
-    if (a->fifo_state != nullptr)
-        rc = sb200_ppo_sample_assign_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed,
-                                         a->step_counter, a->action, a->pd, a->stage_pos, a->stage_act, a->stage_pd,
-                                         a->n_step, a->fifo_state, a->dest, stream);
-    else
-        rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed,
-                                  a->step_counter, a->action, a->pd, a->stage_pos, a->stage_act, a->stage_pd, a->n_step,
-                                  stream);
+    rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed, a->step_counter,
+                              a->action, a->pd, a->stage, a->assign_slots, stream);
     if (rc != SB200_OK || a->action_host == nullptr) return rc;
     SB200_CUDA(cudaMemcpyAsync(a->action_host, a->action, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaMemcpyAsync(a->pd_host, a->pd, (size_t)N * 2 * A * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -674,46 +647,4 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
     }
     SB200_CUDA(cudaStreamSynchronize(st));
     return SB200_OK;
-}
-
-extern "C" int sb200_ppo_window_step_rnn_f32(const float* obs_next_host, const float* obs_reset_host,
-                                             const float* reward_host, const float* done_host, float* obs_next,
-                                             float* obs_reset, float* reward, float* done, int N, int n_step, int stride,
-                                             int obs_dim, int layers, int H, const float* h, const float* c, int A,
-                                             int* stage_pos, float* stage_obs, float* stage_act, float* stage_pd,
-                                             float* stage_rew, float* stage_done, int* dest_scratch, void* fifo_state,
-                                             float* r_obs, float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                             uint64_t* step_counter, int slots_assigned, int force_wide, void* stream) {
-    SB200_REQUIRE(obs_next && obs_reset && reward && done && h && c && stage_pos && stage_obs && stage_act && stage_pd);
-    SB200_REQUIRE(stage_rew && stage_done && dest_scratch && fifo_state && r_obs && r_act && r_pd && r_rew && r_done);
-    SB200_REQUIRE(N >= 1 && n_step >= 1 && stride >= 1 && obs_dim >= 1 && layers >= 1 && H >= 1 && A >= 1);
-    const bool host = obs_reset_host != nullptr;
-    SB200_REQUIRE(host ? (obs_next_host && reward_host && done_host) : (!obs_next_host && !reward_host && !done_host));
-    const int D = obs_dim + 2 * layers * H;
-    const size_t smem = (size_t)2 * D * sizeof(float);
-    const bool wide = smem > 48 * 1024 || force_wide;            // rows too wide to stage in shared memory
-    cudaStream_t st = (cudaStream_t)stream;
-    const float* next = obs_next;
-    if (host) {
-        const size_t row_bytes = (size_t)N * obs_dim * sizeof(float);
-        SB200_CUDA(cudaMemcpyAsync(obs_reset, obs_reset_host, row_bytes, cudaMemcpyHostToDevice, st));
-        if (obs_next_host != obs_reset_host)
-            SB200_CUDA(cudaMemcpyAsync(obs_next, obs_next_host, row_bytes, cudaMemcpyHostToDevice, st));
-        else
-            next = obs_reset;
-        SB200_CUDA(cudaMemcpyAsync(reward, reward_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-        SB200_CUDA(cudaMemcpyAsync(done, done_host, (size_t)N * sizeof(float), cudaMemcpyHostToDevice, st));
-    }
-    if (!slots_assigned)
-        ppo_window_slots_kernel<<<1, 1024, 0, st>>>(N, n_step, stage_pos, dest_scratch, (FifoState*)fifo_state,
-                                                    (unsigned long long*)step_counter);
-    if (wide)
-        ppo_window_commit_rnn_wide_kernel<<<N, 128, 0, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers,
-                                                             H, h, c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
-                                                             stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
-    else
-        ppo_window_commit_rnn_kernel<<<N, 128, smem, st>>>(next, obs_reset, reward, done, N, n_step, stride, obs_dim, layers,
-                                                           H, h, c, A, stage_pos, stage_obs, stage_act, stage_pd, stage_rew,
-                                                           stage_done, dest_scratch, r_obs, r_act, r_pd, r_rew, r_done);
-    return sb200_launch_status(slots_assigned ? 1 : 2);
 }

@@ -21,6 +21,13 @@ struct FifoState {
     int pad_;
 };
 
+// Host check of a staging descriptor: every buffer present and the shape sane (step_counter may be NULL).
+inline bool windows_ok(const sb200_windows* w) {
+    return w != nullptr && w->N >= 1 && w->n_step >= 1 && w->stride >= 1 && w->D >= 1 && w->A >= 1 && w->stage_pos &&
+           w->stage_obs && w->stage_act && w->stage_pd && w->stage_rew && w->stage_done && w->dest && w->fifo_state &&
+           w->r_obs && w->r_act && w->r_pd && w->r_rew && w->r_done;
+}
+
 constexpr int SLOT_NONE = -1;      // deque not full after this step
 constexpr int SLOT_DROPPED = -2;   // window completes but falls straight out of the deque(maxlen)
 

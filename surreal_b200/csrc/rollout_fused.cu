@@ -1360,6 +1360,12 @@ extern "C" int sb200_debug_rf_ctas(long long* host_out, long long* info) {
 }
 #endif
 
+// the chunk's staging descriptor is complete and describes the same N actors and record shape
+static bool rollout_windows_ok(const sb200_ppo_rollout* a) {
+    const sb200_windows* w = a->windows;
+    return windows_ok(w) && w->N == a->N && w->D == a->D && w->A == a->A;
+}
+
 extern "C" int sb200_ppo_rollout_supported(const sb200_mlp* net, int D, int A) {
     return rf_plan(net, D, A, 1, nullptr, nullptr) ? 1 : 0;
 }
@@ -1374,9 +1380,9 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     RfParams p;
     size_t smem = 0;
     if (!rf_plan(a->net, a->D, a->A, 1, &p, &smem)) return SB200_ERR_UNSUPPORTED;
-    SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->n_step >= 1 && a->stride >= 1 && a->W >= 1);
+    SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->W >= 1 && rollout_windows_ok(a));
     SB200_REQUIRE(a->state && a->WsT && a->WaT && a->ep_step && a->action && a->pd && a->obs_next && a->reward && a->done);
-    SB200_REQUIRE(a->log_var && a->stage_pos && a->stage_obs && a->stage_act && a->stage_pd && a->stage_rew && a->stage_done);
+    SB200_REQUIRE(a->log_var);
     SB200_REQUIRE(a->o_obs && a->o_act && a->o_pd && a->o_rew && a->o_done && a->ev_step && a->ev_count);
     for (int l = 0; l < 3; ++l) {
         p.W[l] = a->net->W[l];
@@ -1403,12 +1409,13 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     p.obs_next = a->obs_next;
     p.reward = a->reward;
     p.done = a->done;
-    p.stage_pos = a->stage_pos;
-    p.stage_obs = a->stage_obs;
-    p.stage_act = a->stage_act;
-    p.stage_pd = a->stage_pd;
-    p.stage_rew = a->stage_rew;
-    p.stage_done = a->stage_done;
+    const sb200_windows* w = a->windows;
+    p.stage_pos = w->stage_pos;
+    p.stage_obs = w->stage_obs;
+    p.stage_act = w->stage_act;
+    p.stage_pd = w->stage_pd;
+    p.stage_rew = w->stage_rew;
+    p.stage_done = w->stage_done;
     p.o_obs = a->o_obs;
     p.o_act = a->o_act;
     p.o_pd = a->o_pd;
@@ -1418,10 +1425,10 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     p.ev_count = a->ev_count;
     p.Wout = a->W;
     p.N = a->N;
-    p.n_step = a->n_step;
-    p.stride = a->stride;
+    p.n_step = w->n_step;
+    p.stride = w->stride;
     p.T = a->T;
-    p.step_ctr = (const unsigned long long*)a->step_counter;
+    p.step_ctr = (const unsigned long long*)w->step_counter;
     RfShape sh;
     const int rc = rf_shape(a, &p, &smem, &sh);
     if (rc != SB200_OK) return rc;
@@ -1450,21 +1457,19 @@ extern "C" int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* a, int* sms)
     return SB200_OK;
 }
 
-extern "C" int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* a, int* scratch, void* fifo_state, float* r_obs,
-                                            float* r_act, float* r_pd, float* r_rew, float* r_done,
-                                            uint64_t* step_counter, void* stream) {
-    SB200_REQUIRE(a != nullptr && scratch != nullptr && fifo_state != nullptr);
-    SB200_REQUIRE(r_obs && r_act && r_pd && r_rew && r_done && step_counter);
+extern "C" int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* a, int* scratch, void* stream) {
+    SB200_REQUIRE(a != nullptr && scratch != nullptr && rollout_windows_ok(a) && a->windows->step_counter);
     SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->W >= 1 && a->ev_step && a->ev_count);
+    const sb200_windows* w = a->windows;
     const int words = (a->N + 31) / 32;
     int* bitmap = scratch;
     int* base = bitmap + (size_t)a->T * words;
     int* ev_slot = base + (a->T + 1);
     cudaStream_t st = (cudaStream_t)stream;
     ppo_rollout_rank_kernel<<<1, 1024, 0, st>>>(a->ev_step, a->ev_count, a->N, a->W, a->T, bitmap, base, ev_slot,
-                                                (FifoState*)fifo_state, (unsigned long long*)step_counter);
+                                                (FifoState*)w->fifo_state, (unsigned long long*)w->step_counter);
     ppo_rollout_copy_kernel<<<(unsigned)((long long)a->N * a->W), 256, 0, st>>>(
-        ev_slot, a->n_step, a->D, a->A, a->o_obs, a->o_act, a->o_pd, a->o_rew, a->o_done, r_obs, r_act, r_pd, r_rew,
-        r_done);
+        ev_slot, w->n_step, a->D, a->A, a->o_obs, a->o_act, a->o_pd, a->o_rew, a->o_done, w->r_obs, w->r_act, w->r_pd,
+        w->r_rew, w->r_done);
     return sb200_launch_status(2);
 }

@@ -124,6 +124,17 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         self._outbox = {}
         r = self.replay
         assert (r.n_step, r.D, r.A) == (n, D, A), 'replay record shape does not match the env / n_step'
+        # every buffer the staging entries take, by name: allocated above and in the replay, never reallocated
+        ptrs = {k: getattr(self, k).data_ptr() for k in ('stage_pos', 'stage_obs', 'stage_act', 'stage_pd', 'stage_rew',
+                                                         'stage_done', 'step_counter')}
+        ptrs.update({k: getattr(r, k).data_ptr() for k in ('r_obs', 'r_act', 'r_pd', 'r_rew', 'r_done')})
+        self.windows = _lib.Windows(N=N, n_step=n, stride=self.stride, D=D, A=A, dest=self._dest.data_ptr(),
+                                    fifo_state=r.state.data_ptr(), **ptrs)
+        # the step's rows: the cells are fixed, the rows themselves are filled per step
+        self._rows = _lib.WindowRows(obs_dim=self.obs_dim)
+        if cells is not None:
+            h, c = cells
+            self._rows.layers, self._rows.H, self._rows.h, self._rows.c = h.shape[0], h.shape[2], h.data_ptr(), c.data_ptr()
 
     def reset(self):
         obs, info = self.env.reset()
@@ -163,76 +174,41 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         self._outbox[key] = ob
         return ob
 
-    def slot_assignment_args(self):
-        """For PPOAgent.act: (fifo_state, dest) of sb200_ppo_sample_assign_f32, which folds this step's slot
-        assignment into the sampling launch.  The following step() then skips its own assignment pass."""
+    def mark_slots_assigned(self):
+        """PPOAgent.act folds this step's slot assignment into its sampling launch (sb200_ppo_sample_f32 with
+        assign_slots): the following step() then skips its own assignment pass."""
         self._slots_ready = True
-        return self.replay.state, self._dest
 
     def step(self, action):
         """``action`` = (action_choice, action_info) as PPOAgent.act returns in training mode; the agent has
-        already staged action / pd rows for this step (sb200_ppo_sample[_assign]_f32)."""
+        already staged action / pd rows for this step (sb200_ppo_sample_f32).  An RNN policy's rows get the cells the
+        agent holds NOW, i.e. the ones it acts from on the next observation (`on` and `o` differ only where an episode
+        ended)."""
         a = action[0] if isinstance(action, tuple) else action
-        r = self.replay
         ready, self._slots_ready = self._slots_ready, False
         if ready and hasattr(self.env, 'step_and_commit_window') and self.cells is None:
             return self.env.step_and_commit_window(a, self)        # env step + commit in ONE launch
         obs, reward, done, info = self.env.step(a)
         o = obs_flat(obs)
         on = obs_flat(info['obs_next']) if (isinstance(info, dict) and 'obs_next' in info) else o
-        if self.cells is not None:
-            self._step_rnn(o, on, reward, done, ready, obs_source(obs))
-            return obs, reward, done, info
+        rows, N, Do = self._rows, self.N, self.obs_dim
         if self.host_env:
-            # host env: this step's successor observation / reward / done cross PCIe here (256 KB + 8 KB), issued with
-            # the staging kernels from ONE C call; the device copy of the next observation is handed to the agent's
-            # next act() (cached_device_obs)
-            h_o, h_on = self._pinned('obs', o, (self.N, self.D)), None
-            h_on = h_o if on is o else self._pinned('obs_next', on, (self.N, self.D))
-            h_r, h_d = self._pinned('rew', reward, (self.N,)), self._pinned('done', done, (self.N,))
-            d_o, d_on = self._dev('obs', (self.N, self.D)), self._dev('obs_next', (self.N, self.D))
-            d_r, d_d = self._dev('rew', (self.N,)), self._dev('done', (self.N,))
-            check(_lib.lib().sb200_ppo_window_step_host_f32(
-                h_on, h_o, h_r, h_d, _p(d_on), _p(d_o), _p(d_r), _p(d_d), self.N, self.n_step, self.stride, self.D,
-                self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act), _p(self.stage_pd),
-                _p(self.stage_rew), _p(self.stage_done), _p(self._dest), _p(r.state), _p(r.r_obs), _p(r.r_act),
-                _p(r.r_pd), _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), _st()),
-                'sb200_ppo_window_step_host_f32')
-            self._last_obs_host, self._last_obs_dev = o, d_o
-            return obs, reward, done, info
-        check(_lib.lib().sb200_ppo_window_step_f32(
-            _p(on), _p(o), _p(reward), _p(done), self.N, self.n_step,
-            self.stride, self.D, self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act),
-            _p(self.stage_pd), _p(self.stage_rew), _p(self.stage_done), _p(self._dest), _p(r.state), _p(r.r_obs),
-            _p(r.r_act), _p(r.r_pd), _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), _st()),
-            'sb200_ppo_window_step_f32')
-        return obs, reward, done, info
-
-    def _step_rnn(self, o, on, reward, done, ready, src):
-        """Staging of an RNN policy's step in ONE C call (sb200_ppo_window_step_rnn_f32): both rows get the cells the agent
-        holds NOW, i.e. the ones it acts from on the next observation (`on` and `o` differ only where an episode ended).  A
-        host env's observation / successor / reward / done cross PCIe in that call (uint8 frames as their 32-bit words),
-        and the device copy of the next observation is handed to the agent's next act() (cached_device_obs, keyed by
-        ``src``, the array the env returned)."""
-        N, Do, r = self.N, self.obs_dim, self.replay
-        h, c = self.cells
-        if self.host_env:
-            h_o = self._pinned('obs', o, (N, Do))
-            h_on = h_o if on is o else self._pinned('obs_next', on, (N, Do))
-            h_r, h_d = self._pinned('rew', reward, (N,)), self._pinned('done', done, (N,))
-            d_o, d_on = self._dev('obs', (N, Do)), self._dev('obs_next', (N, Do))
-            d_r, d_d = self._dev('rew', (N,)), self._dev('done', (N,))
+            # host env: this step's successor observation / reward / done cross PCIe (uint8 frames as their 32-bit words),
+            # issued with the staging kernels from ONE C call; the device copy of the next observation is handed to the
+            # agent's next act() (cached_device_obs, keyed by the array the env returned)
+            rows.obs_reset_host = self._pinned('obs', o, (N, Do))
+            rows.obs_next_host = rows.obs_reset_host if on is o else self._pinned('obs_next', on, (N, Do))
+            rows.reward_host, rows.done_host = self._pinned('rew', reward, (N,)), self._pinned('done', done, (N,))
+            d_o = self._dev('obs', (N, Do))
+            rows.obs_reset, rows.obs_next = d_o.data_ptr(), self._dev('obs_next', (N, Do)).data_ptr()
+            rows.reward, rows.done = self._dev('rew', (N,)).data_ptr(), self._dev('done', (N,)).data_ptr()
         else:
-            h_o = h_on = h_r = h_d = None
-            d_o, d_on, d_r, d_d = o, on, reward, done
-        check(_lib.lib().sb200_ppo_window_step_rnn_f32(
-            h_on, h_o, h_r, h_d, _p(d_on), _p(d_o), _p(d_r), _p(d_d), N, self.n_step, self.stride, Do, h.shape[0], h.shape[2],
-            _p(h), _p(c), self.A, _p(self.stage_pos), _p(self.stage_obs), _p(self.stage_act), _p(self.stage_pd),
-            _p(self.stage_rew), _p(self.stage_done), _p(self._dest), _p(r.state), _p(r.r_obs), _p(r.r_act), _p(r.r_pd),
-            _p(r.r_rew), _p(r.r_done), _p(self.step_counter), int(ready), int(self.wide_commit), _st()),
-            'sb200_ppo_window_step_rnn_f32')
+            rows.obs_next, rows.obs_reset, rows.reward, rows.done = on.data_ptr(), o.data_ptr(), reward.data_ptr(), done.data_ptr()
+        rows.slots_assigned, rows.force_wide = int(ready), int(self.wide_commit)
+        check(_lib.lib().sb200_ppo_window_step_f32(C.byref(self.windows), C.byref(rows), _st()), 'sb200_ppo_window_step_f32')
         if self.host_env:
-            self._last_obs_host, self._last_obs_dev = src, d_o
+            self._last_obs_host, self._last_obs_dev = obs_source(obs), d_o
+        return obs, reward, done, info
 
 
 class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
@@ -250,6 +226,12 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         self._dest = torch.zeros(N, dtype=torch.int32, device=self.device)
         self._emit = torch.zeros(N, device=self.device)
         self._obs = torch.zeros(N, D, device=self.device)
+        # every buffer the staging entries take, by name: allocated above and in the replay, never reallocated
+        r = self.replay
+        ptrs = {k: getattr(self, k).data_ptr() for k in ('dq_len', 'dq_obs', 'dq_act', 'dq_rew', 'step_counter')}
+        ptrs.update({k: getattr(r, k).data_ptr() for k in ('r_obs', 'r_obs_next', 'r_act', 'r_rew', 'r_done')})
+        self.ssar = _lib.Ssar(N=N, n_step=n, gamma=float(self.gamma), D=D, A=A, dest=self._dest.data_ptr(),
+                              emit=self._emit.data_ptr(), uniform_state=r.state.data_ptr(), **ptrs)
 
     def reset(self):
         obs, info = self.env.reset()
@@ -265,16 +247,12 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
 
     def step(self, action):
         obs, reward, done, info = self.env.step(action)
-        r = self.replay
         if self.host_env:
             self._step_host(obs, action, reward, done, info)
             return obs, reward, done, info
-        check(_lib.lib().sb200_ssar_step_f32(
-            _p(self._obs), _p(action), _p(info['obs_next']), _p(reward), _p(done), self.N, self.n_step,
-            float(self.gamma), self.D, self.A, _p(self.dq_len), _p(self.dq_obs), _p(self.dq_act), _p(self.dq_rew),
-            _p(self._dest), _p(self._emit), _p(r.state), _p(r.r_obs), _p(r.r_obs_next), _p(r.r_act), _p(r.r_rew),
-            _p(r.r_done), _p(self.step_counter), _st()), 'sb200_ssar_step_f32')
-        r.mark_device_inserts()
+        check(_lib.lib().sb200_ssar_step_f32(C.byref(self.ssar), _p(self._obs), _p(action), _p(info['obs_next']), _p(reward),
+                                             _p(done), _st()), 'sb200_ssar_step_f32')
+        self.replay.mark_device_inserts()
         self._obs.copy_(obs['low_dim']['flat_inputs'])             # s_t of the next transition (reset obs where done)
         return obs, reward, done, info
 
@@ -282,17 +260,14 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         """A host env's step in ONE C call (sb200_ssar_step_host_f32): successor, action, done and the float64 rewards
         cross PCIe, the n-step sums stay float64 until emission, and s_t of the next transition is left in ``_obs`` --
         the device copy the agent's next act() reuses (cached_device_obs)."""
-        N, D, A, r = self.N, self.D, self.A, self.replay
+        N, D, A = self.N, self.D, self.A
         o = obs_flat(obs)
         on = info['obs_next'] if (isinstance(info, dict) and 'obs_next' in info) else o
         h_o = self._pinned('obs', o, (N, D))
         h_on = h_o if on is o else self._pinned('obs_next', on, (N, D))
         check(_lib.lib().sb200_ssar_step_host_f32(
-            h_on, h_o, self._pinned('act', action, (N, A)), self._pinned('rew', reward, (N,), torch.float64),
+            C.byref(self.ssar), h_on, h_o, self._pinned('act', action, (N, A)), self._pinned('rew', reward, (N,), torch.float64),
             self._pinned('done', done, (N,)), _p(self._obs), _p(self._dev('obs_next', (N, D))), _p(self._dev('act', (N, A))),
-            _p(self._dev('rew', (N,), torch.float64)), _p(self._dev('done', (N,))), N, self.n_step, float(self.gamma), D, A,
-            _p(self.dq_len), _p(self.dq_obs), _p(self.dq_act), _p(self.dq_rew), _p(self._dest), _p(self._emit), _p(r.state),
-            _p(r.r_obs), _p(r.r_obs_next), _p(r.r_act), _p(r.r_rew), _p(r.r_done), _p(self.step_counter), _st()),
-            'sb200_ssar_step_host_f32')
-        r.mark_device_inserts()
+            _p(self._dev('rew', (N,), torch.float64)), _p(self._dev('done', (N,))), _st()), 'sb200_ssar_step_host_f32')
+        self.replay.mark_device_inserts()
         self._last_obs_host, self._last_obs_dev = o, self._obs

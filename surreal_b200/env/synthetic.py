@@ -69,13 +69,10 @@ class SyntheticEnv:
     def step_and_commit_window(self, action, w):
         """step() fused with the commit half of ExpSenderWrapperMultiStepMovingWindowWithInfo.step (``w``), for
         steps whose replay slots the sampling kernel has already assigned."""
-        r = w.replay
         check(_lib.lib().sb200_synth_env_window_step_f32(
             _p(self.state), _p(action), _p(self.WsT), _p(self.WaT), self.N, self.D, self.A, self.max_steps,
             _p(self.ep_step), self.seed + 7, _p(self.step_counter), _p(self.obs_next), _p(self.reward), _p(self.done),
-            w.n_step, w.stride, _p(w.stage_pos), _p(w.stage_obs), _p(w.stage_act), _p(w.stage_pd), _p(w.stage_rew),
-            _p(w.stage_done), _p(w._dest), _p(r.r_obs), _p(r.r_act), _p(r.r_pd), _p(r.r_rew), _p(r.r_done),
-            _stream()), 'sb200_synth_env_window_step_f32')
+            C.byref(w.windows), _stream()), 'sb200_synth_env_window_step_f32')
         return {'low_dim': {'flat_inputs': self.state}}, self.reward, self.done, {'obs_next': self.obs_next}
 
     def close(self):
