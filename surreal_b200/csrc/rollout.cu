@@ -38,13 +38,8 @@ __device__ __forceinline__ void sample_one(const float* __restrict__ mean, long 
         const int j = j0 + c;
         if (j >= A) break;
         const float mu = mean[(long long)i * ldm + j];
-        const float sd = __fmul_rn(expf(log_var[j]), sc);
-        float a = mu;
-        if (!deterministic) {
-            const float e = (eps != nullptr) ? eps[(long long)i * A + j] : z[c];
-            a = __fadd_rn(__fmul_rn(e, sd), mu);
-        }
-        a = fminf(fmaxf(a, -1.0f), 1.0f);
+        const float sd = ppo_std(log_var[j], sc);
+        const float a = ppo_action(mu, sd, (eps != nullptr) ? eps[(long long)i * A + j] : z[c], deterministic);
         action[(long long)i * A + j] = a;
         pd[(long long)i * 2 * A + j] = mu;
         pd[(long long)i * 2 * A + A + j] = sd;
@@ -194,10 +189,9 @@ __device__ void synth_env_block(float* __restrict__ state, const float* __restri
         for (int k = 0; k < A; ++k) acc = fmaf(__ldg(Wa + (long long)k * D + d), s_a[q * A + k], acc);
         const Philox4 r = env_noise(seed, ctr, i, d);
         const float2 g = box_muller(r.x, r.y);
-        const float nxt = tanhf(acc) + 0.01f * g.x;
-        const int t = ep_step[i] + 1;
-        const bool dn = (max_steps > 0) && (t >= max_steps);
-        const float st = dn ? box_muller(r.z, r.w).x : nxt;
+        const float nxt = env_successor(acc, g.x);
+        const bool dn = env_done(ep_step[i] + 1, max_steps);
+        const float st = dn ? env_reset_draw(r) : nxt;
         obs_next[(long long)i * D + d] = nxt;
         state[(long long)i * D + d] = st;
         if (s_n != nullptr) {
@@ -205,7 +199,7 @@ __device__ void synth_env_block(float* __restrict__ state, const float* __restri
             s_z[idx] = st;
         }
         if (d == 0) {
-            const float rw = -s_q[q] / (float)D + 0.1f * g.y;
+            const float rw = env_reward(s_q[q], D, g.y);
             reward[i] = rw;
             done[i] = dn ? 1.0f : 0.0f;
             if (s_rew != nullptr) {
@@ -219,7 +213,7 @@ __device__ void synth_env_block(float* __restrict__ state, const float* __restri
         const int i = a0 + q;
         if (i < N) {
             const int t = ep_step[i] + 1;
-            ep_step[i] = ((max_steps > 0) && (t >= max_steps)) ? 0 : t;
+            ep_step[i] = env_done(t, max_steps) ? 0 : t;
         }
     }
 }

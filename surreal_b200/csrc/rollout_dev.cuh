@@ -1,5 +1,6 @@
 // Device-side building blocks shared by the per-step rollout kernels (rollout.cu) and the persistent rollout
-// kernel (rollout_fused.cu): FIFO control block, replay-slot assignment, per-actor window commit.
+// kernel (rollout_fused.cu): FIFO control block, replay-slot assignment, the sampling and env formulas, per-actor
+// window commit.
 #pragma once
 #include "common.cuh"
 
@@ -93,6 +94,33 @@ __device__ void assign_window_slots(int N, int n_step, const int* __restrict__ s
 }
 
 __device__ unsigned int* fifo_ticket(FifoState* fifo) { return &fifo->ticket; }
+
+// ------------------------------------------------------------------------------------------------
+// Per-element formulas of PPO sampling and of the synthetic env, used by the per-step kernels (rollout.cu) and by the
+// persistent rollout (rollout_fused.cu), whose results must agree bit for bit.  Each formula is one expression, so
+// every caller gets the same FMA contraction.
+
+// PPOAgent.act (ppo_agent.py:138-149): std = exp(log_var) * scale, scale = exp(noise_i) (1 without per-actor noise)
+__device__ __forceinline__ float ppo_std(float log_var, float scale) { return __fmul_rn(expf(log_var), scale); }
+
+// action = clip(z * std + mean, -1, 1) with z ~ N(0, 1), or clip(mean) when deterministic
+__device__ __forceinline__ float ppo_action(float mu, float sd, float z, int deterministic) {
+    float a = mu;
+    if (!deterministic) a = __fadd_rn(__fmul_rn(z, sd), mu);
+    return fminf(fmaxf(a, -1.0f), 1.0f);
+}
+
+// The episode ends when its step count `ep` (this step included) reaches max_steps (MaxStepWrapper, env/wrapper.py:142-163)
+__device__ __forceinline__ bool env_done(int ep, int max_steps) { return (max_steps > 0) && (ep >= max_steps); }
+
+// successor s' = tanh(Ws s + Wa a) + 0.01 xi, acc = Ws s + Wa a, xi = box_muller(r.x, r.y).x of env_noise
+__device__ __forceinline__ float env_successor(float acc, float xi) { return tanhf(acc) + 0.01f * xi; }
+
+// reward -|s|^2 / D + 0.1 xi', sq = |s|^2, xi' = box_muller(r.x, r.y).y of env_noise at d = 0
+__device__ __forceinline__ float env_reward(float sq, int D, float xi) { return -sq / (float)D + 0.1f * xi; }
+
+// state component d of the next episode, drawn ~ N(0, 1) when the step ends the episode
+__device__ __forceinline__ float env_reset_draw(const Philox4& r) { return box_muller(r.z, r.w).x; }
 
 __device__ __forceinline__ void copy_floats(float* __restrict__ dst, const float* __restrict__ src, int count, int g,
                                             int G) {

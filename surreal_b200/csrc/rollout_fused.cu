@@ -165,81 +165,9 @@ __device__ __forceinline__ float rf_reduce8(const float (&s)[8], int lane) {
     return v;
 }
 
-// Last hidden layer (G = 1) on the 8 math warps (tid 0..255): warp = (row group rg = warp & 3: rows 8rg..8rg+7, k quarter
-// pair), lane = (column quad, k half) -> 4-way k split, partial tiles summed in a fixed order through Part [4][32][Nc].
-// Each row goes only to the CTA that owns its actor, into its Hout [8][ldout] (input of the head).
-__device__ __forceinline__ void rf2_layer(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
-                                          int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
-                                          int ldout, int col0, float* __restrict__ Part, unsigned smem_base,
-                                          unsigned crank, int rf_t, int rf_id, unsigned bar_off) {
-    const int tid = (int)RF_TID, warp = tid >> 5, lane = tid & 31;
-    const int rg = warp & 3, ks = ((warp >> 2) << 1) | (lane >> 4), cg0 = lane & 15;
-    const int kq = (((K >> 2) + 3) >> 2) << 2;               // k span of one split (multiple of 4)
-    const int k_lo = ks * kq, k_hi = min(K, k_lo + kq);
-    const int nq = Nc >> 2;
-    const float* xr = Xin + (rg * 8) * ldin;
-    for (int c4 = cg0; c4 < nq; c4 += 16) {
-        const float* wp = Ws + c4 * 4;
-        float2 acc[8][2];
-#pragma unroll
-        for (int r = 0; r < 8; ++r) acc[r][0] = acc[r][1] = make_float2(0.0f, 0.0f);
-#pragma unroll 2
-        for (int k = k_lo; k < k_hi; k += 4) {
-            const float4 w0 = *reinterpret_cast<const float4*>(wp + (k + 0) * Nc);
-            const float4 w1 = *reinterpret_cast<const float4*>(wp + (k + 1) * Nc);
-            const float4 w2 = *reinterpret_cast<const float4*>(wp + (k + 2) * Nc);
-            const float4 w3 = *reinterpret_cast<const float4*>(wp + (k + 3) * Nc);
-#pragma unroll
-            for (int r = 0; r < 8; ++r) {
-                const float4 a = *reinterpret_cast<const float4*>(xr + r * ldin + k);
-                float2 aa = make_float2(a.x, a.x);
-                acc[r][0] = fma2(aa, make_float2(w0.x, w0.y), acc[r][0]);
-                acc[r][1] = fma2(aa, make_float2(w0.z, w0.w), acc[r][1]);
-                aa = make_float2(a.y, a.y);
-                acc[r][0] = fma2(aa, make_float2(w1.x, w1.y), acc[r][0]);
-                acc[r][1] = fma2(aa, make_float2(w1.z, w1.w), acc[r][1]);
-                aa = make_float2(a.z, a.z);
-                acc[r][0] = fma2(aa, make_float2(w2.x, w2.y), acc[r][0]);
-                acc[r][1] = fma2(aa, make_float2(w2.z, w2.w), acc[r][1]);
-                aa = make_float2(a.w, a.w);
-                acc[r][0] = fma2(aa, make_float2(w3.x, w3.y), acc[r][0]);
-                acc[r][1] = fma2(aa, make_float2(w3.z, w3.w), acc[r][1]);
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < 8; ++r)
-            *reinterpret_cast<float4*>(Part + ((ks * RF_ROWS + rg * 8 + r) * Nc + c4 * 4)) =
-                make_float4(acc[r][0].x, acc[r][0].y, acc[r][1].x, acc[r][1].y);
-    }
-    RF_STAMP(rf_id, 0);
-    rf_bar_math();
-    RF_STAMP(rf_id + 1, 0);
-    for (int idx = tid; idx < RF_ROWS * nq; idx += 256) {
-        const int row = idx / nq, c4 = idx - row * nq;
-        const float* pp = Part + row * Nc + c4 * 4;
-        const float4 p0 = *reinterpret_cast<const float4*>(pp);
-        const float4 p1 = *reinterpret_cast<const float4*>(pp + RF_ROWS * Nc);
-        const float4 p2 = *reinterpret_cast<const float4*>(pp + 2 * RF_ROWS * Nc);
-        const float4 p3 = *reinterpret_cast<const float4*>(pp + 3 * RF_ROWS * Nc);
-        const float4 bv = *reinterpret_cast<const float4*>(bias_s + c4 * 4);
-        float4 o;
-        o.x = apply_act(((p0.x + p1.x) + (p2.x + p3.x)) + bv.x, act);
-        o.y = apply_act(((p0.y + p1.y) + (p2.y + p3.y)) + bv.y, act);
-        o.z = apply_act(((p0.z + p1.z) + (p2.z + p3.z)) + bv.z, act);
-        o.w = apply_act(((p0.w + p1.w) + (p2.w + p3.w)) + bv.w, act);
-        const unsigned owner = (unsigned)(row / RF_OWN);
-        float* qd = Hout + (row - (int)owner * RF_OWN) * ldout + col0 + c4 * 4;
-        if (owner == crank) {
-            *reinterpret_cast<float4*>(qd) = o;
-        } else {
-            const unsigned pb = mapa_u32(smem_base, owner);
-            rf_st_async_v4(pb + (smem_u32(qd) - smem_base), o, pb + bar_off);
-        }
-    }
-}
-
-// First hidden layer on the 8 math warps WITHOUT a shared-memory reduction: K = D is short (64), so the 4-way k split of
-// rf2_layer spent more on partial tiles, the barrier and the second pass (1.5 K cycles) than on its 4 k quads of FMAs.
+// First hidden layer on the 8 math warps WITHOUT a shared-memory reduction: K = D is short (64), so a 4-way k split
+// reduced through shared memory spent more on partial tiles, the barrier and the second pass (1.5 K cycles) than on its
+// 4 k quads of FMAs.
 // Here warp w owns rows 4w..4w+3, lane = (column quad, k half); the two k halves of a lane pair are summed by shuffle
 // (each lane keeps two of the four rows) and the epilogue stores / pushes straight from registers.
 __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws, int Nc,
@@ -306,18 +234,18 @@ __device__ __forceinline__ void rf2_layer1(const float* __restrict__ Xin, int ld
     }
 }
 
-// Last hidden layer on the 8 math warps WITHOUT the shared-memory reduction of rf2_layer, with the same
-// result bit for bit: the same four k quarters, each accumulated in the same order by one lane, meet through two rounds of
-// shuffles as ((p0 + p1) + (p2 + p3)) + bias (fp32 addition is commutative, so which lane of a pair adds does not
-// matter).  Warp = (row group rg = warp & 3: rows 8rg..8rg+7, column half ch = warp >> 2), lane = (column quad cq = lane & 7,
-// k quarter ks = lane >> 3).  Each row goes to the CTA that owns its actor, as in rf2_layer.
+// Last hidden layer on the 8 math warps, for both schedules, WITHOUT a shared-memory reduction: four k quarters, each
+// accumulated in k order by one lane, meet through two rounds of shuffles as ((p0 + p1) + (p2 + p3)) + bias (fp32
+// addition is commutative, so which lane of a pair adds does not matter).  Warp = (row group rg = warp & 3: rows
+// 8rg..8rg+7, column half ch = warp >> 2), lane = (column quad cq = lane & 7, k quarter ks = lane >> 3).  Each row goes
+// only to the CTA that owns its actor, into its Hout [8][ldout] (input of the head).
 __device__ __forceinline__ void rf2_layer2_direct(const float* __restrict__ Xin, int ldin, int K, const float* __restrict__ Ws,
                                                   int Nc, const float* __restrict__ bias_s, int act, float* __restrict__ Hout,
                                                   int ldout, int col0, unsigned smem_base, unsigned crank, unsigned bar_off) {
     const int tid = (int)RF_TID, warp = tid >> 5, lane = tid & 31;
     const int rg = warp & 3, ch = warp >> 2, cq = lane & 7, ks = lane >> 3;
     const bool u3 = (lane & 8) != 0, u4 = (lane & 16) != 0;
-    const int kq = (((K >> 2) + 3) >> 2) << 2;               // k span of one quarter, as in rf2_layer
+    const int kq = (((K >> 2) + 3) >> 2) << 2;               // k span of one quarter (multiple of 4)
     const int k_lo = ks * kq, k_hi = min(K, k_lo + kq);
     const int nq = Nc >> 2;
     const float* xr = Xin + (rg * 8) * ldin;
@@ -389,75 +317,59 @@ __device__ __forceinline__ void rf2_layer2_direct(const float* __restrict__ Xin,
 __device__ __forceinline__ void rf_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void rf_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
-// Two groups of 32 actors per cluster (G = 2), software-pipelined, so that a chunk of N actors needs half as many
-// clusters.  Warps 0..7 ("layer warps") run hidden layers 1 and 2 for group 0, then for group 1, step after step.
-// Warps 8..15 ("tail warps", warp 8 + a for owned actor a of each group) take the whole tail of a group -- the
-// action-independent env precompute, head, sampling, env step, window staging, the push of the next input rows -- while
-// the layer warps compute the other group.  Arithmetic, operand order and Philox keys are those of the G = 1 schedule
-// (head_mode 1, rf2_layer2_direct = rf2_layer bit for bit), so both give the same results.
-//
-// Hand-offs, per group g (each group has its own tiles, state and three mbarriers):
-//   layer -> peers: H1 rows (all 32) and H2 rows (owners' only) by st.async, counted on the receiver's h1[g] / h2[g];
-//   layer -> tail:  own H2 rows, named barrier 2 + g (layer warps bar.arrive, tail warps bar.sync; 512 threads);
-//   tail  -> peers: next X0 rows by st.async, counted on x0[g];
-//   tail  -> layer: own next X0 rows, named barrier 4 + g (tail warps bar.arrive, layer warps bar.sync).
-// No reverse "buffer free" signal is needed: every buffer of group g is rewritten only behind a chain of hand-offs that
-// starts after its last reader is done.
-//   * X0[g], step t+1: a peer pushes it after its head of step t, which needs this CTA's H2 rows of step t, which the
-//     layer warps push only after all of them passed layer 1 (rf_bar_math), the last reader of X0[g].  The tail warps
-//     rewrite their own rows after their head, i.e. after named barrier 2 + g, which every layer warp reaches after layer 2.
-//   * H1[g], step t+1: a peer pushes it after its layer 1 of step t+1, which needs this CTA's X0 rows of step t+1, which
-//     the tail warps push after named barrier 2 + g: after every layer warp has finished layer 2, the reader of H1[g].
-//   * H2[g], step t+1: written by layer 2 of step t+1 (peers' and own), behind layer 1 of step t+1, behind the X0 rows of
-//     step t+1 of every CTA of the cluster, which this CTA's tail pushes after its head of step t, the reader of H2[g].
-//   * the same chains order every st.async of step t+1 after the mbarrier wait of step t, so no phase receives bytes of
-//     the next one.  Each phase is armed once (expect_tx; arrival count 1) by thread 0 after the previous phase is known
-//     complete: h1[g] and h2[g] after the layer warps' wait on named barrier 4 + g (the tail waited h2[g] of the step
-//     before), x0[g] after the layer warps' own wait on x0[g].
-//   * named barriers 2 + g and 4 + g never see two generations of arrivals at once: each arrival of step t+1 sits behind
-//     the other side's arrival of step t on the other barrier.
-//   * the head slice buffer is used by the tail warps only, between named barrier 6 (tail warps, 256 threads) and the
-//     next group's named barrier 2 + g', which all 256 tail threads must reach.
-__device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
-    constexpr int G = 2;
-    cg::cluster_group cluster = cg::this_cluster();
-    const unsigned crank = cluster.block_rank();
-    extern __shared__ __align__(16) float smem[];
-    const unsigned smem_base = smem_u32(smem);
-    unsigned peer_base[RF_CS - 1];
-#pragma unroll
-    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
-    __shared__ int s_pos[G][RF_OWN], s_ep[G][RF_OWN], s_cnt[G][RF_OWN];
-    __shared__ __align__(8) uint64_t s_bar[G][3];   // per group: hidden layer 1 | last hidden layer rows | next input tile
+// The env matrices: G = 1 keeps them in shared memory, G = 2 reads them from global memory through L1.
+template <int G>
+__device__ __forceinline__ float rf_env_w(const float* w) {
+    if constexpr (G == 2) return __ldg(w);
+    else return *w;
+}
 
+// Group g's tiles and its owned actors' rows in shared memory (G = 2: group 1's lie gstride floats after group 0's).
+struct RfGroup {
+    float *X0, *H1, *H2, *S, *Nx;
+    float *Ac, *Sd, *Zn, *Hp;             // [8][A] each: actions | std | N(0,1) draws | head_mode 0 halves [2][8][A]
+    float *Eacc, *Egx, *Erz, *Eq;         // action-independent env step: [8][D] Ws.s, successor noise, reset draw | [8][2]
+    __device__ __forceinline__ RfGroup(const RfParams& p, float* smem, int g) {
+        float* b = smem + g * p.gstride;
+        X0 = b + p.oX0; H1 = b + p.oH1; H2 = b + p.oH2; S = b + p.oS; Nx = b + p.oNext;
+        Ac = b + p.oAct; Sd = Ac + 2 * RF_OWN * p.A; Zn = Sd + RF_OWN * p.A; Hp = Zn + RF_OWN * p.A;  // (slot 1 unused, see rf_plan)
+        Eacc = b + p.oPre; Egx = Eacc + RF_OWN * p.D; Erz = Egx + RF_OWN * p.D; Eq = Erz + RF_OWN * p.D;
+    }
+};
+
+// One-time loads of a chunk: this CTA's column quarters of the hidden layers' weights and the whole head by cp.async (G = 1:
+// the env matrices too), biases, z-filter columns, the owned actors' deque length and episode step, every group's owned
+// state rows and input tile, the std rows; the mbarriers are initialised.  Ends with the cluster barrier and returns the
+// step counter the chunk starts at.
+template <int G>
+__device__ __forceinline__ unsigned long long rf_setup(const RfParams& p, unsigned crank, int (&s_pos)[G][RF_OWN],
+                                                       int (&s_ep)[G][RF_OWN], int (&s_cnt)[G][RF_OWN],
+                                                       uint64_t (&s_bar)[G][3]) {
+    extern __shared__ __align__(16) float smem[];
     const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
     const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
     const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
     const int ldwh = p.ldw[2];
-    const int gs = p.gstride;
-    float* W1s = smem + p.oW1;
-    float* W2s = smem + p.oW2;
-    float* Whs = smem + p.oWh;
     float* B1s = smem + p.oB;
     float* B2s = B1s + Nc1;
     float* Bhs = B2s + Nc2;
     float* Zm = smem + p.oZf;
     float* Zs = Zm + D;
-    float* Hs = smem + p.oHs;
-    const float* __restrict__ EWs = p.WsT;   // env matrices: global memory, through L1
-    const float* __restrict__ EWa = p.WaT;
     const long long row0 = (long long)(blockIdx.x / RF_CS) * (G * RF_ROWS);
-
-    // ---- one-time loads (as G = 1, without the env matrices; tiles and state of both groups)
     for (int f = tid; f < D * (Nc1 >> 2); f += RF_THREADS) {
         const int k = f / (Nc1 >> 2), q = f - k * (Nc1 >> 2);
-        cp_async16(W1s + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
+        cp_async16(smem + p.oW1 + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
     }
     for (int f = tid; f < H1 * (Nc2 >> 2); f += RF_THREADS) {
         const int k = f / (Nc2 >> 2), q = f - k * (Nc2 >> 2);
-        cp_async16(W2s + k * Nc2 + q * 4, p.W[1] + (long long)k * p.ldw[1] + crank * Nc2 + q * 4, 16);
+        cp_async16(smem + p.oW2 + k * Nc2 + q * 4, p.W[1] + (long long)k * p.ldw[1] + crank * Nc2 + q * 4, 16);
     }
-    for (int f = tid; f < (H2 * ldwh) >> 2; f += RF_THREADS) cp_async16(Whs + f * 4, p.W[2] + f * 4, 16);
+    for (int f = tid; f < (H2 * ldwh) >> 2; f += RF_THREADS) cp_async16(smem + p.oWh + f * 4, p.W[2] + f * 4, 16);
+    if constexpr (G == 1) {
+        float* EWs = smem + p.oEnv;
+        for (int f = tid; f < (D * D) >> 2; f += RF_THREADS) cp_async16(EWs + f * 4, p.WsT + f * 4, 16);
+        for (int f = tid; f < (A * D) >> 2; f += RF_THREADS) cp_async16(EWs + D * D + f * 4, p.WaT + f * 4, 16);
+    }
     cp_async_commit();
     for (int n = tid; n < Nc1; n += RF_THREADS) B1s[n] = p.b[0][crank * Nc1 + n];
     for (int n = tid; n < Nc2; n += RF_THREADS) B2s[n] = p.b[1][crank * Nc2 + n];
@@ -485,29 +397,235 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
         const long long i = row0 + g * RF_ROWS + m;
         float v = (i < p.N) ? p.state[i * D + k] : 0.0f;
         const int own = m - (int)crank * RF_OWN;
-        if (own >= 0 && own < RF_OWN) smem[p.oS + g * gs + own * D + k] = v;
+        if (own >= 0 && own < RF_OWN) smem[p.oS + g * p.gstride + own * D + k] = v;
         if (p.zf != nullptr) v = fminf(fmaxf((v - Zm[k]) / Zs[k], -5.0f), 5.0f);
-        smem[p.oX0 + g * gs + m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
+        smem[p.oX0 + g * p.gstride + m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
     }
-    const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
     if (tid == 0) {
         for (int g = 0; g < G; ++g)
             for (int i = 0; i < 3; ++i) mbar_init(&s_bar[g][i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    // the warps that finish the owned actors (G = 1: warps 0..7, G = 2: warps 8..15) keep their std rows
+    const int own = warp & (RF_OWN - 1);
+    if ((warp < RF_OWN) == (G == 1) && lane < A) {
+        for (int g = 0; g < G; ++g) {
+            const long long i = row0 + g * RF_ROWS + crank * RF_OWN + own;
+            const float sc = (i < p.N && p.log_noise != nullptr) ? expf(p.log_noise[i]) : 1.0f;
+            RfGroup(p, smem, g).Sd[own * A + lane] = ppo_std(p.log_var[lane], sc);
+        }
+    }
+    const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
+    cp_async_wait<0>();
+    cg::this_cluster().sync();
+    return ctr0;
+}
+
+// Head, head_mode 1: k slice sl = [sl H2/16, (sl+1) H2/16) for ALL 8 owned actors (lane = actor x 4 k sub-lanes), so the
+// head weights are read from shared memory once per step instead of once per actor (the 2 x 8 KB per actor were 1 K
+// cycles of the shared-memory pipe).  The slice sums go to Hsum [16][8][ldw[2]].
+__device__ __forceinline__ void rf_head_slice(const RfParams& p, const float* __restrict__ H2rows,
+                                              const float* __restrict__ Whs, int sl, int lane, float* __restrict__ Hsum) {
+    const int ks = p.H2 >> 4;                             // H2 % 16 == 0 (rf_plan)
+    const int ldwh = p.ldw[2];
+    const int a8 = lane >> 2, ksub = lane & 3;
+    const bool u1 = (lane & 2) != 0, u0 = (lane & 1) != 0;
+    const float* hrow = H2rows + a8 * p.ldh2 + sl * ks;
+    const float* wbase = Whs + (sl * ks) * ldwh;
+    for (int n8 = 0; n8 < p.A; n8 += 8) {
+        float s8[8];
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) s8[jj] = 0.0f;
+        const bool second = (n8 + 4 < ldwh);
+        for (int k = ksub; k < ks; k += 4) {
+            const float hv = hrow[k];
+            const float* wr = wbase + k * ldwh + n8;
+            const float4 w0 = *reinterpret_cast<const float4*>(wr);
+            s8[0] = fmaf(hv, w0.x, s8[0]); s8[1] = fmaf(hv, w0.y, s8[1]);
+            s8[2] = fmaf(hv, w0.z, s8[2]); s8[3] = fmaf(hv, w0.w, s8[3]);
+            if (second) {
+                const float4 w1 = *reinterpret_cast<const float4*>(wr + 4);
+                s8[4] = fmaf(hv, w1.x, s8[4]); s8[5] = fmaf(hv, w1.y, s8[5]);
+                s8[6] = fmaf(hv, w1.z, s8[6]); s8[7] = fmaf(hv, w1.w, s8[7]);
+            }
+        }
+        // sum over the 4 k sub-lanes: after two exchange rounds lane ksub holds outputs 2 ksub', 2 ksub' + 1
+        float t4[4], t2[2];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float recv = __shfl_xor_sync(0xffffffffu, u1 ? s8[i] : s8[i + 4], 2);
+            t4[i] = (u1 ? s8[i + 4] : s8[i]) + recv;
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const float recv = __shfl_xor_sync(0xffffffffu, u0 ? t4[i] : t4[i + 2], 1);
+            t2[i] = (u0 ? t4[i + 2] : t4[i]) + recv;
+        }
+        const int j0 = n8 + (u1 ? 4 : 0) + (u0 ? 2 : 0);
+        float* dst = Hsum + ((sl * RF_OWN + a8) * ldwh);
+        if (j0 < p.A) dst[j0] = t2[0];
+        if (j0 + 1 < p.A) dst[j0 + 1] = t2[1];
+    }
+}
+
+// Step t of owned actor `own` of a group, by the warp that finishes it, from the head's sums on: action and its staging,
+// the chunk's final outputs, the action-dependent half of the env step, reward and done, the episode step, and the
+// outbox entry of a window that completes.  Hsum: the head_mode 1 slice sums (rf_head_slice).  Returns the slot for
+// commit_actor; rew / dn are set in every lane.
+template <int G>
+__device__ __forceinline__ int rf_act_env(const RfParams& p, const RfGroup& gr, int t, int own, int lane, long long i_own,
+                                          const float* __restrict__ Hsum, const float* __restrict__ Bhs,
+                                          const float* __restrict__ EWa, int pos, int& ep_s, int& cnt_s, float& rew,
+                                          float& dn) {
+    [[maybe_unused]] const int rf_t = t;              // read by RF_STAMP only
+    const int D = p.D, A = p.A, ldwh = p.ldw[2];
+    const bool valid = i_own < p.N, final_step = (t == p.T - 1);
+    int slot = SLOT_NONE;
+    if (lane < A) {
+        const int j = lane;
+        float pre;
+        if (G == 2 || p.head_mode == 1) {             // G = 2 runs head_mode 1 only (rf_shape)
+            pre = 0.0f;
+#pragma unroll 4
+            for (int w = 0; w < RF_THREADS / 32; ++w) pre += Hsum[(w * RF_OWN + own) * ldwh + j];    // fixed order
+        } else {
+            pre = gr.Hp[own * A + j] + gr.Hp[(RF_OWN + own) * A + j];
+        }
+        RF_STAMP(19, 0);
+        const float mu = apply_act(pre + Bhs[j], p.act[2]);
+        const float sd = gr.Sd[own * A + j];
+        const float a = ppo_action(mu, sd, gr.Zn[own * A + j], p.deterministic);
+        gr.Ac[own * A + j] = a;
+        if (valid) {
+            p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
+            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + j] = mu;
+            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + A + j] = sd;
+            if (final_step) {
+                p.action[i_own * A + j] = a;
+                p.pd[i_own * 2 * A + j] = mu;
+                p.pd[i_own * 2 * A + A + j] = sd;
+            }
+        }
+    }
+    __syncwarp();
+    RF_STAMP(20, 0);
+    float* sown = gr.S + own * D;
+    const int ep = ep_s + 1;
+    const bool is_done = env_done(ep, p.max_steps);
+    dn = is_done ? 1.0f : 0.0f;
+    rew = env_reward(gr.Eq[2 * own], D, gr.Eq[2 * own + 1]);
+    for (int d = lane; d < D; d += 32) {
+        float acc = gr.Eacc[own * D + d];
+#pragma unroll 4
+        for (int k = 0; k < A; ++k) acc = fmaf(rf_env_w<G>(EWa + k * D + d), gr.Ac[own * A + k], acc);
+        const float nxt = env_successor(acc, gr.Egx[own * D + d]);
+        gr.Nx[own * D + d] = nxt;
+        sown[d] = is_done ? gr.Erz[own * D + d] : nxt;
+        if (valid && final_step) p.obs_next[i_own * D + d] = nxt;
+    }
+    RF_STAMP(21, 0);
+    if (lane == 0) {
+        ep_s = is_done ? 0 : ep;
+        if (valid && final_step) {
+            p.reward[i_own] = rew;
+            p.done[i_own] = dn;
+        }
+        if (valid && pos + 1 == p.n_step) {
+            const int w = cnt_s;
+            if (w < p.Wout) {
+                slot = (int)(i_own * p.Wout + w);
+                p.ev_step[slot] = t;
+                cnt_s = w + 1;
+            } else {
+                slot = SLOT_DROPPED;
+            }
+        }
+    }
+    slot = __shfl_sync(0xffffffffu, slot, 0);
+    __syncwarp();
+    return slot;
+}
+
+// Next observation of owned actor `own` (tile row m) -> z-filter -> its row of this CTA's input tile and, by st.async
+// counted on the peers' mbarrier at bar_off, of the three peers' tiles.  Not after a chunk's last step: nobody reads it.
+__device__ __forceinline__ void rf_push_input(const RfParams& p, const RfGroup& gr, int own, int m, long long i_own,
+                                              int lane, unsigned smem_base, const unsigned (&peer_base)[RF_CS - 1],
+                                              unsigned bar_off) {
+    extern __shared__ __align__(16) float smem[];
+    const float* Zm = smem + p.oZf;
+    const float* Zs = Zm + p.D;
+    const int q4 = lane;
+    if (q4 < (p.D >> 2)) {
+        float4 v = *reinterpret_cast<const float4*>(gr.S + own * p.D + q4 * 4);
+        if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (p.zf != nullptr) {
+            const float4 zm = *reinterpret_cast<const float4*>(Zm + q4 * 4);
+            const float4 zs = *reinterpret_cast<const float4*>(Zs + q4 * 4);
+            v.x = fminf(fmaxf((v.x - zm.x) / zs.x, -5.0f), 5.0f);
+            v.y = fminf(fmaxf((v.y - zm.y) / zs.y, -5.0f), 5.0f);
+            v.z = fminf(fmaxf((v.z - zm.z) / zs.z, -5.0f), 5.0f);
+            v.w = fminf(fmaxf((v.w - zm.w) / zs.w, -5.0f), 5.0f);
+            if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        float* qx = gr.X0 + m * p.ldx0 + q4 * 4;
+        *reinterpret_cast<float4*>(qx) = v;
+        const unsigned off = smem_u32(qx) - smem_base;
+#pragma unroll
+        for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off);
+    }
+}
+
+// Two groups of 32 actors per cluster (G = 2), software-pipelined, so that a chunk of N actors needs half as many
+// clusters.  Warps 0..7 ("layer warps") run hidden layers 1 and 2 for group 0, then for group 1, step after step.
+// Warps 8..15 ("tail warps", warp 8 + a for owned actor a of each group) take the whole tail of a group -- the
+// action-independent env precompute, head, sampling, env step, window staging, the push of the next input rows -- while
+// the layer warps compute the other group.  Arithmetic, operand order and Philox keys are those of the G = 1 schedule
+// (head_mode 1, the same layer, head slice and tail functions), so both give the same results.
+//
+// Hand-offs, per group g (each group has its own tiles, state and three mbarriers):
+//   layer -> peers: H1 rows (all 32) and H2 rows (owners' only) by st.async, counted on the receiver's h1[g] / h2[g];
+//   layer -> tail:  own H2 rows, named barrier 2 + g (layer warps bar.arrive, tail warps bar.sync; 512 threads);
+//   tail  -> peers: next X0 rows by st.async, counted on x0[g];
+//   tail  -> layer: own next X0 rows, named barrier 4 + g (tail warps bar.arrive, layer warps bar.sync).
+// No reverse "buffer free" signal is needed: every buffer of group g is rewritten only behind a chain of hand-offs that
+// starts after its last reader is done.
+//   * X0[g], step t+1: a peer pushes it after its head of step t, which needs this CTA's H2 rows of step t, which the
+//     layer warps push only after all of them passed layer 1 (rf_bar_math), the last reader of X0[g].  The tail warps
+//     rewrite their own rows after their head, i.e. after named barrier 2 + g, which every layer warp reaches after layer 2.
+//   * H1[g], step t+1: a peer pushes it after its layer 1 of step t+1, which needs this CTA's X0 rows of step t+1, which
+//     the tail warps push after named barrier 2 + g: after every layer warp has finished layer 2, the reader of H1[g].
+//   * H2[g], step t+1: written by layer 2 of step t+1 (peers' and own), behind layer 1 of step t+1, behind the X0 rows of
+//     step t+1 of every CTA of the cluster, which this CTA's tail pushes after its head of step t, the reader of H2[g].
+//   * the same chains order every st.async of step t+1 after the mbarrier wait of step t, so no phase receives bytes of
+//     the next one.  Each phase is armed once (expect_tx; arrival count 1) by thread 0 after the previous phase is known
+//     complete: h1[g] and h2[g] after the layer warps' wait on named barrier 4 + g (the tail waited h2[g] of the step
+//     before), x0[g] after the layer warps' own wait on x0[g].
+//   * named barriers 2 + g and 4 + g never see two generations of arrivals at once: each arrival of step t+1 sits behind
+//     the other side's arrival of step t on the other barrier.
+//   * the head slice buffer is used by the tail warps only, between named barrier 6 (tail warps, 256 threads) and the
+//     next group's named barrier 2 + g', which all 256 tail threads must reach.
+__device__ __forceinline__ void rf2_two_groups(const RfParams& p, unsigned crank, unsigned long long ctr0,
+                                               int (&s_pos)[2][RF_OWN], int (&s_ep)[2][RF_OWN], int (&s_cnt)[2][RF_OWN],
+                                               uint64_t (&s_bar)[2][3]) {
+    constexpr int G = 2;
+    extern __shared__ __align__(16) float smem[];
+    const unsigned smem_base = smem_u32(smem);
+    unsigned peer_base[RF_CS - 1];
+#pragma unroll
+    for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
+    const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
+    const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
+    const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
+    float* B1s = smem + p.oB;
+    float* B2s = B1s + Nc1;
+    float* Bhs = B2s + Nc2;
+    float* Hs = smem + p.oHs;
+    const float* __restrict__ EWs = p.WsT;   // env matrices: global memory, through L1
+    const long long row0 = (long long)(blockIdx.x / RF_CS) * (G * RF_ROWS);
     // bytes a CTA receives from its three peers per step and group (as G = 1)
     const unsigned tx_h1 = 3u * RF_ROWS * Nc1 * 4u, tx_h2 = 3u * RF_OWN * Nc2 * 4u, tx_x0 = 3u * RF_OWN * D * 4u;
     const bool layer = warp < RF_OWN;
     const int own = warp & (RF_OWN - 1);              // tail warp 8 + own: owned actor `own` of each group
-    if (!layer && lane < A) {
-        for (int g = 0; g < G; ++g) {
-            const long long i = row0 + g * RF_ROWS + crank * RF_OWN + own;
-            const float sc = (i < p.N && p.log_noise != nullptr) ? expf(p.log_noise[i]) : 1.0f;
-            smem[p.oAct + g * gs + 2 * RF_OWN * A + own * A + lane] = __fmul_rn(expf(p.log_var[lane]), sc);
-        }
-    }
-    cp_async_wait<0>();
-    cluster.sync();
 
     if (layer) {
         for (int t = 0; t < p.T; ++t) {
@@ -515,9 +633,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
             [[maybe_unused]] const int rf_t = t;      // read by RF_STAMP only
             RF_STAMP(0, 0);
             for (int g = 0; g < G; ++g) {
-                float* X0 = smem + p.oX0 + g * gs;
-                float* Hb1 = smem + p.oH1 + g * gs;
-                float* Hb2 = smem + p.oH2 + g * gs;
+                const RfGroup gr(p, smem, g);
                 if (t > 0) {                                   // own rows from the tail warps, the peers' rows by st.async
                     rf_bar_sync(4 + g, 2 * 256);
                     rf_mbar_wait(&s_bar[g][2], (unsigned)(t - 1) & 1u);
@@ -527,337 +643,118 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p) {
                     mbar_arrive_expect_tx(&s_bar[g][1], tx_h2);
                     if (!final_step) mbar_arrive_expect_tx(&s_bar[g][2], tx_x0);
                 }
-                rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank,
-                           smem_u32(&s_bar[g][0]) - smem_base);
+                rf2_layer1(gr.X0, p.ldx0, D, smem + p.oW1, Nc1, B1s, p.act[0], gr.H1, p.ldh1, (int)crank * Nc1, smem_base,
+                           crank, smem_u32(&s_bar[g][0]) - smem_base);
                 rf_bar_math();
                 rf_mbar_wait(&s_bar[g][0], (unsigned)t & 1u);
                 RF_STAMP(3 + 2 * g, 0);
-                rf2_layer2_direct(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, smem_base, crank,
-                                  smem_u32(&s_bar[g][1]) - smem_base);
+                rf2_layer2_direct(gr.H1, p.ldh1, H1, smem + p.oW2, Nc2, B2s, p.act[1], gr.H2, p.ldh2, (int)crank * Nc2,
+                                  smem_base, crank, smem_u32(&s_bar[g][1]) - smem_base);
                 RF_STAMP(4 + 2 * g, 0);
                 rf_bar_arrive(2 + g, 2 * 256);
             }
         }
-    } else {
-        for (int t = 0; t < p.T; ++t) {
-            const unsigned long long ctr = ctr0 + (unsigned long long)t;
-            const bool final_step = (t == p.T - 1);
-            [[maybe_unused]] const int rf_t = t;      // read by RF_STAMP only
-            for (int g = 0; g < G; ++g) {
-                float* X0 = smem + p.oX0 + g * gs;
-                float* Hb2 = smem + p.oH2 + g * gs;
-                float* S = smem + p.oS + g * gs;
-                float* Nx = smem + p.oNext + g * gs;
-                float* Ac = smem + p.oAct + g * gs;
-                float* Sd = Ac + 2 * RF_OWN * A;
-                float* Zn = Sd + RF_OWN * A;
-                float* Eacc = smem + p.oPre + g * gs;
-                float* Egx = Eacc + RF_OWN * D;
-                float* Erz = Egx + RF_OWN * D;
-                float* Eq = Erz + RF_OWN * D;
-                const int m_own = (int)crank * RF_OWN + own;
-                const long long i_own = row0 + g * RF_ROWS + m_own;
-                const bool valid = i_own < p.N;
-                RF_STAMP(8 + 4 * g, 256);
-                // ---- everything of the step that does not depend on the action: the env warps' arithmetic of G = 1, but a
-                // lane takes the adjacent columns d, d + 1 together (two independent FMA chains, float2 weight and float4
-                // state loads): here this work is on the step's critical path, next to layer warps that keep the
-                // shared-memory pipe busy, so its loads and dependent latencies are what count
-                {
-                    const float* sh = S + own * D;
-                    float q = 0.0f;
-                    for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
-                    q = warp_sum(q);
-                    const bool h_done = (p.max_steps > 0) && (s_ep[g][own] + 1 >= p.max_steps);
-                    for (int d = 2 * lane; d < D; d += 64) {          // D % 4 == 0: d + 1 < D
-                        float acc0 = 0.0f, acc1 = 0.0f;
-#pragma unroll 4
-                        for (int k = 0; k < D; k += 4) {
-                            const float4 s4 = *reinterpret_cast<const float4*>(sh + k);
-                            const float2 w0 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 0) * D + d));
-                            const float2 w1 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 1) * D + d));
-                            const float2 w2 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 2) * D + d));
-                            const float2 w3 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 3) * D + d));
-                            acc0 = fmaf(w0.x, s4.x, acc0); acc1 = fmaf(w0.y, s4.x, acc1);
-                            acc0 = fmaf(w1.x, s4.y, acc0); acc1 = fmaf(w1.y, s4.y, acc1);
-                            acc0 = fmaf(w2.x, s4.z, acc0); acc1 = fmaf(w2.y, s4.z, acc1);
-                            acc0 = fmaf(w3.x, s4.w, acc0); acc1 = fmaf(w3.y, s4.w, acc1);
-                        }
-                        const Philox4 r0 = env_noise(p.env_seed, ctr, i_own, d);
-                        const Philox4 r1 = env_noise(p.env_seed, ctr, i_own, d + 1);
-                        const float2 gz0 = box_muller(r0.x, r0.y), gz1 = box_muller(r1.x, r1.y);
-                        *reinterpret_cast<float2*>(Eacc + own * D + d) = make_float2(acc0, acc1);
-                        *reinterpret_cast<float2*>(Egx + own * D + d) = make_float2(gz0.x, gz1.x);
-                        *reinterpret_cast<float2*>(Erz + own * D + d) =
-                            h_done ? make_float2(box_muller(r0.z, r0.w).x, box_muller(r1.z, r1.w).x) : make_float2(0.0f, 0.0f);
-                        if (d == 0) {
-                            Eq[2 * own] = q;
-                            Eq[2 * own + 1] = gz0.y;
-                        }
-                    }
-                    if (!p.deterministic && lane < A) Zn[own * A + lane] = action_noise1(p.agent_seed, ctr, i_own, lane);
-                }
-                rf_bar_sync(2 + g, 2 * 256);                   // own rows of the last hidden layer, then the peers' rows
-                rf_mbar_wait(&s_bar[g][1], (unsigned)t & 1u);
-                RF_STAMP(9 + 4 * g, 256);
-                // ---- head, head_mode 1: the 16 k slices of G = 1, two per tail warp, same lane layout and sums
-                {
-                    const int ks = H2 >> 4;
-                    const int a8 = lane >> 2, ksub = lane & 3;
-                    const bool u1 = (lane & 2) != 0, u0 = (lane & 1) != 0;
-                    for (int sl = own; sl < 16; sl += RF_OWN) {
-                        const float* hrow = Hb2 + a8 * p.ldh2 + sl * ks;
-                        const float* wbase = Whs + (sl * ks) * ldwh;
-                        for (int n8 = 0; n8 < A; n8 += 8) {
-                            float s8[8];
-#pragma unroll
-                            for (int jj = 0; jj < 8; ++jj) s8[jj] = 0.0f;
-                            const bool second = (n8 + 4 < ldwh);
-                            for (int k = ksub; k < ks; k += 4) {
-                                const float hv = hrow[k];
-                                const float* wr = wbase + k * ldwh + n8;
-                                const float4 w0 = *reinterpret_cast<const float4*>(wr);
-                                s8[0] = fmaf(hv, w0.x, s8[0]); s8[1] = fmaf(hv, w0.y, s8[1]);
-                                s8[2] = fmaf(hv, w0.z, s8[2]); s8[3] = fmaf(hv, w0.w, s8[3]);
-                                if (second) {
-                                    const float4 w1 = *reinterpret_cast<const float4*>(wr + 4);
-                                    s8[4] = fmaf(hv, w1.x, s8[4]); s8[5] = fmaf(hv, w1.y, s8[5]);
-                                    s8[6] = fmaf(hv, w1.z, s8[6]); s8[7] = fmaf(hv, w1.w, s8[7]);
-                                }
-                            }
-                            float t4[4], t2[2];
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float recv = __shfl_xor_sync(0xffffffffu, u1 ? s8[i] : s8[i + 4], 2);
-                                t4[i] = (u1 ? s8[i + 4] : s8[i]) + recv;
-                            }
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) {
-                                const float recv = __shfl_xor_sync(0xffffffffu, u0 ? t4[i] : t4[i + 2], 1);
-                                t2[i] = (u0 ? t4[i + 2] : t4[i]) + recv;
-                            }
-                            const int j0 = n8 + (u1 ? 4 : 0) + (u0 ? 2 : 0);
-                            float* dst = Hs + ((sl * RF_OWN + a8) * ldwh);
-                            if (j0 < A) dst[j0] = t2[0];
-                            if (j0 + 1 < A) dst[j0 + 1] = t2[1];
-                        }
-                    }
-                }
-                rf_bar_sync(6, 256);
-                RF_STAMP(10 + 4 * g, 256);
-                // ---- action, env step, bookkeeping (the owner warps' code of G = 1)
-                float rew, dn;
-                int slot = SLOT_NONE;
-                {
-                    const int pos = s_pos[g][own];
-                    if (lane < A) {
-                        const int j = lane;
-                        float pre = 0.0f;
-#pragma unroll 4
-                        for (int w = 0; w < RF_THREADS / 32; ++w) pre += Hs[(w * RF_OWN + own) * ldwh + j];
-                        const float mu = apply_act(pre + Bhs[j], p.act[2]);
-                        const float sd = Sd[own * A + j];
-                        float a = mu;
-                        if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
-                        a = fminf(fmaxf(a, -1.0f), 1.0f);
-                        Ac[own * A + j] = a;
-                        if (valid) {
-                            p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
-                            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + j] = mu;
-                            p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + A + j] = sd;
-                            if (final_step) {
-                                p.action[i_own * A + j] = a;
-                                p.pd[i_own * 2 * A + j] = mu;
-                                p.pd[i_own * 2 * A + A + j] = sd;
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    float* sown = S + own * D;
-                    const int ep = s_ep[g][own] + 1;
-                    const bool is_done = (p.max_steps > 0) && (ep >= p.max_steps);
-                    dn = is_done ? 1.0f : 0.0f;
-                    rew = -Eq[2 * own] / (float)D + 0.1f * Eq[2 * own + 1];
-                    for (int d = lane; d < D; d += 32) {
-                        float acc = Eacc[own * D + d];
-#pragma unroll 4
-                        for (int k = 0; k < A; ++k) acc = fmaf(__ldg(EWa + k * D + d), Ac[own * A + k], acc);
-                        const float nxt = tanhf(acc) + 0.01f * Egx[own * D + d];
-                        Nx[own * D + d] = nxt;
-                        sown[d] = is_done ? Erz[own * D + d] : nxt;
-                        if (valid && final_step) p.obs_next[i_own * D + d] = nxt;
-                    }
-                    if (lane == 0) {
-                        s_ep[g][own] = is_done ? 0 : ep;
-                        if (valid && final_step) {
-                            p.reward[i_own] = rew;
-                            p.done[i_own] = dn;
-                        }
-                        if (valid && pos + 1 == p.n_step) {
-                            const int w = s_cnt[g][own];
-                            if (w < p.Wout) {
-                                slot = (int)(i_own * p.Wout + w);
-                                p.ev_step[slot] = t;
-                                s_cnt[g][own] = w + 1;
-                            } else {
-                                slot = SLOT_DROPPED;
-                            }
-                        }
-                    }
-                    slot = __shfl_sync(0xffffffffu, slot, 0);
-                    __syncwarp();
-                }
-                commit_actor(valid, (int)i_own, lane, 32, Nx + own * D, S + own * D, rew, dn, p.n_step, p.stride, D, A,
-                             &s_pos[g][own], slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew, p.stage_done, p.o_obs,
-                             p.o_act, p.o_pd, p.o_rew, p.o_done, WarpBarrier());
-                RF_STAMP(11 + 4 * g, 256);
-                if (!final_step) {                             // next observation -> z-filter -> every CTA's input tile
-                    const int q4 = lane;
-                    if (q4 < (D >> 2)) {
-                        float4 v = *reinterpret_cast<const float4*>(S + own * D + q4 * 4);
-                        if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (p.zf != nullptr) {
-                            const float4 zm = *reinterpret_cast<const float4*>(Zm + q4 * 4);
-                            const float4 zs = *reinterpret_cast<const float4*>(Zs + q4 * 4);
-                            v.x = fminf(fmaxf((v.x - zm.x) / zs.x, -5.0f), 5.0f);
-                            v.y = fminf(fmaxf((v.y - zm.y) / zs.y, -5.0f), 5.0f);
-                            v.z = fminf(fmaxf((v.z - zm.z) / zs.z, -5.0f), 5.0f);
-                            v.w = fminf(fmaxf((v.w - zm.w) / zs.w, -5.0f), 5.0f);
-                            if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        }
-                        float* qx = X0 + m_own * p.ldx0 + q4 * 4;
-                        *reinterpret_cast<float4*>(qx) = v;
-                        const unsigned off = smem_u32(qx) - smem_base;
-                        const unsigned bar_off = smem_u32(&s_bar[g][2]) - smem_base;
-#pragma unroll
-                        for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off);
-                    }
-                    rf_bar_arrive(4 + g, 2 * 256);
-                }
-            }
-        }
+        return;
     }
-    cluster.sync();                                           // nobody leaves while a peer may still address its shared memory
-
-    if (!layer) {
+    for (int t = 0; t < p.T; ++t) {
+        const unsigned long long ctr = ctr0 + (unsigned long long)t;
+        [[maybe_unused]] const int rf_t = t;          // read by RF_STAMP only
         for (int g = 0; g < G; ++g) {
-            const long long i_own = row0 + g * RF_ROWS + (int)crank * RF_OWN + own;
-            if (i_own >= p.N) continue;
-            const float* S = smem + p.oS + g * gs;
-            for (int d = lane; d < D; d += 32) p.state[i_own * D + d] = S[own * D + d];
-            if (lane == 0) {
-                p.stage_pos[i_own] = s_pos[g][own];
-                p.ep_step[i_own] = s_ep[g][own];
-                p.ev_count[i_own] = s_cnt[g][own];
+            const RfGroup gr(p, smem, g);
+            const int m_own = (int)crank * RF_OWN + own;
+            const long long i_own = row0 + g * RF_ROWS + m_own;
+            RF_STAMP(8 + 4 * g, 256);
+            // ---- everything of the step that does not depend on the action: the env warps' arithmetic of G = 1, but a
+            // lane takes the adjacent columns d, d + 1 together (two independent FMA chains, float2 weight and float4
+            // state loads): here this work is on the step's critical path, next to layer warps that keep the
+            // shared-memory pipe busy, so its loads and dependent latencies are what count
+            {
+                const float* sh = gr.S + own * D;
+                float q = 0.0f;
+                for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
+                q = warp_sum(q);
+                const bool h_done = env_done(s_ep[g][own] + 1, p.max_steps);
+                for (int d = 2 * lane; d < D; d += 64) {          // D % 4 == 0: d + 1 < D
+                    float acc0 = 0.0f, acc1 = 0.0f;
+#pragma unroll 4
+                    for (int k = 0; k < D; k += 4) {
+                        const float4 s4 = *reinterpret_cast<const float4*>(sh + k);
+                        const float2 w0 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 0) * D + d));
+                        const float2 w1 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 1) * D + d));
+                        const float2 w2 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 2) * D + d));
+                        const float2 w3 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 3) * D + d));
+                        acc0 = fmaf(w0.x, s4.x, acc0); acc1 = fmaf(w0.y, s4.x, acc1);
+                        acc0 = fmaf(w1.x, s4.y, acc0); acc1 = fmaf(w1.y, s4.y, acc1);
+                        acc0 = fmaf(w2.x, s4.z, acc0); acc1 = fmaf(w2.y, s4.z, acc1);
+                        acc0 = fmaf(w3.x, s4.w, acc0); acc1 = fmaf(w3.y, s4.w, acc1);
+                    }
+                    const Philox4 r0 = env_noise(p.env_seed, ctr, i_own, d);
+                    const Philox4 r1 = env_noise(p.env_seed, ctr, i_own, d + 1);
+                    const float2 gz0 = box_muller(r0.x, r0.y), gz1 = box_muller(r1.x, r1.y);
+                    *reinterpret_cast<float2*>(gr.Eacc + own * D + d) = make_float2(acc0, acc1);
+                    *reinterpret_cast<float2*>(gr.Egx + own * D + d) = make_float2(gz0.x, gz1.x);
+                    *reinterpret_cast<float2*>(gr.Erz + own * D + d) =
+                        h_done ? make_float2(env_reset_draw(r0), env_reset_draw(r1)) : make_float2(0.0f, 0.0f);
+                    if (d == 0) {
+                        gr.Eq[2 * own] = q;
+                        gr.Eq[2 * own + 1] = gz0.y;
+                    }
+                }
+                if (!p.deterministic && lane < A) gr.Zn[own * A + lane] = action_noise1(p.agent_seed, ctr, i_own, lane);
+            }
+            rf_bar_sync(2 + g, 2 * 256);                   // own rows of the last hidden layer, then the peers' rows
+            rf_mbar_wait(&s_bar[g][1], (unsigned)t & 1u);
+            RF_STAMP(9 + 4 * g, 256);
+            // ---- head: the 16 k slices of G = 1, two per tail warp; their sums meet in the head slice buffer
+            for (int sl = own; sl < 16; sl += RF_OWN) rf_head_slice(p, gr.H2, smem + p.oWh, sl, lane, Hs);
+            rf_bar_sync(6, 256);
+            RF_STAMP(10 + 4 * g, 256);
+            float rew, dn;
+            const int slot = rf_act_env<G>(p, gr, t, own, lane, i_own, Hs, Bhs, p.WaT, s_pos[g][own], s_ep[g][own],
+                                           s_cnt[g][own], rew, dn);
+            commit_actor(i_own < p.N, (int)i_own, lane, 32, gr.Nx + own * D, gr.S + own * D, rew, dn, p.n_step, p.stride,
+                         D, A, &s_pos[g][own], slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew, p.stage_done,
+                         p.o_obs, p.o_act, p.o_pd, p.o_rew, p.o_done, WarpBarrier());
+            RF_STAMP(11 + 4 * g, 256);
+            if (t < p.T - 1) {
+                rf_push_input(p, gr, own, m_own, i_own, lane, smem_base, peer_base, smem_u32(&s_bar[g][2]) - smem_base);
+                rf_bar_arrive(4 + g, 2 * 256);
             }
         }
     }
 }
 
-template <int G>
-__global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
-    ppo_rollout2_kernel(const __grid_constant__ RfParams p) {
-    RF_CTA_STAMP(1);
-    if constexpr (G == 2) {
-        rf2_two_groups(p);
-        RF_CTA_STAMP(2);
-        return;
-    }
-    cg::cluster_group cluster = cg::this_cluster();
-    const unsigned crank = cluster.block_rank();
+// One group of 32 actors per cluster (G = 1).  Warps 0..7 run the hidden layers, then each finishes owned actor `warp`;
+// warps 8..15 do the action-independent half of the env step of owned actor `warp & 7` beside the layers.  The block
+// barriers of the step order every hand-off inside the CTA.
+__device__ __forceinline__ void rf_one_group(const RfParams& p, unsigned crank, unsigned long long ctr0,
+                                             int (&s_pos)[RF_OWN], int (&s_ep)[RF_OWN], int (&s_cnt)[RF_OWN],
+                                             uint64_t (&s_bar)[3]) {
     extern __shared__ __align__(16) float smem[];
     const unsigned smem_base = smem_u32(smem);
     unsigned peer_base[RF_CS - 1];
 #pragma unroll
     for (int c = 1; c < RF_CS; ++c) peer_base[c - 1] = mapa_u32(smem_base, (crank + (unsigned)c) % RF_CS);
-    __shared__ int s_pos[RF_OWN], s_ep[RF_OWN], s_cnt[RF_OWN];
-    __shared__ __align__(8) uint64_t s_bar[3];      // hidden layer 1 | last hidden layer rows | next input tile
-
     // (tried: the two roles on swapped warp halves, in case the scheduler's preference for one end of the warp index range
     // starved the layers -- no difference in clock64 traces)
     const int tid = (int)RF_TID, lane = tid & 31, warp = tid >> 5;
     const int D = p.D, H1 = p.H1, H2 = p.H2, A = p.A;
     const int Nc1 = H1 / RF_CS, Nc2 = H2 / RF_CS;
     const int ldwh = p.ldw[2];
-    float* W1s = smem + p.oW1;
-    float* W2s = smem + p.oW2;
     float* Whs = smem + p.oWh;
     float* B1s = smem + p.oB;
     float* B2s = B1s + Nc1;
     float* Bhs = B2s + Nc2;
-    float* X0 = smem + p.oX0;
-    float* Hb1 = smem + p.oH1;
-    float* Hb2 = smem + p.oH2;
     float* Part = smem + p.oPart;
-    float* Zm = smem + p.oZf;
-    float* Zs = Zm + D;
     float* EWs = smem + p.oEnv;
     float* EWa = EWs + D * D;
-    float* S = smem + p.oS;
-    float* Nx = smem + p.oNext;
-    float* Ac = smem + p.oAct;
-    float* Sd = Ac + 2 * RF_OWN * A;     // (slot 1 unused, see rf_plan)
-    float* Zn = Sd + RF_OWN * A;
-    float* Hp = Zn + RF_OWN * A;         // [2][8][A] head partial sums of the two k halves
-    float* Eacc = smem + p.oPre;
-    float* Egx = Eacc + RF_OWN * D;
-    float* Erz = Egx + RF_OWN * D;
-    float* Eq = Erz + RF_OWN * D;
+    const RfGroup gr(p, smem, 0);
     const long long row0 = (long long)(blockIdx.x / RF_CS) * RF_ROWS;
-
-    // ---- one-time loads: weight slices, biases, env matrices (cp.async burst), z-filter columns, actor state
-    for (int f = tid; f < D * (Nc1 >> 2); f += RF_THREADS) {
-        const int k = f / (Nc1 >> 2), q = f - k * (Nc1 >> 2);
-        cp_async16(W1s + k * Nc1 + q * 4, p.W[0] + (long long)k * p.ldw[0] + crank * Nc1 + q * 4, 16);
-    }
-    for (int f = tid; f < H1 * (Nc2 >> 2); f += RF_THREADS) {
-        const int k = f / (Nc2 >> 2), q = f - k * (Nc2 >> 2);
-        cp_async16(W2s + k * Nc2 + q * 4, p.W[1] + (long long)k * p.ldw[1] + crank * Nc2 + q * 4, 16);
-    }
-    for (int f = tid; f < (H2 * ldwh) >> 2; f += RF_THREADS) cp_async16(Whs + f * 4, p.W[2] + f * 4, 16);
-    for (int f = tid; f < (D * D) >> 2; f += RF_THREADS) cp_async16(EWs + f * 4, p.WsT + f * 4, 16);
-    for (int f = tid; f < (A * D) >> 2; f += RF_THREADS) cp_async16(EWa + f * 4, p.WaT + f * 4, 16);
-    cp_async_commit();
-    for (int n = tid; n < Nc1; n += RF_THREADS) B1s[n] = p.b[0][crank * Nc1 + n];
-    for (int n = tid; n < Nc2; n += RF_THREADS) B2s[n] = p.b[1][crank * Nc2 + n];
-    for (int n = tid; n < ldwh; n += RF_THREADS) Bhs[n] = (n < A) ? p.b[2][n] : 0.0f;
-    if (p.zf != nullptr) {
-        const float cnt = p.zf[2 * D];
-        for (int k = tid; k < D; k += RF_THREADS) {
-            const float mean = p.zf[k] / cnt;
-            const float var = p.zf[D + k] / cnt - mean * mean;
-            Zm[k] = mean;
-            Zs[k] = fmaxf(sqrtf(var), p.zf_eps);
-        }
-    }
-    if (tid < RF_OWN) {
-        const long long i = row0 + crank * RF_OWN + tid;
-        s_pos[tid] = (i < p.N) ? p.stage_pos[i] : 0;
-        s_ep[tid] = (i < p.N) ? p.ep_step[i] : 0;
-        s_cnt[tid] = 0;
-    }
-    __syncthreads();
-    for (int idx = tid; idx < RF_ROWS * D; idx += RF_THREADS) {
-        const int m = idx / D, k = idx - m * D;
-        const long long i = row0 + m;
-        float v = (i < p.N) ? p.state[i * D + k] : 0.0f;
-        const int own = m - (int)crank * RF_OWN;
-        if (own >= 0 && own < RF_OWN) S[own * D + k] = v;
-        if (p.zf != nullptr) v = fminf(fmaxf((v - Zm[k]) / Zs[k], -5.0f), 5.0f);
-        X0[m * p.ldx0 + k] = (i < p.N) ? v : 0.0f;
-    }
-    const unsigned long long ctr0 = (p.step_ctr != nullptr) ? *p.step_ctr : 0ull;
-    if (tid == 0) {
-        for (int i = 0; i < 3; ++i) mbar_init(&s_bar[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     const unsigned bar_off_h1 = smem_u32(&s_bar[0]) - smem_base, bar_off_h2 = smem_u32(&s_bar[1]) - smem_base;
     const unsigned bar_off_x0 = smem_u32(&s_bar[2]) - smem_base;
     // bytes a CTA receives from its three peers per step: their column quarters of hidden layer 1 for all 32 rows, their
     // column quarters of the last hidden layer for the 8 owned rows, their 8 rows of the next input tile
     const unsigned tx_h1 = 3u * RF_ROWS * Nc1 * 4u, tx_h2 = 3u * RF_OWN * Nc2 * 4u, tx_x0 = 3u * RF_OWN * D * 4u;
-    cp_async_wait<0>();
-    cluster.sync();
 
     const bool math = warp < RF_OWN;                  // warps 0..7: layers, then owner of actor `warp`
     const int own = warp & (RF_OWN - 1);              // owned actor this warp works for (owner or env warp)
@@ -865,16 +762,11 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
     const int m_own = (int)crank * RF_OWN + own;
     const long long i_own = row0 + m_own;
     const bool valid = owner && (i_own < p.N);
-    {
-        const float sc = (i_own < p.N && p.log_noise != nullptr) ? expf(p.log_noise[i_own]) : 1.0f;
-        if (owner && lane < A) Sd[own * A + lane] = __fmul_rn(expf(p.log_var[lane]), sc);
-    }
-    __syncthreads();
 
     for (int t = 0; t < p.T; ++t) {
         const unsigned long long ctr = ctr0 + (unsigned long long)t;
         const bool final_step = (t == p.T - 1);
-        const int rf_t = t;
+        [[maybe_unused]] const int rf_t = t;          // read by RF_STAMP only
         RF_STAMP(0, 0);
         if (tid == 0) {                                       // arm this step's phases (the previous ones were consumed)
             mbar_arrive_expect_tx(&s_bar[0], tx_h1);
@@ -887,13 +779,14 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
             }
             RF_STAMP(18, 0);
             if (tid == 0 && !final_step) mbar_arrive_expect_tx(&s_bar[2], tx_x0);     // next tile's phase: only now is the previous one complete
-            rf2_layer1(X0, p.ldx0, D, W1s, Nc1, B1s, p.act[0], Hb1, p.ldh1, (int)crank * Nc1, smem_base, crank, bar_off_h1);
+            rf2_layer1(gr.X0, p.ldx0, D, smem + p.oW1, Nc1, B1s, p.act[0], gr.H1, p.ldh1, (int)crank * Nc1, smem_base, crank,
+                       bar_off_h1);
             RF_STAMP(3, 0);
             rf_bar_math();
             rf_mbar_wait(&s_bar[0], (unsigned)t & 1u);
             RF_STAMP(4, 0);
-            rf2_layer(Hb1, p.ldh1, H1, W2s, Nc2, B2s, p.act[1], Hb2, p.ldh2, (int)crank * Nc2, Part, smem_base, crank, rf_t, 5,
-                      bar_off_h2);
+            rf2_layer2_direct(gr.H1, p.ldh1, H1, smem + p.oW2, Nc2, B2s, p.act[1], gr.H2, p.ldh2, (int)crank * Nc2, smem_base,
+                              crank, bar_off_h2);
             RF_STAMP(7, 0);
         } else {
             // ---- env warp h: everything of this step that does not depend on the action (the arithmetic of sample_one() /
@@ -901,77 +794,37 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
             RF_STAMP(16, 256);
             const int h = own;
             const long long ih = row0 + (int)crank * RF_OWN + h;
-            const float* sh = S + h * D;
+            const float* sh = gr.S + h * D;
             float q = 0.0f;
             for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
             q = warp_sum(q);
-            const bool h_done = (p.max_steps > 0) && (s_ep[h] + 1 >= p.max_steps);
+            const bool h_done = env_done(s_ep[h] + 1, p.max_steps);
             for (int d = lane; d < D; d += 32) {
                 float acc = 0.0f;
 #pragma unroll 8
                 for (int k = 0; k < D; ++k) acc = fmaf(EWs[k * D + d], sh[k], acc);
                 const Philox4 r = env_noise(p.env_seed, ctr, ih, d);
                 const float2 gz = box_muller(r.x, r.y);
-                Eacc[h * D + d] = acc;
-                Egx[h * D + d] = gz.x;
-                Erz[h * D + d] = h_done ? box_muller(r.z, r.w).x : 0.0f;
+                gr.Eacc[h * D + d] = acc;
+                gr.Egx[h * D + d] = gz.x;
+                gr.Erz[h * D + d] = h_done ? env_reset_draw(r) : 0.0f;
                 if (d == 0) {
-                    Eq[2 * h] = q;
-                    Eq[2 * h + 1] = gz.y;
+                    gr.Eq[2 * h] = q;
+                    gr.Eq[2 * h + 1] = gz.y;
                 }
             }
-            if (!p.deterministic && lane < A) Zn[h * A + lane] = action_noise1(p.agent_seed, ctr, ih, lane);
+            if (!p.deterministic && lane < A) gr.Zn[h * A + lane] = action_noise1(p.agent_seed, ctr, ih, lane);
             RF_STAMP(17, 256);
         }
         __syncthreads();                                      // last hidden layer: own columns (block barrier) + the peers' columns
         rf_mbar_wait(&s_bar[1], (unsigned)t & 1u);
-        // ---- head.  p.head_mode 1: warp w takes the k slice [w H2/16, (w+1) H2/16) for ALL 8 owned actors (lane = actor x 4 k
-        // sub-lanes), so the head weights are read from shared memory once per step instead of once per actor (the 2 x 8 KB
-        // per actor were 1 K cycles of the shared-memory pipe); the 16 slice sums meet in the (idle) Part buffer.
+        // ---- head.  p.head_mode 1: warp w takes k slice w (rf_head_slice); the 16 slice sums meet in the (idle) Part buffer.
         // head_mode 0: warps w and w + 8 take the two k halves of owned actor w & 7.
         if (p.head_mode == 1) {
-            const int ks = H2 >> 4;                           // H2 % 16 == 0 (rf_plan)
-            const int a8 = lane >> 2, ksub = lane & 3;
-            const float* hrow = Hb2 + a8 * p.ldh2 + warp * ks;
-            const float* wbase = Whs + (warp * ks) * ldwh;
-            for (int n8 = 0; n8 < A; n8 += 8) {
-                float s8[8];
-#pragma unroll
-                for (int jj = 0; jj < 8; ++jj) s8[jj] = 0.0f;
-                const bool second = (n8 + 4 < ldwh);
-                for (int k = ksub; k < ks; k += 4) {
-                    const float hv = hrow[k];
-                    const float* wr = wbase + k * ldwh + n8;
-                    const float4 w0 = *reinterpret_cast<const float4*>(wr);
-                    s8[0] = fmaf(hv, w0.x, s8[0]); s8[1] = fmaf(hv, w0.y, s8[1]);
-                    s8[2] = fmaf(hv, w0.z, s8[2]); s8[3] = fmaf(hv, w0.w, s8[3]);
-                    if (second) {
-                        const float4 w1 = *reinterpret_cast<const float4*>(wr + 4);
-                        s8[4] = fmaf(hv, w1.x, s8[4]); s8[5] = fmaf(hv, w1.y, s8[5]);
-                        s8[6] = fmaf(hv, w1.z, s8[6]); s8[7] = fmaf(hv, w1.w, s8[7]);
-                    }
-                }
-                // sum over the 4 k sub-lanes: after two exchange rounds lane ksub holds outputs 2 ksub', 2 ksub' + 1
-                const bool u1 = (lane & 2) != 0, u0 = (lane & 1) != 0;
-                float t4[4], t2[2];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    const float recv = __shfl_xor_sync(0xffffffffu, u1 ? s8[i] : s8[i + 4], 2);
-                    t4[i] = (u1 ? s8[i + 4] : s8[i]) + recv;
-                }
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const float recv = __shfl_xor_sync(0xffffffffu, u0 ? t4[i] : t4[i + 2], 1);
-                    t2[i] = (u0 ? t4[i + 2] : t4[i]) + recv;
-                }
-                const int j0 = n8 + (u1 ? 4 : 0) + (u0 ? 2 : 0);
-                float* dst = Part + ((warp * RF_OWN + a8) * ldwh);
-                if (j0 < A) dst[j0] = t2[0];
-                if (j0 + 1 < A) dst[j0 + 1] = t2[1];
-            }
+            rf_head_slice(p, gr.H2, Whs, warp, lane, Part);
         } else {
             const int half = warp >> 3;
-            const float* hrow = Hb2 + own * p.ldh2;
+            const float* hrow = gr.H2 + own * p.ldh2;
             const int kh = H2 >> 1;
             for (int n8 = 0; n8 < A; n8 += 8) {
                 float s8[8];
@@ -992,7 +845,7 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
                 }
                 const float v = rf_reduce8(s8, lane);
                 const int j = n8 + (((lane >> 4) & 1) << 2) + (((lane >> 3) & 1) << 1) + ((lane >> 2) & 1);
-                if ((lane & 3) == 0 && j < A) Hp[(half * RF_OWN + own) * A + j] = v;
+                if ((lane & 3) == 0 && j < A) gr.Hp[(half * RF_OWN + own) * A + j] = v;
             }
         }
         RF_STAMP(9, 0);
@@ -1000,111 +853,43 @@ __global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
         RF_STAMP(10, 0);
         float rew = 0.0f, dn = 0.0f;
         int slot = SLOT_NONE;
-        if (owner) {
-            const int pos = s_pos[own];
-            if (lane < A) {
-                const int j = lane;
-                float pre;
-                if (p.head_mode == 1) {
-                    pre = 0.0f;
-#pragma unroll 4
-                    for (int w = 0; w < RF_THREADS / 32; ++w) pre += Part[(w * RF_OWN + own) * ldwh + j];    // fixed order
-                } else {
-                    pre = Hp[own * A + j] + Hp[(RF_OWN + own) * A + j];
-                }
-                RF_STAMP(19, 0);
-                const float mu = apply_act(pre + Bhs[j], p.act[2]);
-                const float sd = Sd[own * A + j];
-                float a = mu;
-                if (!p.deterministic) a = __fadd_rn(__fmul_rn(Zn[own * A + j], sd), mu);
-                a = fminf(fmaxf(a, -1.0f), 1.0f);
-                Ac[own * A + j] = a;
-                if (valid) {
-                    p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
-                    p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + j] = mu;
-                    p.stage_pd[((long long)i_own * p.n_step + pos) * 2 * A + A + j] = sd;
-                    if (final_step) {
-                        p.action[i_own * A + j] = a;
-                        p.pd[i_own * 2 * A + j] = mu;
-                        p.pd[i_own * 2 * A + A + j] = sd;
-                    }
-                }
-            }
-            __syncwarp();
-            RF_STAMP(20, 0);
-            float* sown = S + own * D;
-            const int ep = s_ep[own] + 1;
-            const bool is_done = (p.max_steps > 0) && (ep >= p.max_steps);
-            dn = is_done ? 1.0f : 0.0f;
-            rew = -Eq[2 * own] / (float)D + 0.1f * Eq[2 * own + 1];
-            for (int d = lane; d < D; d += 32) {
-                float acc = Eacc[own * D + d];
-#pragma unroll 4
-                for (int k = 0; k < A; ++k) acc = fmaf(EWa[k * D + d], Ac[own * A + k], acc);
-                const float nxt = tanhf(acc) + 0.01f * Egx[own * D + d];
-                Nx[own * D + d] = nxt;
-                sown[d] = is_done ? Erz[own * D + d] : nxt;
-                if (valid && final_step) p.obs_next[i_own * D + d] = nxt;
-            }
-            RF_STAMP(21, 0);
-            if (lane == 0) {
-                s_ep[own] = is_done ? 0 : ep;
-                if (valid && final_step) {
-                    p.reward[i_own] = rew;
-                    p.done[i_own] = dn;
-                }
-                if (valid && pos + 1 == p.n_step) {
-                    const int w = s_cnt[own];
-                    if (w < p.Wout) {
-                        slot = (int)(i_own * p.Wout + w);
-                        p.ev_step[slot] = t;
-                        s_cnt[own] = w + 1;
-                    } else {
-                        slot = SLOT_DROPPED;
-                    }
-                }
-            }
-            slot = __shfl_sync(0xffffffffu, slot, 0);
-            __syncwarp();
-        }
+        if (owner) slot = rf_act_env<1>(p, gr, t, own, lane, i_own, Part, Bhs, EWa, s_pos[own], s_ep[own], s_cnt[own], rew, dn);
         RF_STAMP(11, 0);
-        commit_actor(valid, (int)i_own, lane, 32, Nx + own * D, S + own * D, rew, dn, p.n_step, p.stride, D, A, s_pos + own,
-                     slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew, p.stage_done, p.o_obs, p.o_act, p.o_pd, p.o_rew,
-                     p.o_done);
+        commit_actor(valid, (int)i_own, lane, 32, gr.Nx + own * D, gr.S + own * D, rew, dn, p.n_step, p.stride, D, A,
+                     s_pos + own, slot, p.stage_obs, p.stage_act, p.stage_pd, p.stage_rew, p.stage_done, p.o_obs, p.o_act,
+                     p.o_pd, p.o_rew, p.o_done);
         RF_STAMP(12, 0);
-        if (owner) {
-            const int q4 = lane;
-            if (q4 < (D >> 2)) {
-                float4 v = *reinterpret_cast<const float4*>(S + own * D + q4 * 4);
-                if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (p.zf != nullptr) {
-                    const float4 zm = *reinterpret_cast<const float4*>(Zm + q4 * 4);
-                    const float4 zs = *reinterpret_cast<const float4*>(Zs + q4 * 4);
-                    v.x = fminf(fmaxf((v.x - zm.x) / zs.x, -5.0f), 5.0f);
-                    v.y = fminf(fmaxf((v.y - zm.y) / zs.y, -5.0f), 5.0f);
-                    v.z = fminf(fmaxf((v.z - zm.z) / zs.z, -5.0f), 5.0f);
-                    v.w = fminf(fmaxf((v.w - zm.w) / zs.w, -5.0f), 5.0f);
-                    if (i_own >= p.N) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-                float* qx = X0 + m_own * p.ldx0 + q4 * 4;
-                *reinterpret_cast<float4*>(qx) = v;
-                const unsigned off = smem_u32(qx) - smem_base;
-                if (!final_step) {
-#pragma unroll
-                    for (int c = 0; c < RF_CS - 1; ++c) rf_st_async_v4(peer_base[c] + off, v, peer_base[c] + bar_off_x0);
-                }
-            }
-        }
+        if (owner && !final_step) rf_push_input(p, gr, own, m_own, i_own, lane, smem_base, peer_base, bar_off_x0);
         RF_STAMP(13, 0);
     }
-    cluster.sync();                                           // nobody leaves while a peer may still address its shared memory
+}
 
-    if (valid) {
-        for (int d = lane; d < D; d += 32) p.state[i_own * D + d] = S[own * D + d];
-        if (lane == 0) {
-            p.stage_pos[i_own] = s_pos[own];
-            p.ep_step[i_own] = s_ep[own];
-            p.ev_count[i_own] = s_cnt[own];
+template <int G>
+__global__ void __cluster_dims__(RF_CS, 1, 1) __launch_bounds__(RF_THREADS, 1)
+    ppo_rollout2_kernel(const __grid_constant__ RfParams p) {
+    RF_CTA_STAMP(1);
+    __shared__ int s_pos[G][RF_OWN], s_ep[G][RF_OWN], s_cnt[G][RF_OWN];
+    __shared__ __align__(8) uint64_t s_bar[G][3];   // per group: hidden layer 1 | last hidden layer rows | next input tile
+    const unsigned crank = cg::this_cluster().block_rank();
+    const unsigned long long ctr0 = rf_setup<G>(p, crank, s_pos, s_ep, s_cnt, s_bar);
+    if constexpr (G == 2) rf2_two_groups(p, crank, ctr0, s_pos, s_ep, s_cnt, s_bar);
+    else rf_one_group(p, crank, ctr0, s_pos[0], s_ep[0], s_cnt[0], s_bar[0]);
+    cg::this_cluster().sync();                                // nobody leaves while a peer may still address its shared memory
+
+    // write-back by the warps that finished the owned actors
+    extern __shared__ __align__(16) float smem[];
+    const int lane = (int)RF_TID & 31, warp = (int)RF_TID >> 5, own = warp & (RF_OWN - 1);
+    if ((warp < RF_OWN) == (G == 1)) {
+        for (int g = 0; g < G; ++g) {
+            const long long i = (long long)(blockIdx.x / RF_CS) * (G * RF_ROWS) + g * RF_ROWS + (int)crank * RF_OWN + own;
+            if (i >= p.N) continue;
+            const float* S = smem + p.oS + g * p.gstride + own * p.D;
+            for (int d = lane; d < p.D; d += 32) p.state[i * p.D + d] = S[d];
+            if (lane == 0) {
+                p.stage_pos[i] = s_pos[g][own];
+                p.ep_step[i] = s_ep[g][own];
+                p.ev_count[i] = s_cnt[g][own];
+            }
         }
     }
     RF_CTA_STAMP(2);
@@ -1193,11 +978,11 @@ __global__ void __launch_bounds__(256) ppo_rollout_copy_kernel(const int* __rest
     copy_floats(r_done + (long long)slot * n_step, o_done + e * n_step, n_step, g, G);
 }
 
-// Shared-memory plan of ppo_rollout2_kernel<G>.  G = 1: weights, the cluster's activation tiles, the k-split partial
-// tiles (Part), the env matrices and the owned actors' state.  G = 2: no Part (both layers are reduction-free), the env
-// matrices stay in global memory (read through L1 by the tail warps, off the layers' path), a 4 KB head slice buffer,
-// and the per-group tiles and state twice, `gstride` floats apart.  At the configs[1] shape [64, 256, 256, 8]:
-// G = 1 204 512 B, G = 2 219 552 B.
+// Shared-memory plan of ppo_rollout2_kernel<G>.  G = 1: weights, the cluster's activation tiles, Part (4 x 32 x
+// max(Nc1, Nc2) floats: the head's slice sums, whose fit decides head_mode), the env matrices and the owned actors'
+// state.  G = 2: no Part, the env matrices stay in global memory (read through L1 by the tail warps, off the layers'
+// path), a 4 KB head slice buffer, and the per-group tiles and state twice, `gstride` floats apart.  At the configs[1]
+// shape [64, 256, 256, 8]: G = 1 204 512 B, G = 2 219 552 B.
 bool rf_plan(const sb200_mlp* net, int D, int A, int G, RfParams* p, size_t* smem_bytes) {
     if (net == nullptr || net->n_layers != 3 || net->aux_layer >= 0 || sb200_mlp_has_ln(net)) return false;
     const int H1 = net->dims[1], H2 = net->dims[2];

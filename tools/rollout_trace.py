@@ -20,9 +20,8 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 OUT = os.path.join(ROOT, 'tools', '_trace')
 LIB = os.path.join(OUT, 'libsurreal_b200_trace.so')
 # one-group stamps of thread 0 in step order after the step top (stamp 0), each timing the interval since the one before
-NAMES = [(18, 'input-tile wait'), (3, 'L1 fma + push'), (4, 'H1 wait'), (5, 'L2 fma done'), (6, 'L2 sync'),
-         (7, 'L2 reduce+push'), (9, 'H2 wait + head'), (10, 'head sync'), (11, 'phase 2 (sample+env)'), (12, 'commit_actor'),
-         (13, 'x0 push')]
+NAMES = [(18, 'input-tile wait'), (3, 'L1 fma + push'), (4, 'H1 wait'), (7, 'L2 fma + push'), (9, 'H2 wait + head'),
+         (10, 'head sync'), (11, 'phase 2 (sample+env)'), (12, 'commit_actor'), (13, 'x0 push')]
 
 
 def build():
