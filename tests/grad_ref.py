@@ -128,12 +128,12 @@ def policy_loss_head(pre, log_var, actions, adv, behave, mode, **hyper):
     return _result(loss, st, [pre, lv], ['g_pre', 'g_log_var'])
 
 
-def ppo_policy(layers, log_var, x, actions, adv, behave, mode, **hyper):
+def ppo_policy(layers, log_var, x, actions, adv, behave, mode, masks=None, **hyper):
     """One policy update's loss on the actor ``layers`` over (already whitened) inputs ``x``: ``grads`` per layer,
-    ``g_log_var``, ``g_pre``, plus the loss statistics."""
+    ``g_log_var``, ``g_pre``, plus the loss statistics.  ``masks`` as in trunk."""
     L = _leaves(layers)
     lv = f64(log_var).reshape(-1).requires_grad_(True)
-    pre = trunk(f64(x), L)
+    pre = trunk(f64(x), L, masks=masks)
     ref = hyper.pop('ref', None)
     loss, st = _policy_loss(pre, lv, f64(actions), f64(adv), f64(behave), mode,
                             ref=f64(ref) if ref is not None else None, **hyper)
@@ -142,13 +142,14 @@ def ppo_policy(layers, log_var, x, actions, adv, behave, mode, **hyper):
     return out
 
 
-def value(layers, x, ret):
-    """_value_update's loss mean((v - ret)^2) and explained variance; ``grads`` per layer, ``g_pre`` = dL/dv."""
+def value(layers, x, ret, masks=None):
+    """_value_update's loss mean((v - ret)^2) and explained variance; ``grads`` per layer, ``g_pre`` = dL/dv, ``v``.
+    ``masks`` as in trunk."""
     L = _leaves(layers)
-    v = trunk(f64(x), L)
+    v = trunk(f64(x), L, masks=masks)
     ret = f64(ret).reshape(-1, 1)
     loss = (v - ret).pow(2).mean()
-    st = {'loss': loss, 'explained_var': 1 - torch.var(ret - v) / torch.var(ret), 'ret_mean': ret.mean()}
+    st = {'loss': loss, 'explained_var': 1 - torch.var(ret - v) / torch.var(ret), 'ret_mean': ret.mean(), 'v': v}
     out = _result(loss, st, _flat(L) + [v], ['_g%d' % i for i in range(2 * len(L))] + ['g_pre'])
     out['grads'] = _pairs([out.pop('_g%d' % i) for i in range(2 * len(L))])
     return out

@@ -49,3 +49,128 @@ def test_shapes_the_kernel_rejects_fall_back():
     assert not ops.EpochPair.supported(_block([64, 256, 256, 40], 0), v)         # head wider than 32
     four = ops.FlatNet([64, 128, 128, 128, 8], [ops.ACT_RELU] * 3 + [ops.ACT_TANH], 'cpu', extra=8)
     assert four.n_layers == 4                                                    # PPOLearner._epoch_kernels screens these out
+
+
+# ---- the plan's edges, against a restatement of e2_plan -------------------------------------------------------------
+RB, MAX_OUT, MAX_WIDTH = 16, 32, 512
+SMEM_FLOATS = 220 * 1024 // 4
+
+
+def _ru4(v):
+    return (v + 3) & ~3
+
+
+def _mirror(jobs, G, max_width=MAX_WIDTH):
+    """e2_plan restated: ``jobs`` = [(dims, M, splits)] -> [(s, rps)] per job, or None when the pair is rejected.  The
+    activation region (16 rows of x, h1, h2, d2, head, dpre) doubles as the A operand of the weight-gradient items
+    (16 x (rps + 4)); then the GEMM partials (4 x 17 rows of the widest layer), W3 and the per-row loss operands."""
+    for dims, _, _ in jobs:
+        if len(dims) != 4 or min(dims) < 1 or dims[3] > MAX_OUT or max(dims[:3]) > max_width:
+            return None
+    ld_xs = max([4] + [_ru4(d[0]) for d, _, _ in jobs])
+    ld_h1 = max([4] + [_ru4(d[1]) for d, _, _ in jobs])
+    ld_h2 = max([4] + [_ru4(d[2]) for d, _, _ in jobs])
+    max_w3 = max([4] + [d[2] * _ru4(d[3]) for d, _, _ in jobs])
+    blocks = sum(-(-d[1] // RB) + -(-d[0] // RB) + 1 for d, _, _ in jobs)
+    out, max_as = [], 0
+    for _, M, splits in jobs:
+        s = min(max(1, G // blocks), splits, max(1, M // 64))
+        rps = _ru4(-(-M // s))
+        out.append((s, rps))
+        max_as = max(max_as, RB * (_ru4(rps) + 4))
+    act = RB * (ld_xs + ld_h1 + 2 * ld_h2 + 2 * MAX_OUT)
+    off = max(act, _ru4(max_as)) + 4 * (RB + 1) * max(ld_h1, ld_h2) + _ru4(max_w3) + RB * (5 * MAX_OUT + 1)
+    return out if off <= SMEM_FLOATS else None
+
+
+def _plan_sms():
+    """SMs the plan is sized for (the device's, or 132 without one)."""
+    p, v = _block([64, 256, 256, 8], 0), _block([64, 256, 256, 1], 2)
+    return ops.EpochPair.plan(p, v)['norm_chunks']
+
+
+def _at_rows(blocks, M):
+    """Re-point the plan inputs of EpochKernel blocks at M rows with MlpTrainer's default row splits (planning only: the
+    buffers behind them are not touched)."""
+    for b in blocks:
+        b.args.M, b.args.splits = M, max(1, min(16, M // 128))
+    return blocks
+
+
+def _jobs(blocks):
+    return [(list(C.cast(b.args.net, C.POINTER(_lib.Mlp)).contents.dims)[:4], b.args.M, b.args.splits) for b in blocks]
+
+
+def _accepts(blocks):
+    return ops.EpochPair.supported(*blocks)
+
+
+def _last_true(ok, lo, hi):
+    """Largest v in [lo, hi) with ok(v), given ok(lo) and not ok(hi)."""
+    assert ok(lo) and not ok(hi), (lo, hi)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if ok(mid) else (lo, mid)
+    return lo
+
+
+def _pair_blocks(H1, H2, D=64, A=8, M=1024, mode=0):
+    return [_block([D, H1, H2, A], mode, M=M), _block([D, H1, H2, 1], 2, M=M)]
+
+
+def largest_rows(H1=256, H2=256, D=64, A=8):
+    """Largest batch the kernel takes for this pair of networks (MlpTrainer's default splits), by bisection."""
+    blocks = _pair_blocks(H1, H2, D, A)
+    return _last_true(lambda M: _accepts(_at_rows(blocks, M)), 2, 1 << 20)
+
+
+def widest_square(M=1024, D=64, A=8):
+    """Widest H the kernel takes for D-H-H-A / D-H-H-1 at M rows, by bisection."""
+    return _last_true(lambda H: _accepts(_at_rows(_pair_blocks(H, H, D, A), M)), 4, MAX_WIDTH + 1)
+
+
+def test_plan_matches_its_restatement():
+    """Acceptance, row splits and rows per split of the library's plan equal _mirror's at shapes on both sides of every
+    width, head and row edge: a change to the plan has to change the restatement with it."""
+    G = _plan_sms()
+    nets = [([17, 15, 17, 5], [17, 16, 15, 1]), ([3, 257, 260, 9], [3, 256, 257, 1]), ([16, 416, 416, 8], [16, 416, 416, 1]),
+            ([64, 420, 416, 8], [64, 416, 416, 1]), ([64, 256, 256, 32], [64, 256, 256, 1]),
+            ([64, 256, 256, 33], [64, 256, 256, 1]), ([512, 16, 16, 4], [512, 16, 16, 1]),
+            ([513, 16, 16, 4], [513, 16, 16, 1]), ([8, 513, 8, 4], [8, 8, 8, 1]), ([8, 8, 512, 1], [8, 8, 8, 1])]
+    seen = [0, 0]
+    for pd, vd in nets:
+        blocks = [_block(pd, 0, M=256), _block(vd, 2, M=256)]
+        for M in (2, 3, 16, 63, 64, 127, 128, 129, 255, 256, 577, 1000, 1024, 4096, 6408, 6409, 9000):
+            _at_rows(blocks, M)
+            exp = _mirror(_jobs(blocks), G)
+            assert _accepts(blocks) == (exp is not None), (pd, vd, M, exp)
+            seen[exp is not None] += 1
+            if exp is not None:
+                pl = ops.EpochPair.plan(*blocks)
+                assert [(pl['s'][j], pl['rps'][j]) for j in range(2)] == exp, (pd, vd, M, pl, exp)
+    assert min(seen) >= 20, seen
+
+
+def test_plan_limits():
+    """The edges the GPU envelope test runs at, found by bisection and pinned to the restatement: the bench shape's
+    largest batch, the widest square hidden layers at 1024 rows and those networks' largest batch.  Widths past 512 and
+    heads past 32 are rejected by the width rule, not only by the shared-memory budget."""
+    G = _plan_sms()
+    m_bench = largest_rows()
+    assert _mirror([([64, 256, 256, 8], m_bench, max(1, min(16, m_bench // 128))),
+                    ([64, 256, 256, 1], m_bench, max(1, min(16, m_bench // 128)))], G) is not None
+    m1 = m_bench + 1
+    assert _mirror([([64, 256, 256, 8], m1, max(1, min(16, m1 // 128))), ([64, 256, 256, 1], m1, max(1, min(16, m1 // 128)))], G) is None
+    assert m_bench >= 4096, m_bench                              # every bench batch size (1024 and 4096) is taken
+    h = widest_square()
+    assert 256 <= h < MAX_WIDTH, h                               # the shared-memory budget binds before the width rule
+    assert _accepts(_pair_blocks(h, h)) and not _accepts(_pair_blocks(h + 1, h + 1))
+    m_wide = largest_rows(h, h)
+    assert 1024 <= m_wide < m_bench, (m_wide, m_bench)
+    # the width rule: 512 wide inputs are taken, 513 are not, although the budget would have room for them
+    wide_in = [([513, 16, 16, 4], 256, 2), ([513, 16, 16, 1], 256, 2)]
+    assert _accepts(_at_rows([_block([512, 16, 16, 4], 0, M=256), _block([512, 16, 16, 1], 2, M=256)], 256))
+    assert not _accepts(_at_rows([_block([513, 16, 16, 4], 0, M=256), _block([513, 16, 16, 1], 2, M=256)], 256))
+    assert _mirror(wide_in, G) is None and _mirror(wide_in, G, max_width=1024) is not None
+    assert _accepts([_block([64, 256, 256, 32], 0), _block([64, 256, 256, 1], 2)])
+    print('plan limits at %d SMs: bench shape M <= %d, square H <= %d at 1024 rows, M <= %d at H = %d' % (G, m_bench, h, m_wide, h))

@@ -682,11 +682,13 @@ def test_ddpg_learn_gradients_fullsize():
 
 # (actor dims, critic dims, rows, mode, grids).  The grid sets epoch2's row splits s = min(G // blocks, splits, M // 64),
 # blocks = sum over both nets of ceil(H1 / 16) + ceil(D / 16) + 1: the 1000-row case runs s = 1, 2, 3, 4 over 63 row
-# blocks (2 and 4 do not divide it), the 200-row case s = 3 and 1, the 515-row case (A = 32, E2_MAX_OUT) s = 1 and 8.
+# blocks (2 and 4 do not divide it), the 200-row case s = 3 and 1, the 515-row case (A = 32, E2_MAX_OUT) s = 1 and 8; the
+# 3-row case is one row block with a one-unit head and widths 1 and 3 mod 4.
 E2_CASES = [([17, 300, 200, 6], [17, 100, 68, 1], 200, 'clip', (132, 40)),
             ([17, 300, 200, 6], [17, 100, 68, 1], 1000, 'adapt-hinge', (16, 64, 100, 132)),
             ([20, 64, 64, 1], [20, 64, 64, 1], 77, 'adapt', (7, 132)),
-            ([24, 64, 48, 32], [24, 64, 48, 1], 515, 'clip', (24, 132))]
+            ([24, 64, 48, 32], [24, 64, 48, 1], 515, 'clip', (24, 132)),
+            ([5, 17, 15, 1], [5, 15, 17, 1], 3, 'adapt', (1, 132))]
 E2_BAR = 3e-5
 
 
