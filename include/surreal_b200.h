@@ -393,6 +393,12 @@ int sb200_clip_adam_f32(float* params, const float* grad, float* exp_avg, float*
                         const int* stop_flag, void* stream);
 /* target = target*(1-tau) + tau*src (soft target update, ddpg.py:410-418); a no-op when *stop_flag != 0. */
 int sb200_soft_update_f32(float* target, const float* src, int64_t n, double tau, const int* stop_flag, void* stream);
+/* Hard target update with the update counter on the device (ddpg.py:419-428: counter += 1; copy every `interval`-th
+ * update), so that several learner updates and the copy among them fit in one CUDA graph.  tick != 0: *counter += 1
+ * first (pass it for the first buffer of an update, 0 for the others sharing the counter); then target = src when
+ * *counter % interval == 0.  Neither happens when *stop_flag != 0. */
+int sb200_hard_update_every_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t interval, int tick,
+                                const int* stop_flag, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * DDPG element-wise pieces (surreal/learner/ddpg.py:261-262,279,305,324-331,335-341); the networks run through
@@ -695,6 +701,23 @@ int sb200_replay_gather_f32(const float* src, int64_t record_floats, const int* 
  * outs[f][b] = srcs[f][idx[b]].  Replaces the per-key np.stack loops of aggregator.py:52-103,151-205. */
 int sb200_replay_gather_multi_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
                                   int nfields, const int* idx32, const int64_t* idx64, int batch, void* stream);
+/* UniformReplay.sample (uniform_replay.py:43-47) on the device: `batch` i.i.d. draws WITH replacement over a sampling
+ * view and the gather of every field of the drawn records (field arrays as in replay_gather_multi), in ONE launch with
+ * no host input that depends on the ring's fill level -- so sample -> learn can be one CUDA graph.
+ *   view (device): {int64 start, count, capacity}; draw r in [0, count) is ring slot (start + r) % capacity.
+ *   sampler (device): sb200_uniform_sampler_bytes() bytes {uint64 draw_counter; int32 status; uint32 ticket}, zeroed
+ *     once.  The launch advances draw_counter itself: replaying a captured graph draws fresh indices.
+ *   Index stream: Philox4x32-10 call p, keyed (seed, draw_counter, p), serves draws 2p (words x:y) and 2p+1 (z:w); a
+ *     draw is floor(u * count / 2^64) of its 64 bits u.  No rejection loop; bias <= count / 2^64 per index (< 2^-43 for
+ *     a 2^20-slot ring).  NOT the reference's random.randint stream (that one is sb200_mt19937_randint_fill_h below).
+ *   indices [batch]: the drawn ring slots.  count == 0: no ring access, outputs untouched, status = 1, counter kept.
+ * uniform_view: the view between two chunks of inserts that excludes every slot the next `reserve` inserts can write:
+ *   size + reserve <= capacity: {0, size}; else {(next_idx + reserve) % capacity, capacity - reserve}. */
+size_t sb200_uniform_sampler_bytes(void);
+int sb200_uniform_view(const void* uniform_state, int64_t reserve, int64_t* view, void* stream);
+int sb200_uniform_sample_gather_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
+                                    int nfields, const int64_t* view, uint64_t seed, void* sampler, int batch,
+                                    int64_t* indices, void* stream);
 /* Experience staging of DDPG: ExpSenderWrapperSSARNStepBootstrap._step (exp_sender_wrapper.py:96-112) for N actors +
  * UniformReplay.insert (uniform_replay.py:36-41): k-th insert -> slot k % capacity, actor order.  One descriptor of the
  * buffers involved (device memory, allocated once by the caller), taken whole by both ssar_step entries.

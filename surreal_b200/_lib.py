@@ -208,6 +208,9 @@ def _declare(lib):
         'sb200_replay_gather_f32': (I, [P, L, P, P, I, P, P]),
         'sb200_replay_gather_multi_f32': (I, [P, P, P, I, P, P, I, P]),
         'sb200_uniform_state_bytes': (S, []),
+        'sb200_uniform_sampler_bytes': (S, []),
+        'sb200_uniform_view': (I, [P, L, P, P]),
+        'sb200_uniform_sample_gather_f32': (I, [P, P, P, I, P, C.c_uint64, P, I, P, P]),
         'sb200_ssar_step_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P]),
         'sb200_ssar_step_host_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P, P, P, P, P, P]),
         'sb200_mt19937_state_bytes': (S, []),
@@ -224,6 +227,7 @@ def _declare(lib):
         'sb200_grad_reduce_norm_f32': (I, [P, L, I, P, L, D, I, P, P, P]),
         'sb200_clip_adam_f32': (I, [P, P, P, P, L, P, D, D, D, D, I, D, P, P, P, P]),
         'sb200_soft_update_f32': (I, [P, P, L, D, P, P]),
+        'sb200_hard_update_every_f32': (I, [P, P, L, P, L, I, P, P]),
         'sb200_ddpg_bad_action_offset': (S, []),
         'sb200_gae_window_f32': (I, [P, P, P, I, I, I, D, D, D, I, P, P, P, P]),
     }

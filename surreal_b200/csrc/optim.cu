@@ -62,6 +62,23 @@ __global__ void __launch_bounds__(OT) soft_update_kernel(float* __restrict__ tar
         target[i] = __fadd_rn(__fmul_rn(target[i], keep), __fmul_rn(tau, src[i]));
 }
 
+// Hard target update on the device (ddpg.py:419-428): the update counter lives in device memory so that several
+// learner updates, and the one among them that copies, fit in one CUDA graph.  `tick` counts one update; the copy
+// runs when the counter is a multiple of `interval`.  Both leave everything alone when *stop != 0.
+__global__ void hard_update_tick_kernel(long long* counter, const int* __restrict__ stop) {
+    if (stop != nullptr && *stop) return;
+    *counter += 1;
+}
+
+__global__ void __launch_bounds__(OT) hard_update_kernel(float* __restrict__ target, const float* __restrict__ src,
+                                                         long long n, const long long* __restrict__ counter,
+                                                         long long interval, const int* __restrict__ stop) {
+    if (stop != nullptr && *stop) return;
+    if (*counter % interval != 0) return;
+    for (long long i = (long long)blockIdx.x * OT + threadIdx.x; i < n; i += (long long)gridDim.x * OT)
+        target[i] = src[i];
+}
+
 inline int grid_for(long long n) {
     long long b = (n + 4 * OT - 1) / (4 * OT);   // >= 4 elements per thread: small nets finish in one short wave
     if (b > 264) b = 264;          // 2 x 132 SMs, grid-stride
@@ -100,4 +117,13 @@ extern "C" int sb200_soft_update_f32(float* target, const float* src, int64_t n,
     SB200_REQUIRE(target && src && n >= 1);
     soft_update_kernel<<<grid_for(n), OT, 0, (cudaStream_t)stream>>>(target, src, n, (float)tau, stop_flag);
     return sb200_launch_status();
+}
+
+extern "C" int sb200_hard_update_every_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t interval,
+                                           int tick, const int* stop_flag, void* stream) {
+    SB200_REQUIRE(target && src && counter && n >= 1 && interval >= 1);
+    if (tick) hard_update_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((long long*)counter, stop_flag);
+    hard_update_kernel<<<grid_for(n), OT, 0, (cudaStream_t)stream>>>(target, src, n, (const long long*)counter, interval,
+                                                                     stop_flag);
+    return sb200_launch_status(tick ? 2 : 1);
 }

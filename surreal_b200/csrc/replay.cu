@@ -1,6 +1,7 @@
 // HBM-resident replay: FIFO queue control, gather of sampled records into the learner's batch buffers,
-// the DDPG n-step SSAR staging + UniformReplay ring insert, and a host-side MT19937 that reproduces
-// CPython's random.randint index stream bit for bit.
+// the DDPG n-step SSAR staging + UniformReplay ring insert, a host-side MT19937 that reproduces
+// CPython's random.randint index stream bit for bit, and the on-device uniform sampler (Philox indices + gather in one
+// launch) that lets sample -> learn live inside one CUDA graph.
 //
 // Replaces surreal/replay/fifo_replay.py:6-48, uniform_replay.py:6-74, the aggregators' np.stack loops
 // (aggregator.py:52-103,151-262) and ExpSenderWrapperSSARNStepBootstrap (exp_sender_wrapper.py:72-112).
@@ -269,26 +270,98 @@ struct GatherFields {
     int nf;
 };
 
+// record `s` of every field -> batch row `b`, by the 32 lanes of one warp
+__device__ __forceinline__ void gather_record(const GatherFields& f, long long s, long long b, int lane) {
+    const int total = f.chunk_end[f.nf - 1];
+    for (int c = lane; c < total; c += 32) {
+        int q = 0;
+#pragma unroll
+        for (int k = 0; k < GATHER_MAX_FIELDS - 1; ++k) q += (k < f.nf - 1 && c >= f.chunk_end[k]) ? 1 : 0;
+        const int local = c - (q > 0 ? f.chunk_end[q - 1] : 0);
+        if (f.unit[q] == 4) {
+            reinterpret_cast<float4*>(f.out[q] + b * f.rec[q])[local] = ld_stream4(f.src[q] + s * f.rec[q] + 4 * local);
+        } else {
+            f.out[q][b * f.rec[q] + local] = __ldg(f.src[q] + s * f.rec[q] + local);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256) gather_multi_kernel(const __grid_constant__ GatherFields f, const int* __restrict__ idx,
                                                            const long long* __restrict__ idx64, int batch) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     const int nwarps = (gridDim.x * blockDim.x) >> 5;
-    const int total = f.chunk_end[f.nf - 1];
     for (int b = warp; b < batch; b += nwarps) {
         const long long s = (idx64 != nullptr) ? idx64[b] : (long long)idx[b];
-        for (int c = lane; c < total; c += 32) {
-            int q = 0;
-#pragma unroll
-            for (int k = 0; k < GATHER_MAX_FIELDS - 1; ++k) q += (k < f.nf - 1 && c >= f.chunk_end[k]) ? 1 : 0;
-            const int local = c - (q > 0 ? f.chunk_end[q - 1] : 0);
-            if (f.unit[q] == 4) {
-                reinterpret_cast<float4*>(f.out[q] + (long long)b * f.rec[q])[local] =
-                    ld_stream4(f.src[q] + s * f.rec[q] + 4 * local);
-            } else {
-                f.out[q][(long long)b * f.rec[q] + local] = __ldg(f.src[q] + s * f.rec[q] + local);
+        gather_record(f, s, b, lane);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// UniformReplay.sample (uniform_replay.py:43-47) without the host: `batch` i.i.d. draws WITH replacement, uniform over
+// the `count` records of a sampling view {start, count, capacity} that lives in device memory, and the gather of the
+// drawn records, in one launch.  Draw r of the view is ring slot (start + r) % capacity.
+//
+// Index stream: Philox call p = philox4x32_10(seed, draw_counter, p) serves draws 2p (words x:y) and 2p + 1 (words z:w);
+// a draw takes its 64 random bits u = hi:lo and r = floor(u * count / 2^64) (__umul64hi).  No rejection loop: every
+// thread does the same work, at a bias of at most count / 2^64 per index (< 2^-43 for a 2^20-slot ring).  The launch
+// advances draw_counter itself (the last block to finish, after every block has read it), so a captured graph draws
+// fresh indices at every replay.  Not the reference's stream: random.randint parity is sb200_mt19937_randint_fill_h.
+struct UniformView {
+    long long start;
+    long long count;
+    long long capacity;
+};
+struct UniformSampler {
+    unsigned long long draw_counter;
+    int status;              // 1: the last launch found an empty view and sampled nothing
+    unsigned int ticket;
+};
+
+// One warp per Philox call = two records: lane 0 draws, the warp copies.
+__global__ void __launch_bounds__(256) uniform_sample_gather_kernel(const __grid_constant__ GatherFields f,
+                                                                    const UniformView* __restrict__ view,
+                                                                    unsigned long long seed, UniformSampler* sm, int batch,
+                                                                    long long* __restrict__ indices) {
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    const int nwarps = (gridDim.x * blockDim.x) >> 5;
+    const long long start = view->start, count = view->count, cap = view->capacity;
+    const unsigned long long ctr = *(volatile unsigned long long*)&sm->draw_counter;
+    if (count >= 1) {
+        for (int p = warp; 2 * p < batch; p += nwarps) {
+            unsigned long long r0 = 0, r1 = 0;
+            if (lane == 0) {
+                const Philox4 z = philox4x32_10(seed, ctr, (unsigned long long)p);
+                r0 = __umul64hi(((unsigned long long)z.x << 32) | z.y, (unsigned long long)count);
+                r1 = __umul64hi(((unsigned long long)z.z << 32) | z.w, (unsigned long long)count);
             }
+            r0 = __shfl_sync(0xffffffffu, r0, 0);
+            r1 = __shfl_sync(0xffffffffu, r1, 0);
+            const long long s0 = (start + (long long)r0) % cap, s1 = (start + (long long)r1) % cap;
+            const bool two = 2 * p + 1 < batch;
+            if (lane == 0) {
+                indices[2 * p] = s0;
+                if (two) indices[2 * p + 1] = s1;
+            }
+            gather_record(f, s0, 2 * p, lane);
+            if (two) gather_record(f, s1, 2 * p + 1, lane);
         }
     }
+    if (last_block_ticket(&sm->ticket, gridDim.x) && threadIdx.x == 0) {
+        sm->status = (count >= 1) ? 0 : 1;
+        if (count >= 1) sm->draw_counter = ctr + 1ull;
+    }
+}
+
+// The sampling view of the ring between two chunks of inserts: every filled slot that the next `reserve` inserts cannot
+// overwrite.  While those inserts still land beyond the filled part the view is [0, size); once they wrap into live
+// records it starts behind them, start = (next_idx + reserve) % capacity, and offers capacity - reserve records (the
+// `reserve` oldest, about to be overwritten, are left out).
+__global__ void uniform_view_kernel(const UniformState* __restrict__ us, long long reserve, UniformView* view) {
+    const long long cap = us->capacity, size = us->size;
+    const bool fits = size + reserve <= cap;
+    view->start = fits ? 0 : (us->next_idx + reserve) % cap;
+    view->count = fits ? size : cap - reserve;
+    view->capacity = cap;
 }
 
 }  // namespace
@@ -316,27 +389,56 @@ extern "C" int sb200_replay_gather_f32(const float* src, int64_t record_floats, 
     return sb200_launch_status();
 }
 
-extern "C" int sb200_replay_gather_multi_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
-                                             int nfields, const int* idx32, const int64_t* idx64, int batch, void* stream) {
-    SB200_REQUIRE(srcs && outs && record_floats && (idx32 || idx64) && batch >= 1);
-    SB200_REQUIRE(nfields >= 1 && nfields <= GATHER_MAX_FIELDS);
-    GatherFields f;
+// Field table of the multi-field gathers from the caller's HOST arrays; false when an entry is unusable.
+static bool gather_fields_ok(const float* const* srcs, float* const* outs, const int64_t* record_floats, int nfields,
+                             GatherFields* f) {
+    if (!srcs || !outs || !record_floats || nfields < 1 || nfields > GATHER_MAX_FIELDS) return false;
     int end = 0;
     for (int k = 0; k < nfields; ++k) {
-        SB200_REQUIRE(srcs[k] && outs[k] && record_floats[k] >= 1 && record_floats[k] < (1ll << 28));
-        f.src[k] = srcs[k];
-        f.out[k] = outs[k];
-        f.rec[k] = record_floats[k];
+        if (!srcs[k] || !outs[k] || record_floats[k] < 1 || record_floats[k] >= (1ll << 28)) return false;
+        f->src[k] = srcs[k];
+        f->out[k] = outs[k];
+        f->rec[k] = record_floats[k];
         const bool vec = (record_floats[k] % 4 == 0) && ((((uintptr_t)srcs[k]) | ((uintptr_t)outs[k])) & 15) == 0;
-        f.unit[k] = vec ? 4 : 1;
-        end += (int)(record_floats[k] / f.unit[k]);
-        f.chunk_end[k] = end;
+        f->unit[k] = vec ? 4 : 1;
+        end += (int)(record_floats[k] / f->unit[k]);
+        f->chunk_end[k] = end;
     }
-    for (int k = nfields; k < GATHER_MAX_FIELDS; ++k) { f.src[k] = nullptr; f.out[k] = nullptr; f.rec[k] = 0; f.unit[k] = 1; f.chunk_end[k] = end; }
-    f.nf = nfields;
+    for (int k = nfields; k < GATHER_MAX_FIELDS; ++k) { f->src[k] = nullptr; f->out[k] = nullptr; f->rec[k] = 0; f->unit[k] = 1; f->chunk_end[k] = end; }
+    f->nf = nfields;
+    return true;
+}
+
+extern "C" int sb200_replay_gather_multi_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
+                                             int nfields, const int* idx32, const int64_t* idx64, int batch, void* stream) {
+    SB200_REQUIRE((idx32 || idx64) && batch >= 1);
+    GatherFields f;
+    SB200_REQUIRE(gather_fields_ok(srcs, outs, record_floats, nfields, &f));
     int blocks = (batch + 7) / 8;
     if (blocks > 132 * 8) blocks = 132 * 8;
     gather_multi_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(f, idx32, (const long long*)idx64, batch);
+    return sb200_launch_status();
+}
+
+extern "C" size_t sb200_uniform_sampler_bytes(void) { return sizeof(UniformSampler); }
+
+extern "C" int sb200_uniform_view(const void* uniform_state, int64_t reserve, int64_t* view, void* stream) {
+    SB200_REQUIRE(uniform_state && view && reserve >= 0);
+    uniform_view_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((const UniformState*)uniform_state, reserve, (UniformView*)view);
+    return sb200_launch_status();
+}
+
+extern "C" int sb200_uniform_sample_gather_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
+                                               int nfields, const int64_t* view, uint64_t seed, void* sampler, int batch,
+                                               int64_t* indices, void* stream) {
+    SB200_REQUIRE(view && sampler && indices && batch >= 1);
+    GatherFields f;
+    SB200_REQUIRE(gather_fields_ok(srcs, outs, record_floats, nfields, &f));
+    int blocks = ((batch + 1) / 2 + 7) / 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    uniform_sample_gather_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(f, (const UniformView*)view, seed,
+                                                                          (UniformSampler*)sampler, batch,
+                                                                          (long long*)indices);
     return sb200_launch_status();
 }
 

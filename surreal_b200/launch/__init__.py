@@ -1,1 +1,1 @@
-from .launcher import Launcher, SurrealDefaultLauncher, PipelinedEngine  # noqa: F401
+from .launcher import Launcher, SurrealDefaultLauncher, PipelinedEngine, ReplayEngine  # noqa: F401

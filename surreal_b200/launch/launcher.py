@@ -127,6 +127,109 @@ class PipelinedEngine:
         self.torch.cuda.synchronize()
 
 
+# ReplayEngine defaults: 32 env steps per chunk and one learner update per batched env step (the textbook DDPG ratio).
+# Which ratio keeps both streams of an H100 busy has not been measured; pass rollout_steps / updates_per_chunk to tune.
+REPLAY_ROLLOUT_STEPS = 32
+
+
+class ReplayEngine:
+    """PipelinedEngine's shape for an off-policy learner on a uniform replay (DDPG): the actors keep inserting into the
+    ring while the learner runs K updates per chunk on records it samples ON the device, so neither stream waits for the
+    host between two updates.  The single-process form of the reference's free-running actor and learner processes.
+
+      stream A:  [wait view_k, pub]  chunk_{k+1}: T env steps -> ring ..................  -> roll_{k+1}
+      stream L:  [wait roll_k] view_k -> view | learn_from_replay(K) (one CUDA graph) | publish -> pub
+
+    view_k (replay.snapshot_view) fixes what the K updates of step k sample from: the ring as chunk k left it, minus the
+    W = N * T slots chunk k+1 can overwrite.  Chunk k+1 therefore never writes a slot the learner reads, no record is ever
+    torn, and the sampled data do not depend on how the streams interleave: a run equals the one-stream schedule
+    (``overlap=False``: chunk, then K updates, in program order) bit for bit.  Against UniformReplay.sample, records
+    inserted during the current chunk become eligible one chunk later and the W oldest leave one chunk early.
+
+    Until ``replay.start_sample_condition()`` first holds only the actors run, with one host read of the ring's control
+    block per chunk; afterwards the only host synchronisation of a step is the learner's statistics read-back.
+    Ordering between the streams is carried by events only (view happens-after chunk k and happens-before chunk k+1;
+    publish happens-before fetch happens-before next publish)."""
+
+    def __init__(self, agent, replay, learner, rollout_steps, updates_per_chunk, overlap=True):
+        import torch
+        from ..session import ConfigError
+        self.torch = torch
+        self.agent, self.replay, self.learner = agent, replay, learner
+        self.T, self.K = int(rollout_steps), int(updates_per_chunk)
+        if agent._obs is None:
+            agent._obs, _ = agent.env.reset()
+        if not agent._device_resident(agent._obs):
+            raise ConfigError('ReplayEngine runs device-resident envs only; drive a host env by hand: '
+                              'agent.main_loop(T) and, once replay.start_sample_condition() holds, learner.main_loop()')
+        self.W = agent.num_envs * self.T                    # most records one chunk can insert
+        if replay.memory_size < 2 * self.W:
+            raise ConfigError('replay.memory_size {} is less than two chunks of inserts (2 x {} actors x {} steps): the '
+                              'sampling view would be empty'.format(replay.memory_size, agent.num_envs, self.T))
+        if self.T < 1 or self.K < 1 or replay.learner_config.replay.sampling_start_size < 0:
+            raise ConfigError('rollout_steps and updates_per_chunk must be >= 1 and sampling_start_size >= 0')
+        self.sA = torch.cuda.Stream(priority=-1)
+        self.sL = torch.cuda.Stream() if overlap else self.sA
+        self.ev_roll = self.ev_view = self.ev_pub = self.ev_fetch = None
+        self.iterations = 0
+        self.started = False                                 # the ring has held more than sampling_start_size records
+        cur = torch.cuda.current_stream()
+        self.sA.wait_stream(cur)
+        self.sL.wait_stream(cur)
+
+    def _rollout(self):
+        torch = self.torch
+        with torch.cuda.stream(self.sA):
+            if self.ev_view is not None:
+                self.sA.wait_event(self.ev_view)
+            if self.ev_pub is not None:
+                self.sA.wait_event(self.ev_pub)
+            self.agent.main_loop(max_steps=self.T)          # parameter fetch (if due) + T batched env steps
+            self.ev_fetch = torch.cuda.Event()
+            self.ev_fetch.record(self.sA)
+            self.ev_roll = torch.cuda.Event()
+            self.ev_roll.record(self.sA)
+
+    def prime(self):
+        """First chunk (nothing to overlap with yet)."""
+        self._rollout()
+
+    def step(self):
+        """One chunk of the actors beside K learner updates on the previous chunks' records.  Returns the learner
+        statistics, or None while the ring is still filling."""
+        torch = self.torch
+        L = self.learner
+        if not self.started:
+            with torch.cuda.stream(self.sA):
+                self.replay.mark_device_inserts()            # a replayed chunk graph inserts without telling the host
+                self.started = self.replay.start_sample_condition()     # host read, after the last chunk
+            if not self.started:
+                self._rollout()
+                self.iterations += 1
+                return None
+        with torch.cuda.stream(self.sL):
+            self.sL.wait_event(self.ev_roll)
+            self.replay.snapshot_view(reserve=self.W)
+            self.ev_view = torch.cuda.Event()
+            self.ev_view.record(self.sL)
+        self._rollout()                                      # enqueue chunk k+1 BEFORE blocking on the read-back
+        with torch.cuda.stream(self.sL):
+            with L.learn_timer.time():
+                stats = L.learn_from_replay(self.replay, self.K)
+            self.sL.wait_event(self.ev_fetch)                # the snapshot buffers may still be read by a fetch
+            if L.should_publish_parameter():
+                L.publish_parameter(L.current_iter, message='batch ' + str(L.current_iter))
+            self.ev_pub = torch.cuda.Event()
+            self.ev_pub.record(self.sL)
+            L.iter_timer.lap()
+            L.current_iter += self.K
+        self.iterations += 1
+        return stats
+
+    def drain(self):
+        self.torch.cuda.synchronize()
+
+
 class SurrealDefaultLauncher(Launcher):
     def __init__(self, agent_class, learner_class, replay_class, session_config, env_config, learner_config,
                  eval_mode='eval_stochastic', agent_batch_size=8, eval_batch_size=8, render=False):
@@ -142,6 +245,8 @@ class SurrealDefaultLauncher(Launcher):
         self.eval_batch_size = eval_batch_size
         self.log = U.get_logger('launcher')
         self.replay = self.learner = self.agent = None
+        self.iterations = None               # engine steps `launch` runs (None: until interrupted)
+        self.rollout_steps = self.updates_per_chunk = None     # ReplayEngine chunk shape (None: its defaults)
 
     # -- constructors the reference exposes (launcher.py:192-217, 317-332, 369-381) ----------------------
     def setup_replay(self, replay_id=0):
@@ -180,11 +285,21 @@ class SurrealDefaultLauncher(Launcher):
         self.agent.main_setup(env)
         return self.agent, self.replay, self.learner
 
-    def run_engine(self, iterations=None, rollout_steps=None, pipelined=None):
-        """Run actors + learner.  pipelined (default when one rollout chunk yields exactly one learner batch):
+    def run_engine(self, iterations=None, rollout_steps=None, pipelined=None, updates_per_chunk=None):
+        """Run actors + learner.  A learner with ``learn_from_replay`` on a replay with ``sample_device`` (DDPG on the
+        uniform replay) runs in a ReplayEngine: ``iterations`` counts its steps, ``updates_per_chunk`` defaults to one
+        update per env step of the chunk.  pipelined (default when one rollout chunk yields exactly one learner batch):
         PipelinedEngine -- actors and learner on two concurrent streams.  Otherwise alternate a rollout chunk with
         as many learner iterations as the replay can feed."""
         agent, replay, learner = self.setup_engine()
+        if hasattr(learner, 'learn_from_replay') and hasattr(replay, 'sample_device'):
+            T = rollout_steps or self.rollout_steps or REPLAY_ROLLOUT_STEPS
+            eng = ReplayEngine(agent, replay, learner, T, updates_per_chunk or self.updates_per_chunk or T)
+            eng.prime()
+            while iterations is None or eng.iterations < iterations:
+                eng.step()
+            eng.drain()
+            return learner
         T = rollout_steps or self.learner_config.algo.stride
         n, stride = self.learner_config.algo.n_step, self.learner_config.algo.stride
         one_batch_per_chunk = (n == stride == T and agent.num_envs == self.learner_config.replay.batch_size and
@@ -211,7 +326,7 @@ class SurrealDefaultLauncher(Launcher):
     def launch(self, component_name_in):
         name = component_name_in.split('-')[0] if '-' in component_name_in else component_name_in
         if name in ('learner', 'engine', 'all'):
-            return self.run_engine()
+            return self.run_engine(self.iterations)
         if name in ('agent', 'agents', 'eval', 'evals', 'replay', 'replay_worker') or name in _NOOP_COMPONENTS:
             self.log.warning('component "%s" is collapsed into the learner process of surreal_b200 '
                              '(one process per GPU); launch `learner` instead', component_name_in)

@@ -96,6 +96,13 @@ class DDPGLearner(Learner):
         self.check_action_range = True
         self.use_cuda_graph = ops.graphs_enabled()
         self._graph = ops.GraphRunner()
+        # learn_from_replay: K updates per graph.  _stop latches the bad-action flag for the rest of the call, the hard
+        # target counter lives on the device, and everything the host wants afterwards lands in ONE read-back buffer
+        # (float64: statistics [0:16], critic 2's [16:32], latched stop flag [32], hard-update counter [33])
+        self._stop = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._hard_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self._readback = torch.zeros(34, dtype=torch.float64, device=self.device)
+        self._replay_graphs = {}
 
     # ------------------------------------------------------------------------------------------------
     def preprocess(self, batch):
@@ -138,9 +145,11 @@ class DDPGLearner(Learner):
             self._noise_draws = torch.zeros(self.batch_size, self.action_dim, dtype=torch.float32, device=self.device)
         self._noise_draws.copy_(torch.as_tensor(draws, dtype=torch.float32).reshape(self.batch_size, self.action_dim))
 
-    def _optimize_device(self):
-        """ddpg.py:244-333 as one fixed launch sequence (CUDA-graph body; no host round trip inside)."""
+    def _optimize_device(self, stop=None):
+        """ddpg.py:244-333 as one fixed launch sequence (CUDA-graph body; no host round trip inside).  ``stop``: the
+        flag that no-ops the optimiser / target kernels -- this update's bad-action flag, or a flag that latches it."""
         L = _lib.lib()
+        stop = self._bad if stop is None else stop
         B, A = self.batch_size, self.action_dim
         m, mt, st = self.model, self.model_target, ops._stream()
         b = self._own
@@ -165,13 +174,15 @@ class DDPGLearner(Learner):
             check(L.sb200_ddpg_target_f32(_ptr(rewards), _ptr(self._q_t), 1, _ptr(dones), _ptr(actions), A, B, A,
                                           disc, _ptr(self._y), _ptr(self._stats), _ptr(self._ws), st),
                   'sb200_ddpg_target_f32')
+        if stop is not self._bad:
+            torch.maximum(stop, self._bad, out=stop)
         ct = self.critic_optim
         q = ct.forward(obs, aux=actions)                                                # Q(s_t, a_t)
         check(L.sb200_ddpg_critic_loss_f32(_ptr(q), q.stride(0), _ptr(self._y), B, _ptr(ct.d[-1]),
                                            ct.d[-1].stride(0), _ptr(self._stats), _ptr(self._ws), st),
               'sb200_ddpg_critic_loss_f32')
         ct.backward()
-        ct.step(stop_flag=self._bad)
+        ct.step(stop_flag=stop)
         if self.use_double_critic:                                                       # ddpg.py:298-303,311-321
             c2 = self.critic_optim2
             q2 = c2.forward(obs, aux=actions)
@@ -179,7 +190,7 @@ class DDPGLearner(Learner):
                                                c2.d[-1].stride(0), _ptr(self._stats2), _ptr(self._ws), st),
                   'sb200_ddpg_critic_loss_f32')
             c2.backward()
-            c2.step(stop_flag=self._bad)
+            c2.step(stop_flag=stop)
         at = self.actor_optim
         a_pi = at.forward(obs)
         q_pi = ct.forward(obs, aux=at.h[-1])                  # through the UPDATED critic (ddpg.py:324-327)
@@ -190,14 +201,14 @@ class DDPGLearner(Learner):
         check(L.sb200_tanh_bwd_f32(_ptr(self._dA), self._dA.stride(0), _ptr(a_pi), a_pi.stride(0), B, A,
                                    _ptr(at.d[-1]), at.d[-1].stride(0), st), 'sb200_tanh_bwd_f32')
         at.backward()
-        at.step(stop_flag=self._bad)
+        at.step(stop_flag=stop)
         if self.target_update_type == 'soft':                                           # ddpg.py:410-418
             pairs = [(mt.actor, m.actor), (mt.critic, m.critic)]
             if self.use_double_critic:
                 pairs.append((self.model_target2.critic, self.model2.critic))
             for t, s_ in pairs:
                 check(L.sb200_soft_update_f32(_ptr(t.params), _ptr(s_.params), t.size, float(self.target_update_tau),
-                                              _ptr(self._bad), st), 'sb200_soft_update_f32')
+                                              _ptr(stop), st), 'sb200_soft_update_f32')
 
     def _optimize(self):
         with self.forward_time.time():
@@ -210,15 +221,7 @@ class DDPGLearner(Learner):
         s2 = self._stats2.cpu().numpy() if self.use_double_critic else None
         if self.check_action_range and s[DS['ABSMAX']] > 1.0:
             raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
-        stats = {'actor_loss': float(s[DS['ACTOR_LOSS']]), 'critic_loss': float(s[DS['CRITIC_LOSS']]),
-                 'action_norm': float(s[DS['ACTION_NORM']]), 'rewards': float(s[DS['REWARDS']]),
-                 'Q_target': float(s[DS['Q_TARGET']]), 'Q_policy': float(s[DS['Q_POLICY']]),
-                 'performance/forward_time': self.forward_time.avg}
-        # (the reference's critic_update_time / actor_update_time split does not exist here: the whole update is one
-        #  CUDA graph; performance/forward_time covers it)
-        if s2 is not None:                                       # ddpg.py:316,345-346: critic_loss is critic 2's
-            stats['critic_loss'] = float(s2[DS['CRITIC_LOSS']])
-            stats['Q_policy2'] = float(s2[DS['Q_POLICY']])
+        stats = self._statistics(s, s2)
         if self.target_update_type == 'hard':                     # host-side counter (ddpg.py:419-428)
             self.target_update_counter += 1
             if self.target_update_counter % self.target_update_interval == 0:
@@ -228,12 +231,79 @@ class DDPGLearner(Learner):
                     self.model_target2.critic.params.copy_(self.model2.critic.params)
         return stats
 
+    def _statistics(self, s, s2):
+        stats = {'actor_loss': float(s[DS['ACTOR_LOSS']]), 'critic_loss': float(s[DS['CRITIC_LOSS']]),
+                 'action_norm': float(s[DS['ACTION_NORM']]), 'rewards': float(s[DS['REWARDS']]),
+                 'Q_target': float(s[DS['Q_TARGET']]), 'Q_policy': float(s[DS['Q_POLICY']]),
+                 'performance/forward_time': self.forward_time.avg}
+        # (the reference's critic_update_time / actor_update_time split does not exist here: the whole update is one
+        #  CUDA graph; performance/forward_time covers it)
+        if s2 is not None:                                       # ddpg.py:316,345-346: critic_loss is critic 2's
+            stats['critic_loss'] = float(s2[DS['CRITIC_LOSS']])
+            stats['Q_policy2'] = float(s2[DS['Q_POLICY']])
+        return stats
+
     def learn(self, batch):
         """ddpg.py:354-374."""
         self.current_iteration += 1
         with self.total_learn_time.time():
             self.preprocess(batch)
             stats = self._optimize()
+            stats['performance/total_learn_time'] = self.total_learn_time.avg
+            self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
+            self.periodic_checkpoint(global_steps=self.current_iteration, score=None)
+        return stats
+
+    def _replay_updates_device(self, replay, updates):
+        """``updates`` x [sample on the device -> update -> target update] and the read-back staging, as one fixed
+        launch sequence.  A bad-action batch stops every later optimiser / target kernel of the sequence (_stop)."""
+        L, st = _lib.lib(), ops._stream()
+        self._stop.zero_()
+        for _ in range(updates):
+            replay.sample_device(self.batch_size, out=self._own)
+            self._optimize_device(stop=self._stop)
+            if self.target_update_type == 'hard':                                        # ddpg.py:419-428
+                pairs = [(self.model_target.actor, self.model.actor), (self.model_target.critic, self.model.critic)]
+                if self.use_double_critic:
+                    pairs.append((self.model_target2.critic, self.model2.critic))
+                for i, (t, s_) in enumerate(pairs):
+                    check(L.sb200_hard_update_every_f32(_ptr(t.params), _ptr(s_.params), t.size, _ptr(self._hard_counter),
+                                                        int(self.target_update_interval), int(i == 0), _ptr(self._stop),
+                                                        st), 'sb200_hard_update_every_f32')
+        rb = self._readback
+        rb[0:16].copy_(self._stats)
+        rb[16:32].copy_(self._stats2)
+        rb[32:33].copy_(self._stop)
+        rb[33:34].copy_(self._hard_counter)
+
+    def learn_from_replay(self, replay, updates=1):
+        """``updates`` learner updates fed by ``replay.sample_device`` -- ddpg.py:354-374 ``updates`` times over, with no
+        host step between them: one CUDA graph (the same launches eagerly when graphs are off), then ONE read-back.
+        Returns the statistics of the last update.  Hard target updates (ddpg.py:419-428) run on the device, gated by a
+        device counter that starts from ``target_update_counter`` and is read back into it.  An out-of-range action in
+        any sampled batch raises AssertionError after the read-back; that update and every later one of the call changed
+        nothing."""
+        K = int(updates)
+        assert K >= 1
+        self.current_iteration += K
+        with self.total_learn_time.time():
+            if self.target_update_type == 'hard':
+                self._hard_counter.fill_(self.target_update_counter)
+            with self.forward_time.time():
+                if self.use_cuda_graph:
+                    key = (id(replay), K)
+                    if key not in self._replay_graphs:
+                        self._replay_graphs[key] = (ops.GraphRunner(), replay)
+                    self._replay_graphs[key][0].run(lambda: self._replay_updates_device(replay, K))
+                else:
+                    self._replay_updates_device(replay, K)
+            rb = self._readback.cpu().numpy()
+            self.last_d2h_bytes = rb.nbytes
+            if self.target_update_type == 'hard':
+                self.target_update_counter = int(rb[33])
+            if self.check_action_range and rb[32] != 0:
+                raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
+            stats = self._statistics(rb[0:16], rb[16:32] if self.use_double_critic else None)
             stats['performance/total_learn_time'] = self.total_learn_time.avg
             self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
             self.periodic_checkpoint(global_steps=self.current_iteration, score=None)

@@ -68,6 +68,11 @@ def ddpg_argparser():
     p.add_argument('--agent-batch', type=int, default=1)
     p.add_argument('--eval-batch', type=int, default=1)
     p.add_argument('--unit-test', action='store_true')
+    # the single-GPU engine (launch.ReplayEngine): env steps per actor chunk, learner updates beside each chunk (default:
+    # one per env step), and an optional cap on engine steps (default: run until interrupted)
+    p.add_argument('--rollout-steps', type=int, default=None)
+    p.add_argument('--updates-per-chunk', type=int, default=None)
+    p.add_argument('--iterations', type=int, default=None)
     return p
 
 
@@ -101,6 +106,8 @@ class DDPGLauncher:
                     self.session_config.checkpoint.restore_folder = args.restore_folder
                 self.agent_batch_size = args.agent_batch
                 self.eval_batch_size = args.eval_batch
+                self.rollout_steps, self.updates_per_chunk = args.rollout_steps, args.updates_per_chunk
+                self.iterations = args.iterations
                 if args.unit_test:
                     self.learner_config.replay.sampling_start_size = 5
                     self.learner_config.replay.replay_shards = 1

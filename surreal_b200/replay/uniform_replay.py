@@ -7,7 +7,12 @@ in slot k % memory_size, on-device actors insert through the ssar_step kernel (n
 Sampling is bit-exact with the reference: ``batch_size`` i.i.d. ``random.randint(0, len-1)`` draws WITH
 replacement.  The draws come from a C++ MT19937 that continues Python's *global* ``random`` stream (state
 transplanted in, advanced state written back), 16 KB of indices are uploaded, and a gather kernel assembles
-the batch (aggregator.py:52-103 layout: rewards / dones as [B,1])."""
+the batch (aggregator.py:52-103 layout: rewards / dones as [B,1]).
+
+``sample_device`` is the second sampler: Philox indices drawn ON the device over a sampling view that also lives there,
+and the gather, in one launch (sb200_uniform_sample_gather_f32).  It never touches the host, so it can sit inside a CUDA
+graph next to the learner's update; its index stream is its own (not ``random.randint``'s), which is why ``sample``
+stays the default and the parity path."""
 import ctypes as C
 import random
 
@@ -77,6 +82,13 @@ class UniformReplay(Replay):
         self._idx_event = None
         self._idx_dev = None
         self._pin = None
+        # device sampler: the view {start, count, capacity} it draws from, its {draw counter, status} block and the seed
+        rc = self.learner_config.replay
+        self.sampler_seed = int(rc.sampler_seed) if 'sampler_seed' in rc else 0
+        assert _lib.lib().sb200_uniform_sampler_bytes() == 16
+        self.view = torch.zeros(3, dtype=torch.int64, device=self.device)
+        self.sampler = torch.zeros(2, dtype=torch.int64, device=self.device)
+        self._dev_indices = torch.zeros(self.batch_size, dtype=torch.int64, device=self.device)
 
     def mark_device_inserts(self):
         """Called by the on-device experience wrapper: the control block changed on the GPU."""
@@ -154,3 +166,44 @@ class UniformReplay(Replay):
         return {'obs': {'low_dim': {'flat_inputs': out['obs']}}, 'obs_next': {'low_dim': {'flat_inputs': out['obs_next']}},
                 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'],
                 'indices': indices}
+
+    # -- device sampler ----------------------------------------------------------------------------------
+    def snapshot_view(self, reserve=0):
+        """Fix the population ``sample_device`` draws from: every record in the ring now, minus the slots the next
+        ``reserve`` inserts can overwrite (sb200_uniform_view).  One one-thread launch on the current stream; call it
+        where that stream is ordered after the inserts so far and before the next ones."""
+        check(_lib.lib().sb200_uniform_view(_p(self.state), int(reserve), _p(self.view), _st()), 'sb200_uniform_view')
+
+    @property
+    def draw_counter(self):
+        """Sample launches that have drawn so far (host read: synchronises)."""
+        return int(self.sampler[0])
+
+    @property
+    def sampler_status(self):
+        """1 when the last ``sample_device`` found an empty view and sampled nothing (host read: synchronises)."""
+        return int(self.sampler.view(torch.int32)[2])
+
+    def sample_device(self, batch_size, out=None):
+        """The batch dict of ``sample`` drawn from ``self.view`` without the host: no fill-level read, no pinned buffer,
+        no event -- one launch, capturable.  ``indices`` is a device tensor owned by the replay (overwritten by the next
+        call); a batch size other than ``replay.batch_size`` must be used once outside a capture first."""
+        D, A = self.D, self.A
+        if self._dev_indices.numel() < batch_size:
+            self._dev_indices = torch.zeros(batch_size, dtype=torch.int64, device=self.device)
+        idx = self._dev_indices[:batch_size]
+        if out is None:
+            f = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)  # noqa: E731
+            out = dict(obs=f(batch_size, D), obs_next=f(batch_size, D), actions=f(batch_size, A),
+                       rewards=f(batch_size, 1), dones=f(batch_size, 1))
+        pairs = [(self.r_obs, out['obs'], D), (self.r_obs_next, out['obs_next'], D), (self.r_act, out['actions'], A),
+                 (self.r_rew, out['rewards'], 1), (self.r_done, out['dones'], 1)]
+        n = len(pairs)
+        srcs = (C.c_void_p * n)(*[p[0].data_ptr() for p in pairs])
+        outs = (C.c_void_p * n)(*[p[1].data_ptr() for p in pairs])
+        recs = (C.c_int64 * n)(*[int(p[2]) for p in pairs])
+        check(_lib.lib().sb200_uniform_sample_gather_f32(srcs, outs, recs, n, _p(self.view), self.sampler_seed,
+                                                         _p(self.sampler), int(batch_size), _p(idx), _st()),
+              'sb200_uniform_sample_gather_f32')
+        return {'obs': {'low_dim': {'flat_inputs': out['obs']}}, 'obs_next': {'low_dim': {'flat_inputs': out['obs_next']}},
+                'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'], 'indices': idx}
