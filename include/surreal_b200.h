@@ -687,6 +687,42 @@ int sb200_ppo_rollout_f32(const sb200_ppo_rollout* args, void* stream);
 int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* args, int* sms);
 int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, void* stream);
 
+/* Persistent rollout of the recurrent policy (csrc/rollout_rnn.cu): T steps of z-filter -> LSTM layers -> actor head ->
+ * sampling -> synthetic env step -> window staging for ALL N actors in ONE launch.  Replaces T x (sb200_ppo_act_rnn_f32
+ * with `stage` and assign_slots + sb200_synth_env_step_f32 + sb200_ppo_window_step_f32 with the cells), i.e. the actor
+ * main loop of surreal/agent/base.py:224-271 with the LSTM policy of ppo_net.py:317-351 and ppo_agent.py:84-93,133-154,
+ * for a device-resident env.  A CTA owns 8 actors; their
+ * env state and [L][H] cells stay in shared memory for the whole chunk.  Same records, Philox keys and FIFO order as
+ * that chain: the action noise of step t is keyed by *step_counter + t, the env noise by *step_counter + t + 1.
+ *   base: a filled sb200_ppo_rollout for the env, sampling, outbox and windows; base->net is the actor head
+ *     (H -> ... -> A), base->D the env's observation width; the window records are base->D + 2 * layers * H wide
+ *     ([obs | h_0 .. h_{L-1} | c_0 .. c_{L-1}], utils.rnn_cell_layout).  Commit with sb200_ppo_rollout_commit_f32 on a
+ *     copy of `base` whose D is the record width.
+ *   ih / whh / bhh / layers / H / h / c / h_before / c_before: as in sb200_ppo_act_rnn.  The cells are read at entry and
+ *     written back at exit; h_before / c_before receive the cells before the chunk's last step.
+ *   Each staged row carries the cells the actor acts from on that row's observation (the successor row and, after done,
+ *   the reset row alike: the cells carry over across episodes).
+ *   rollout_rnn_supported: 1 when the shapes fit the kernel, from the shapes alone (no device needed): 1 ..
+ *     SB200_MAX_RNN_LAYERS layers, H <= 128, D <= 256, a head of 1 .. SB200_MAX_LAYERS layers each <= 512 wide,
+ *     A <= 32, each ih[k] one Linear (in -> 4H, no activation), no LayerNorm, no aux input; else 0, and rollout_rnn_f32 /
+ *     rollout_rnn_footprint return SB200_ERR_UNSUPPORTED: use the per-step entries.
+ *   rollout_rnn_footprint: SMs the chunk holds from start to end when its grid is at most one CTA per SM (one wave);
+ *     0 otherwise. */
+typedef struct sb200_ppo_rollout_rnn {
+    const sb200_ppo_rollout* base;
+    const sb200_mlp* ih[SB200_MAX_RNN_LAYERS];  /* input projection of layer k: in -> 4H (W_ih^T, b_ih) */
+    const float* whh[SB200_MAX_RNN_LAYERS];     /* W_hh^T [H][4H] of layer k */
+    const float* bhh[SB200_MAX_RNN_LAYERS];     /* b_hh [4H] of layer k */
+    int layers, H;
+    float* h;                           /* [layers][N][H] cells, updated in place */
+    float* c;
+    float* h_before;                    /* [layers][N][H] cells before the last step */
+    float* c_before;
+} sb200_ppo_rollout_rnn;
+int sb200_ppo_rollout_rnn_supported(const sb200_ppo_rollout_rnn* args);
+int sb200_ppo_rollout_rnn_f32(const sb200_ppo_rollout_rnn* args, void* stream);
+int sb200_ppo_rollout_rnn_footprint(const sb200_ppo_rollout_rnn* args, int* sms);
+
 /* ---------------------------------------------------------------------------------------------
  * HBM replay (the PPO window staging that fills the FIFO ring is sb200_windows above).
  *   fifo_pop: FIFOReplay.sample (fifo_replay.py:37-39): slot ids of the `batch` oldest windows; *status = 1

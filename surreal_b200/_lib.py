@@ -73,6 +73,13 @@ class PPORollout(C.Structure):
 MAX_RNN_LAYERS = 8
 
 
+class PPORolloutRnn(C.Structure):
+    """sb200_ppo_rollout_rnn (include/surreal_b200.h)."""
+    _fields_ = [('base', C.POINTER(PPORollout)), ('ih', C.POINTER(Mlp) * MAX_RNN_LAYERS),
+                ('whh', C.c_void_p * MAX_RNN_LAYERS), ('bhh', C.c_void_p * MAX_RNN_LAYERS), ('layers', C.c_int),
+                ('H', C.c_int), ('h', C.c_void_p), ('c', C.c_void_p), ('h_before', C.c_void_p), ('c_before', C.c_void_p)]
+
+
 class ZFilter(C.Structure):
     _fields_ = [('stats', C.c_void_p), ('eps', C.c_float)]
 
@@ -177,6 +184,9 @@ def _declare(lib):
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),
         'sb200_ppo_rollout_footprint': (I, [C.POINTER(PPORollout), C.POINTER(C.c_int)]),
         'sb200_ppo_rollout_commit_f32': (I, [C.POINTER(PPORollout), P, P]),
+        'sb200_ppo_rollout_rnn_supported': (I, [C.POINTER(PPORolloutRnn)]),
+        'sb200_ppo_rollout_rnn_f32': (I, [C.POINTER(PPORolloutRnn), P]),
+        'sb200_ppo_rollout_rnn_footprint': (I, [C.POINTER(PPORolloutRnn), C.POINTER(C.c_int)]),
         'sb200_linear_bwd_dx_f32': (I, [P, L, P, I, P, L, P, L, I, I, I, P]),
         'sb200_linear_bwd_dw_f32': (I, [P, L, P, L, P, P, L, I, I, I, I, I, P]),
         'sb200_layernorm_bwd_f32': (I, [P, L, P, L, P, P, I, I, I, P, L, P, P, L, I, P]),

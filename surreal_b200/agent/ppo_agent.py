@@ -335,20 +335,23 @@ class PPOAgent(Agent):
         return self._host_result(False, self._unbatched(obs), [])
 
     def rollout_chunk_supported(self):
-        """True when ``steps`` consecutive act -> env.step -> staging iterations can run as the persistent rollout
-        kernel (sb200_ppo_rollout_f32): training mode, the in-tree device env behind the window wrapper, and a policy
-        that fits the kernel's shared-memory plan."""
+        """True when ``steps`` consecutive act -> env.step -> staging iterations can run as one persistent rollout
+        kernel: training mode, the in-tree device env behind the window wrapper, and a policy that fits the kernel's
+        plan -- the MLP policy on sb200_ppo_rollout_f32, the low-dim LSTM policy on sb200_ppo_rollout_rnn_f32."""
         import os
         from ..env import SyntheticEnv
         env = self.env
         if self.agent_mode != 'training' or os.environ.get('SB200_PERSISTENT_ROLLOUT', '1') == '0':
             return False
-        if self.model.rnn_stem is not None or self.model.cnn_stem is not None:
-            return False                       # the persistent kernel runs the plain MLP policy only
+        if self.model.cnn_stem is not None:
+            return False                       # pixel policies run on the per-step launch chain
         if not isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo) or not env.persistent_rollout:
             return False
         if type(env.env) is not SyntheticEnv:
             return False
+        if self.model.rnn_stem is not None:
+            a, keep = self._rollout_rnn_args(self._rollout_args())
+            return bool(_lib.lib().sb200_ppo_rollout_rnn_supported(C.byref(a)))
         d = self.model.actor.desc()
         return bool(_lib.lib().sb200_ppo_rollout_supported(C.byref(d), self.model.low_dim, self.action_dim))
 
@@ -357,26 +360,27 @@ class PPOAgent(Agent):
         chunk takes several waves or does not run on that kernel."""
         if not self.rollout_chunk_supported():
             return 0
-        m = self.model
-        a = _lib.PPORollout()
-        d = m.actor.desc()
-        a.net = C.pointer(d)
-        a.N, a.D, a.A = self.num_envs, m.low_dim, self.action_dim
         n = C.c_int(0)
         _lib.ensure_device()
-        check(_lib.lib().sb200_ppo_rollout_footprint(C.byref(a), C.byref(n)), 'sb200_ppo_rollout_footprint')
+        a = self._rollout_args()
+        if self.model.rnn_stem is not None:
+            r, keep = self._rollout_rnn_args(a)
+            check(_lib.lib().sb200_ppo_rollout_rnn_footprint(C.byref(r), C.byref(n)), 'sb200_ppo_rollout_rnn_footprint')
+        else:
+            check(_lib.lib().sb200_ppo_rollout_footprint(C.byref(a), C.byref(n)), 'sb200_ppo_rollout_footprint')
         return int(n.value)
 
-    def rollout_chunk(self, steps):
-        """``steps`` iterations of the actor loop (agent/base.py:244-262) in one launch + the ordered commit pass."""
-        w = self.env
-        e, m = w.env, self.model
-        ob = w.rollout_outbox(steps)
-        if ob is None:
-            return False
+    def _rollout_args(self, ob=None, steps=0):
+        """sb200_ppo_rollout of this agent's policy, env and window wrapper; with ``ob`` (the wrapper's outbox for chunks of
+        ``steps``) every buffer of a chunk.  ``net`` is the actor (the LSTM policy's head); D the env's observation width."""
+        m, w = self.model, self.env
         a = _lib.PPORollout()
         d = m.actor.desc()
         a.net = C.pointer(d)
+        a.N, a.D, a.A, a.T = self.num_envs, m.low_dim, self.action_dim, int(steps)
+        if ob is None:
+            return a
+        e = w.env
         a.zf_stats = m.z_stats.data_ptr() if m.z_stats is not None else None
         a.zf_eps = float(m.z_eps)
         a.log_var, a.log_noise = m.log_var.data_ptr(), self._log_noise.data_ptr()
@@ -389,9 +393,40 @@ class PPOAgent(Agent):
         a.o_obs, a.o_act, a.o_pd = ob['o_obs'].data_ptr(), ob['o_act'].data_ptr(), ob['o_pd'].data_ptr()
         a.o_rew, a.o_done = ob['o_rew'].data_ptr(), ob['o_done'].data_ptr()
         a.ev_step, a.ev_count, a.W = ob['ev_step'].data_ptr(), ob['ev_count'].data_ptr(), ob['W']
-        a.N, a.D, a.A, a.T = self.num_envs, m.low_dim, self.action_dim, int(steps)
+        return a
+
+    def _rollout_rnn_args(self, a):
+        """sb200_ppo_rollout_rnn around ``a``: the LSTM stem's weights and the agent's cells.  Returns it with the
+        descriptors it points to (kept alive by the caller for the duration of the call)."""
+        from ..model.lstm_stem import _sfx
+        stem = self.model.rnn_stem
+        self._rnn_state()
+        r = _lib.PPORolloutRnn()
+        r.base = C.pointer(a)
+        ihs = [stem.ihs[k].desc(stem.seg('ih' + _sfx(k))) for k in range(stem.layers)]
+        for k in range(stem.layers):
+            r.ih[k] = C.pointer(ihs[k])
+            hh, lay = stem.seg('hh' + _sfx(k)), stem.hhs[k].layout[0]
+            r.whh[k], r.bhh[k] = hh.data_ptr() + 4 * lay['w'], hh.data_ptr() + 4 * lay['b']
+        r.layers, r.H = stem.layers, stem.H
+        r.h, r.c = self._hs.data_ptr(), self._cs.data_ptr()
+        r.h_before, r.c_before = self._hs_before.data_ptr(), self._cs_before.data_ptr()
+        return r, (a, ihs)
+
+    def rollout_chunk(self, steps):
+        """``steps`` iterations of the actor loop (agent/base.py:244-262) in one launch + the ordered commit pass."""
+        w = self.env
+        ob = w.rollout_outbox(steps)
+        if ob is None:
+            return False
+        a = self._rollout_args(ob, steps)
         L, st = _lib.lib(), ops._stream()
-        check(L.sb200_ppo_rollout_f32(C.byref(a), st), 'sb200_ppo_rollout_f32')
+        if self.model.rnn_stem is not None:
+            r, keep = self._rollout_rnn_args(a)
+            check(L.sb200_ppo_rollout_rnn_f32(C.byref(r), st), 'sb200_ppo_rollout_rnn_f32')
+            a.D = w.D                              # the records carry the cells: [obs | h | c]
+        else:
+            check(L.sb200_ppo_rollout_f32(C.byref(a), st), 'sb200_ppo_rollout_f32')
         check(L.sb200_ppo_rollout_commit_f32(C.byref(a), _p(ob['scratch']), st), 'sb200_ppo_rollout_commit_f32')
         return True
 
@@ -411,8 +446,6 @@ class PPOAgent(Agent):
         env = super().prepare_env_agent(env)
         if self.model.rnn_stem is not None:
             self._rnn_state()
-            w = ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config,
-                                                              cells=(self._hs, self._cs))
-            w.persistent_rollout = False
-            return w
+            return ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config,
+                                                                 cells=(self._hs, self._cs))
         return ExpSenderWrapperMultiStepMovingWindowWithInfo(env, self.learner_config, self.session_config)

@@ -10,10 +10,9 @@
 // Gate order i, f, g, o (torch).  Weights in the kernel layout: WhhT[k][4H] (transpose of torch's weight_hh_l0 [4H][H]).
 // Sequences are tiny here (B = 64 windows x <= 26 steps x H = 100): latency-bound, weights come from L2 every step.
 #include "common.cuh"
+#include "lstm_dev.cuh"
 
 namespace {
-
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // out[(b*L + t)][0..D) = zfilter(x[b*batch_stride + t*row_stride + 0..D))   (z_filter.py:59-79); zf == nullptr: plain gather
 __global__ void __launch_bounds__(256) rows_zfilter_kernel(const float* __restrict__ x, long long row_stride, long long batch_stride,
@@ -60,18 +59,18 @@ __global__ void __launch_bounds__(1024) lstm_fwd_kernel(const float* __restrict_
         if (j < G) {
             float acc = 0.0f;
             for (int k = 0; k < H; ++k) acc = fmaf(hs[k], WhhT[(long long)k * G + j], acc);
-            gs[j] = pre_x[r * G + j] + (acc + b_hh[j]);       // F.linear(x, w_ih, b_ih) + F.linear(h, w_hh, b_hh)
+            gs[j] = lstm_gate_pre(pre_x[r * G + j], acc, b_hh[j]);
         }
         __syncthreads();
         if (j < H) {
-            const float ig = sigmoidf_(gs[j]), fg = sigmoidf_(gs[H + j]), gg = tanhf(gs[2 * H + j]), og = sigmoidf_(gs[3 * H + j]);
-            const float c = fg * cs[j] + ig * gg;
-            const float h = og * tanhf(c);
+            LstmGates q;
+            float c = cs[j];
+            const float h = lstm_cell(gs[j], gs[H + j], gs[2 * H + j], gs[3 * H + j], c, q);
             cs[j] = c;
             hs[j] = h;
             h_out[r * ldh + j] = h;
             if (gates != nullptr) {
-                gates[r * G + j] = ig; gates[r * G + H + j] = fg; gates[r * G + 2 * H + j] = gg; gates[r * G + 3 * H + j] = og;
+                gates[r * G + j] = q.i; gates[r * G + H + j] = q.f; gates[r * G + 2 * H + j] = q.g; gates[r * G + 3 * H + j] = q.o;
             }
             if (c_seq != nullptr) c_seq[r * H + j] = c;
         }
