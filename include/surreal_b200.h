@@ -410,6 +410,8 @@ int sb200_hard_update_every_f32(float* target, const float* src, int64_t n, int6
 #define SB200_DSTAT_Q_TARGET 4
 #define SB200_DSTAT_Q_POLICY 5
 #define SB200_DSTAT_ACTION_ABSMAX 6   /* for the deferred `assert |a| <= 1` of ddpg.py:261-262 */
+#define SB200_DSTAT_TD_ERROR 7        /* weighted critic loss only: mean |q - y| (the reference DQN's td_error) */
+#define SB200_DSTAT_IS_WEIGHT 8       /* weighted critic loss only: mean importance weight */
 /* byte offset inside the DDPG workspace of the int32 "bad action" flag: sb200_ddpg_target*_f32 set it to 1 when
  * max|a| > 1 (the reference asserts this BEFORE any update, ddpg.py:261-262); pass its address as stop_flag to the
  * optimiser / soft-update calls of the same learn() so an out-of-range batch leaves every parameter untouched. */
@@ -422,6 +424,12 @@ int sb200_ddpg_target_f32(const float* rewards, const float* q_next, int64_t ldq
 /* MSE(q, y): dq = 2 (q - y) / B. */
 int sb200_ddpg_critic_loss_f32(const float* q, int64_t ldq, const float* y, int B, float* dq, int64_t ldd,
                                float* stats, void* workspace, void* stream);
+/* The critic loss of prioritized replay (dqn.py:148-168): mean(w (q - y)^2), dq = 2 w (q - y) / B, with importance
+ * weights w [B]; stats also get TD_ERROR and IS_WEIGHT.  priorities [B] (or NULL): |q - y| + eps per row, the new
+ * priorities of the sampled records.  With every w == 1 dq and the loss equal sb200_ddpg_critic_loss_f32's bit for bit. */
+int sb200_ddpg_critic_loss_weighted_f32(const float* q, int64_t ldq, const float* y, int B, const float* weights,
+                                        float* dq, int64_t ldd, float* priorities, double eps, float* stats,
+                                        void* workspace, void* stream);
 /* TD3 options (ddpg.py:267-283): target2 = ddpg_target with y = min(y, y2) over two target critics; smooth_action =
  * clamp(pi + clip(policy_noise * N(0,1), -noise_clip, noise_clip), -1, 1) (unit_noise [B][A] injected draws, or NULL
  * for Philox keyed by (seed, *step_counter, row)). */
@@ -754,6 +762,51 @@ int sb200_uniform_view(const void* uniform_state, int64_t reserve, int64_t* view
 int sb200_uniform_sample_gather_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,
                                     int nfields, const int64_t* view, uint64_t seed, void* sampler, int batch,
                                     int64_t* indices, void* stream);
+/* Prioritized replay (Schaul et al. 2016; the reference's prioritized_replay.py + segment_tree.py) over the uniform
+ * ring: a sum tree and a min tree of p^alpha over the ring's slots, in device memory, and the entries that admit new
+ * records, sample with importance weights and write new priorities, all capturable (no host read, fixed grids).
+ *   Trees: `leaves` = capacity rounded up to a power of two (>= 2), heap order (node 1 is the root, node i has children
+ *   2i and 2i+1, leaf j is node leaves + j).  leaf [leaves] fp32 p^alpha, 0 for a slot never inserted (and for slots
+ *   >= capacity); sum [leaves] fp64 internal nodes, parent = left + right; mn [leaves] fp32 internal min nodes, where a 0
+ *   leaf counts as +inf.  Internal nodes are rebuilt from their children, one CTA per `subtree` leaves (only subtrees
+ *   flagged in dirty [leaves / subtree]), then the levels above, so tree values never depend on thread scheduling.
+ *   owner [capacity]: int32 scratch of the priority update, all -1 at construction and after every update.
+ *   ctrl: sb200_per_ctrl_bytes() bytes {int64 admitted; int64 updates; float max_priority; uint32 ticket}, zeroed with
+ *   max_priority = 1.0 at construction.
+ * per_tree_layout: `leaves` and `subtree` of a ring of `capacity` slots.
+ * per_admit: every slot inserted since the last admit (total_in of the uniform state against ctrl.admitted, with wrap;
+ *   all slots once the gap reaches capacity) gets max_priority^alpha, then the tree is rebuilt.  Call it before
+ *   sb200_uniform_view.
+ * per_rebuild: rebuild dirty subtrees (every subtree when full != 0) and the levels above.
+ * per_sample_gather: as uniform_sample_gather (same view, Philox call/counter convention and empty-view rule), but draw
+ *   k takes u = (64-bit word >> 11) * 2^-53 and mass = u * S, S the leaf sum over the view (split in two segments when it
+ *   wraps), and descends the sum tree by prefix sum from the view's first slot (find_prefixsum_idx), clamped into the
+ *   view.  weights [batch]: (leaf / min over the view)^(-beta), in fp64, with beta = beta_override when >= 0, else
+ *   beta0 + min(updates / beta_anneal_iters, 1) (1 - beta0) (beta0 alone when beta_anneal_iters <= 0).  The launch
+ *   advances the sampler's draw_counter and ctrl.updates.
+ * per_update: leaf[indices[b]] = priorities[b]^alpha, the last b winning among equal indices, max_priority = max(it,
+ *   priorities); then the rebuild.  Nothing happens while *stop_flag != 0 (stop_flag may be NULL). */
+typedef struct sb200_per_tree {
+    int64_t capacity;
+    int64_t leaves;
+    int64_t subtree;
+    float* leaf;
+    double* sum;
+    float* mn;
+    uint32_t* dirty;
+    int32_t* owner;
+    void* ctrl;
+} sb200_per_tree;
+size_t sb200_per_ctrl_bytes(void);
+int sb200_per_tree_layout(int64_t capacity, int64_t* leaves, int64_t* subtree);
+int sb200_per_admit(const sb200_per_tree* tree, const void* uniform_state, double alpha, void* stream);
+int sb200_per_rebuild(const sb200_per_tree* tree, int full, void* stream);
+int sb200_per_sample_gather_f32(const sb200_per_tree* tree, const float* const* srcs, float* const* outs,
+                                const int64_t* record_floats, int nfields, const int64_t* view, uint64_t seed,
+                                void* sampler, int batch, double beta0, double beta_anneal_iters, double beta_override,
+                                int64_t* indices, float* weights, void* stream);
+int sb200_per_update_f32(const sb200_per_tree* tree, const int64_t* indices, const float* priorities, int batch,
+                         double alpha, const int* stop_flag, void* stream);
 /* Experience staging of DDPG: ExpSenderWrapperSSARNStepBootstrap._step (exp_sender_wrapper.py:96-112) for N actors +
  * UniformReplay.insert (uniform_replay.py:36-41): k-th insert -> slot k % capacity, actor order.  One descriptor of the
  * buffers involved (device memory, allocated once by the caller), taken whole by both ssar_step entries.

@@ -58,6 +58,13 @@ class Ssar(C.Structure):
                 ('step_counter', C.c_void_p)]
 
 
+class PerTree(C.Structure):
+    """sb200_per_tree (include/surreal_b200.h): the sum / min trees of a prioritized replay and their scratch."""
+    _fields_ = [('capacity', C.c_int64), ('leaves', C.c_int64), ('subtree', C.c_int64), ('leaf', C.c_void_p),
+                ('sum', C.c_void_p), ('mn', C.c_void_p), ('dirty', C.c_void_p), ('owner', C.c_void_p),
+                ('ctrl', C.c_void_p)]
+
+
 class PPORollout(C.Structure):
     """sb200_ppo_rollout (include/surreal_b200.h)."""
     _fields_ = [('net', C.POINTER(Mlp)), ('zf_stats', C.c_void_p), ('zf_eps', C.c_float), ('log_var', C.c_void_p),
@@ -221,6 +228,12 @@ def _declare(lib):
         'sb200_uniform_sampler_bytes': (S, []),
         'sb200_uniform_view': (I, [P, L, P, P]),
         'sb200_uniform_sample_gather_f32': (I, [P, P, P, I, P, C.c_uint64, P, I, P, P]),
+        'sb200_per_ctrl_bytes': (S, []),
+        'sb200_per_tree_layout': (I, [L, C.POINTER(L), C.POINTER(L)]),
+        'sb200_per_admit': (I, [C.POINTER(PerTree), P, D, P]),
+        'sb200_per_rebuild': (I, [C.POINTER(PerTree), I, P]),
+        'sb200_per_sample_gather_f32': (I, [C.POINTER(PerTree), P, P, P, I, P, C.c_uint64, P, I, D, D, D, P, P, P]),
+        'sb200_per_update_f32': (I, [C.POINTER(PerTree), P, P, I, D, P, P]),
         'sb200_ssar_step_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P]),
         'sb200_ssar_step_host_f32': (I, [C.POINTER(Ssar), P, P, P, P, P, P, P, P, P, P, P]),
         'sb200_mt19937_state_bytes': (S, []),
@@ -231,6 +244,7 @@ def _declare(lib):
         'sb200_ddpg_workspace_bytes': (S, [I]),
         'sb200_ddpg_target_f32': (I, [P, P, L, P, P, L, I, I, D, P, P, P, P]),
         'sb200_ddpg_critic_loss_f32': (I, [P, L, P, I, P, L, P, P, P]),
+        'sb200_ddpg_critic_loss_weighted_f32': (I, [P, L, P, I, P, P, L, P, D, P, P, P]),
         'sb200_ddpg_actor_seed_f32': (I, [P, L, I, P, L, P, P, P]),
         'sb200_tanh_bwd_f32': (I, [P, L, P, L, I, I, P, L, P]),
         'sb200_optim_workspace_bytes': (S, []),

@@ -82,34 +82,57 @@ __global__ void __launch_bounds__(DT) ddpg_target_kernel(const float* __restrict
 }
 
 // critic loss: MSE(q, y) (nn.MSELoss, ddpg.py:305) -> dq = 2(q-y)/B; stats: critic_loss, Q_policy.
+// With importance weights w (prioritized replay, dqn.py:148-168): mean(w (q-y)^2) -> dq = 2 w (q-y)/B, the stats
+// td_error = mean|q-y| and is_weight = mean w, and (prio non-NULL) the row's new priority |q-y| + eps.
 __global__ void __launch_bounds__(DT) ddpg_critic_loss_kernel(const float* __restrict__ q, long long ldq,
                                                               const float* __restrict__ y, int B,
                                                               float* __restrict__ dq, long long ldd,
-                                                              float* __restrict__ stats, DdpgWs* ws) {
+                                                              float* __restrict__ stats, DdpgWs* ws,
+                                                              const float* __restrict__ w, float* __restrict__ prio,
+                                                              double eps) {
     __shared__ double sh[32];
     const int tid = threadIdx.x, b = blockIdx.x * DT + tid;
-    double se = 0.0, qs = 0.0;
+    double se = 0.0, qs = 0.0, ad = 0.0, ws_ = 0.0;
     if (b < B) {
         const float qq = q[(long long)b * ldq];
         const float d = qq - y[b];
         se = (double)d * (double)d;
         qs = (double)qq;
-        dq[(long long)b * ldd] = (float)(2.0 * (double)d / (double)B);
+        double g = 2.0 * (double)d;
+        if (w != nullptr) {
+            const double wb = (double)w[b];
+            se = wb * se;
+            g = g * wb;
+            ad = fabs((double)d);
+            ws_ = wb;
+            if (prio != nullptr) prio[b] = (float)(ad + eps);
+        }
+        dq[(long long)b * ldd] = (float)(g / (double)B);
         for (int j = 1; j < (int)ldd; ++j) dq[(long long)b * ldd + j] = 0.0f;
     }
     double* part = ws->partial + (size_t)blockIdx.x * 4;
     double t;
     t = block_sum(se, sh);  if (tid == 0) part[0] = t;
     t = block_sum(qs, sh);  if (tid == 0) part[1] = t;
+    if (w != nullptr) {
+        t = block_sum(ad, sh);   if (tid == 0) part[2] = t;
+        t = block_sum(ws_, sh);  if (tid == 0) part[3] = t;
+    }
     if (last_block_ticket(&ws->counter, gridDim.x)) {
         if (tid == 0) {
-            double s0 = 0, s1 = 0;
+            double s0 = 0, s1 = 0, s2 = 0, s3 = 0;
             for (unsigned int k = 0; k < gridDim.x; ++k) {
                 s0 += ws->partial[(size_t)k * 4 + 0];
                 s1 += ws->partial[(size_t)k * 4 + 1];
+                s2 += ws->partial[(size_t)k * 4 + 2];
+                s3 += ws->partial[(size_t)k * 4 + 3];
             }
             stats[SB200_DSTAT_CRITIC_LOSS] = (float)(s0 / B);
             stats[SB200_DSTAT_Q_POLICY] = (float)(s1 / B);
+            if (w != nullptr) {
+                stats[SB200_DSTAT_TD_ERROR] = (float)(s2 / B);
+                stats[SB200_DSTAT_IS_WEIGHT] = (float)(s3 / B);
+            }
         }
     }
 }
@@ -215,7 +238,17 @@ extern "C" int sb200_ddpg_smooth_action_f32(const float* pi, int64_t ldp, const 
 extern "C" int sb200_ddpg_critic_loss_f32(const float* q, int64_t ldq, const float* y, int B, float* dq, int64_t ldd,
                                           float* stats, void* workspace, void* stream) {
     SB200_REQUIRE(q && y && dq && stats && workspace && B >= 1 && ldd >= 1);
-    ddpg_critic_loss_kernel<<<nb(B), DT, 0, (cudaStream_t)stream>>>(q, ldq, y, B, dq, ldd, stats, (DdpgWs*)workspace);
+    ddpg_critic_loss_kernel<<<nb(B), DT, 0, (cudaStream_t)stream>>>(q, ldq, y, B, dq, ldd, stats, (DdpgWs*)workspace,
+                                                                    nullptr, nullptr, 0.0);
+    return sb200_launch_status();
+}
+
+extern "C" int sb200_ddpg_critic_loss_weighted_f32(const float* q, int64_t ldq, const float* y, int B,
+                                                   const float* weights, float* dq, int64_t ldd, float* priorities,
+                                                   double eps, float* stats, void* workspace, void* stream) {
+    SB200_REQUIRE(q && y && weights && dq && stats && workspace && B >= 1 && ldd >= 1);
+    ddpg_critic_loss_kernel<<<nb(B), DT, 0, (cudaStream_t)stream>>>(q, ldq, y, B, dq, ldd, stats, (DdpgWs*)workspace,
+                                                                    weights, priorities, eps);
     return sb200_launch_status();
 }
 

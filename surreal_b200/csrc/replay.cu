@@ -7,7 +7,7 @@
 // (aggregator.py:52-103,151-262) and ExpSenderWrapperSSARNStepBootstrap (exp_sender_wrapper.py:72-112).
 // Records are stored SoA (one array per field, record-major) so that every field of a record is one
 // contiguous, 16-byte aligned run: gathers move whole sectors.
-#include "common.cuh"
+#include "replay_dev.cuh"
 #include <string.h>
 
 namespace {
@@ -89,12 +89,7 @@ __global__ void __launch_bounds__(256) gather_kernel(const float* __restrict__ s
 // POSITION, the reference's warm-up quirk); the new transition is appended; when the deque holds n_step
 // entries the oldest is emitted.  Emitted records go to ring slot (next_idx + rank) % capacity in actor
 // order (uniform_replay.py:36-41).
-struct UniformState {
-    long long next_idx;
-    long long size;
-    long long capacity;
-    long long total_in;
-};
+// (UniformState {next_idx, size, capacity, total_in}: replay_dev.cuh)
 
 // Rew: float for device envs, double for host envs, whose float64 rewards the reference sums as Python floats.
 template <typename Rew>
@@ -257,35 +252,7 @@ inline uint32_t mt_next(MT* g) {
     return y;
 }
 
-// All fields of a record in ONE launch: out_f[b] = src_f[idx[b]] for f < nf.  A warp owns a record; its lanes walk the
-// record's chunks across fields (16-byte chunks for fields whose record size / alignment allow, 4-byte otherwise), so a
-// 552-byte SSAR record (obs 64, obs_next 64, action 8, reward 1, done 1 floats) is two loads + two stores per lane.
-constexpr int GATHER_MAX_FIELDS = 8;
-struct GatherFields {
-    const float* src[GATHER_MAX_FIELDS];
-    float* out[GATHER_MAX_FIELDS];
-    long long rec[GATHER_MAX_FIELDS];     // floats per record
-    int unit[GATHER_MAX_FIELDS];          // 4 (float4 chunks) or 1
-    int chunk_end[GATHER_MAX_FIELDS];     // prefix sums of chunks per record
-    int nf;
-};
-
-// record `s` of every field -> batch row `b`, by the 32 lanes of one warp
-__device__ __forceinline__ void gather_record(const GatherFields& f, long long s, long long b, int lane) {
-    const int total = f.chunk_end[f.nf - 1];
-    for (int c = lane; c < total; c += 32) {
-        int q = 0;
-#pragma unroll
-        for (int k = 0; k < GATHER_MAX_FIELDS - 1; ++k) q += (k < f.nf - 1 && c >= f.chunk_end[k]) ? 1 : 0;
-        const int local = c - (q > 0 ? f.chunk_end[q - 1] : 0);
-        if (f.unit[q] == 4) {
-            reinterpret_cast<float4*>(f.out[q] + b * f.rec[q])[local] = ld_stream4(f.src[q] + s * f.rec[q] + 4 * local);
-        } else {
-            f.out[q][b * f.rec[q] + local] = __ldg(f.src[q] + s * f.rec[q] + local);
-        }
-    }
-}
-
+// GatherFields / gather_record: replay_dev.cuh
 __global__ void __launch_bounds__(256) gather_multi_kernel(const __grid_constant__ GatherFields f, const int* __restrict__ idx,
                                                            const long long* __restrict__ idx64, int batch) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -306,16 +273,7 @@ __global__ void __launch_bounds__(256) gather_multi_kernel(const __grid_constant
 // thread does the same work, at a bias of at most count / 2^64 per index (< 2^-43 for a 2^20-slot ring).  The launch
 // advances draw_counter itself (the last block to finish, after every block has read it), so a captured graph draws
 // fresh indices at every replay.  Not the reference's stream: random.randint parity is sb200_mt19937_randint_fill_h.
-struct UniformView {
-    long long start;
-    long long count;
-    long long capacity;
-};
-struct UniformSampler {
-    unsigned long long draw_counter;
-    int status;              // 1: the last launch found an empty view and sampled nothing
-    unsigned int ticket;
-};
+// UniformView / UniformSampler: replay_dev.cuh
 
 // One warp per Philox call = two records: lane 0 draws, the warp copies.
 __global__ void __launch_bounds__(256) uniform_sample_gather_kernel(const __grid_constant__ GatherFields f,
@@ -387,26 +345,6 @@ extern "C" int sb200_replay_gather_f32(const float* src, int64_t record_floats, 
     gather_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(src, record_floats, idx32, (const long long*)idx64, batch, out,
                                                             vec);
     return sb200_launch_status();
-}
-
-// Field table of the multi-field gathers from the caller's HOST arrays; false when an entry is unusable.
-static bool gather_fields_ok(const float* const* srcs, float* const* outs, const int64_t* record_floats, int nfields,
-                             GatherFields* f) {
-    if (!srcs || !outs || !record_floats || nfields < 1 || nfields > GATHER_MAX_FIELDS) return false;
-    int end = 0;
-    for (int k = 0; k < nfields; ++k) {
-        if (!srcs[k] || !outs[k] || record_floats[k] < 1 || record_floats[k] >= (1ll << 28)) return false;
-        f->src[k] = srcs[k];
-        f->out[k] = outs[k];
-        f->rec[k] = record_floats[k];
-        const bool vec = (record_floats[k] % 4 == 0) && ((((uintptr_t)srcs[k]) | ((uintptr_t)outs[k])) & 15) == 0;
-        f->unit[k] = vec ? 4 : 1;
-        end += (int)(record_floats[k] / f->unit[k]);
-        f->chunk_end[k] = end;
-    }
-    for (int k = nfields; k < GATHER_MAX_FIELDS; ++k) { f->src[k] = nullptr; f->out[k] = nullptr; f->rec[k] = 0; f->unit[k] = 1; f->chunk_end[k] = end; }
-    f->nf = nfields;
-    return true;
 }
 
 extern "C" int sb200_replay_gather_multi_f32(const float* const* srcs, float* const* outs, const int64_t* record_floats,

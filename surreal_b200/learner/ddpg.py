@@ -16,7 +16,8 @@ from ..session import ConfigError
 from .aggregator import SSARAggregator
 from .base import Learner
 
-DS = dict(ACTOR_LOSS=0, CRITIC_LOSS=1, ACTION_NORM=2, REWARDS=3, Q_TARGET=4, Q_POLICY=5, ABSMAX=6)
+DS = dict(ACTOR_LOSS=0, CRITIC_LOSS=1, ACTION_NORM=2, REWARDS=3, Q_TARGET=4, Q_POLICY=5, ABSMAX=6, TD_ERROR=7,
+          IS_WEIGHT=8)
 
 
 def _ptr(t):
@@ -103,6 +104,13 @@ class DDPGLearner(Learner):
         self._hard_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self._readback = torch.zeros(34, dtype=torch.float64, device=self.device)
         self._replay_graphs = {}
+        # prioritized replay: a batch with importance weights takes the weighted critic loss (dqn.py:148-168), whose
+        # rows also give the sampled records' new priorities |q1 - y| + eps (critic 1's TD error, before the step)
+        rc = lc.replay
+        self.priority_eps = float(rc.priority_eps) if 'priority_eps' in rc else 1e-6
+        self._w = f(B, 1)                                      # learn(): the batch's weights, at a fixed address
+        self._prio = f(B)
+        self._graph_w = ops.GraphRunner()
 
     # ------------------------------------------------------------------------------------------------
     def preprocess(self, batch):
@@ -145,9 +153,27 @@ class DDPGLearner(Learner):
             self._noise_draws = torch.zeros(self.batch_size, self.action_dim, dtype=torch.float32, device=self.device)
         self._noise_draws.copy_(torch.as_tensor(draws, dtype=torch.float32).reshape(self.batch_size, self.action_dim))
 
-    def _optimize_device(self, stop=None):
+    @property
+    def td_priorities(self):
+        """Device [B]: |q1 - y| + priority_eps of the last weighted update's rows (the priorities to write back)."""
+        return self._prio
+
+    def _critic_loss(self, trainer, q, stats, weights, prio):
+        L, st, B = _lib.lib(), ops._stream(), self.batch_size
+        d = trainer.d[-1]
+        if weights is None:
+            check(L.sb200_ddpg_critic_loss_f32(_ptr(q), q.stride(0), _ptr(self._y), B, _ptr(d), d.stride(0), _ptr(stats),
+                                               _ptr(self._ws), st), 'sb200_ddpg_critic_loss_f32')
+        else:
+            check(L.sb200_ddpg_critic_loss_weighted_f32(_ptr(q), q.stride(0), _ptr(self._y), B, _ptr(weights), _ptr(d),
+                                                        d.stride(0), _ptr(prio), self.priority_eps, _ptr(stats),
+                                                        _ptr(self._ws), st), 'sb200_ddpg_critic_loss_weighted_f32')
+
+    def _optimize_device(self, stop=None, weights=None):
         """ddpg.py:244-333 as one fixed launch sequence (CUDA-graph body; no host round trip inside).  ``stop``: the
-        flag that no-ops the optimiser / target kernels -- this update's bad-action flag, or a flag that latches it."""
+        flag that no-ops the optimiser / target kernels -- this update's bad-action flag, or a flag that latches it.
+        ``weights`` (device [B, 1]): importance weights of a prioritized batch; both critic losses are weighted and
+        critic 1's rows leave the new priorities in ``td_priorities``."""
         L = _lib.lib()
         stop = self._bad if stop is None else stop
         B, A = self.batch_size, self.action_dim
@@ -178,17 +204,13 @@ class DDPGLearner(Learner):
             torch.maximum(stop, self._bad, out=stop)
         ct = self.critic_optim
         q = ct.forward(obs, aux=actions)                                                # Q(s_t, a_t)
-        check(L.sb200_ddpg_critic_loss_f32(_ptr(q), q.stride(0), _ptr(self._y), B, _ptr(ct.d[-1]),
-                                           ct.d[-1].stride(0), _ptr(self._stats), _ptr(self._ws), st),
-              'sb200_ddpg_critic_loss_f32')
+        self._critic_loss(ct, q, self._stats, weights, self._prio)
         ct.backward()
         ct.step(stop_flag=stop)
         if self.use_double_critic:                                                       # ddpg.py:298-303,311-321
             c2 = self.critic_optim2
             q2 = c2.forward(obs, aux=actions)
-            check(L.sb200_ddpg_critic_loss_f32(_ptr(q2), q2.stride(0), _ptr(self._y), B, _ptr(c2.d[-1]),
-                                               c2.d[-1].stride(0), _ptr(self._stats2), _ptr(self._ws), st),
-                  'sb200_ddpg_critic_loss_f32')
+            self._critic_loss(c2, q2, self._stats2, weights, None)
             c2.backward()
             c2.step(stop_flag=stop)
         at = self.actor_optim
@@ -210,9 +232,14 @@ class DDPGLearner(Learner):
                 check(L.sb200_soft_update_f32(_ptr(t.params), _ptr(s_.params), t.size, float(self.target_update_tau),
                                               _ptr(stop), st), 'sb200_soft_update_f32')
 
-    def _optimize(self):
+    def _optimize(self, weighted=False):
         with self.forward_time.time():
-            if self.use_cuda_graph:
+            if weighted:
+                if self.use_cuda_graph:
+                    self._graph_w.run(lambda: self._optimize_device(weights=self._w))
+                else:
+                    self._optimize_device(weights=self._w)
+            elif self.use_cuda_graph:
                 self._graph.run(self._optimize_device)
             else:
                 self._optimize_device()
@@ -221,7 +248,7 @@ class DDPGLearner(Learner):
         s2 = self._stats2.cpu().numpy() if self.use_double_critic else None
         if self.check_action_range and s[DS['ABSMAX']] > 1.0:
             raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
-        stats = self._statistics(s, s2)
+        stats = self._statistics(s, s2, weighted)
         if self.target_update_type == 'hard':                     # host-side counter (ddpg.py:419-428)
             self.target_update_counter += 1
             if self.target_update_counter % self.target_update_interval == 0:
@@ -231,7 +258,7 @@ class DDPGLearner(Learner):
                     self.model_target2.critic.params.copy_(self.model2.critic.params)
         return stats
 
-    def _statistics(self, s, s2):
+    def _statistics(self, s, s2, weighted=False):
         stats = {'actor_loss': float(s[DS['ACTOR_LOSS']]), 'critic_loss': float(s[DS['CRITIC_LOSS']]),
                  'action_norm': float(s[DS['ACTION_NORM']]), 'rewards': float(s[DS['REWARDS']]),
                  'Q_target': float(s[DS['Q_TARGET']]), 'Q_policy': float(s[DS['Q_POLICY']]),
@@ -241,14 +268,25 @@ class DDPGLearner(Learner):
         if s2 is not None:                                       # ddpg.py:316,345-346: critic_loss is critic 2's
             stats['critic_loss'] = float(s2[DS['CRITIC_LOSS']])
             stats['Q_policy2'] = float(s2[DS['Q_POLICY']])
+        if weighted:                                             # prioritized replay only (dqn.py's td_error)
+            stats['td_error'] = float(s[DS['TD_ERROR']])
+            stats['avg_is_weight'] = float(s[DS['IS_WEIGHT']])
         return stats
 
     def learn(self, batch):
-        """ddpg.py:354-374."""
+        """ddpg.py:354-374.  A batch with ``weights`` (prioritized replay) takes the weighted critic loss; when it also
+        carries ``indices`` and the attached replay has priorities, the new ones are written back to it."""
         self.current_iteration += 1
+        get = (lambda k: batch.get(k)) if isinstance(batch, dict) else (lambda k: getattr(batch, k, None))
+        weights, indices = get('weights'), get('indices')
         with self.total_learn_time.time():
             self.preprocess(batch)
-            stats = self._optimize()
+            if weights is not None:
+                self._w.copy_(torch.as_tensor(weights, dtype=torch.float32).reshape(self._w.shape), non_blocking=True)
+            stats = self._optimize(weighted=weights is not None)
+            if weights is not None and indices is not None and hasattr(self._replay, 'update_priorities_device'):
+                idx = torch.as_tensor(indices, dtype=torch.int64).to(self.device).reshape(-1)
+                self._replay.update_priorities_device(idx, self._prio, stop_flag=self._bad)
             stats['performance/total_learn_time'] = self.total_learn_time.avg
             self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
             self.periodic_checkpoint(global_steps=self.current_iteration, score=None)
@@ -256,12 +294,16 @@ class DDPGLearner(Learner):
 
     def _replay_updates_device(self, replay, updates):
         """``updates`` x [sample on the device -> update -> target update] and the read-back staging, as one fixed
-        launch sequence.  A bad-action batch stops every later optimiser / target kernel of the sequence (_stop)."""
+        launch sequence.  A bad-action batch stops every later optimiser / target kernel of the sequence (_stop).  On a
+        prioritized replay each update is weighted and writes its priorities back (sample -> update -> priorities)."""
         L, st = _lib.lib(), ops._stream()
+        per = hasattr(replay, 'update_priorities_device')
         self._stop.zero_()
         for _ in range(updates):
-            replay.sample_device(self.batch_size, out=self._own)
-            self._optimize_device(stop=self._stop)
+            b = replay.sample_device(self.batch_size, out=self._own)
+            self._optimize_device(stop=self._stop, weights=b['weights'] if per else None)
+            if per:                                                  # no-op once _stop is latched
+                replay.update_priorities_device(b['indices'], self._prio, stop_flag=self._stop)
             if self.target_update_type == 'hard':                                        # ddpg.py:419-428
                 pairs = [(self.model_target.actor, self.model.actor), (self.model_target.critic, self.model.critic)]
                 if self.use_double_critic:
@@ -303,7 +345,8 @@ class DDPGLearner(Learner):
                 self.target_update_counter = int(rb[33])
             if self.check_action_range and rb[32] != 0:
                 raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
-            stats = self._statistics(rb[0:16], rb[16:32] if self.use_double_critic else None)
+            stats = self._statistics(rb[0:16], rb[16:32] if self.use_double_critic else None,
+                                     hasattr(replay, 'update_priorities_device'))
             stats['performance/total_learn_time'] = self.total_learn_time.avg
             self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
             self.periodic_checkpoint(global_steps=self.current_iteration, score=None)

@@ -73,6 +73,9 @@ def ddpg_argparser():
     p.add_argument('--rollout-steps', type=int, default=None)
     p.add_argument('--updates-per-chunk', type=int, default=None)
     p.add_argument('--iterations', type=int, default=None)
+    # proportional prioritized replay (replay.PrioritizedReplay) instead of the uniform ring; its alpha, beta0,
+    # beta_anneal_iters and priority_eps come from learner_config.replay when set there
+    p.add_argument('--prioritized-replay', action='store_true')
     return p
 
 
@@ -83,7 +86,7 @@ class DDPGLauncher:
         from ..launch import SurrealDefaultLauncher
         from ..agent import DDPGAgent
         from ..learner import DDPGLearner
-        from ..replay import UniformReplay
+        from ..replay import UniformReplay, PrioritizedReplay
         from .ppo_configs import make_synthetic_env_config
 
         class _DDPGLauncher(SurrealDefaultLauncher):
@@ -108,6 +111,8 @@ class DDPGLauncher:
                 self.eval_batch_size = args.eval_batch
                 self.rollout_steps, self.updates_per_chunk = args.rollout_steps, args.updates_per_chunk
                 self.iterations = args.iterations
+                if args.prioritized_replay:
+                    self.replay_class = PrioritizedReplay
                 if args.unit_test:
                     self.learner_config.replay.sampling_start_size = 5
                     self.learner_config.replay.replay_shards = 1
