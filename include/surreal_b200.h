@@ -447,6 +447,54 @@ int sb200_tanh_bwd_f32(const float* dout, int64_t ldo, const float* out, int64_t
                        float* dpre, int64_t ldd, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * DQN (surreal/learner/dqn.py, agent/q_agent.py, model/q_net.py).  The Q towers run through sb200_mlp_forward_f32 /
+ * the packed forward (one call per tower: the action tower [rows][n_actions], with dueling also the state tower
+ * [rows][1]); these entries combine them, Q = (A - mean_j A) + V, or Q = A without a state tower.
+ *
+ * act: one warp per actor, argmax_j Q_j (first index among ties), then epsilon-greedy.  epsilon is
+ *   schedule(*act_counter) when `schedule` is given -- the device array [t_0..t_{P-1} | v_0..v_{P-1} | outside] of a
+ *   PiecewiseSchedule with P = n_points (utils/schedule.py:34-73; LinearSchedule is [(0, 1), (T, final)] with outside
+ *   value final) -- else fixed_eps.  Philox4x32-10 keyed (seed, *act_counter, actor): u = x / 2^32 < epsilon explores
+ *   with action floor(y * n_actions / 2^32).  Writes the action index as a float (the record's action field),
+ *   optionally a one-hot row [N][ldo] (ldo >= n_actions, the tail zero) and the index as int64.  The caller advances
+ *   *act_counter after the call (q_agent.py:45: T += 1 per act).
+ * act_host: act on host observations in one call: H2D of obs_host (NULL: obs_dev already holds them), the tower
+ *   forwards, act, D2H of the int64 actions into action_host and one stream synchronisation. */
+#define SB200_DQN_MAX_ACTIONS 1024
+int sb200_dqn_act_f32(const float* adv, int64_t lda, const float* value, int64_t ldv, int N, int n_actions,
+                      const double* schedule, int n_points, double fixed_eps, uint64_t seed, const int64_t* act_counter,
+                      float* action, float* one_hot, int64_t ldo, int64_t* action_i64, void* stream);
+int sb200_dqn_act_host_f32(const sb200_mlp* adv_net, const sb200_mlp* value_net, const float* obs_host, float* obs_dev,
+                           int N, float* adv_dev, float* value_dev, const double* schedule, int n_points,
+                           double fixed_eps, uint64_t seed, const int64_t* act_counter, float* action_dev,
+                           int64_t* action_i64_dev, int64_t* action_host, void* stream);
+/* TD step of one update (dqn.py:44-69), one thread per row: q = Q(s)[a] from the online towers (q_a, q_v), the target
+ * towers at s' (t_a, t_v) and, for double Q, the online towers at s' (o_a, o_v; NULL for max over the target row).
+ * y = r + gamma (1 - done) q', td = q - y, loss = mean(w huber(td)) with the Huber of delta 1 (w = 1 when weights is
+ * NULL).  Writes d_a / d_v, the gradients w.r.t. the towers' outputs (dQ_a = w clamp(td, -1, 1) / B; dueling:
+ * dA_j = dQ_j - mean_k dQ_k, dV = sum_k dQ_k; padding columns zero), priorities[b] = |td| + priority_eps when given, the
+ * SB200_QSTAT_* statistics as fixed-order sums, and the workspace's bad-action flag: 1 when some action is not an
+ * integer in [0, n_actions) (such rows compute with action 0).  Pass the flag as stop_flag to the optimiser calls of the
+ * update.  workspace: sb200_dqn_workspace_bytes(B), zero-initialised once. */
+#define SB200_QSTAT_LOSS 0
+#define SB200_QSTAT_TD_ERROR 1        /* mean |td| (dqn.py:87-90) */
+#define SB200_QSTAT_Q 2               /* mean Q(s, a) */
+#define SB200_QSTAT_IS_WEIGHT 3       /* mean importance weight (1 without weights) */
+#define SB200_QSTAT_BAD_ROWS 4        /* rows whose action is out of range */
+size_t sb200_dqn_workspace_bytes(int B);
+size_t sb200_dqn_bad_action_offset(void);
+int sb200_dqn_td_f32(const float* q_a, int64_t ld_qa, const float* q_v, int64_t ld_qv, const float* t_a, int64_t ld_ta,
+                     const float* t_v, int64_t ld_tv, const float* o_a, int64_t ld_oa, const float* o_v, int64_t ld_ov,
+                     const float* actions, const float* rewards, const float* dones, const float* weights, int B,
+                     int n_actions, double gamma, double priority_eps, float* d_a, int64_t ld_da, float* d_v,
+                     int64_t ld_dv, float* priorities, float* stats, void* workspace, void* stream);
+/* Hard target copy with PeriodicTracker(period).track_increment(incr) semantics on a device counter of samples
+ * (dqn.py:84-86, incr = batch size): tick != 0 adds incr first (pass it for the first buffer of an update); then
+ * target = src when the count crossed a multiple of period in that increment.  Neither happens when *stop_flag != 0. */
+int sb200_hard_update_samples_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t period,
+                                  int64_t incr, int tick, const int* stop_flag, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Experience staging of PPO: ExpSenderWrapperMultiStepMovingWindowWithInfo._step (exp_sender_wrapper.py:209-228) for N
  * actors + FIFOReplay.insert (fifo_replay.py:27,34-35).  Every entry that stages a step takes this one descriptor of the
  * buffers involved (all device memory, allocated once by the caller).

@@ -253,6 +253,13 @@ def _declare(lib):
         'sb200_soft_update_f32': (I, [P, P, L, D, P, P]),
         'sb200_hard_update_every_f32': (I, [P, P, L, P, L, I, P, P]),
         'sb200_ddpg_bad_action_offset': (S, []),
+        'sb200_dqn_act_f32': (I, [P, L, P, L, I, I, P, I, D, C.c_uint64, P, P, P, L, P, P]),
+        'sb200_dqn_act_host_f32': (I, [C.POINTER(Mlp), C.POINTER(Mlp), P, P, I, P, P, P, I, D, C.c_uint64, P, P, P, P,
+                                       P]),
+        'sb200_dqn_workspace_bytes': (S, [I]),
+        'sb200_dqn_bad_action_offset': (S, []),
+        'sb200_dqn_td_f32': (I, [P, L, P, L, P, L, P, L, P, L, P, L, P, P, P, P, I, I, D, D, P, L, P, L, P, P, P, P]),
+        'sb200_hard_update_samples_f32': (I, [P, P, L, P, L, L, I, P, P]),
         'sb200_gae_window_f32': (I, [P, P, P, I, I, I, D, D, D, I, P, P, P, P]),
     }
     sig.update(_EXTRA_SIGS)

@@ -13,7 +13,7 @@ from .. import _lib
 from .._lib import check
 from ..distributed import LocalHub
 from ..session import ConfigError
-from ..utils import obs_flat, obs_source
+from ..utils import obs_flat, obs_source, record_action_dim
 
 
 def _p(t):
@@ -36,7 +36,9 @@ class _WrapperBase:
                                'wraps its env (the ZeroMQ collector address of the reference is gone)')
         # D: floats per staged observation row = the env's obs_dim + obs_extra trailing floats (an RNN agent's LSTM cells,
         # utils.record_obs_dim)
-        self.N, self.D, self.A = env.N, env.D + int(obs_extra), env.A
+        # A: floats per staged action = the replay's record width (utils.record_action_dim: 1 for a discrete spec)
+        self.N, self.D = env.N, env.D + int(obs_extra)
+        self.A = record_action_dim(self.replay.env_config.action_spec)
         self.obs_dim = env.D
         # a batched HOST env (numpy in / numpy out, attributes N, D, A) has no device: the staging lives with the replay
         self.device = env.device if hasattr(env, 'device') else self.replay.device
@@ -246,7 +248,11 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         return obs, info
 
     def step(self, action):
+        """``action``: what the env steps with, or the pair (env action, record action) of a discrete agent (QAgent.act:
+        one-hot rows for the env, the indices as floats for the record)."""
         obs, reward, done, info = self.env.step(action)
+        if isinstance(action, tuple):
+            action = action[1]
         if self.host_env:
             self._step_host(obs, action, reward, done, info)
             return obs, reward, done, info

@@ -79,6 +79,19 @@ class SyntheticEnv:
         pass
 
 
+class DiscreteSyntheticEnv(SyntheticEnv):
+    """SyntheticEnv with ``n_actions`` discrete actions: the same arithmetic driven by one-hot rows a = e_k, so the action
+    term Wa a is column k of Wa [D][n_actions].  step() takes the one-hot rows [N, n_actions] (or QAgent.act's
+    (one-hot rows, indices) pair)."""
+
+    def __init__(self, num_envs, obs_dim=64, n_actions=18, limit_episode_length=200, seed=0, device=None):
+        super().__init__(num_envs, obs_dim, n_actions, limit_episode_length, seed, device)
+        self.n_actions = int(n_actions)
+
+    def action_spec(self):
+        return {'dim': (self.n_actions,), 'type': 'discrete'}
+
+
 class SyntheticPixelEnv:
     """Batched device-resident PIXEL env of BASELINE configs[3] (SURVEY §8d cfg 4): every step each actor observes a fresh
     uint8 frame [C, H, W] of uniform random bytes; reward = -mean(a^2) + 0.1 xi; episodes end at ``limit_episode_length``.

@@ -156,13 +156,14 @@ class StemTrainer:
         self.exp_avg_sq.copy_(torch.as_tensor(sd['exp_avg_sq']).to(self.stem.device))
 
 
-def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None):
+def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None, adam_eps=1e-8):
     """One optimiser step over a head network (ops.MlpTrainer) AND the shared stems: the reference clips the global norm
     of head + stem parameters together (get_actor_params / get_critic_params chain actor, cnn_stem and rnn_stem,
     ppo_net.py:202-224; ppo.py:244-246,349-351) and steps ONE Adam over all of them.  ``stem_trs`` is the list of stem
     trainers (StemTrainer / lstm_stem.RnnTrainer); ``grad`` = [head gradient | stem gradients in that order] is
     one contiguous buffer so that the norm (and a data-parallel all-reduce) sees everything at once; head.ws carries the
-    shared step count / norm."""
+    shared step count / norm.  A stem trainer may also be an ops.MlpTrainer (its ``net`` is then the stem: the DQN
+    state tower, clipped jointly with the action tower).  ``adam_eps``: Adam's eps for every segment."""
     L, st = _lib.lib(), ops._stream()
     nh = head.net.size
     segs, o = [(head.net.params, grad[:nh], head.exp_avg, head.exp_avg_sq, nh, norm_out)], nh
@@ -170,11 +171,12 @@ def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None):
     check(L.sb200_grad_reduce_norm_f32(_p(head.slabs), nh, head.splits, _p(grad[:nh]), nh, 1.0, 0, _p(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(head)')
     for tr in stem_trs:
-        ns = tr.stem.size
+        stem = tr.stem if hasattr(tr, 'stem') else tr.net
+        ns = stem.size
         gs = grad[o:o + ns]
         check(L.sb200_grad_reduce_norm_f32(_p(tr.slabs), ns, tr.splits, _p(gs), ns, 1.0, 0, _p(head.ws), sf, st),
               'sb200_grad_reduce_norm_f32(stem)')
-        segs.append((tr.stem.params, gs, tr.exp_avg, tr.exp_avg_sq, ns, None))
+        segs.append((stem.params, gs, tr.exp_avg, tr.exp_avg_sq, ns, None))
         o += ns
     dp = getattr(head, 'dp', None)
     scale = 1.0
@@ -184,5 +186,5 @@ def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None):
     check(L.sb200_grad_reduce_norm_f32(_p(grad), o, 1, _p(grad), o, scale, 1, _p(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(joint norm)')
     for params, g, m, v, n, no in segs:
-        check(L.sb200_clip_adam_f32(_p(params), _p(g), _p(m), _p(v), n, _p(head.lr), 0.9, 0.999, 1e-8, head.weight_decay,
+        check(L.sb200_clip_adam_f32(_p(params), _p(g), _p(m), _p(v), n, _p(head.lr), 0.9, 0.999, adam_eps, head.weight_decay,
                                     head.clip_mode, head.clip_value, _p(head.ws), _p(no), sf, st), 'sb200_clip_adam_f32')

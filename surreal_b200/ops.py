@@ -342,7 +342,8 @@ class MlpTrainer:
     """Forward-with-saved-activations, hand-written backward and Adam for one FlatNet on a fixed
     batch size M.  All buffers are allocated once; every method only launches kernels (graph-safe)."""
 
-    def __init__(self, net, M, lr, clip_mode=0, clip_value=0.0, weight_decay=0.0, splits=None, input_grad=False):
+    def __init__(self, net, M, lr, clip_mode=0, clip_value=0.0, weight_decay=0.0, splits=None, input_grad=False,
+                 adam_eps=1e-8):
         L = _lib.lib()
         self.net, self.M = net, M
         dev = net.device
@@ -353,6 +354,7 @@ class MlpTrainer:
         self.ws = torch.zeros(L.sb200_optim_workspace_bytes(), dtype=torch.uint8, device=dev)
         self.lr = torch.tensor([lr], dtype=torch.float64, device=dev)
         self.clip_mode, self.clip_value, self.weight_decay = clip_mode, float(clip_value), float(weight_decay)
+        self.adam_eps = float(adam_eps)                           # torch.optim.Adam's eps (DQN: 1e-4, dqn.py:18-22)
         self.x_in = z(M, _ru(net.dims[0], 4))
         self.h = [z(M, _ru(n, 4)) for n in net.dims[1:]]          # post-activation outputs
         self.d = [z(M, _ru(n, 4)) for n in net.dims[1:]]          # gradients w.r.t. pre-activations
@@ -493,7 +495,7 @@ class MlpTrainer:
                                                    1.0 / dp.world, 1, _ptr(self.ws), _ptr(stop_flag), st),
                       'sb200_grad_reduce_norm_f32')
         check(L.sb200_clip_adam_f32(_ptr(net.params), _ptr(self.grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq),
-                                    net.size, _ptr(self.lr), 0.9, 0.999, 1e-8, self.weight_decay, self.clip_mode,
+                                    net.size, _ptr(self.lr), 0.9, 0.999, self.adam_eps, self.weight_decay, self.clip_mode,
                                     self.clip_value, _ptr(self.ws), _ptr(norm_out), _ptr(stop_flag), st),
               'sb200_clip_adam_f32')
 

@@ -25,7 +25,8 @@ from .. import _lib
 from .._lib import check
 from .uniform_replay import UniformReplay, _p, _st
 
-# learner_config.replay keys read when present (the reference's PrioritizedReplay / DQN 'prioritized' defaults)
+# learner_config.replay keys read when present (the reference's PrioritizedReplay / DQN 'prioritized' defaults); a
+# learner config with an algo.prioritized block (DQN) takes all four from there instead
 PER_DEFAULTS = {'alpha': 0.6, 'beta0': 0.4, 'beta_anneal_iters': None, 'priority_eps': 1e-6}
 
 
@@ -34,6 +35,10 @@ class PrioritizedReplay(UniformReplay):
         super().__init__(learner_config, env_config, session_config, index)
         rc = self.learner_config.replay
         get = lambda k: rc[k] if k in rc else PER_DEFAULTS[k]  # noqa: E731
+        algo = self.learner_config.algo
+        if 'prioritized' in algo:                 # DQN's algo.prioritized block (dqn.py:115-119) is the one source there
+            pc = algo.prioritized
+            get = lambda k: pc['eps' if k == 'priority_eps' else k]  # noqa: E731
         self.alpha = float(get('alpha'))
         self.beta0 = float(get('beta0'))
         anneal = get('beta_anneal_iters')

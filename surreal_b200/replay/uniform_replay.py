@@ -21,6 +21,7 @@ import torch
 
 from .. import _lib
 from .._lib import check
+from ..utils import record_action_dim
 from .base import Replay, gather_fields
 
 
@@ -66,7 +67,7 @@ class UniformReplay(Replay):
         self.memory_size = self.learner_config.replay.memory_size
         self.batch_size = self.learner_config.replay.batch_size
         self.D = sum(v[0] for v in self.env_config.obs_spec['low_dim'].values())
-        self.A = self.env_config.action_spec.dim[0]
+        self.A = record_action_dim(self.env_config.action_spec)
         C_, D, A = self.memory_size, self.D, self.A
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
         self.r_obs, self.r_obs_next, self.r_act = f(C_, D), f(C_, D), f(C_, A)

@@ -230,3 +230,55 @@ def record_obs_dim(learner_config, env_config):
     (ppo_agent.py:133-137, exp_sender_wrapper.py:244-264); here they simply ride with every observation row."""
     lay = rnn_cell_layout(learner_config, env_config)
     return lay.width if lay is not None else obs_packed_dim(env_config.obs_spec)
+
+
+def action_is_discrete(action_spec):
+    """True for a discrete action spec ({'dim': (n_actions,), 'type': 'discrete'})."""
+    return 'type' in action_spec and action_spec['type'] == 'discrete'
+
+
+def record_action_dim(action_spec):
+    """Floats per action in the HBM staging / replay records and the learner's batch buffers: the action width A of a
+    continuous spec, 1 for a discrete one (the action index as a float, the [B, 1] column dqn.py:46-49 gathers with)."""
+    return 1 if action_is_discrete(action_spec) else int(action_spec['dim'][0])
+
+
+class LinearSchedule:
+    """initial_p + min(t / schedule_timesteps, 1) (final_p - initial_p) (surreal/utils/schedule.py:76-99)."""
+
+    def __init__(self, schedule_timesteps, final_p, initial_p=1.0):
+        self.schedule_timesteps, self.final_p, self.initial_p = schedule_timesteps, final_p, initial_p
+
+    def value(self, t):
+        fraction = min(float(t) / self.schedule_timesteps, 1.0)
+        return self.initial_p + fraction * (self.final_p - self.initial_p)
+
+    def device_points(self):
+        """The same schedule as PiecewiseSchedule([(0, initial_p), (T, v_T)], outside_value=v_T) with v_T = value(T)
+        (initial_p + (final_p - initial_p), which may differ from final_p in the last bit): the [t_0 .. | v_0 .. |
+        outside] array of sb200_dqn_act_f32, equal to value(t) at every t >= 0."""
+        v_t = self.value(self.schedule_timesteps)
+        return PiecewiseSchedule([(0, self.initial_p), (self.schedule_timesteps, v_t)], outside_value=v_t).device_points()
+
+
+class PiecewiseSchedule:
+    """Linear interpolation between (time, value) endpoints, ``outside_value`` elsewhere
+    (surreal/utils/schedule.py:34-73)."""
+
+    def __init__(self, endpoints, outside_value=None):
+        idxes = [e[0] for e in endpoints]
+        assert idxes == sorted(idxes)
+        self._endpoints, self._outside_value = list(endpoints), outside_value
+
+    def value(self, t):
+        for (l_t, l), (r_t, r) in zip(self._endpoints[:-1], self._endpoints[1:]):
+            if l_t <= t < r_t:
+                alpha = float(t - l_t) / (r_t - l_t)
+                return l + alpha * (r - l)
+        assert self._outside_value is not None
+        return self._outside_value
+
+    def device_points(self):
+        ts = [float(e[0]) for e in self._endpoints]
+        vs = [float(e[1]) for e in self._endpoints]
+        return ts + vs + [float(self._outside_value)]
