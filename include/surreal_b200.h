@@ -393,12 +393,13 @@ int sb200_clip_adam_f32(float* params, const float* grad, float* exp_avg, float*
                         const int* stop_flag, void* stream);
 /* target = target*(1-tau) + tau*src (soft target update, ddpg.py:410-418); a no-op when *stop_flag != 0. */
 int sb200_soft_update_f32(float* target, const float* src, int64_t n, double tau, const int* stop_flag, void* stream);
-/* Hard target update with the update counter on the device (ddpg.py:419-428: counter += 1; copy every `interval`-th
- * update), so that several learner updates and the copy among them fit in one CUDA graph.  tick != 0: *counter += 1
- * first (pass it for the first buffer of an update, 0 for the others sharing the counter); then target = src when
- * *counter % interval == 0.  Neither happens when *stop_flag != 0. */
-int sb200_hard_update_every_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t interval, int tick,
-                                const int* stop_flag, void* stream);
+/* Hard target update with PeriodicTracker(period).track_increment(incr) semantics on a device counter, so that several
+ * learner updates and the copies among them fit in one CUDA graph: DDPG counts updates (ddpg.py:419-428, incr = 1),
+ * DQN counts samples (dqn.py:84-86, incr = batch size).  tick != 0: *counter += incr first (pass it for the first
+ * buffer of an update, 0 for the others sharing the counter); then target = src when the count crossed a multiple of
+ * period in that increment.  Neither happens when *stop_flag != 0. */
+int sb200_hard_update_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t period, int64_t incr,
+                          int tick, const int* stop_flag, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * DDPG element-wise pieces (surreal/learner/ddpg.py:261-262,279,305,324-331,335-341); the networks run through
@@ -488,11 +489,6 @@ int sb200_dqn_td_f32(const float* q_a, int64_t ld_qa, const float* q_v, int64_t 
                      const float* actions, const float* rewards, const float* dones, const float* weights, int B,
                      int n_actions, double gamma, double priority_eps, float* d_a, int64_t ld_da, float* d_v,
                      int64_t ld_dv, float* priorities, float* stats, void* workspace, void* stream);
-/* Hard target copy with PeriodicTracker(period).track_increment(incr) semantics on a device counter of samples
- * (dqn.py:84-86, incr = batch size): tick != 0 adds incr first (pass it for the first buffer of an update); then
- * target = src when the count crossed a multiple of period in that increment.  Neither happens when *stop_flag != 0. */
-int sb200_hard_update_samples_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t period,
-                                  int64_t incr, int tick, const int* stop_flag, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Experience staging of PPO: ExpSenderWrapperMultiStepMovingWindowWithInfo._step (exp_sender_wrapper.py:209-228) for N

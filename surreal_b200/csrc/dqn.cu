@@ -1,6 +1,6 @@
 // DQN pieces around the shared MLP forward / backward / optimiser kernels (surreal/learner/dqn.py, agent/q_agent.py,
-// model/q_net.py): the epsilon-greedy act over the dueling combine, the TD target / Huber loss / dueling backward of one
-// update, and the hard target copy counted in samples.
+// model/q_net.py): the epsilon-greedy act over the dueling combine and the TD target / Huber loss / dueling backward of
+// one update.  The hard target copy is sb200_hard_update_f32 (optim.cu) with the counter in samples.
 #include "common.cuh"
 #include <stddef.h>
 
@@ -175,23 +175,6 @@ __global__ void __launch_bounds__(QT) dqn_td_kernel(const float* __restrict__ qa
     }
 }
 
-// PeriodicTracker(period).track_increment(incr) on a device counter of samples (dqn.py:84-86): tick adds incr; the copy
-// runs when the count crossed a multiple of the period, i.e. floor(c / period) > floor((c - incr) / period).
-__global__ void hard_update_samples_tick_kernel(long long* counter, long long incr, const int* __restrict__ stop) {
-    if (stop != nullptr && *stop) return;
-    *counter += incr;
-}
-
-__global__ void __launch_bounds__(QT) hard_update_samples_kernel(float* __restrict__ target, const float* __restrict__ src,
-                                                                 long long n, const long long* __restrict__ counter,
-                                                                 long long period, long long incr,
-                                                                 const int* __restrict__ stop) {
-    if (stop != nullptr && *stop) return;
-    const long long c = *counter;
-    if (c / period <= (c - incr) / period) return;
-    for (long long i = (long long)blockIdx.x * QT + threadIdx.x; i < n; i += (long long)gridDim.x * QT) target[i] = src[i];
-}
-
 inline int nb(int B) { return (B + QT - 1) / QT; }
 
 int act_launch(const float* adv, int64_t lda, const float* value, int64_t ldv, int N, int n_actions, const double* sched,
@@ -277,16 +260,4 @@ extern "C" int sb200_dqn_td_f32(const float* q_a, int64_t ld_qa, const float* q_
                                                          (float)gamma, priority_eps, d_a, ld_da, d_v, ld_dv, priorities,
                                                          stats, (DqnWs*)workspace);
     return sb200_launch_status();
-}
-
-extern "C" int sb200_hard_update_samples_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t period,
-                                             int64_t incr, int tick, const int* stop_flag, void* stream) {
-    SB200_REQUIRE(target && src && counter && n >= 1 && period >= 1 && incr >= 0);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (tick) hard_update_samples_tick_kernel<<<1, 1, 0, st>>>((long long*)counter, incr, stop_flag);
-    long long blocks = (n + 4 * QT - 1) / (4 * QT);
-    if (blocks > 264) blocks = 264;
-    hard_update_samples_kernel<<<(unsigned)blocks, QT, 0, st>>>(target, src, n, (const long long*)counter, period, incr,
-                                                                 stop_flag);
-    return sb200_launch_status(tick ? 2 : 1);
 }

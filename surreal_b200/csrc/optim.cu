@@ -62,19 +62,22 @@ __global__ void __launch_bounds__(OT) soft_update_kernel(float* __restrict__ tar
         target[i] = __fadd_rn(__fmul_rn(target[i], keep), __fmul_rn(tau, src[i]));
 }
 
-// Hard target update on the device (ddpg.py:419-428): the update counter lives in device memory so that several
-// learner updates, and the one among them that copies, fit in one CUDA graph.  `tick` counts one update; the copy
-// runs when the counter is a multiple of `interval`.  Both leave everything alone when *stop != 0.
-__global__ void hard_update_tick_kernel(long long* counter, const int* __restrict__ stop) {
+// Hard target update on the device, PeriodicTracker(period).track_increment(incr) on a device counter (ddpg.py:419-428
+// counts updates, incr = 1; dqn.py:84-86 counts samples, incr = batch size), so that several learner updates, and the
+// ones among them that copy, fit in one CUDA graph.  `tick` adds incr; the copy runs when the count crossed a multiple
+// of the period, floor(c / period) > floor((c - incr) / period) -- for incr = 1 and c >= 1 that is c % period == 0.
+// Both leave everything alone when *stop != 0.
+__global__ void hard_update_tick_kernel(long long* counter, long long incr, const int* __restrict__ stop) {
     if (stop != nullptr && *stop) return;
-    *counter += 1;
+    *counter += incr;
 }
 
 __global__ void __launch_bounds__(OT) hard_update_kernel(float* __restrict__ target, const float* __restrict__ src,
                                                          long long n, const long long* __restrict__ counter,
-                                                         long long interval, const int* __restrict__ stop) {
+                                                         long long period, long long incr, const int* __restrict__ stop) {
     if (stop != nullptr && *stop) return;
-    if (*counter % interval != 0) return;
+    const long long c = *counter;
+    if (c / period <= (c - incr) / period) return;
     for (long long i = (long long)blockIdx.x * OT + threadIdx.x; i < n; i += (long long)gridDim.x * OT)
         target[i] = src[i];
 }
@@ -119,11 +122,11 @@ extern "C" int sb200_soft_update_f32(float* target, const float* src, int64_t n,
     return sb200_launch_status();
 }
 
-extern "C" int sb200_hard_update_every_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t interval,
-                                           int tick, const int* stop_flag, void* stream) {
-    SB200_REQUIRE(target && src && counter && n >= 1 && interval >= 1);
-    if (tick) hard_update_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((long long*)counter, stop_flag);
-    hard_update_kernel<<<grid_for(n), OT, 0, (cudaStream_t)stream>>>(target, src, n, (const long long*)counter, interval,
-                                                                     stop_flag);
+extern "C" int sb200_hard_update_f32(float* target, const float* src, int64_t n, int64_t* counter, int64_t period,
+                                     int64_t incr, int tick, const int* stop_flag, void* stream) {
+    SB200_REQUIRE(target && src && counter && n >= 1 && period >= 1 && incr >= 0);
+    if (tick) hard_update_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>((long long*)counter, incr, stop_flag);
+    hard_update_kernel<<<grid_for(n), OT, 0, (cudaStream_t)stream>>>(target, src, n, (const long long*)counter, period,
+                                                                     incr, stop_flag);
     return sb200_launch_status(tick ? 2 : 1);
 }

@@ -3,28 +3,24 @@ target nets -> Bellman target -> critic MSE step -> actor step THROUGH the updat
 Statistics names and the order of operations follow ddpg.py:244-352, including the TD3 options
 (``use_double_critic``: second critic + target, y = min(y, y2); ``use_action_regularization``: clipped noise on the
 target action -- added, as in the reference, only AFTER Q'_1 was evaluated, so it reaches critic 2 alone)."""
-import ctypes as C
-
-import numpy as np
 import torch
 
 from .. import _lib, ops
 from .._lib import check
 from .. import utils as U
 from ..model.ddpg_net import DDPGModel
+from ..ops import _ptr
 from ..session import ConfigError
 from .aggregator import SSARAggregator
-from .base import Learner
+from .off_policy import OffPolicyLearner
 
 DS = dict(ACTOR_LOSS=0, CRITIC_LOSS=1, ACTION_NORM=2, REWARDS=3, Q_TARGET=4, Q_POLICY=5, ABSMAX=6, TD_ERROR=7,
           IS_WEIGHT=8)
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+class DDPGLearner(OffPolicyLearner):
+    bad_action_message = 'actions outside [-1, 1] (ddpg.py:261-262)'
 
-
-class DDPGLearner(Learner):
     def __init__(self, learner_config, env_config, session_config):
         super().__init__(learner_config, env_config, session_config)
         if not torch.cuda.is_available():
@@ -40,7 +36,15 @@ class DDPGLearner(Learner):
         self.use_double_critic = lc.algo.network.use_double_critic
         self.use_action_regularization = lc.algo.network.use_action_regularization
         self._num_gpus = 1
-        self._target_update_init()
+        cfg = lc.algo.network.target_update                                 # ddpg.py:403-428
+        self.target_update_type = cfg.type
+        if cfg.type == 'soft':
+            self.target_update_tau = cfg.tau
+        elif cfg.type == 'hard':
+            self.target_update_counter = 0
+            self.target_update_interval = cfg.interval
+        else:
+            raise ConfigError('Unsupported ddpg update type: {}'.format(cfg.type))
         net = lc.algo.network
         self.clip_actor_gradient = net.clip_actor_gradient
         self.actor_gradient_clip_value = net.actor_gradient_value_clip if self.clip_actor_gradient else 0.0
@@ -78,68 +82,29 @@ class DDPGLearner(Learner):
         self.total_learn_time = U.TimeRecorder()
         self.forward_time = U.TimeRecorder()
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
-        self._own = dict(obs=f(B, D), obs_next=f(B, D), actions=f(B, A), rewards=f(B, 1), dones=f(B, 1))
         self._pi_t, self._q_t, self._y = f(B, A), f(B, 1), f(B)
         self._dA = f(B, ops._ru(A, 4))
-        self._stats = f(16)
-        self._stats2 = f(16)                                   # critic 2's loss / Q (critic_loss is overwritten by it)
         self._pi_t2, self._q_t2 = f(B, A), f(B, 1)
         self.policy_noise, self.noise_clip = 0.2, 0.5           # hard-coded in the reference (ddpg.py:269-270)
         self._noise_draws = None                                # tests: injected N(0,1) draws [B, A], see setter below
         self._td3_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self._td3_seed = 77
         self._ws = torch.zeros(_lib.lib().sb200_ddpg_workspace_bytes(B), dtype=torch.uint8, device=self.device)
-        # device flag raised by the target kernel when max|a| > 1: every optimiser / soft-update kernel of that learn()
-        # then no-ops, so the AssertionError below leaves the learner exactly as the reference's pre-update assert does
-        off = int(_lib.lib().sb200_ddpg_bad_action_offset())
-        self._bad = self._ws[off:off + 4].view(torch.int32)
-        self._pin = {}
-        self.check_action_range = True
-        self.use_cuda_graph = ops.graphs_enabled()
-        self._graph = ops.GraphRunner()
-        # learn_from_replay: K updates per graph.  _stop latches the bad-action flag for the rest of the call, the hard
-        # target counter lives on the device, and everything the host wants afterwards lands in ONE read-back buffer
-        # (float64: statistics [0:16], critic 2's [16:32], latched stop flag [32], hard-update counter [33])
-        self._stop = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self._hard_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
-        self._readback = torch.zeros(34, dtype=torch.float64, device=self.device)
-        self._replay_graphs = {}
         # prioritized replay: a batch with importance weights takes the weighted critic loss (dqn.py:148-168), whose
         # rows also give the sampled records' new priorities |q1 - y| + eps (critic 1's TD error, before the step)
         rc = lc.replay
         self.priority_eps = float(rc.priority_eps) if 'priority_eps' in rc else 1e-6
-        self._w = f(B, 1)                                      # learn(): the batch's weights, at a fixed address
-        self._prio = f(B)
-        self._graph_w = ops.GraphRunner()
+        # the target kernel raises the workspace's bad-action flag when max|a| > 1: every optimiser / target kernel of
+        # the call then no-ops, so the AssertionError leaves the learner exactly as the reference's pre-update assert does
+        hard = self.target_update_type == 'hard'
+        self._init_off_policy(D, A, 32, self._ws, int(_lib.lib().sb200_ddpg_bad_action_offset()),
+                              tau=None if hard else self.target_update_tau,
+                              counter='target_update_counter' if hard else None,
+                              period=self.target_update_interval if hard else 1)
+        self._stats = self._stats_block[0:16]
+        self._stats2 = self._stats_block[16:32]                # critic 2's loss / Q (critic_loss is overwritten by it)
 
     # ------------------------------------------------------------------------------------------------
-    def preprocess(self, batch):
-        """ddpg.py:186-242: numpy -> fp32 device tensors (pinned staging); device batches are used in place."""
-        B, D, A = self.batch_size, self.low_dim, self.action_dim
-        get = (lambda k: batch[k]) if isinstance(batch, dict) else (lambda k: getattr(batch, k))
-        flat = lambda o: o['low_dim']['flat_inputs'] if isinstance(o, dict) else o  # noqa: E731
-        src = dict(obs=flat(get('obs')), obs_next=flat(get('obs_next')), actions=get('actions'),
-                   rewards=get('rewards'), dones=get('dones'))
-        nbytes = 0
-        for k, v in src.items():
-            dst = self._own[k]
-            if isinstance(v, torch.Tensor):
-                if v.data_ptr() != dst.data_ptr():                # foreign tensors are copied in: the captured graph
-                    dst.copy_(v.reshape(dst.shape), non_blocking=True)   # always reads the same addresses
-                    if not v.is_cuda:
-                        nbytes += dst.numel() * 4
-                continue
-            if k not in self._pin:
-                self._pin[k] = torch.empty(dst.shape, dtype=torch.float32, pin_memory=True)
-            self._pin[k].numpy()[...] = np.asarray(v).reshape(tuple(dst.shape))
-            dst.copy_(self._pin[k], non_blocking=True)
-            nbytes += dst.numel() * 4
-        self.last_h2d_bytes = nbytes
-        return batch
-
-    def replay_out_buffers(self):
-        return self._own
-
     @property
     def policy_noise_draws(self):
         return self._noise_draws
@@ -153,11 +118,6 @@ class DDPGLearner(Learner):
             self._noise_draws = torch.zeros(self.batch_size, self.action_dim, dtype=torch.float32, device=self.device)
         self._noise_draws.copy_(torch.as_tensor(draws, dtype=torch.float32).reshape(self.batch_size, self.action_dim))
 
-    @property
-    def td_priorities(self):
-        """Device [B]: |q1 - y| + priority_eps of the last weighted update's rows (the priorities to write back)."""
-        return self._prio
-
     def _critic_loss(self, trainer, q, stats, weights, prio):
         L, st, B = _lib.lib(), ops._stream(), self.batch_size
         d = trainer.d[-1]
@@ -169,15 +129,13 @@ class DDPGLearner(Learner):
                                                         d.stride(0), _ptr(prio), self.priority_eps, _ptr(stats),
                                                         _ptr(self._ws), st), 'sb200_ddpg_critic_loss_weighted_f32')
 
-    def _optimize_device(self, stop=None, weights=None):
-        """ddpg.py:244-333 as one fixed launch sequence (CUDA-graph body; no host round trip inside).  ``stop``: the
-        flag that no-ops the optimiser / target kernels -- this update's bad-action flag, or a flag that latches it.
-        ``weights`` (device [B, 1]): importance weights of a prioritized batch; both critic losses are weighted and
-        critic 1's rows leave the new priorities in ``td_priorities``."""
+    def _optimize_device(self, weights):
+        """ddpg.py:244-333 as one fixed launch sequence (CUDA-graph body; no host round trip inside).  ``weights``
+        (device [B, 1]): importance weights of a prioritized batch; both critic losses are weighted and critic 1's rows
+        leave the new priorities |q1 - y| + priority_eps in ``td_priorities``."""
         L = _lib.lib()
-        stop = self._bad if stop is None else stop
         B, A = self.batch_size, self.action_dim
-        m, mt, st = self.model, self.model_target, ops._stream()
+        mt, st = self.model_target, ops._stream()
         b = self._own
         obs, obs_next, actions, rewards, dones = b['obs'], b['obs_next'], b['actions'], b['rewards'], b['dones']
         ops.mlp_forward(mt.actor, obs_next, out=self._pi_t)                              # ddpg.py:266
@@ -200,8 +158,7 @@ class DDPGLearner(Learner):
             check(L.sb200_ddpg_target_f32(_ptr(rewards), _ptr(self._q_t), 1, _ptr(dones), _ptr(actions), A, B, A,
                                           disc, _ptr(self._y), _ptr(self._stats), _ptr(self._ws), st),
                   'sb200_ddpg_target_f32')
-        if stop is not self._bad:
-            torch.maximum(stop, self._bad, out=stop)
+        stop = self._latch_bad_action()
         ct = self.critic_optim
         q = ct.forward(obs, aux=actions)                                                # Q(s_t, a_t)
         self._critic_loss(ct, q, self._stats, weights, self._prio)
@@ -224,132 +181,27 @@ class DDPGLearner(Learner):
                                    _ptr(at.d[-1]), at.d[-1].stride(0), st), 'sb200_tanh_bwd_f32')
         at.backward()
         at.step(stop_flag=stop)
-        if self.target_update_type == 'soft':                                           # ddpg.py:410-418
-            pairs = [(mt.actor, m.actor), (mt.critic, m.critic)]
-            if self.use_double_critic:
-                pairs.append((self.model_target2.critic, self.model2.critic))
-            for t, s_ in pairs:
-                check(L.sb200_soft_update_f32(_ptr(t.params), _ptr(s_.params), t.size, float(self.target_update_tau),
-                                              _ptr(stop), st), 'sb200_soft_update_f32')
 
-    def _optimize(self, weighted=False):
-        with self.forward_time.time():
-            if weighted:
-                if self.use_cuda_graph:
-                    self._graph_w.run(lambda: self._optimize_device(weights=self._w))
-                else:
-                    self._optimize_device(weights=self._w)
-            elif self.use_cuda_graph:
-                self._graph.run(self._optimize_device)
-            else:
-                self._optimize_device()
-        s = self._stats.cpu().numpy()
-        self.last_d2h_bytes = s.nbytes
-        s2 = self._stats2.cpu().numpy() if self.use_double_critic else None
-        if self.check_action_range and s[DS['ABSMAX']] > 1.0:
-            raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
-        stats = self._statistics(s, s2, weighted)
-        if self.target_update_type == 'hard':                     # host-side counter (ddpg.py:419-428)
-            self.target_update_counter += 1
-            if self.target_update_counter % self.target_update_interval == 0:
-                self.model_target.actor.params.copy_(self.model.actor.params)
-                self.model_target.critic.params.copy_(self.model.critic.params)
-                if self.use_double_critic:
-                    self.model_target2.critic.params.copy_(self.model2.critic.params)
-        return stats
+    def _target_pairs(self):
+        pairs = [(self.model_target.actor, self.model.actor), (self.model_target.critic, self.model.critic)]
+        if self.use_double_critic:
+            pairs.append((self.model_target2.critic, self.model2.critic))
+        return pairs
 
-    def _statistics(self, s, s2, weighted=False):
+    def _statistics(self, s, weighted):
         stats = {'actor_loss': float(s[DS['ACTOR_LOSS']]), 'critic_loss': float(s[DS['CRITIC_LOSS']]),
                  'action_norm': float(s[DS['ACTION_NORM']]), 'rewards': float(s[DS['REWARDS']]),
                  'Q_target': float(s[DS['Q_TARGET']]), 'Q_policy': float(s[DS['Q_POLICY']]),
                  'performance/forward_time': self.forward_time.avg}
         # (the reference's critic_update_time / actor_update_time split does not exist here: the whole update is one
         #  CUDA graph; performance/forward_time covers it)
-        if s2 is not None:                                       # ddpg.py:316,345-346: critic_loss is critic 2's
+        if self.use_double_critic:                               # ddpg.py:316,345-346: critic_loss is critic 2's
+            s2 = s[16:32]
             stats['critic_loss'] = float(s2[DS['CRITIC_LOSS']])
             stats['Q_policy2'] = float(s2[DS['Q_POLICY']])
         if weighted:                                             # prioritized replay only (dqn.py's td_error)
             stats['td_error'] = float(s[DS['TD_ERROR']])
             stats['avg_is_weight'] = float(s[DS['IS_WEIGHT']])
-        return stats
-
-    def learn(self, batch):
-        """ddpg.py:354-374.  A batch with ``weights`` (prioritized replay) takes the weighted critic loss; when it also
-        carries ``indices`` and the attached replay has priorities, the new ones are written back to it."""
-        self.current_iteration += 1
-        get = (lambda k: batch.get(k)) if isinstance(batch, dict) else (lambda k: getattr(batch, k, None))
-        weights, indices = get('weights'), get('indices')
-        with self.total_learn_time.time():
-            self.preprocess(batch)
-            if weights is not None:
-                self._w.copy_(torch.as_tensor(weights, dtype=torch.float32).reshape(self._w.shape), non_blocking=True)
-            stats = self._optimize(weighted=weights is not None)
-            if weights is not None and indices is not None and hasattr(self._replay, 'update_priorities_device'):
-                idx = torch.as_tensor(indices, dtype=torch.int64).to(self.device).reshape(-1)
-                self._replay.update_priorities_device(idx, self._prio, stop_flag=self._bad)
-            stats['performance/total_learn_time'] = self.total_learn_time.avg
-            self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
-            self.periodic_checkpoint(global_steps=self.current_iteration, score=None)
-        return stats
-
-    def _replay_updates_device(self, replay, updates):
-        """``updates`` x [sample on the device -> update -> target update] and the read-back staging, as one fixed
-        launch sequence.  A bad-action batch stops every later optimiser / target kernel of the sequence (_stop).  On a
-        prioritized replay each update is weighted and writes its priorities back (sample -> update -> priorities)."""
-        L, st = _lib.lib(), ops._stream()
-        per = hasattr(replay, 'update_priorities_device')
-        self._stop.zero_()
-        for _ in range(updates):
-            b = replay.sample_device(self.batch_size, out=self._own)
-            self._optimize_device(stop=self._stop, weights=b['weights'] if per else None)
-            if per:                                                  # no-op once _stop is latched
-                replay.update_priorities_device(b['indices'], self._prio, stop_flag=self._stop)
-            if self.target_update_type == 'hard':                                        # ddpg.py:419-428
-                pairs = [(self.model_target.actor, self.model.actor), (self.model_target.critic, self.model.critic)]
-                if self.use_double_critic:
-                    pairs.append((self.model_target2.critic, self.model2.critic))
-                for i, (t, s_) in enumerate(pairs):
-                    check(L.sb200_hard_update_every_f32(_ptr(t.params), _ptr(s_.params), t.size, _ptr(self._hard_counter),
-                                                        int(self.target_update_interval), int(i == 0), _ptr(self._stop),
-                                                        st), 'sb200_hard_update_every_f32')
-        rb = self._readback
-        rb[0:16].copy_(self._stats)
-        rb[16:32].copy_(self._stats2)
-        rb[32:33].copy_(self._stop)
-        rb[33:34].copy_(self._hard_counter)
-
-    def learn_from_replay(self, replay, updates=1):
-        """``updates`` learner updates fed by ``replay.sample_device`` -- ddpg.py:354-374 ``updates`` times over, with no
-        host step between them: one CUDA graph (the same launches eagerly when graphs are off), then ONE read-back.
-        Returns the statistics of the last update.  Hard target updates (ddpg.py:419-428) run on the device, gated by a
-        device counter that starts from ``target_update_counter`` and is read back into it.  An out-of-range action in
-        any sampled batch raises AssertionError after the read-back; that update and every later one of the call changed
-        nothing."""
-        K = int(updates)
-        assert K >= 1
-        self.current_iteration += K
-        with self.total_learn_time.time():
-            if self.target_update_type == 'hard':
-                self._hard_counter.fill_(self.target_update_counter)
-            with self.forward_time.time():
-                if self.use_cuda_graph:
-                    key = (id(replay), K)
-                    if key not in self._replay_graphs:
-                        self._replay_graphs[key] = (ops.GraphRunner(), replay)
-                    self._replay_graphs[key][0].run(lambda: self._replay_updates_device(replay, K))
-                else:
-                    self._replay_updates_device(replay, K)
-            rb = self._readback.cpu().numpy()
-            self.last_d2h_bytes = rb.nbytes
-            if self.target_update_type == 'hard':
-                self.target_update_counter = int(rb[33])
-            if self.check_action_range and rb[32] != 0:
-                raise AssertionError('actions outside [-1, 1] (ddpg.py:261-262)')
-            stats = self._statistics(rb[0:16], rb[16:32] if self.use_double_critic else None,
-                                     hasattr(replay, 'update_priorities_device'))
-            stats['performance/total_learn_time'] = self.total_learn_time.avg
-            self.tensorplex.add_scalars(stats, global_step=self.current_iteration)
-            self.periodic_checkpoint(global_steps=self.current_iteration, score=None)
         return stats
 
     def module_dict(self):
@@ -366,36 +218,6 @@ class DDPGLearner(Learner):
             if self.use_double_critic:
                 attrs += ['critic_optim2']
         return attrs
-
-    def _target_update_init(self):
-        cfg = self.learner_config.algo.network.target_update
-        self.target_update_type = cfg.type
-        if self.target_update_type == 'soft':
-            self.target_update_tau = cfg.tau
-        elif self.target_update_type == 'hard':
-            self.target_update_counter = 0
-            self.target_update_interval = cfg.interval
-        else:
-            raise ConfigError('Unsupported ddpg update type: {}'.format(cfg.type))
-
-    def _target_update(self):
-        """ddpg.py:403-428."""
-        m, mt = self.model, self.model_target
-        if self.target_update_type == 'soft':
-            L, st = _lib.lib(), ops._stream()
-            pairs = [(mt.actor, m.actor), (mt.critic, m.critic)]
-            if self.use_double_critic:
-                pairs.append((self.model_target2.critic, self.model2.critic))
-            for t, s in pairs:
-                check(L.sb200_soft_update_f32(_ptr(t.params), _ptr(s.params), t.size, float(self.target_update_tau), None, st),
-                      'sb200_soft_update_f32')
-        else:
-            self.target_update_counter += 1
-            if self.target_update_counter % self.target_update_interval == 0:
-                mt.actor.params.copy_(m.actor.params)
-                mt.critic.params.copy_(m.critic.params)
-                if self.use_double_critic:
-                    self.model_target2.critic.params.copy_(self.model2.critic.params)
 
     def _prefetcher_preprocess(self, batch):
         if isinstance(batch, dict):

@@ -6,7 +6,6 @@ Same constructor, config keys, method names, statistics names and control flow a
 ``learn(batch)`` call receives has the aggregator's layout (aggregator.py:176-183); its arrays may be
 numpy (copied through pinned memory) or CUDA tensors (zero copy).
 """
-import ctypes as C
 import os
 
 import numpy as np
@@ -18,6 +17,7 @@ from .._lib import check
 from ..model.lstm_stem import rows_zfilter
 from ..model.ppo_net import PPOModel, DiagGauss
 from ..model.stem_chain import ChainTrainer, StemChain
+from ..ops import _ptr
 from ..session import ConfigError
 from .aggregator import MultistepAggregatorWithInfo
 from .base import Learner
@@ -25,10 +25,6 @@ from .scheduler import make_lr_scheduler
 
 S = dict(SURR=0, LOSS=1, ENTROPY=2, KL_PRE=3, KL_POST=4, GN_ACTOR=5, VAL_LOSS=6, EXPL_VAR=7, GN_CRITIC=8,
          RET_MEAN=9, LOG_SIG=10, BEHAVE_LIK=11, IS_WEIGHT=12, REF_BEHAVE=13, EPOCHS=14, VAL_MOMENTS=16, COUNT=32)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 class PPOLearner(Learner):
