@@ -413,9 +413,10 @@ int sb200_hard_update_f32(float* target, const float* src, int64_t n, int64_t* c
 #define SB200_DSTAT_ACTION_ABSMAX 6   /* for the deferred `assert |a| <= 1` of ddpg.py:261-262 */
 #define SB200_DSTAT_TD_ERROR 7        /* weighted critic loss only: mean |q - y| (the reference DQN's td_error) */
 #define SB200_DSTAT_IS_WEIGHT 8       /* weighted critic loss only: mean importance weight */
-/* byte offset inside the DDPG workspace of the int32 "bad action" flag: sb200_ddpg_target*_f32 set it to 1 when
- * max|a| > 1 (the reference asserts this BEFORE any update, ddpg.py:261-262); pass its address as stop_flag to the
- * optimiser / soft-update calls of the same learn() so an out-of-range batch leaves every parameter untouched. */
+/* byte offset inside the DDPG workspace of the int32 "bad action" flag: sb200_ddpg_target*_f32 set it to 1 unless
+ * max|a| <= 1, so a NaN action raises it too (the reference asserts this BEFORE any update, ddpg.py:261-262); pass its
+ * address as stop_flag to the optimiser / soft-update calls of the same learn() so an out-of-range batch leaves every
+ * parameter untouched. */
 size_t sb200_ddpg_bad_action_offset(void);
 size_t sb200_ddpg_workspace_bytes(int B);
 /* y = rewards + discount * q_next * (1 - dones), discount = gamma ** n_step. */

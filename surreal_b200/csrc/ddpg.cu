@@ -8,9 +8,12 @@ namespace {
 
 constexpr int DT = 256;
 
+// max that keeps NaN, as torch.max does: the reference's `actions.max() <= 1` rejects a NaN action (fmax would drop it)
+__device__ __forceinline__ double max_keep_nan(double a, double b) { return (b > a || b != b) ? b : a; }
+
 struct DdpgWs {
     unsigned int counter;
-    int bad_action;          // 1 when max|a| > 1 (ddpg.py:261-262): optimiser / target kernels of this learn() no-op
+    int bad_action;          // 1 unless max|a| <= 1 (ddpg.py:261-262), NaN included: optimiser / target kernels no-op
     double partial[1];       // [blocks][4]
 };
 
@@ -41,7 +44,8 @@ __global__ void __launch_bounds__(DT) ddpg_target_kernel(const float* __restrict
         for (int j = 0; j < A; ++j) {
             const float a = actions[(long long)b * lda + j];
             s += a * a;
-            mx = fmaxf(mx, fabsf(a));
+            const float x = fabsf(a);
+            if (x > mx || x != x) mx = x;
         }
         an = (double)sqrtf(s);
         amax = (double)mx;
@@ -55,12 +59,12 @@ __global__ void __launch_bounds__(DT) ddpg_target_kernel(const float* __restrict
     __syncthreads();
     double m = amax;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    for (int o = 16; o > 0; o >>= 1) m = max_keep_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((tid & 31) == 0) sh[tid >> 5] = m;
     __syncthreads();
     if (tid == 0) {
         double mm = 0.0;
-        for (int w = 0; w < DT / 32; ++w) mm = fmax(mm, sh[w]);
+        for (int w = 0; w < DT / 32; ++w) mm = max_keep_nan(mm, sh[w]);
         part[3] = mm;
     }
     if (last_block_ticket(&ws->counter, gridDim.x)) {
@@ -70,13 +74,13 @@ __global__ void __launch_bounds__(DT) ddpg_target_kernel(const float* __restrict
                 s0 += ws->partial[(size_t)k * 4 + 0];
                 s1 += ws->partial[(size_t)k * 4 + 1];
                 s2 += ws->partial[(size_t)k * 4 + 2];
-                mx = fmax(mx, ws->partial[(size_t)k * 4 + 3]);
+                mx = max_keep_nan(mx, ws->partial[(size_t)k * 4 + 3]);
             }
             stats[SB200_DSTAT_REWARDS] = (float)(s0 / B);
             stats[SB200_DSTAT_ACTION_NORM] = (float)(s1 / B);
             stats[SB200_DSTAT_Q_TARGET] = (float)(s2 / B);
             stats[SB200_DSTAT_ACTION_ABSMAX] = (float)mx;
-            ws->bad_action = (mx > 1.0) ? 1 : 0;
+            ws->bad_action = (mx <= 1.0) ? 0 : 1;
         }
     }
 }

@@ -234,12 +234,17 @@ def value_rnn(stem, layers, x, h0, c0, ret, zs=None, masks=None):
     return out
 
 
-def ddpg_critic(layers, x, actions, y, aux_layer=1):
-    """nn.MSELoss()(Q(s, a), y) of oracle/ddpg.py: ``grads`` per critic layer, ``g_pre`` = dL/dQ, stat ``q_mean``."""
+def ddpg_critic(layers, x, actions, y, aux_layer=1, weights=None):
+    """nn.MSELoss()(Q(s, a), y) of oracle/ddpg.py: ``grads`` per critic layer, ``g_pre`` = dL/dQ, stats ``q_mean`` and
+    ``q`` [B, 1].  ``weights`` [B] (prioritized replay's importance weights, dqn.py:148-168): mean(w (Q - y)^2)."""
     L = _leaves(layers)
     q = trunk(f64(x), L, aux=f64(actions), aux_layer=aux_layer)
-    loss = F.mse_loss(q, f64(y).reshape(-1, 1))
-    out = _result(loss, {'loss': loss, 'q_mean': q.mean()}, _flat(L) + [q],
+    y = f64(y).reshape(-1, 1).to(q.device)
+    if weights is None:
+        loss = F.mse_loss(q, y)
+    else:
+        loss = (f64(weights).reshape(-1, 1).to(q.device) * (q - y).pow(2)).mean()
+    out = _result(loss, {'loss': loss, 'q_mean': q.mean(), 'q': q}, _flat(L) + [q],
                   ['_g%d' % i for i in range(2 * len(L))] + ['g_pre'])
     out['grads'] = _pairs([out.pop('_g%d' % i) for i in range(2 * len(L))])
     return out

@@ -148,7 +148,7 @@ def test_ddpg_engine_end_to_end():
 
 
 def test_ddpg_out_of_range_actions_leave_state_untouched():
-    """The reference asserts |a| <= 1 BEFORE any update (ddpg.py:261-262).  Here the whole update is one graph, so the
+    """The reference asserts |a| <= 1 BEFORE any update (ddpg.py:261-262), and a NaN action fails it too.  Here the whole update is one graph, so the
     target kernel raises a device flag that turns every optimiser / soft-update kernel of that learn() into a no-op:
     the AssertionError must leave actor, critic, targets and Adam moments bit-identical."""
     from surreal_b200.learner import DDPGLearner
@@ -162,12 +162,15 @@ def test_ddpg_out_of_range_actions_leave_state_untouched():
     L.learn(mk(1.0))                                            # a good batch first (captures the graph, moves Adam)
     snap = [t.clone() for t in (L.model.actor.params, L.model.critic.params, L.model_target.actor.params,
                                 L.model_target.critic.params, L.actor_optim.exp_avg, L.critic_optim.exp_avg_sq)]
-    with pytest.raises(AssertionError):
-        L.learn(mk(3.0))
-    torch.cuda.synchronize()
-    for a, b in zip(snap, (L.model.actor.params, L.model.critic.params, L.model_target.actor.params,
-                           L.model_target.critic.params, L.actor_optim.exp_avg, L.critic_optim.exp_avg_sq)):
-        assert torch.equal(a, b)
+    nan_batch = mk(1.0)
+    nan_batch['actions'][9, 2] = np.nan                         # torch.max propagates NaN: the reference rejects it
+    for bad in (mk(3.0), nan_batch):
+        with pytest.raises(AssertionError):
+            L.learn(bad)
+        torch.cuda.synchronize()
+        for a, b in zip(snap, (L.model.actor.params, L.model.critic.params, L.model_target.actor.params,
+                               L.model_target.critic.params, L.actor_optim.exp_avg, L.critic_optim.exp_avg_sq)):
+            assert torch.equal(a, b)
     before = L.model.critic.params.clone()
     L.learn(mk(1.0))                                            # and the learner keeps working afterwards
     assert not torch.equal(before, L.model.critic.params)

@@ -128,6 +128,16 @@ def test_ddpg_losses_match_oracle():
         _close(r['grads'][l][0], c32[l][0].grad, ('critic W', l))
         _close(r['grads'][l][1], c32[l][1].grad, ('critic b', l))
     assert abs(float(r['q_mean']) - float(q.mean())) <= 1e-6
+    # importance weights: mean(w (q - y)^2); unit weights are the plain MSE
+    w = torch.rand(B, generator=gen) + 0.1
+    c32 = [(w_.clone().requires_grad_(True), b.clone().requires_grad_(True)) for w_, b in cl]
+    (w.view(-1, 1) * (onets.ddpg_critic(obs, act, c32) - y) ** 2).mean().backward()
+    rw = R.ddpg_critic(cl, obs, act, y, weights=w)
+    r1 = R.ddpg_critic(cl, obs, act, y, weights=torch.ones(B))
+    for l in range(3):
+        _close(rw['grads'][l][0], c32[l][0].grad, ('weighted critic W', l))
+        _close(rw['grads'][l][1], c32[l][1].grad, ('weighted critic b', l))
+        assert torch.equal(r1['grads'][l][0], r['grads'][l][0]) and torch.equal(r1['grads'][l][1], r['grads'][l][1])
     a32 = [(w.clone().requires_grad_(True), b.clone().requires_grad_(True)) for w, b in al]
     (-onets.ddpg_critic(obs, onets.ddpg_actor(obs, a32), cl).mean()).backward()
     r = R.ddpg_actor(al, cl, obs)
