@@ -272,6 +272,7 @@ extern "C" int sb200_conv_backward_dw_f32(int layer, const void* x, int in_u8, c
                                           int W, double in_scale, float* slab_w, float* slab_b, int64_t slab_stride, int splits,
                                           void* stream) {
     SB200_REQUIRE(x && dy && slab_w && slab_b && frames >= 1 && CIN >= 1 && splits >= 1 && (layer == 1 || layer == 2));
+    SB200_REQUIRE(layer == 1 ? (H >= 8 && W >= 8) : (H >= 4 && W >= 4));     // (H - KS) / ST truncates to 0 below KS
     cudaStream_t st = (cudaStream_t)stream;
     if (layer == 1)
         return in_u8 ? launch_dw<8, 4, 16, unsigned char>(x, dy, (int)frames, CIN, H, W, (float)in_scale, slab_w, slab_b, slab_stride,
@@ -284,7 +285,8 @@ extern "C" int sb200_conv_backward_dw_f32(int layer, const void* x, int in_u8, c
 // dx[frames][CIN][H][W] = relu'(act) * conv_transpose(dy, Wk) for layer 2 (its input is layer 1's post-ReLU output `act`).
 extern "C" int sb200_conv_backward_dx_f32(int layer, const float* dy, const float* Wk, const float* act, int64_t frames, int CIN,
                                           int H, int W, float* dx, void* stream) {
-    SB200_REQUIRE(dy && Wk && dx && frames >= 1 && layer == 2 && CIN >= 1);
+    SB200_REQUIRE(dy && Wk && dx && frames >= 1 && layer == 2 && CIN >= 1 && H >= 4 && W >= 4);
+    SB200_REQUIRE((((uintptr_t)Wk) & 15) == 0);
     const int HO = (H - 4) / 2 + 1, WO = (W - 4) / 2 + 1;
     const size_t smem = ((size_t)CIN * 16 * 32 + (size_t)HO * WO * 32) * sizeof(float);
     if (smem > STEM_SMEM_MAX) return SB200_ERR_UNSUPPORTED;
