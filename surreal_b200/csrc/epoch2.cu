@@ -172,9 +172,13 @@ __device__ __forceinline__ float4 ldw4(const float* p) {                 // L1-a
     asm volatile("ld.global.ca.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
     return r;
 }
+// rb_gemm is a called function, not inlined: inlined at its six call sites it shared the 128 registers with the epoch
+// loop's live state, so the kernel spilled (1300 B) and reloaded operands from local memory inside the k loop, and its
+// code was several times larger.  Called, it spills 4 B and the kernel 612 B (-Xptxas -v); the epoch kernel at the
+// bench shape runs 12 % faster on 68 SMs and 16 % faster on all 132 (H100 SXM, tools/prof_epoch2.py).
 template <bool COLSUM>
-__device__ __forceinline__ void rb_gemm(const float* __restrict__ As, int lda, int K, const float* __restrict__ W, int ldw,
-                                        float* __restrict__ Part, int ldp, int c40) {
+__device__ __noinline__ void rb_gemm(const float* __restrict__ As, int lda, int K, const float* __restrict__ W, int ldw,
+                                     float* __restrict__ Part, int ldp, int c40) {
     const int tid = threadIdx.x, cq = tid & 63, rg = (tid >> 6) & 1, kh = tid >> 7;
     const int Kp = (K + 3) & ~3;
     const int kq = (((Kp >> 2) + 3) >> 2) << 2;
@@ -911,10 +915,11 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
                 w0[j] = n_w;
                 if (train[j]) n_w += (((p.H1 + RB - 1) / RB) + ((p.D + RB - 1) / RB) + 1) * p.s;
             }
-            // CTA 0 spends this phase on the loss statistics (below, ~8 us of serial work): when the items fit on the other
-            // CTAs it takes none, so that nobody waits for it at the barrier
-            const int skip0 = (n_w <= G - 1) ? 1 : 0;
-            for (int it = c - skip0; it >= 0 && it < n_w; it += G) {
+            // CTA 0 spends this phase on the loss statistics (above, ~10 us of serial work): when the other CTAs cover the
+            // items in as many rounds as the whole grid would (one round at the full grid, two on the learner's 68-SM budget)
+            // it takes none, so that nobody waits for it at the barrier
+            const int skip0 = (G > 1 && (n_w + G - 2) / (G - 1) == (n_w + G - 1) / G) ? 1 : 0;
+            for (int it = c - skip0; it >= 0 && it < n_w; it += G - skip0) {
                 const int j = (NJ == 2 && train[1] && it >= w0[1]) ? 1 : 0;
                 const Job& p = P.job[j];
                 int q = it - w0[j];

@@ -329,10 +329,12 @@ struct RfGroup {
     float *X0, *H1, *H2, *S, *Nx;
     float *Ac, *Sd, *Zn, *Hp;             // [8][A] each: actions | std | N(0,1) draws | head_mode 0 halves [2][8][A]
     float *Eacc, *Egx, *Erz, *Eq;         // action-independent env step: [8][D] Ws.s, successor noise, reset draw | [8][2]
+    // G = 2 keeps the action draws of a step in the buffer of its parity (rf2_action_noise): Zn | Act slot 1
+    __device__ __forceinline__ float* zn2(int par, int A) const { return par ? Ac + RF_OWN * A : Zn; }
     __device__ __forceinline__ RfGroup(const RfParams& p, float* smem, int g) {
         float* b = smem + g * p.gstride;
         X0 = b + p.oX0; H1 = b + p.oH1; H2 = b + p.oH2; S = b + p.oS; Nx = b + p.oNext;
-        Ac = b + p.oAct; Sd = Ac + 2 * RF_OWN * p.A; Zn = Sd + RF_OWN * p.A; Hp = Zn + RF_OWN * p.A;  // (slot 1 unused, see rf_plan)
+        Ac = b + p.oAct; Sd = Ac + 2 * RF_OWN * p.A; Zn = Sd + RF_OWN * p.A; Hp = Zn + RF_OWN * p.A;  // (slot 1: zn2, see rf_plan)
         Eacc = b + p.oPre; Egx = Eacc + RF_OWN * p.D; Erz = Egx + RF_OWN * p.D; Eq = Erz + RF_OWN * p.D;
     }
 };
@@ -480,6 +482,7 @@ __device__ __forceinline__ int rf_act_env(const RfParams& p, const RfGroup& gr, 
     [[maybe_unused]] const int rf_t = t;              // read by RF_STAMP only
     const int D = p.D, A = p.A, ldwh = p.ldw[2];
     const bool valid = i_own < p.N, final_step = (t == p.T - 1);
+    const float* zn = (G == 2) ? gr.zn2(t & 1, A) : gr.Zn;
     int slot = SLOT_NONE;
     if (lane < A) {
         const int j = lane;
@@ -494,7 +497,7 @@ __device__ __forceinline__ int rf_act_env(const RfParams& p, const RfGroup& gr, 
         RF_STAMP(19, 0);
         const float mu = apply_act(pre + Bhs[j], p.act[2]);
         const float sd = gr.Sd[own * A + j];
-        const float a = ppo_action(mu, sd, gr.Zn[own * A + j], p.deterministic);
+        const float a = ppo_action(mu, sd, zn[own * A + j], p.deterministic);
         gr.Ac[own * A + j] = a;
         if (valid) {
             p.stage_act[((long long)i_own * p.n_step + pos) * A + j] = a;
@@ -575,6 +578,25 @@ __device__ __forceinline__ void rf_push_input(const RfParams& p, const RfGroup& 
     }
 }
 
+// Two groups: the action draws N(0, 1) of step t of group g (owned actors i0 .. i0 + 7) by the layer warps, into the
+// buffer of parity t & 1 (RfGroup::zn2).  They depend on neither state nor action, so the layer warps take them while
+// they would otherwise wait for the other group's input rows, and the tail warps, whose chain sets the step, no longer
+// run a Philox round and two Box-Muller draws per actor for them.  The values are those of action_noise1 at the same
+// counter.  A called function: inlined, its registers pushed the layer code into spills.
+__device__ __noinline__ void rf2_action_noise(const RfParams& p, const RfGroup& gr, long long i0, unsigned long long ctr,
+                                              int par, int tid) {
+    const int A = p.A, nq = (A + 3) >> 2;
+    float* zn = gr.zn2(par, A);
+    for (int idx = tid; idx < RF_OWN * nq; idx += RF_THREADS / 2) {
+        const int a = idx / nq, q = idx - a * nq;
+        const float4 z = action_noise4(p.agent_seed, ctr, i0 + a, q);
+        const float zv[4] = {z.x, z.y, z.z, z.w};
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            if (4 * q + c < A) zn[a * A + 4 * q + c] = zv[c];
+    }
+}
+
 // Two groups of 32 actors per cluster (G = 2), software-pipelined, so that a chunk of N actors needs half as many
 // clusters.  Warps 0..7 ("layer warps") run hidden layers 1 and 2 for group 0, then for group 1, step after step.
 // Warps 8..15 ("tail warps", warp 8 + a for owned actor a of each group) take the whole tail of a group -- the
@@ -634,6 +656,8 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p, unsigned crank
             RF_STAMP(0, 0);
             for (int g = 0; g < G; ++g) {
                 const RfGroup gr(p, smem, g);
+                const long long i0 = row0 + g * RF_ROWS + (int)crank * RF_OWN;
+                if (t == 0 && !p.deterministic) rf2_action_noise(p, gr, i0, ctr0, 0, tid);
                 if (t > 0) {                                   // own rows from the tail warps, the peers' rows by st.async
                     rf_bar_sync(4 + g, 2 * 256);
                     rf_mbar_wait(&s_bar[g][2], (unsigned)(t - 1) & 1u);
@@ -652,6 +676,10 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p, unsigned crank
                                   smem_base, crank, smem_u32(&s_bar[g][1]) - smem_base);
                 RF_STAMP(4 + 2 * g, 0);
                 rf_bar_arrive(2 + g, 2 * 256);
+                // the next step's action draws: their buffer's last reader, the tail's env step of step t - 1, is behind
+                // named barrier 4 + g above; the tail reads them behind barrier 2 + g of step t + 1
+                if (!final_step && !p.deterministic)
+                    rf2_action_noise(p, gr, i0, ctr0 + (unsigned long long)(t + 1), (t + 1) & 1, tid);
             }
         }
         return;
@@ -664,34 +692,48 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p, unsigned crank
             const int m_own = (int)crank * RF_OWN + own;
             const long long i_own = row0 + g * RF_ROWS + m_own;
             RF_STAMP(8 + 4 * g, 256);
-            // ---- everything of the step that does not depend on the action: the env warps' arithmetic of G = 1, but a
-            // lane takes the adjacent columns d, d + 1 together (two independent FMA chains, float2 weight and float4
-            // state loads): here this work is on the step's critical path, next to layer warps that keep the
-            // shared-memory pipe busy, so its loads and dependent latencies are what count
+            // ---- everything of the step that does not depend on the action: the env warps' arithmetic of G = 1.  Here
+            // this work is on the step's critical path, next to layer warps that keep the shared-memory pipe busy, so
+            // what it puts through L1 counts.  Ws.s for the group's 8 owned actors is one register-tiled product on
+            // tail warps 8..11 (tt < 128): a thread takes column d of 4 actors, so each weight is read through L1 twice
+            // per group and step instead of once per actor, and the state rows are warp-wide float4 broadcasts.  Each
+            // output is one fmaf chain over k in ascending order, as in the G = 1 env warps, so both give the same bits.
+            // Eacc is read by the actors' warps behind named barrier 6 (the head), and rewritten only after every tail
+            // warp passed barrier 6 of the other group, behind its last reader; the state rows read here were last
+            // written before that same barrier.
             {
+                const int tt = tid - RF_THREADS / 2;
+                if (tt < 128) {
+                    const int a0 = (tt >> 6) * 4;
+                    const float* s0 = gr.S + a0 * D;
+                    for (int d = tt & 63; d < D; d += 64) {
+                        float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll 4
+                        for (int k = 0; k < D; k += 4) {
+                            const float w0 = __ldg(EWs + (k + 0) * D + d), w1 = __ldg(EWs + (k + 1) * D + d);
+                            const float w2 = __ldg(EWs + (k + 2) * D + d), w3 = __ldg(EWs + (k + 3) * D + d);
+#pragma unroll
+                            for (int a = 0; a < 4; ++a) {
+                                const float4 s4 = *reinterpret_cast<const float4*>(s0 + a * D + k);
+                                acc[a] = fmaf(w0, s4.x, acc[a]);
+                                acc[a] = fmaf(w1, s4.y, acc[a]);
+                                acc[a] = fmaf(w2, s4.z, acc[a]);
+                                acc[a] = fmaf(w3, s4.w, acc[a]);
+                            }
+                        }
+#pragma unroll
+                        for (int a = 0; a < 4; ++a) gr.Eacc[(a0 + a) * D + d] = acc[a];
+                    }
+                }
                 const float* sh = gr.S + own * D;
                 float q = 0.0f;
                 for (int d = lane; d < D; d += 32) q += sh[d] * sh[d];
                 q = warp_sum(q);
                 const bool h_done = env_done(s_ep[g][own] + 1, p.max_steps);
                 for (int d = 2 * lane; d < D; d += 64) {          // D % 4 == 0: d + 1 < D
-                    float acc0 = 0.0f, acc1 = 0.0f;
-#pragma unroll 4
-                    for (int k = 0; k < D; k += 4) {
-                        const float4 s4 = *reinterpret_cast<const float4*>(sh + k);
-                        const float2 w0 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 0) * D + d));
-                        const float2 w1 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 1) * D + d));
-                        const float2 w2 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 2) * D + d));
-                        const float2 w3 = __ldg(reinterpret_cast<const float2*>(EWs + (k + 3) * D + d));
-                        acc0 = fmaf(w0.x, s4.x, acc0); acc1 = fmaf(w0.y, s4.x, acc1);
-                        acc0 = fmaf(w1.x, s4.y, acc0); acc1 = fmaf(w1.y, s4.y, acc1);
-                        acc0 = fmaf(w2.x, s4.z, acc0); acc1 = fmaf(w2.y, s4.z, acc1);
-                        acc0 = fmaf(w3.x, s4.w, acc0); acc1 = fmaf(w3.y, s4.w, acc1);
-                    }
                     const Philox4 r0 = env_noise(p.env_seed, ctr, i_own, d);
                     const Philox4 r1 = env_noise(p.env_seed, ctr, i_own, d + 1);
                     const float2 gz0 = box_muller(r0.x, r0.y), gz1 = box_muller(r1.x, r1.y);
-                    *reinterpret_cast<float2*>(gr.Eacc + own * D + d) = make_float2(acc0, acc1);
                     *reinterpret_cast<float2*>(gr.Egx + own * D + d) = make_float2(gz0.x, gz1.x);
                     *reinterpret_cast<float2*>(gr.Erz + own * D + d) =
                         h_done ? make_float2(env_reset_draw(r0), env_reset_draw(r1)) : make_float2(0.0f, 0.0f);
@@ -699,8 +741,7 @@ __device__ __forceinline__ void rf2_two_groups(const RfParams& p, unsigned crank
                         gr.Eq[2 * own] = q;
                         gr.Eq[2 * own + 1] = gz0.y;
                     }
-                }
-                if (!p.deterministic && lane < A) gr.Zn[own * A + lane] = action_noise1(p.agent_seed, ctr, i_own, lane);
+                }                                             // the action draws come from the layer warps
             }
             rf_bar_sync(2 + g, 2 * 256);                   // own rows of the last hidden layer, then the peers' rows
             rf_mbar_wait(&s_bar[g][1], (unsigned)t & 1u);
@@ -995,8 +1036,7 @@ bool rf_plan(const sb200_mlp* net, int D, int A, int G, RfParams* p, size_t* sme
     const int oB = take(Nc1 + Nc2 + ldwh);
     const int ldx0 = D + 4, ldh1 = H1 + 4, ldh2 = H2 + 4;
     int oX0, oH1, oH2, oPart = -1, oZf, oEnv = -1, oS, oNext, oAct, oPre, oHs = -1, gstride = 0;
-    // Act: actions | unused | std | N(0,1) draws | two head halves; the unused slot stays so that the plan, and with it the
-    // supported envelope and the one- / two-group choice, does not move
+    // Act: actions | N(0,1) draws of odd steps (G = 2; unused with one group) | std | N(0,1) draws | two head halves
     if (G == 1) {
         oX0 = take(RF_ROWS * ldx0); oH1 = take(RF_ROWS * ldh1); oH2 = take(RF_OWN * ldh2);
         oPart = take(4LL * RF_ROWS * (Nc1 > Nc2 ? Nc1 : Nc2));

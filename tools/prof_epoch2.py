@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """Phase profile of the one-launch learner kernel (csrc/epoch2.cu) at the bench shape: accumulated clock64 cycles per phase
-(CTA 0 and the last CTA) over a few learn() calls, printed as microseconds per learn()."""
+(CTA 0 and the last CTA) over a few learn() calls, printed as microseconds per learn().
+
+    python tools/prof_epoch2.py [clip|adapt] [--sm-budget N]    # N CTAs, as PipelinedEngine caps the learner (0: all SMs)
+"""
 import os
 import sys
 
@@ -15,10 +18,16 @@ def main():
     from helpers import ppo_configs
     from surreal_b200.learner import PPOLearner
     B, n, D, A = 1024, 128, 64, 8
-    mode = sys.argv[1] if len(sys.argv) > 1 else 'clip'
+    import argparse
+    ap = argparse.ArgumentParser()
+    ap.add_argument('mode', nargs='?', default='clip', choices=('clip', 'adapt'))
+    ap.add_argument('--sm-budget', type=int, default=0)
+    args = ap.parse_args()
+    mode = args.mode
     lc, ec, sc = ppo_configs(D=D, A=A, actor_h=(256, 256), critic_h=(256, 256), n_step=n, stride=n, B=B, mode=mode, lr=1e-4)
     lc.algo.consts.kl_target = 1e6                      # no KL early stop: every policy epoch runs, as in the bench
     L = PPOLearner(lc, ec, sc)
+    L.set_sm_budget(args.sm_budget)
     rng = np.random.default_rng(0)
 
     def batch():
@@ -39,7 +48,7 @@ def main():
     pair.cta_profile()
     reps = 10
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    print('policy epochs of the last learn():', L.last_n_policy_epochs)
+    print('policy epochs of the last learn():', L.last_n_policy_epochs, '| SM budget:', args.sm_budget or 'all SMs')
     ev0.record()
     for _ in range(reps):
         pair.run()                                      # the kernel alone, on the resident batch
