@@ -268,6 +268,9 @@ static int gae_resident_ctas(int n, size_t smem) {
 }
 
 int sb200_gae_init() {
+    // the generic MLP-branch kernel takes up to 48 KB of tables (n <= 6144) on top of its static reduction scratch, past
+    // the 48 KB a kernel gets without opting in
+    SB200_CUDA(cudaFuncSetAttribute(gae_full_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024));
     SB200_CUDA(cudaFuncSetAttribute(gae_horizon_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     return SB200_OK;
 }
