@@ -460,16 +460,38 @@ int sb200_tanh_bwd_f32(const float* dout, int64_t ldo, const float* out, int64_t
  *   with action floor(y * n_actions / 2^32).  Writes the action index as a float (the record's action field),
  *   optionally a one-hot row [N][ldo] (ldo >= n_actions, the tail zero) and the index as int64.  The caller advances
  *   *act_counter after the call (q_agent.py:45: T += 1 per act).
- * act_host: act on host observations in one call: H2D of obs_host (NULL: obs_dev already holds them), the tower
- *   forwards, act, D2H of the int64 actions into action_host and one stream synchronisation. */
+ * agent_act: QAgent.act in one call, for host and device observations: [H2D obs_host -> obs unless obs_host is NULL] ->
+ *   the tower forwards (on the packed weights when adv_packed is given: both towers' packs, the per-step copy a rollout
+ *   chunk packs once; else the fused forward) -> act -> [when action_host is not NULL: D2H of the int64 actions and ONE
+ *   stream synchronisation].  With the host pointers NULL no copy to or from the host and no synchronisation is
+ *   issued: the call is graph-capturable.  value_net / value_packed / value: the state tower, all NULL without dueling. */
 #define SB200_DQN_MAX_ACTIONS 1024
 int sb200_dqn_act_f32(const float* adv, int64_t lda, const float* value, int64_t ldv, int N, int n_actions,
                       const double* schedule, int n_points, double fixed_eps, uint64_t seed, const int64_t* act_counter,
                       float* action, float* one_hot, int64_t ldo, int64_t* action_i64, void* stream);
-int sb200_dqn_act_host_f32(const sb200_mlp* adv_net, const sb200_mlp* value_net, const float* obs_host, float* obs_dev,
-                           int N, float* adv_dev, float* value_dev, const double* schedule, int n_points,
-                           double fixed_eps, uint64_t seed, const int64_t* act_counter, float* action_dev,
-                           int64_t* action_i64_dev, int64_t* action_host, void* stream);
+typedef struct {
+    const sb200_mlp* adv_net;           /* action tower: D -> ... -> n_actions */
+    const sb200_mlp* value_net;         /* state tower: D -> ... -> 1, or NULL */
+    const float* adv_packed;            /* packed weights of both towers, or NULL: the fused forward */
+    const float* value_packed;
+    int N;
+    const float* obs_host;              /* [N][D] pinned, or NULL: obs already holds this step's observations */
+    float* obs;                         /* [N][ld_obs] */
+    int64_t ld_obs;
+    float* adv;                         /* [N][n_actions] */
+    float* value;                       /* [N][1] or NULL */
+    const double* schedule;             /* as in sb200_dqn_act_f32 */
+    int n_points;
+    double fixed_eps;
+    uint64_t seed;
+    const int64_t* act_counter;
+    float* action;                      /* [N] action indices as floats */
+    float* one_hot;                     /* [N][ldo] or NULL */
+    int64_t ldo;
+    int64_t* action_i64;                /* [N] or NULL; required with action_host */
+    int64_t* action_host;               /* [N] pinned; NULL: no D2H and no synchronisation */
+} sb200_dqn_agent_act;
+int sb200_dqn_agent_act_f32(const sb200_dqn_agent_act* args, void* stream);
 /* TD step of one update (dqn.py:44-69), one thread per row: q = Q(s)[a] from the online towers (q_a, q_v), the target
  * towers at s' (t_a, t_v) and, for double Q, the online towers at s' (o_a, o_v; NULL for max over the target row).
  * y = r + gamma (1 - done) q', td = q - y, loss = mean(w huber(td)) with the Huber of delta 1 (w = 1 when weights is
@@ -575,23 +597,6 @@ int sb200_synth_env_window_step_f32(float* state, const float* action, const flo
                                     const uint64_t* step_counter, float* obs_next, float* reward, float* done,
                                     const sb200_windows* windows, void* stream);
 
-/* Host-env fast path (one C call per agent.act() / ExpSender-wrapper step when the environment lives on the host; the
- * wrapper's step is sb200_ppo_window_step_f32 with host rows):
- *   ppo_act_host: [H2D obs_host -> obs_dev unless obs_host is NULL] -> policy forward -> ppo_sample (with `stage` and
- *     assign_slots) -> D2H action / pd -> ONE stream synchronisation.  Host pointers must be pinned. */
-int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter* zf, const float* obs_host, float* obs_dev, int N,
-                           float* mean_dev, const float* log_var, const float* log_noise, int deterministic,
-                           uint64_t seed, uint64_t* step_counter, float* action_dev, float* pd_dev,
-                           const sb200_windows* stage, int assign_slots, float* action_host, float* pd_host,
-                           void* stream);
-/*   ddpg_act_host: DDPGAgent.act on a host observation batch: [H2D obs_host -> obs_dev unless obs_host is NULL] -> actor
- *     forward -> ddpg_ou_noise (when ou_state != NULL, with sigma64) or ddpg_noise (with sigma) -> D2H action -> ONE stream
- *     synchronisation.  unit_noise: injected N(0,1) draws [N][A] or NULL (Philox).  2 kernels below 2048 actors. */
-int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* obs_dev, int N, float* mean_dev,
-                            const float* sigma, const double* sigma64, const float* unit_noise, int deterministic,
-                            uint64_t seed, const uint64_t* step_counter, double theta, double dt, double* ou_state,
-                            float* action_dev, float* action_host, void* stream);
-
 /* ---------------------------------------------------------------------------------------------
  * DDPG parameter-space exploration noise (surreal/agent/param_noise.py:9-74, ddpg_agent.py:136-153,174-175): every
  * actor acts with its own perturbed copy of the policy.  Images are [N][actor_stride] floats, each in the layout of
@@ -619,27 +624,66 @@ int sb200_ddpg_param_noise_apply_f32(const sb200_mlp* net, int N, float* images,
 int sb200_mlp_forward_per_actor_f32(const sb200_mlp* net, int64_t actor_stride, const float* x, int64_t ldx, int N,
                                     float* out, int64_t ld_out, const sb200_mlp* shared, float* dist, int dist_interval,
                                     sb200_param_noise_state* state, void* stream);
-/* ddpg_act_host_per_actor: sb200_ddpg_act_host_f32 (DDPGAgent.act on host observations, ddpg_agent.py:155-184) with the
- *   per-actor forward in place of the shared one: [H2D obs] -> per-actor forward -> ddpg_noise / ddpg_ou_noise -> D2H
- *   action -> ONE stream synchronisation.  2 kernels. */
-int sb200_ddpg_act_host_per_actor_f32(const sb200_mlp* net, int64_t actor_stride, const sb200_mlp* shared, float* dist,
-                                      int dist_interval, sb200_param_noise_state* state, const float* obs_host,
-                                      float* obs_dev, int N, float* mean_dev, const float* sigma, const double* sigma64,
-                                      const float* unit_noise, int deterministic, uint64_t seed,
-                                      const uint64_t* step_counter, double theta, double dt, double* ou_state,
-                                      float* action_dev, float* action_host, void* stream);
+/* DDPGAgent.act (ddpg_agent.py:155-184) in one call, for host and device observations: [H2D obs_host -> obs unless
+ *   obs_host is NULL] -> actor forward -> ddpg_ou_noise (when ou_state != NULL, with sigma64) or ddpg_noise (with sigma)
+ *   -> [when action_host is not NULL: D2H action and ONE stream synchronisation].  With the host pointers NULL no copy to
+ *   or from the host and no synchronisation is issued: the call is graph-capturable.  The forward is chosen explicitly,
+ *   because a per-actor forward with actor_stride 0 and no state (normal parameter noise before the first fetch) has the
+ *   same arguments as the fused one:
+ *     SB200_DDPG_FWD_FUSED: sb200_mlp_forward_f32 of `net`;
+ *     SB200_DDPG_FWD_PACKED: sb200_mlp_forward_packed_f32 of `net` on `packed` (the per-step copy a rollout chunk packs);
+ *     SB200_DDPG_FWD_PER_ACTOR: sb200_mlp_forward_per_actor_f32 with `net` the descriptor of image 0, actor_stride,
+ *       shared, dist, dist_interval and pn_state.
+ *   unit_noise: injected N(0,1) draws [N][A] or NULL (Philox).  2 kernels below 2048 actors. */
+#define SB200_DDPG_FWD_FUSED 0
+#define SB200_DDPG_FWD_PACKED 1
+#define SB200_DDPG_FWD_PER_ACTOR 2
+typedef struct {
+    int forward;                        /* SB200_DDPG_FWD_* */
+    const sb200_mlp* net;               /* actor: D -> ... -> A */
+    const float* packed;                /* SB200_DDPG_FWD_PACKED only */
+    int64_t actor_stride;               /* SB200_DDPG_FWD_PER_ACTOR only, as in sb200_mlp_forward_per_actor_f32 */
+    const sb200_mlp* shared;
+    float* dist;
+    int dist_interval;
+    sb200_param_noise_state* pn_state;
+    int N;
+    const float* obs_host;              /* [N][D] pinned, or NULL: obs already holds this step's observations */
+    float* obs;                         /* [N][ld_obs] */
+    int64_t ld_obs;
+    float* mean;                        /* [N][A] actor output */
+    const float* sigma;                 /* [N] float32: normal noise */
+    const double* sigma64;              /* [N] float64: OU noise */
+    const float* unit_noise;
+    int deterministic;
+    uint64_t seed;
+    const uint64_t* step_counter;
+    double theta, dt;                   /* OU noise only */
+    double* ou_state;                   /* [N][A] float64, or NULL: normal noise */
+    float* action;                      /* [N][A] */
+    float* action_host;                 /* pinned; NULL: no D2H and no synchronisation */
+} sb200_ddpg_act;
+int sb200_ddpg_act_f32(const sb200_ddpg_act* args, void* stream);
 
-/* RNN-mode PPOAgent.act (ppo_net.py:317-351, ppo_agent.py:133-149) for host or device observations, one call:
- *   [H2D obs_host -> obs unless obs_host is NULL] -> h, c copied to h_before, c_before (the step's onetime_infos) ->
- *   rows_zfilter -> per layer k: input projection (mlp_forward of ih[k] into pre_x) and lstm_forward from layer k's cells,
- *   updated in place -> head forward -> ppo_sample (with `stage` and assign_slots) -> [when action_host is not
- *   NULL: D2H action / pd, and h_before / c_before when h_before_host is not NULL, then ONE stream synchronisation].
- *   Cells are [layers][N][H] (h_before_host / c_before_host receive that layout).  Layer k writes h_out[(layers-1-k) % 2].
- *   Kernels: 2 * layers + 3 while every forward stays below 2048 rows (one kernel each).  With the host pointers NULL no
- *   copy to or from the host and no synchronisation is issued: the call is graph-capturable. */
+/* PPOAgent.act (ppo_net.py:268-279,317-351,368-375, ppo_agent.py:133-149) in one call, for host and device observations
+ * and every policy form:
+ *   layers = 0, no frames: the MLP policy.  The head reads the observation rows with the z-filter fused into its forward
+ *     (on head_packed, the per-step copy a rollout chunk packs once, when given).
+ *   layers = 0, frames: the CNN policy: the CNN stem stage below into xf, then the head on xf.
+ *   layers >= 1: the LSTM policy: h, c copied to h_before, c_before (the step's onetime_infos) -> rows_zfilter of the
+ *     observations into xf (or the CNN stem stage with frames) -> per layer k: input projection (mlp_forward of ih[k] into
+ *     pre_x) and lstm_forward from layer k's cells, updated in place -> head on the last layer's output.
+ *   Every form: [H2D obs_host -> obs or frames_host -> frames first, unless NULL] -> ... -> ppo_sample (with `stage` and
+ *   assign_slots) -> [when action_host is not NULL: D2H action / pd, and h_before / c_before when h_before_host is not
+ *   NULL, then ONE stream synchronisation].  Cells are [layers][N][H] (h_before_host / c_before_host receive that layout).
+ *   Layer k writes h_out[(layers-1-k) % 2].  Kernels while every forward stays below 2048 rows (one kernel each): 2 for
+ *   the MLP policy, 5 for the CNN policy, 2 * layers + 3 for the LSTM policy, 2 more with frames (the stem's 3 in place
+ *   of the z-filter).  With the host pointers NULL no copy to or from the host and no synchronisation is issued: the
+ *   call is graph-capturable. */
 #define SB200_MAX_RNN_LAYERS 8
 typedef struct {
-    const sb200_mlp* head;              /* actor head: H -> ... -> A */
+    const sb200_mlp* head;              /* actor head: D (layers = 0) or H -> ... -> A */
+    const float* head_packed;           /* packed head weights (MLP policy only), or NULL: the fused forward */
     sb200_zfilter zf;                   /* z-filter of the observation rows */
     const sb200_mlp* ih[SB200_MAX_RNN_LAYERS];  /* input projection of layer k: in -> 4H (W_ih^T, b_ih) */
     const float* whh[SB200_MAX_RNN_LAYERS];     /* W_hh^T [H][4H] of layer k */
@@ -648,7 +692,7 @@ typedef struct {
     const float* obs_host;              /* [N][D] pinned, or NULL: obs already holds this step's observations */
     float* obs;                         /* [N][ld_obs] */
     int64_t ld_obs;
-    float* xf;                          /* [N][ld_xf] z-filtered rows */
+    float* xf;                          /* [N][ld_xf] z-filtered rows or stem features (not read by the MLP policy) */
     int64_t ld_xf;
     float* pre_x;                       /* [N][4H] */
     float* h_out[2];                    /* [N][ldh] each; h_out[1] only for layers > 1 */
@@ -672,10 +716,10 @@ typedef struct {
     float* pd_host;
     float* h_before_host;               /* pinned; NULL: the cells stay on the device */
     float* c_before_host;
-    /* Optional CNN stem stage (pixel input, ppo_net.py:268-279): with frames != NULL layer 0 reads the stem's features
-     * instead of the z-filtered observations (obs and zf are not read):  [H2D frames_host -> frames unless NULL] ->
-     * conv_forward(1) of frames / 255 -> conv_forward(2) -> fc (Linear + ReLU) into xf [N][ld_xf], D = fc's output width.
-     * frames == NULL: no stem, the launches above unchanged.  3 kernels more while every forward stays below 2048 rows. */
+    /* Optional CNN stem stage (pixel input, ppo_net.py:268-279): with frames != NULL the first layer (or the head) reads
+     * the stem's features instead of the observations (obs and zf are not read):  [H2D frames_host -> frames unless
+     * NULL] -> conv_forward(1) of frames / 255 -> conv_forward(2) -> fc (Linear + ReLU) into xf [N][ld_xf], D = fc's
+     * output width. */
     const uint8_t* frames_host;         /* [N][frame_c][frame_h][frame_w] pinned, or NULL: frames already hold this step's */
     uint8_t* frames;                    /* [N][frame_c][frame_h][frame_w] uint8 on the device, or NULL */
     int frame_c, frame_h, frame_w;
@@ -686,8 +730,8 @@ typedef struct {
     const sb200_mlp* fc;                /* the stem's Linear + ReLU: 32 * H2 * W2 -> D */
     float* a1;                          /* [N][16][H1][W1] */
     float* a2;                          /* [N][32 * H2 * W2] */
-} sb200_ppo_act_rnn;
-int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* args, void* stream);
+} sb200_ppo_act;
+int sb200_ppo_act_f32(const sb200_ppo_act* args, void* stream);
 
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N
  * actors in ONE launch (a 4-CTA cluster owns 32 actors for the whole chunk; the policy weights stay resident in
@@ -741,7 +785,7 @@ int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* args, int* sms);
 int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, void* stream);
 
 /* Persistent rollout of the recurrent policy (csrc/rollout_rnn.cu): T steps of z-filter -> LSTM layers -> actor head ->
- * sampling -> synthetic env step -> window staging for ALL N actors in ONE launch.  Replaces T x (sb200_ppo_act_rnn_f32
+ * sampling -> synthetic env step -> window staging for ALL N actors in ONE launch.  Replaces T x (sb200_ppo_act_f32
  * with `stage` and assign_slots + sb200_synth_env_step_f32 + sb200_ppo_window_step_f32 with the cells), i.e. the actor
  * main loop of surreal/agent/base.py:224-271 with the LSTM policy of ppo_net.py:317-351 and ppo_agent.py:84-93,133-154,
  * for a device-resident env.  A CTA owns 8 actors; their
@@ -751,7 +795,7 @@ int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, vo
  *     (H -> ... -> A), base->D the env's observation width; the window records are base->D + 2 * layers * H wide
  *     ([obs | h_0 .. h_{L-1} | c_0 .. c_{L-1}], utils.rnn_cell_layout).  Commit with sb200_ppo_rollout_commit_f32 on a
  *     copy of `base` whose D is the record width.
- *   ih / whh / bhh / layers / H / h / c / h_before / c_before: as in sb200_ppo_act_rnn.  The cells are read at entry and
+ *   ih / whh / bhh / layers / H / h / c / h_before / c_before: as in sb200_ppo_act.  The cells are read at entry and
  *     written back at exit; h_before / c_before receive the cells before the chunk's last step.
  *   Each staged row carries the cells the actor acts from on that row's observation (the successor row and, after done,
  *   the reset row alike: the cells carry over across episodes).

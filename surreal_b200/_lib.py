@@ -91,21 +91,44 @@ class ZFilter(C.Structure):
     _fields_ = [('stats', C.c_void_p), ('eps', C.c_float)]
 
 
-class PPOActRnn(C.Structure):
-    """sb200_ppo_act_rnn (include/surreal_b200.h)."""
-    _fields_ = [('head', C.POINTER(Mlp)), ('zf', ZFilter), ('ih', C.POINTER(Mlp) * MAX_RNN_LAYERS),
-                ('whh', C.c_void_p * MAX_RNN_LAYERS), ('bhh', C.c_void_p * MAX_RNN_LAYERS), ('layers', C.c_int),
-                ('N', C.c_int), ('D', C.c_int), ('H', C.c_int), ('obs_host', C.c_void_p), ('obs', C.c_void_p),
-                ('ld_obs', C.c_int64), ('xf', C.c_void_p), ('ld_xf', C.c_int64), ('pre_x', C.c_void_p),
-                ('h_out', C.c_void_p * 2), ('ldh', C.c_int), ('h', C.c_void_p), ('c', C.c_void_p), ('h_before', C.c_void_p),
-                ('c_before', C.c_void_p), ('mean', C.c_void_p), ('log_var', C.c_void_p), ('log_noise', C.c_void_p),
-                ('eps', C.c_void_p), ('deterministic', C.c_int), ('seed', C.c_uint64), ('step_counter', C.c_void_p),
-                ('action', C.c_void_p), ('pd', C.c_void_p), ('stage', C.POINTER(Windows)), ('assign_slots', C.c_int),
-                ('action_host', C.c_void_p), ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p),
-                ('c_before_host', C.c_void_p), ('frames_host', C.c_void_p), ('frames', C.c_void_p), ('frame_c', C.c_int),
-                ('frame_h', C.c_int), ('frame_w', C.c_int), ('conv_w1', C.c_void_p), ('conv_b1', C.c_void_p),
-                ('conv_w2', C.c_void_p), ('conv_b2', C.c_void_p), ('fc', C.POINTER(Mlp)), ('a1', C.c_void_p),
-                ('a2', C.c_void_p)]
+class PPOAct(C.Structure):
+    """sb200_ppo_act (include/surreal_b200.h)."""
+    _fields_ = [('head', C.POINTER(Mlp)), ('head_packed', C.c_void_p), ('zf', ZFilter),
+                ('ih', C.POINTER(Mlp) * MAX_RNN_LAYERS), ('whh', C.c_void_p * MAX_RNN_LAYERS),
+                ('bhh', C.c_void_p * MAX_RNN_LAYERS), ('layers', C.c_int), ('N', C.c_int), ('D', C.c_int), ('H', C.c_int),
+                ('obs_host', C.c_void_p), ('obs', C.c_void_p), ('ld_obs', C.c_int64), ('xf', C.c_void_p),
+                ('ld_xf', C.c_int64), ('pre_x', C.c_void_p), ('h_out', C.c_void_p * 2), ('ldh', C.c_int), ('h', C.c_void_p),
+                ('c', C.c_void_p), ('h_before', C.c_void_p), ('c_before', C.c_void_p), ('mean', C.c_void_p),
+                ('log_var', C.c_void_p), ('log_noise', C.c_void_p), ('eps', C.c_void_p), ('deterministic', C.c_int),
+                ('seed', C.c_uint64), ('step_counter', C.c_void_p), ('action', C.c_void_p), ('pd', C.c_void_p),
+                ('stage', C.POINTER(Windows)), ('assign_slots', C.c_int), ('action_host', C.c_void_p),
+                ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p), ('c_before_host', C.c_void_p),
+                ('frames_host', C.c_void_p), ('frames', C.c_void_p), ('frame_c', C.c_int), ('frame_h', C.c_int),
+                ('frame_w', C.c_int), ('conv_w1', C.c_void_p), ('conv_b1', C.c_void_p), ('conv_w2', C.c_void_p),
+                ('conv_b2', C.c_void_p), ('fc', C.POINTER(Mlp)), ('a1', C.c_void_p), ('a2', C.c_void_p)]
+
+
+DDPG_FWD_FUSED, DDPG_FWD_PACKED, DDPG_FWD_PER_ACTOR = 0, 1, 2
+
+
+class DDPGAct(C.Structure):
+    """sb200_ddpg_act (include/surreal_b200.h)."""
+    _fields_ = [('forward', C.c_int), ('net', C.POINTER(Mlp)), ('packed', C.c_void_p), ('actor_stride', C.c_int64),
+                ('shared', C.POINTER(Mlp)), ('dist', C.c_void_p), ('dist_interval', C.c_int), ('pn_state', C.c_void_p),
+                ('N', C.c_int), ('obs_host', C.c_void_p), ('obs', C.c_void_p), ('ld_obs', C.c_int64), ('mean', C.c_void_p),
+                ('sigma', C.c_void_p), ('sigma64', C.c_void_p), ('unit_noise', C.c_void_p), ('deterministic', C.c_int),
+                ('seed', C.c_uint64), ('step_counter', C.c_void_p), ('theta', C.c_double), ('dt', C.c_double),
+                ('ou_state', C.c_void_p), ('action', C.c_void_p), ('action_host', C.c_void_p)]
+
+
+class DQNAgentAct(C.Structure):
+    """sb200_dqn_agent_act (include/surreal_b200.h)."""
+    _fields_ = [('adv_net', C.POINTER(Mlp)), ('value_net', C.POINTER(Mlp)), ('adv_packed', C.c_void_p),
+                ('value_packed', C.c_void_p), ('N', C.c_int), ('obs_host', C.c_void_p), ('obs', C.c_void_p),
+                ('ld_obs', C.c_int64), ('adv', C.c_void_p), ('value', C.c_void_p), ('schedule', C.c_void_p),
+                ('n_points', C.c_int), ('fixed_eps', C.c_double), ('seed', C.c_uint64), ('act_counter', C.c_void_p),
+                ('action', C.c_void_p), ('one_hot', C.c_void_p), ('ldo', C.c_int64), ('action_i64', C.c_void_p),
+                ('action_host', C.c_void_p)]
 
 
 class Par(C.Structure):
@@ -178,14 +201,10 @@ def _declare(lib):
         'sb200_mlp_pack_floats': (S, [C.POINTER(Mlp)]),
         'sb200_mlp_pack_tf32': (I, [C.POINTER(Mlp), P, P]),
         'sb200_mlp_forward_packed_f32': (I, [C.POINTER(Mlp), P, C.POINTER(ZFilter), C.POINTER(Rows), P, L, P]),
-        'sb200_ppo_act_host_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), P, P, I, P, P, P, I, C.c_uint64, P, P, P,
-                                       C.POINTER(Windows), I, P, P, P]),
-        'sb200_ddpg_act_host_f32': (I, [C.POINTER(Mlp), P, P, I, P, P, P, P, I, C.c_uint64, P, D, D, P, P, P, P]),
+        'sb200_ddpg_act_f32': (I, [C.POINTER(DDPGAct), P]),
         'sb200_ddpg_param_noise_apply_f32': (I, [C.POINTER(Mlp), I, P, L, P, P, C.c_uint64, C.c_uint64, P, P, D, D, P]),
         'sb200_mlp_forward_per_actor_f32': (I, [C.POINTER(Mlp), L, P, L, I, P, L, C.POINTER(Mlp), P, I, P, P]),
-        'sb200_ddpg_act_host_per_actor_f32': (I, [C.POINTER(Mlp), L, C.POINTER(Mlp), P, I, P, P, P, I, P, P, P, P, I,
-                                                  C.c_uint64, P, D, D, P, P, P, P]),
-        'sb200_ppo_act_rnn_f32': (I, [C.POINTER(PPOActRnn), P]),
+        'sb200_ppo_act_f32': (I, [C.POINTER(PPOAct), P]),
         'sb200_ppo_rollout_supported': (I, [C.POINTER(Mlp), I, I]),
         'sb200_ppo_rollout_scratch_ints': (S, [I, I, I]),
         'sb200_ppo_rollout_f32': (I, [C.POINTER(PPORollout), P]),
@@ -254,8 +273,7 @@ def _declare(lib):
         'sb200_hard_update_f32': (I, [P, P, L, P, L, L, I, P, P]),
         'sb200_ddpg_bad_action_offset': (S, []),
         'sb200_dqn_act_f32': (I, [P, L, P, L, I, I, P, I, D, C.c_uint64, P, P, P, L, P, P]),
-        'sb200_dqn_act_host_f32': (I, [C.POINTER(Mlp), C.POINTER(Mlp), P, P, I, P, P, P, I, D, C.c_uint64, P, P, P, P,
-                                       P]),
+        'sb200_dqn_agent_act_f32': (I, [C.POINTER(DQNAgentAct), P]),
         'sb200_dqn_workspace_bytes': (S, [I]),
         'sb200_dqn_bad_action_offset': (S, []),
         'sb200_dqn_td_f32': (I, [P, L, P, L, P, L, P, L, P, L, P, L, P, P, P, P, I, I, D, D, P, L, P, L, P, P, P, P]),

@@ -70,7 +70,7 @@ class DDPGAgent(Agent):
                                actor_fc_hidden_sizes=self.learner_config.model.actor_fc_hidden_sizes,
                                critic_fc_hidden_sizes=self.learner_config.model.critic_fc_hidden_sizes,
                                device=self.device)
-        A, D = self.action_dim, self.model.input_dim
+        A = self.action_dim
         self._sigma = torch.tensor(self.sigma, dtype=torch.float32, device=self.device)
         self._ou_state = None
         if self.noise_type == 'ou_noise':
@@ -84,8 +84,6 @@ class DDPGAgent(Agent):
         else:
             self._init_param_noise(ex)
         self._action = torch.zeros(N, A, device=self.device)
-        self._obs_dev = torch.zeros(N, D, device=self.device)
-        self._obs_pin = None
         self._counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.seed = 5 + 1000003 * int(agent_id)
 
@@ -145,77 +143,59 @@ class DDPGAgent(Agent):
         return actor.desc(self._pn_images), self.param_noise_stride, (shared if self._pn_adaptive else None)
 
     def act(self, obs, unit_noise=None):
+        """DDPGAgent.act (ddpg_agent.py:155-184) for all N actors in ONE call of sb200_ddpg_act_f32, host and device
+        observations alike: [H2D] -> the actor forward (fused, packed inside a rollout chunk, or per actor under parameter
+        noise) -> exploration noise -> [D2H, one sync].  Device observations give the device action tensor; numpy in,
+        float32 numpy out (1-D for one actor's 1-D observation)."""
         N, A, D = self.num_envs, self.action_dim, self.model.input_dim
         if self.sleep_time > 0.0:
             time.sleep(self.sleep_time)
         x = obs['low_dim']['flat_inputs'] if isinstance(obs, dict) else obs
-        if not isinstance(x, torch.Tensor):
-            return self._act_host(np.asarray(x), unit_noise)
-        x = x.reshape(N, D)
-        if self.param_noise_type is not None:
+        host = not isinstance(x, torch.Tensor)
+        a = _lib.DDPGAct()
+        if host:
+            x = np.asarray(x)
+            a.obs_host, obs_dev = self._host_obs(x, (N, D))
+            a.obs, a.ld_obs = obs_dev.data_ptr(), D
+            if getattr(self, '_act_pin', None) is None:
+                self._act_pin = torch.empty(N, A, dtype=torch.float32, pin_memory=True)
+            a.action_host = self._act_pin.data_ptr()
+        else:
+            x = x.reshape(N, D)
             if x.stride(1) != 1:
                 x = x.contiguous()
-            d, stride, shared = self._pn_descs()
-            check(_lib.lib().sb200_mlp_forward_per_actor_f32(
-                C.byref(d), stride, _p(x), x.stride(0), N, _p(self._mean), A,
-                C.byref(shared) if shared is not None else None, _p(self._pn_dist), PARAM_NOISE_DIST_INTERVAL,
-                _p(self._pn_state), ops._stream()), 'sb200_mlp_forward_per_actor_f32')
-        elif self._in_chunk and self._packed.supported and x.stride(1) == 1:
-            # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
-            ops.mlp_forward_packed(self._packed, x, out=self._mean)
-        else:
-            ops.mlp_forward(self.model.actor, x, out=self._mean)
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        env = self.env
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        un = None
-        if unit_noise is not None:
-            un = torch.as_tensor(np.asarray(unit_noise, dtype=np.float32).reshape(N, A)).to(self.device)
-        if self._ou_state is not None:
-            check(_lib.lib().sb200_ddpg_ou_noise_f32(_p(self._mean), A, _p(self._sigma64), _p(un), N, A, int(det),
-                                                     self.seed, _p(counter), self.ou_theta, self.ou_dt,
-                                                     _p(self._ou_state), _p(self._action), ops._stream()),
-                  'sb200_ddpg_ou_noise_f32')
-        else:
-            check(_lib.lib().sb200_ddpg_noise_f32(_p(self._mean), A, _p(self._sigma), _p(un), N, A, int(det), self.seed,
-                                                  _p(counter), _p(self._action), ops._stream()), 'sb200_ddpg_noise_f32')
-        if counter is self._counter:
-            self._counter += 1
-        return self._action
-
-    def _act_host(self, x, unit_noise):
-        """act() on a HOST observation batch through sb200_ddpg_act_host_f32 (H2D obs unless the wrapper already moved it
-        -> actor forward -> exploration noise -> D2H action -> one sync): numpy in, float32 numpy out."""
-        N, A, D = self.num_envs, self.action_dim, self.model.input_dim
-        obs_host, obs_dev = self._host_obs(x, D)
-        if getattr(self, '_act_pin', None) is None:
-            self._act_pin = torch.empty(N, A, dtype=torch.float32, pin_memory=True)
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        env = self.env
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        un = None
-        if unit_noise is not None:
-            un = torch.as_tensor(np.asarray(unit_noise, dtype=np.float32).reshape(N, A)).to(self.device)
-        ou = self._ou_state is not None
+            a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
         if self.param_noise_type is not None:
             d, stride, shared = self._pn_descs()
-            check(_lib.lib().sb200_ddpg_act_host_per_actor_f32(
-                C.byref(d), stride, C.byref(shared) if shared is not None else None, _p(self._pn_dist),
-                PARAM_NOISE_DIST_INTERVAL, _p(self._pn_state), obs_host, _p(obs_dev), N, _p(self._mean), _p(self._sigma),
-                _p(self._sigma64 if ou else None), _p(un), int(det), self.seed, _p(counter),
-                self.ou_theta if ou else 0.0, self.ou_dt if ou else 0.0, _p(self._ou_state), _p(self._action),
-                C.c_void_p(self._act_pin.data_ptr()), ops._stream()), 'sb200_ddpg_act_host_per_actor_f32')
+            a.forward, a.actor_stride, a.dist_interval = _lib.DDPG_FWD_PER_ACTOR, stride, PARAM_NOISE_DIST_INTERVAL
+            a.shared = C.pointer(shared) if shared is not None else None
+            a.dist = self._pn_dist.data_ptr() if self._pn_dist is not None else None
+            a.pn_state = self._pn_state.data_ptr() if self._pn_state is not None else None
         else:
             d = self.model.actor.desc()
-            check(_lib.lib().sb200_ddpg_act_host_f32(
-                C.byref(d), obs_host, _p(obs_dev), N, _p(self._mean), _p(self._sigma), _p(self._sigma64 if ou else None),
-                _p(un), int(det), self.seed, _p(counter), self.ou_theta if ou else 0.0, self.ou_dt if ou else 0.0,
-                _p(self._ou_state), _p(self._action), C.c_void_p(self._act_pin.data_ptr()), ops._stream()),
-                'sb200_ddpg_act_host_f32')
+            if self._in_chunk and self._packed.supported:
+                # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
+                a.forward, a.packed = _lib.DDPG_FWD_PACKED, self._packed.buf.data_ptr()
+        a.net = C.pointer(d)
+        a.N, a.mean, a.action = N, self._mean.data_ptr(), self._action.data_ptr()
+        a.sigma = self._sigma.data_ptr()
+        if self._ou_state is not None:
+            a.sigma64, a.theta, a.dt, a.ou_state = self._sigma64.data_ptr(), self.ou_theta, self.ou_dt, self._ou_state.data_ptr()
+        un = None
+        if unit_noise is not None:
+            un = torch.as_tensor(np.asarray(unit_noise, dtype=np.float32).reshape(N, A)).to(self.device)
+            a.unit_noise = un.data_ptr()
+        env = self.env
+        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
+        a.deterministic = int(self.agent_mode in ['eval_deterministic', 'eval_deterministic_local'])
+        a.seed, a.step_counter = self.seed, counter.data_ptr()
+        check(_lib.lib().sb200_ddpg_act_f32(C.byref(a), ops._stream()), 'sb200_ddpg_act_f32')
         if counter is self._counter:
             self._counter += 1
-        a = self._act_pin.numpy().copy()
-        return a.reshape(-1) if (N == 1 and x.ndim == 1) else a
+        if not host:
+            return self._action
+        act = self._act_pin.numpy().copy()
+        return act.reshape(-1) if (N == 1 and x.ndim == 1) else act
 
     def pre_episode(self):
         super().pre_episode()

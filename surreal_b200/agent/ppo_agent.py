@@ -49,14 +49,12 @@ class PPOAgent(Agent):
         self.model = PPOModel(obs_spec=self.obs_spec, action_dim=self.action_dim, model_config=self.learner_config.model,
                               use_cuda=True, init_log_sig=self.init_log_sig, use_z_filter=self.use_z_filter,
                               if_pixel_input=pixel, rnn_config=self.rnn_config, device=self.device)
-        A, D = self.action_dim, self.model.low_dim
+        A = self.action_dim
         self._log_noise = torch.tensor(self.noise, dtype=torch.float32, device=self.device)
         self._mean = torch.zeros(N, A, device=self.device)
         self._packed = ops.PackedWeights(self.model.actor)          # per-step inference copy of the policy weights
         self._action = torch.zeros(N, A, device=self.device)
         self._pd = torch.zeros(N, 2 * A, device=self.device)
-        self._obs_dev = torch.zeros(N, D, device=self.device)
-        self._obs_pin = None
         self._out_pin = None
         self._counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.seed = 2 + 1000003 * int(agent_id)
@@ -66,68 +64,118 @@ class PPOAgent(Agent):
         self._log_noise.copy_(torch.tensor(self.noise, dtype=torch.float32))
 
     def act(self, obs, eps=None):
-        """-> action (eval) or (action, [onetime_infos, [pd]]) in training, like ppo_agent.py:151-154.
-        Device observations give device results; numpy in, numpy out."""
-        N, D = self.num_envs, self.model.low_dim
-        if self.model.rnn_stem is not None:
-            return self._act_rnn(obs, eps)
-        if self.model.cnn_stem is not None:
-            return self._act_pixel(obs, eps)
-        x = obs
-        if isinstance(obs, dict):
+        """-> action (eval) or (action, [onetime_infos, [pd]]) in training, like ppo_agent.py:151-154, through ONE call of
+        sb200_ppo_act_f32 for every policy form (MLP, CNN, LSTM, CNN + LSTM) and for host and device observations alike:
+        [H2D] -> [CNN stem] -> [z-filter -> LSTM layers, each actor's cells updated in place] -> actor head -> sampling
+        (ppo_net.py:268-279,317-351,368-375, ppo_agent.py:133-149) -> [D2H, one sync].  The LSTM policy's onetime_infos are
+        its cells BEFORE the step.  Device observations give device results; numpy in, numpy out.  Pixel input is uint8
+        frames [N, C, H, W] (device tensor or numpy)."""
+        from ..model.lstm_stem import _sfx
+        N, A, m = self.num_envs, self.action_dim, self.model
+        cnn, stem = m.cnn_stem, m.rnn_stem
+        if cnn is not None:
+            x = obs['pixel']['camera0'] if isinstance(obs, dict) else obs
+        elif isinstance(obs, dict):
             xs = [obs['low_dim'][k] for k in obs['low_dim']]
-            x = xs[0] if len(xs) == 1 else (torch.cat(xs, -1) if isinstance(xs[0], torch.Tensor)
-                                            else np.concatenate(xs, -1))
-        host = not isinstance(x, torch.Tensor)
-        if host and eps is None and isinstance(x, np.ndarray):
-            return self._act_host(obs, x)                          # one C call: copies, kernels, one sync
-        if host:
-            cached = self.env.cached_device_obs(x) if hasattr(self.env, 'cached_device_obs') else None
-            if cached is not None:
-                x = cached                                         # the wrapper already moved this observation
-            else:
-                if self._obs_pin is None:
-                    self._obs_pin = torch.empty(N, D, dtype=torch.float32, pin_memory=True)
-                xt = torch.from_numpy(x) if (isinstance(x, np.ndarray) and x.dtype == np.float32 and
-                                             x.flags['C_CONTIGUOUS'] and x.flags['WRITEABLE']) else None
-                if xt is not None and xt.is_pinned():              # observation already in pinned memory: DMA directly
-                    self._obs_dev.copy_(xt.view(N, D), non_blocking=True)
-                else:
-                    self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.float32).reshape(N, D)
-                    self._obs_dev.copy_(self._obs_pin, non_blocking=True)
-                x = self._obs_dev
-        x = x.reshape(N, D)
-        m = self.model
-        if self._in_chunk and self._packed.supported and x.stride(1) == 1:
-            # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
-            ops.mlp_forward_packed(self._packed, x, zf_stats=m.z_stats, zf_eps=m.z_eps, out=self._mean)
+            x = xs[0] if len(xs) == 1 else (torch.cat(xs, -1) if isinstance(xs[0], torch.Tensor) else np.concatenate(xs, -1))
         else:
-            ops.mlp_forward(m.actor, x, zf_stats=m.z_stats, zf_eps=m.z_eps, out=self._mean)
-        self._sample(eps)
-        return self._host_result(True, self._unbatched(obs), []) if host else self._result(self._action, self._pd, [])
+            x = obs
+        host = not isinstance(x, torch.Tensor)
+        training = self.agent_mode == 'training'
+        a = _lib.PPOAct()
+        D, xf = m.low_dim, None
+        if cnn is not None:
+            # CNN stem stage of the same call: frames -> conv1 -> conv2 -> fc + ReLU -> the LSTM's or the head's input rows
+            D, shape = cnn.d_out, (N, cnn.C, cnn.H, cnn.W)
+            if host:
+                a.frames_host, frames = self._host_obs(np.asarray(x), shape, np.uint8)
+            else:
+                if x.dtype != torch.uint8 or x.numel() != N * cnn.C * cnn.H * cnn.W or not x.is_cuda:
+                    raise ValueError('pixel act() wants uint8 CUDA frames [%d, %d, %d, %d], got %s %s'
+                                     % (N, cnn.C, cnn.H, cnn.W, x.dtype, tuple(x.shape)))
+                frames = x = x.contiguous()                      # held until the call below has been issued
+            a.frames = frames.data_ptr()
+            a.frame_c, a.frame_h, a.frame_w = cnn.C, cnn.H, cnn.W
+            a.conv_w1, a.conv_b1 = cnn.seg('w1').data_ptr(), cnn.seg('b1').data_ptr()
+            a.conv_w2, a.conv_b2 = cnn.seg('w2').data_ptr(), cnn.seg('b2').data_ptr()
+            fc = cnn.fc.desc()
+            a.fc = C.pointer(fc)
+            if getattr(self, '_stem_bufs', None) is None:
+                self._stem_bufs = cnn.buffers(N)
+            a.a1, a.a2 = self._stem_bufs['a1'].data_ptr(), self._stem_bufs['a2'].data_ptr()
+            xf = self._stem_bufs['feat']
+        elif host:
+            a.obs_host, obs_dev = self._host_obs(np.asarray(x), (N, D))
+            a.obs, a.ld_obs = obs_dev.data_ptr(), D
+        else:
+            x = x.reshape(N, D)
+            if x.stride(1) != 1:
+                x = x.contiguous()
+            a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
+            if stem is None and self._in_chunk and self._packed.supported:
+                a.head_packed = self._packed.buf.data_ptr()      # weights are fixed inside a chunk: packed at its top
+        if stem is not None:
+            self._rnn_state()
+            L, H = stem.layers, stem.H
+            ihs = [stem.ihs[k].desc(stem.seg('ih' + _sfx(k))) for k in range(L)]
+            for k in range(L):
+                a.ih[k] = C.pointer(ihs[k])
+                hh, lay = stem.seg('hh' + _sfx(k)), stem.hhs[k].layout[0]
+                a.whh[k], a.bhh[k] = hh.data_ptr() + 4 * lay['w'], hh.data_ptr() + 4 * lay['b']
+            a.layers, a.H = L, H
+            bufs = self._rnn_bufs
+            a.pre_x = bufs['pre_x'].data_ptr()
+            a.h_out[0], a.ldh = bufs['h_out'].data_ptr(), bufs['h_out'].stride(0)
+            if L > 1:
+                a.h_out[1] = bufs['h_out1'].data_ptr()
+            a.h, a.c, a.h_before, a.c_before = self._hs.data_ptr(), self._cs.data_ptr(), self._hs_before.data_ptr(), self._cs_before.data_ptr()
+            xf = self._xf
+        if xf is not None:
+            a.xf, a.ld_xf = xf.data_ptr(), xf.stride(0)
+        if host:
+            out = self._pinned_out()
+            a.action_host, a.pd_host = out[0].data_ptr(), out[1].data_ptr()
+            if training and stem is not None:
+                if getattr(self, '_cells_pin', None) is None:
+                    self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
+                                       torch.empty(L, N, H, dtype=torch.float32, pin_memory=True))
+                a.h_before_host, a.c_before_host = self._cells_pin[0].data_ptr(), self._cells_pin[1].data_ptr()
+        head = m.actor.desc()
+        a.head = C.pointer(head)
+        a.zf = ops.zfilter_desc(m.z_stats, m.z_eps)
+        a.N, a.D = N, D
+        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
+        env = self.env
+        staged = training and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
+        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
+        eps_dev = None
+        if eps is not None:
+            eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
+            a.eps = eps_dev.data_ptr()
+        a.mean, a.log_var, a.log_noise = self._mean.data_ptr(), m.log_var.data_ptr(), self._log_noise.data_ptr()
+        a.deterministic, a.seed, a.step_counter = int(det), self.seed, counter.data_ptr()
+        a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
+        if staged:
+            a.stage = C.pointer(env.windows)
+        a.assign_slots = self._assign_slots(staged, counter)
+        check(_lib.lib().sb200_ppo_act_f32(C.byref(a), ops._stream()), 'sb200_ppo_act_f32')
+        self._count_step(staged, counter)
+        if stem is None:                                            # the CNN policy keeps the batch dimension
+            return self._host_result(cnn is None and self._unbatched(obs), []) if host else \
+                self._result(self._action, self._pd, [])
+        if not host:
+            return self._result(self._action, self._pd, [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)])
+        onetime = None
+        if training:                                                # [N, layers, H]
+            onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
+            if N == 1:
+                onetime = [onetime[0][0], onetime[1][0]]
+        return self._host_result(N == 1, onetime)
 
     def _unbatched(self, obs):
         """One actor's observation without the batch dimension (numpy in: its results lose theirs too)."""
         return self.num_envs == 1 and np.asarray(obs['low_dim'][next(iter(obs['low_dim']))] if isinstance(obs, dict)
                                                  else obs).ndim == 1
-
-    def _sample(self, eps):
-        """The sampling kernel on self._mean: each actor's exploration scale, N(mean, std), clip, behaviour policy -- and,
-        in training behind the window wrapper, this step's staging (+ its replay-slot assignment when the wrapper fuses
-        launches) -- then the step counter."""
-        N, A, m, env = self.num_envs, self.action_dim, self.model, self.env
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        eps_dev = None
-        if eps is not None:
-            eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-        assign = self._assign_slots(staged, counter)
-        check(_lib.lib().sb200_ppo_sample_f32(
-            _p(self._mean), A, _p(m.log_var), _p(self._log_noise), _p(eps_dev), N, A, int(det), self.seed, _p(counter),
-            _p(self._action), _p(self._pd), C.byref(env.windows) if staged else None, int(assign), ops._stream()),
-            'sb200_ppo_sample_f32')
-        self._count_step(staged, counter)
 
     def _assign_slots(self, staged, counter):
         """Whether this step's sampling launch also assigns the step's replay slots and advances the wrapper's step
@@ -149,15 +197,10 @@ class PPOAgent(Agent):
                              torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
         return self._out_pin
 
-    def _host_result(self, d2h, single, onetime):
-        """act()'s numpy result from the pinned outputs: with ``d2h`` the D2H copies of action / pd and one sync for both
-        (else the C call has done them); float64 actions, as the reference hands the env (ppo_net.py:83); ``single``: one
-        actor's unbatched observation gives unbatched results."""
+    def _host_result(self, single, onetime):
+        """act()'s numpy result from the pinned outputs the C call has filled: float64 actions, as the reference hands the
+        env (ppo_net.py:83); ``single``: one actor's unbatched observation gives unbatched results."""
         out = self._pinned_out()
-        if d2h:
-            out[0].copy_(self._action, non_blocking=True)
-            out[1].copy_(self._pd, non_blocking=True)
-            torch.cuda.current_stream().synchronize()
         action, pd = out[0].numpy().astype(np.float64), out[1].numpy().copy()
         if single:
             action, pd = action.reshape(-1), pd.reshape(-1)
@@ -187,152 +230,6 @@ class PPOAgent(Agent):
             self._xf = z(N, ops._ru(D, 4))[:, :D]
             self._rnn_bufs = self.model.rnn_stem.buffers(N, 1, save=False)
         return self._h, self._c
-
-    def _act_rnn(self, obs, eps=None):
-        """act() with the LSTM stem, for host and device observations alike through ONE call of sb200_ppo_act_rnn_f32:
-        z-filter -> per layer one LSTM step from each actor's cells, updated in place -> actor head -> sampling
-        (ppo_net.py:317-351, ppo_agent.py:133-149).  The cells BEFORE the step are the step's onetime_info.  Host input:
-        H2D of the observation (unless the wrapper already moved it), D2H of the results and one stream sync in that call.
-        Pixel input: uint8 frames [N, C, H, W] (device tensor or numpy) go through the CNN stem stage of the same call
-        instead of the z-filter."""
-        from ..model.lstm_stem import _sfx
-        N, A, D = self.num_envs, self.action_dim, self.model.low_dim
-        m, stem = self.model, self.model.rnn_stem
-        self._rnn_state()
-        L, H = stem.layers, stem.H
-        cnn = m.cnn_stem
-        x = obs
-        if cnn is not None:
-            x = obs['pixel']['camera0'] if isinstance(obs, dict) else obs
-        elif isinstance(obs, dict):
-            xs = [obs['low_dim'][k] for k in obs['low_dim']]
-            x = xs[0] if len(xs) == 1 else (torch.cat(xs, -1) if isinstance(xs[0], torch.Tensor) else np.concatenate(xs, -1))
-        host = not isinstance(x, torch.Tensor)
-        training = self.agent_mode == 'training'
-        a = _lib.PPOActRnn()
-        if cnn is not None:
-            # CNN stem stage of the same call: frames -> conv1 -> conv2 -> fc + ReLU -> the LSTM's input rows
-            D = cnn.d_out
-            if not host:
-                if x.dtype != torch.uint8 or x.numel() != N * cnn.C * cnn.H * cnn.W or not x.is_cuda:
-                    raise ValueError('pixel act() wants uint8 CUDA frames [%d, %d, %d, %d], got %s %s'
-                                     % (N, cnn.C, cnn.H, cnn.W, x.dtype, tuple(x.shape)))
-                x = x.contiguous()                               # held until the call below has been issued
-                a.frames = x.data_ptr()
-            else:
-                cached = self.env.cached_device_obs(x) if hasattr(self.env, 'cached_device_obs') else None
-                if cached is not None:                           # the wrapper already moved these frames (as words)
-                    a.frames = cached.data_ptr()
-                else:                                            # H2D inside the call, from pinned staging
-                    if self._obs_pin is None:
-                        self._obs_pin = torch.empty(N, cnn.C, cnn.H, cnn.W, dtype=torch.uint8, pin_memory=True)
-                        self._frames_dev = torch.empty(N, cnn.C, cnn.H, cnn.W, dtype=torch.uint8, device=self.device)
-                    self._obs_pin.numpy()[...] = np.asarray(x, dtype=np.uint8).reshape(N, cnn.C, cnn.H, cnn.W)
-                    a.frames_host, a.frames = self._obs_pin.data_ptr(), self._frames_dev.data_ptr()
-            a.frame_c, a.frame_h, a.frame_w = cnn.C, cnn.H, cnn.W
-            a.conv_w1, a.conv_b1 = cnn.seg('w1').data_ptr(), cnn.seg('b1').data_ptr()
-            a.conv_w2, a.conv_b2 = cnn.seg('w2').data_ptr(), cnn.seg('b2').data_ptr()
-            fc = cnn.fc.desc()
-            a.fc = C.pointer(fc)
-            if getattr(self, '_stem_bufs', None) is None:
-                self._stem_bufs = cnn.buffers(N)
-            a.a1, a.a2 = self._stem_bufs['a1'].data_ptr(), self._stem_bufs['a2'].data_ptr()
-        if host:
-            if cnn is None:
-                obs_host, obs_dev = self._host_obs(np.asarray(x), D)
-                a.obs_host, a.obs, a.ld_obs = (obs_host.value if obs_host is not None else None), obs_dev.data_ptr(), D
-            out = self._pinned_out()
-            a.action_host, a.pd_host = out[0].data_ptr(), out[1].data_ptr()
-            if training:
-                if getattr(self, '_cells_pin', None) is None:
-                    self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
-                                       torch.empty(L, N, H, dtype=torch.float32, pin_memory=True))
-                a.h_before_host, a.c_before_host = self._cells_pin[0].data_ptr(), self._cells_pin[1].data_ptr()
-        elif cnn is None:
-            x = x.reshape(N, D)
-            a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
-        head = m.actor.desc()
-        ihs = [stem.ihs[k].desc(stem.seg('ih' + _sfx(k))) for k in range(L)]
-        a.head = C.pointer(head)
-        a.zf = ops.zfilter_desc(m.z_stats, m.z_eps)
-        for k in range(L):
-            a.ih[k] = C.pointer(ihs[k])
-            hh, lay = stem.seg('hh' + _sfx(k)), stem.hhs[k].layout[0]
-            a.whh[k], a.bhh[k] = hh.data_ptr() + 4 * lay['w'], hh.data_ptr() + 4 * lay['b']
-        a.layers, a.N, a.D, a.H = L, N, D, H
-        bufs = self._rnn_bufs
-        a.xf, a.ld_xf, a.pre_x = self._xf.data_ptr(), self._xf.stride(0), bufs['pre_x'].data_ptr()
-        a.h_out[0], a.ldh = bufs['h_out'].data_ptr(), bufs['h_out'].stride(0)
-        if L > 1:
-            a.h_out[1] = bufs['h_out1'].data_ptr()
-        a.h, a.c, a.h_before, a.c_before = self._hs.data_ptr(), self._cs.data_ptr(), self._hs_before.data_ptr(), self._cs_before.data_ptr()
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        env = self.env
-        staged = training and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        eps_dev = None
-        if eps is not None:
-            eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-            a.eps = eps_dev.data_ptr()
-        a.mean, a.log_var, a.log_noise = self._mean.data_ptr(), m.log_var.data_ptr(), self._log_noise.data_ptr()
-        a.deterministic, a.seed, a.step_counter = int(det), self.seed, counter.data_ptr()
-        a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
-        if staged:
-            a.stage = C.pointer(env.windows)
-        a.assign_slots = self._assign_slots(staged, counter)
-        check(_lib.lib().sb200_ppo_act_rnn_f32(C.byref(a), ops._stream()), 'sb200_ppo_act_rnn_f32')
-        self._count_step(staged, counter)
-        if not host:
-            return self._result(self._action, self._pd, [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)])
-        onetime = None
-        if training:                                                # [N, layers, H]
-            onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
-            if N == 1:
-                onetime = [onetime[0][0], onetime[1][0]]
-        return self._host_result(False, N == 1, onetime)
-
-    def _act_pixel(self, obs, eps=None):
-        """act() on uint8 frames [N, C, H, W] (device tensor or numpy): CNN stem -> actor head -> sampling kernel
-        (ppo_net.py:268-273,368-375; ppo_agent.py:138-149)."""
-        N = self.num_envs
-        m, stem = self.model, self.model.cnn_stem
-        fr = obs['pixel']['camera0'] if isinstance(obs, dict) else obs
-        host = not isinstance(fr, torch.Tensor)
-        if host:
-            if self._obs_pin is None:
-                self._obs_pin = torch.empty(N, stem.C, stem.H, stem.W, dtype=torch.uint8, pin_memory=True)
-                self._frames_dev = torch.empty(N, stem.C, stem.H, stem.W, dtype=torch.uint8, device=self.device)
-            self._obs_pin.numpy()[...] = np.asarray(fr, dtype=np.uint8).reshape(N, stem.C, stem.H, stem.W)
-            self._frames_dev.copy_(self._obs_pin, non_blocking=True)
-            fr = self._frames_dev
-        fr = fr.reshape(N, stem.C, stem.H, stem.W)
-        if getattr(self, '_stem_bufs', None) is None:
-            self._stem_bufs = stem.buffers(N)
-        feat = stem.forward(fr, self._stem_bufs)
-        ops.mlp_forward(m.actor, feat, out=self._mean)
-        self._sample(eps)
-        return self._host_result(True, False, []) if host else self._result(self._action, self._pd, [])
-
-    def _act_host(self, obs, x):
-        """act() for a HOST observation batch through sb200_ppo_act_host_f32 (H2D -> forward -> sample -> D2H -> sync
-        issued back to back from C): numpy in, numpy out, same results as the generic path."""
-        N, D = self.num_envs, self.model.low_dim
-        m, env = self.model, self.env
-        out = self._pinned_out()
-        obs_host, obs_dev = self._host_obs(x, D)
-        det = self.agent_mode in ['eval_deterministic', 'eval_deterministic_local']
-        staged = self.agent_mode == 'training' and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
-        counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
-        assign = self._assign_slots(staged, counter)
-        d = m.actor.desc()
-        zf = ops.zfilter_desc(m.z_stats, m.z_eps)
-        check(_lib.lib().sb200_ppo_act_host_f32(
-            C.byref(d), C.byref(zf), obs_host, _p(obs_dev), N, _p(self._mean), _p(m.log_var), _p(self._log_noise),
-            int(det), self.seed, _p(counter), _p(self._action), _p(self._pd), C.byref(env.windows) if staged else None,
-            int(assign), C.c_void_p(out[0].data_ptr()), C.c_void_p(out[1].data_ptr()), ops._stream()),
-            'sb200_ppo_act_host_f32')
-        self._count_step(staged, counter)
-        return self._host_result(False, self._unbatched(obs), [])
 
     def rollout_chunk_supported(self):
         """True when ``steps`` consecutive act -> env.step -> staging iterations can run as one persistent rollout

@@ -23,10 +23,6 @@ from .base import Agent
 DETERMINISTIC_MODES = ('eval_deterministic', 'eval_deterministic_local')
 
 
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
 def exploration_schedule(exploration):
     """q_agent.py:67-87: LinearSchedule(steps, final_eps, 1.0), or PiecewiseSchedule([(0, 1.0)] + zip(steps, final_eps),
     outside_value=final_eps[-1])."""
@@ -72,15 +68,13 @@ class QAgent(Agent):
             self._n_points = (len(pts) - 1) // 2
         elif self.agent_mode not in DETERMINISTIC_MODES:
             self.fixed_eps = float(lc.eval.eps)
-        N, D = self.num_envs, self.model.input_dim
+        N = self.num_envs
         self._packed = _PackedTowers(self.model.nets())
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
         self._adv, self._val = f(N, n), (f(N, 1) if self.model.dueling else None)
         self._action = f(N, 1)                                   # the record's action field: the index as a float
         self._one_hot = f(N, n)                                  # what the device env steps with
         self._action_i64 = torch.zeros(N, dtype=torch.int64, device=self.device)
-        self._obs_dev = f(N, D)
-        self._obs_pin = None
         self._act_pin = None
         self._counter = torch.zeros(1, dtype=torch.int64, device=self.device)      # T of q_agent.py:45
         self.seed = 11 + 1000003 * int(agent_id)
@@ -96,52 +90,50 @@ class QAgent(Agent):
             return self.fixed_eps
         return self.exploration.value(self.T if t is None else t)
 
-    def _sched_args(self):
-        if self._schedule is None:
-            return None, 0, self.fixed_eps
-        return _p(self._schedule), self._n_points, 0.0
-
     def act(self, obs):
-        """Device observations [N, D]: (one-hot rows [N, n_actions] for the device env, action indices [N, 1] as floats
-        for the records).  Host observations (numpy): int64 actions [N] (a scalar for one actor and a 1-D observation)."""
+        """QAgent.act for all N actors in ONE call of sb200_dqn_agent_act_f32, host and device observations alike: [H2D] ->
+        the tower forwards (packed inside a rollout chunk) -> epsilon-greedy -> [D2H, one sync].  Device observations [N, D]:
+        (one-hot rows [N, n_actions] for the device env, action indices [N, 1] as floats for the records).  Host
+        observations (numpy): int64 actions [N] (a scalar for one actor and a 1-D observation)."""
         N, D = self.num_envs, self.model.input_dim
         if self.sleep_time > 0.0:
             time.sleep(self.sleep_time)
         x = obs['low_dim']['flat_inputs'] if isinstance(obs, dict) else obs
-        if not isinstance(x, torch.Tensor):
-            return self._act_host(np.asarray(x))
-        x = x.reshape(N, D)
-        if self._in_chunk and self._packed.supported and x.stride(1) == 1:
-            # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
-            ops.mlp_forward_packed(self._packed.packs[0], x, out=self._adv)
-            if self.model.dueling:
-                ops.mlp_forward_packed(self._packed.packs[1], x, out=self._val)
+        host = not isinstance(x, torch.Tensor)
+        a = _lib.DQNAgentAct()
+        if host:
+            x = np.asarray(x)
+            a.obs_host, obs_dev = self._host_obs(x, (N, D))
+            a.obs, a.ld_obs = obs_dev.data_ptr(), D
+            if self._act_pin is None:
+                self._act_pin = torch.empty(N, dtype=torch.int64, pin_memory=True)
+            a.action_i64, a.action_host = self._action_i64.data_ptr(), self._act_pin.data_ptr()
         else:
-            self.model.forward_towers(x, self._adv, self._val)
-        sched, P, eps = self._sched_args()
-        check(_lib.lib().sb200_dqn_act_f32(_p(self._adv), self._adv.stride(0), _p(self._val), 1, N, self.n_actions, sched,
-                                           P, eps, self.seed, _p(self._counter), _p(self._action), _p(self._one_hot),
-                                           self._one_hot.stride(0), None, ops._stream()), 'sb200_dqn_act_f32')
-        self._counter += 1
-        return self._one_hot, self._action
-
-    def _act_host(self, x):
-        """act() on a HOST observation batch through sb200_dqn_act_host_f32 (H2D obs unless the wrapper already moved it
-        -> tower forwards -> epsilon-greedy -> D2H int64 actions -> one sync)."""
-        N, D = self.num_envs, self.model.input_dim
-        obs_host, obs_dev = self._host_obs(x, D)
-        if self._act_pin is None:
-            self._act_pin = torch.empty(N, dtype=torch.int64, pin_memory=True)
-        sched, P, eps = self._sched_args()
-        vd = self.model.state_net.desc() if self.model.dueling else None
+            x = x.reshape(N, D)
+            if x.stride(1) != 1:
+                x = x.contiguous()
+            a.obs, a.ld_obs = x.data_ptr(), x.stride(0)
+            a.one_hot, a.ldo = self._one_hot.data_ptr(), self._one_hot.stride(0)
+            if self._in_chunk and self._packed.supported:
+                # inside a multi-step chunk the weights are fixed: the chunk packed them once, at its top
+                a.adv_packed = self._packed.packs[0].buf.data_ptr()
+                if self.model.dueling:
+                    a.value_packed = self._packed.packs[1].buf.data_ptr()
         ad = self.model.action_net.desc()
-        check(_lib.lib().sb200_dqn_act_host_f32(
-            C.byref(ad), C.byref(vd) if vd is not None else None, obs_host, _p(obs_dev), N, _p(self._adv), _p(self._val),
-            sched, P, eps, self.seed, _p(self._counter), _p(self._action), _p(self._action_i64),
-            C.c_void_p(self._act_pin.data_ptr()), ops._stream()), 'sb200_dqn_act_host_f32')
+        vd = self.model.state_net.desc() if self.model.dueling else None
+        a.adv_net, a.value_net = C.pointer(ad), (C.pointer(vd) if vd is not None else None)
+        a.N, a.adv, a.value = N, self._adv.data_ptr(), (self._val.data_ptr() if self._val is not None else None)
+        if self._schedule is not None:
+            a.schedule, a.n_points = self._schedule.data_ptr(), self._n_points
+        else:
+            a.fixed_eps = self.fixed_eps
+        a.seed, a.act_counter, a.action = self.seed, self._counter.data_ptr(), self._action.data_ptr()
+        check(_lib.lib().sb200_dqn_agent_act_f32(C.byref(a), ops._stream()), 'sb200_dqn_agent_act_f32')
         self._counter += 1
-        a = self._act_pin.numpy().copy()
-        return a[0] if (N == 1 and x.ndim == 1) else a
+        if not host:
+            return self._one_hot, self._action
+        act = self._act_pin.numpy().copy()
+        return act[0] if (N == 1 and x.ndim == 1) else act
 
     def module_dict(self, model=None):
         return {'q_func': self.model if model is None else model}

@@ -48,6 +48,17 @@ static inline bool sb200_mlp_has_ln(const sb200_mlp* net) {
     return false;
 }
 
+// sb200_mlp_forward_f32 of the rows [rows][ldx] at x, saving only the last layer's output into out [rows][ld_out].
+static inline int sb200_forward_out(const sb200_mlp* net, const sb200_zfilter* zf, const float* x, int64_t ldx,
+                                    int64_t rows, float* out, int64_t ld_out, void* stream) {
+    const sb200_rows in = {x, nullptr, ldx, rows, 0, nullptr, 0, nullptr, 0};
+    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
+    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
+    save[net->n_layers - 1] = out;
+    lds[net->n_layers - 1] = ld_out;
+    return sb200_mlp_forward_f32(net, zf, &in, save, lds, stream);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -209,35 +209,35 @@ extern "C" int sb200_dqn_act_f32(const float* adv, int64_t lda, const float* val
                       one_hot, ldo, action_i64, (cudaStream_t)stream);
 }
 
-extern "C" int sb200_dqn_act_host_f32(const sb200_mlp* adv_net, const sb200_mlp* value_net, const float* obs_host,
-                                      float* obs_dev, int N, float* adv_dev, float* value_dev, const double* schedule,
-                                      int n_points, double fixed_eps, uint64_t seed, const int64_t* act_counter,
-                                      float* action_dev, int64_t* action_i64_dev, int64_t* action_host, void* stream) {
-    SB200_REQUIRE(adv_net != nullptr && obs_dev != nullptr && action_i64_dev != nullptr && action_host != nullptr);
-    SB200_REQUIRE((value_net == nullptr) == (value_dev == nullptr));
-    const int D = adv_net->dims[0], n = adv_net->dims[adv_net->n_layers];
-    SB200_REQUIRE(value_net == nullptr || (value_net->dims[0] == D && value_net->dims[value_net->n_layers] == 1));
-    SB200_REQUIRE(act_args_ok(adv_dev, n, value_dev, 1, N, n, schedule, n_points, fixed_eps, action_dev, nullptr, 0));
+extern "C" int sb200_dqn_agent_act_f32(const sb200_dqn_agent_act* a, void* stream) {
+    SB200_REQUIRE(a != nullptr && a->adv_net != nullptr && a->obs != nullptr);
+    const sb200_mlp* nets[2] = {a->adv_net, a->value_net};
+    const float* packs[2] = {a->adv_packed, a->value_packed};
+    float* outs[2] = {a->adv, a->value};
+    const int N = a->N, D = nets[0]->dims[0], n = nets[0]->dims[nets[0]->n_layers];
+    SB200_REQUIRE((nets[1] == nullptr) == (outs[1] == nullptr));
+    SB200_REQUIRE(nets[1] == nullptr || (nets[1]->dims[0] == D && nets[1]->dims[nets[1]->n_layers] == 1));
+    SB200_REQUIRE(packs[0] != nullptr ? (packs[1] == nullptr) == (nets[1] == nullptr) : packs[1] == nullptr);
+    SB200_REQUIRE(a->ld_obs >= D && (a->obs_host == nullptr || a->ld_obs == D));
+    SB200_REQUIRE(a->action_host == nullptr || a->action_i64 != nullptr);
+    SB200_REQUIRE(act_args_ok(outs[0], n, outs[1], 1, N, n, a->schedule, a->n_points, a->fixed_eps, a->action, a->one_hot,
+                              a->ldo));
     cudaStream_t st = (cudaStream_t)stream;
-    if (obs_host != nullptr)
-        SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (a->obs_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
     const sb200_zfilter nozf = {nullptr, 1e-5f};
-    const sb200_rows in = {obs_dev, nullptr, D, N, 0, nullptr, 0, nullptr, 0};
-    const sb200_mlp* nets[2] = {adv_net, value_net};
-    float* outs[2] = {adv_dev, value_dev};
+    const sb200_rows in = {a->obs, nullptr, a->ld_obs, N, 0, nullptr, 0, nullptr, 0};
     for (int k = 0; k < 2; ++k) {
         if (nets[k] == nullptr) continue;
-        float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
-        int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
-        save[nets[k]->n_layers - 1] = outs[k];
-        lds[nets[k]->n_layers - 1] = k == 0 ? n : 1;
-        const int rc = sb200_mlp_forward_f32(nets[k], &nozf, &in, save, lds, stream);
+        const int64_t ld = k == 0 ? n : 1;
+        const int rc = packs[k] != nullptr ? sb200_mlp_forward_packed_f32(nets[k], packs[k], &nozf, &in, outs[k], ld, stream)
+                                           : sb200_forward_out(nets[k], &nozf, a->obs, a->ld_obs, N, outs[k], ld, stream);
         if (rc != SB200_OK) return rc;
     }
-    const int rc = act_launch(adv_dev, n, value_dev, 1, N, n, schedule, n_points, fixed_eps, seed, act_counter,
-                              action_dev, nullptr, 0, action_i64_dev, st);
-    if (rc != SB200_OK) return rc;
-    SB200_CUDA(cudaMemcpyAsync(action_host, action_i64_dev, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    const int rc = act_launch(outs[0], n, outs[1], 1, N, n, a->schedule, a->n_points, a->fixed_eps, a->seed, a->act_counter,
+                              a->action, a->one_hot, a->ldo, a->action_i64, st);
+    if (rc != SB200_OK || a->action_host == nullptr) return rc;
+    SB200_CUDA(cudaMemcpyAsync(a->action_host, a->action_i64, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaStreamSynchronize(st));
     return SB200_OK;
 }

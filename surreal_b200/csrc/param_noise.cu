@@ -123,30 +123,3 @@ extern "C" int sb200_ddpg_param_noise_apply_f32(const sb200_mlp* net, int N, flo
         (unsigned long long)fetch_index, dist, state, alpha, (float)target_stddev);
     return sb200_launch_status();
 }
-
-extern "C" int sb200_ddpg_act_host_per_actor_f32(const sb200_mlp* net, int64_t actor_stride, const sb200_mlp* shared,
-                                                 float* dist, int dist_interval, sb200_param_noise_state* state,
-                                                 const float* obs_host, float* obs_dev, int N, float* mean_dev,
-                                                 const float* sigma, const double* sigma64, const float* unit_noise,
-                                                 int deterministic, uint64_t seed, const uint64_t* step_counter,
-                                                 double theta, double dt, double* ou_state, float* action_dev,
-                                                 float* action_host, void* stream) {
-    SB200_REQUIRE(net != nullptr && obs_dev != nullptr && mean_dev != nullptr && action_dev && action_host && N >= 1);
-    SB200_REQUIRE(ou_state != nullptr ? sigma64 != nullptr : sigma != nullptr);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int D = net->dims[0], A = net->dims[net->n_layers];
-    if (obs_host != nullptr)
-        SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    int rc = sb200_mlp_forward_per_actor_f32(net, actor_stride, obs_dev, D, N, mean_dev, A, shared, dist, dist_interval,
-                                             state, stream);
-    if (rc != SB200_OK) return rc;
-    if (ou_state != nullptr)
-        rc = sb200_ddpg_ou_noise_f32(mean_dev, A, sigma64, unit_noise, N, A, deterministic, seed, step_counter, theta, dt,
-                                     ou_state, action_dev, stream);
-    else
-        rc = sb200_ddpg_noise_f32(mean_dev, A, sigma, unit_noise, N, A, deterministic, seed, step_counter, action_dev, stream);
-    if (rc != SB200_OK) return rc;
-    SB200_CUDA(cudaMemcpyAsync(action_host, action_dev, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
-    SB200_CUDA(cudaStreamSynchronize(st));
-    return SB200_OK;
-}

@@ -377,13 +377,19 @@ __global__ void __launch_bounds__(RT) synth_env_window_step_kernel(
 
 }  // namespace
 
+static bool sample_args_ok(const float* mean, int64_t ldm, const float* log_var, int N, int A,
+                           const uint64_t* step_counter, const float* action, const float* pd, const sb200_windows* stage,
+                           int assign_slots) {
+    return mean && log_var && action && pd && N >= 1 && A >= 1 && ldm >= A &&
+           (stage == nullptr || (windows_ok(stage) && stage->N == N && stage->A == A)) &&
+           // the fused slot assignment advances the staging's step counter, which must be the one the draws are keyed by
+           (!assign_slots || (stage != nullptr && step_counter != nullptr && step_counter == stage->step_counter));
+}
+
 extern "C" int sb200_ppo_sample_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
                                     const float* eps, int N, int A, int deterministic, uint64_t seed, uint64_t* step_counter,
                                     float* action, float* pd, const sb200_windows* stage, int assign_slots, void* stream) {
-    SB200_REQUIRE(mean && log_var && action && pd && N >= 1 && A >= 1 && ldm >= A);
-    SB200_REQUIRE(stage == nullptr || (windows_ok(stage) && stage->N == N && stage->A == A));
-    // the fused slot assignment advances the staging's step counter, which must be the one the draws are keyed by
-    SB200_REQUIRE(!assign_slots || (stage != nullptr && step_counter != nullptr && step_counter == stage->step_counter));
+    SB200_REQUIRE(sample_args_ok(mean, ldm, log_var, N, A, step_counter, action, pd, stage, assign_slots));
     ppo_sample_kernel<<<(N * ((A + 3) / 4) + RT - 1) / RT, RT, 0, (cudaStream_t)stream>>>(
         mean, ldm, log_var, log_noise, eps, N, A, deterministic, (unsigned long long)seed,
         (const unsigned long long*)step_counter, action, pd, stage ? stage->stage_pos : nullptr,
@@ -488,132 +494,69 @@ extern "C" int sb200_ppo_window_step_f32(const sb200_windows* w, const sb200_win
 }
 
 // ------------------------------------------------------------------------------------------------
-// Host-env fast path: one C call per agent.act() / wrapper.step() with a HOST environment.  The per-step work is
-// tens of microseconds of GPU time, so the ~10 separate Python-level copy / launch calls of the generic path cost
-// more than the kernels; here the PCIe copies, launches and the single stream synchronisation are issued back to
-// back from C.  Host pointers must be pinned (cudaHostAlloc / torch pin_memory) for the copies to be asynchronous.
-extern "C" int sb200_ppo_act_host_f32(const sb200_mlp* net, const sb200_zfilter* zf, const float* obs_host,
-                                      float* obs_dev, int N, float* mean_dev, const float* log_var,
-                                      const float* log_noise, int deterministic, uint64_t seed,
-                                      uint64_t* step_counter, float* action_dev, float* pd_dev,
-                                      const sb200_windows* stage, int assign_slots, float* action_host, float* pd_host,
-                                      void* stream) {
-    SB200_REQUIRE(net != nullptr && obs_dev != nullptr && mean_dev != nullptr && N >= 1);
-    SB200_REQUIRE(action_dev && pd_dev && action_host && pd_host && step_counter);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int D = net->dims[0], A = net->dims[net->n_layers];
-    if (obs_host != nullptr)
-        SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    sb200_rows in = {};
-    in.x = obs_dev;
-    in.x_next = nullptr;
-    in.ldx = D;
-    in.rows = N;
-    in.win_n = 0;
-    in.aux = nullptr;
-    in.aux_ld = 0;
-    in.save_x = nullptr;
-    in.ld_save_x = 0;
-    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
-    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
-    save[net->n_layers - 1] = mean_dev;
-    lds[net->n_layers - 1] = A;
-    int rc = sb200_mlp_forward_f32(net, zf, &in, save, lds, stream);
-    if (rc != SB200_OK) return rc;
-    rc = sb200_ppo_sample_f32(mean_dev, A, log_var, log_noise, nullptr, N, A, deterministic, seed, step_counter, action_dev,
-                              pd_dev, stage, assign_slots, stream);
-    if (rc != SB200_OK) return rc;
-    SB200_CUDA(cudaMemcpyAsync(action_host, action_dev, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
-    SB200_CUDA(cudaMemcpyAsync(pd_host, pd_dev, (size_t)N * 2 * A * sizeof(float), cudaMemcpyDeviceToHost, st));
-    SB200_CUDA(cudaStreamSynchronize(st));
-    return SB200_OK;
-}
-
-extern "C" int sb200_ddpg_act_host_f32(const sb200_mlp* net, const float* obs_host, float* obs_dev, int N, float* mean_dev,
-                                       const float* sigma, const double* sigma64, const float* unit_noise, int deterministic,
-                                       uint64_t seed, const uint64_t* step_counter, double theta, double dt,
-                                       double* ou_state, float* action_dev, float* action_host, void* stream) {
-    SB200_REQUIRE(net != nullptr && obs_dev != nullptr && mean_dev != nullptr && action_dev && action_host && N >= 1);
-    SB200_REQUIRE(ou_state != nullptr ? sigma64 != nullptr : sigma != nullptr);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int D = net->dims[0], A = net->dims[net->n_layers];
-    if (obs_host != nullptr)
-        SB200_CUDA(cudaMemcpyAsync(obs_dev, obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-    const sb200_zfilter nozf = {nullptr, 1e-5f};
-    const sb200_rows in = {obs_dev, nullptr, D, N, 0, nullptr, 0, nullptr, 0};
-    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
-    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
-    save[net->n_layers - 1] = mean_dev;
-    lds[net->n_layers - 1] = A;
-    int rc = sb200_mlp_forward_f32(net, &nozf, &in, save, lds, stream);
-    if (rc != SB200_OK) return rc;
-    if (ou_state != nullptr)
-        rc = sb200_ddpg_ou_noise_f32(mean_dev, A, sigma64, unit_noise, N, A, deterministic, seed, step_counter, theta, dt,
-                                     ou_state, action_dev, stream);
-    else
-        rc = sb200_ddpg_noise_f32(mean_dev, A, sigma, unit_noise, N, A, deterministic, seed, step_counter, action_dev, stream);
-    if (rc != SB200_OK) return rc;
-    SB200_CUDA(cudaMemcpyAsync(action_host, action_dev, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
-    SB200_CUDA(cudaStreamSynchronize(st));
-    return SB200_OK;
-}
-
-extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
-    SB200_REQUIRE(a != nullptr && a->head != nullptr && a->layers >= 1 && a->layers <= SB200_MAX_RNN_LAYERS);
-    const bool stem = a->frames != nullptr;
-    SB200_REQUIRE(a->N >= 1 && a->D >= 1 && a->H >= 1 && a->ldh >= a->H && a->ld_xf >= a->D);
-    // stem geometry (k8 s4 then k4 s2), checked before anything is issued
+// Act entries: one C call per agent.act() for host and device observations alike.  The per-step work is tens of
+// microseconds of GPU time, so separate Python-level copy / launch calls would cost more than the kernels; here the PCIe
+// copies, launches and the single stream synchronisation are issued back to back from C, after every argument has been
+// checked.  Host pointers must be pinned (cudaHostAlloc / torch pin_memory) for the copies to be asynchronous.
+extern "C" int sb200_ppo_act_f32(const sb200_ppo_act* a, void* stream) {
+    SB200_REQUIRE(a != nullptr && a->head != nullptr && a->head->n_layers >= 1 && a->head->n_layers <= SB200_MAX_LAYERS);
+    SB200_REQUIRE(a->layers >= 0 && a->layers <= SB200_MAX_RNN_LAYERS && a->N >= 1 && a->D >= 1);
+    const bool stem = a->frames != nullptr, rnn = a->layers > 0;
+    const int N = a->N, D = a->D, H = a->H, L = a->layers, A = a->head->dims[a->head->n_layers];
+    // stem geometry (k8 s4 then k4 s2)
     const int H1 = (a->frame_h - 8) / 4 + 1, W1 = (a->frame_w - 8) / 4 + 1;
     const int H2 = (H1 - 4) / 2 + 1, W2 = (W1 - 4) / 2 + 1;
     SB200_REQUIRE(stem ? (a->fc && a->conv_w1 && a->conv_b1 && a->conv_w2 && a->conv_b2 && a->a1 && a->a2 &&
                           a->obs_host == nullptr && a->frame_c >= 1 && a->frame_h >= 8 && a->frame_w >= 8 && H1 >= 4 &&
-                          W1 >= 4 && a->fc->n_layers == 1 && a->fc->dims[0] == 32 * H2 * W2 && a->fc->dims[1] == a->D)
-                       : (a->obs && a->ld_obs >= a->D && a->frames_host == nullptr));
-    SB200_REQUIRE(a->xf && a->pre_x && a->h_out[0] && (a->layers == 1 || a->h_out[1]));
-    SB200_REQUIRE(a->h && a->c && a->h_before && a->c_before && a->mean && a->log_var && a->action && a->pd);
-    SB200_REQUIRE(a->obs_host == nullptr || a->ld_obs == a->D);
+                          W1 >= 4 && a->fc->n_layers == 1 && a->fc->dims[0] == 32 * H2 * W2 && a->fc->dims[1] == D)
+                       : (a->obs && a->ld_obs >= D && a->frames_host == nullptr));
+    SB200_REQUIRE(a->obs_host == nullptr || a->ld_obs == D);
+    SB200_REQUIRE(!(stem || rnn) || (a->xf && a->ld_xf >= D));
+    SB200_REQUIRE(a->head_packed == nullptr || !(stem || rnn));
+    SB200_REQUIRE(a->head->dims[0] == (rnn ? H : D));
+    if (rnn) {
+        SB200_REQUIRE(H >= 1 && a->ldh >= H && a->pre_x && a->h_out[0] && (L == 1 || a->h_out[1]));
+        SB200_REQUIRE(a->h && a->c && a->h_before && a->c_before);
+        for (int k = 0; k < L; ++k)
+            SB200_REQUIRE(a->ih[k] && a->whh[k] && a->bhh[k] && a->ih[k]->n_layers == 1 && a->ih[k]->dims[1] == 4 * H);
+    }
     SB200_REQUIRE(a->action_host == nullptr || a->pd_host != nullptr);
-    SB200_REQUIRE((a->h_before_host == nullptr) == (a->c_before_host == nullptr));
-    for (int k = 0; k < a->layers; ++k) SB200_REQUIRE(a->ih[k] && a->whh[k] && a->bhh[k] && a->ih[k]->dims[1] == 4 * a->H);
+    SB200_REQUIRE((a->h_before_host == nullptr) == (a->c_before_host == nullptr) && (a->h_before_host == nullptr || rnn));
+    SB200_REQUIRE(sample_args_ok(a->mean, A, a->log_var, N, A, a->step_counter, a->action, a->pd, a->stage,
+                                 a->assign_slots));
     // no LayerNorm in the recurrent policy's head, input projections or CNN stem
-    if (sb200_mlp_has_ln(a->head) || (stem && sb200_mlp_has_ln(a->fc))) return SB200_ERR_UNSUPPORTED;
-    for (int k = 0; k < a->layers; ++k)
+    if ((rnn && sb200_mlp_has_ln(a->head)) || (stem && sb200_mlp_has_ln(a->fc))) return SB200_ERR_UNSUPPORTED;
+    for (int k = 0; k < L; ++k)
         if (sb200_mlp_has_ln(a->ih[k])) return SB200_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
-    const int N = a->N, D = a->D, H = a->H, L = a->layers, A = a->head->dims[a->head->n_layers];
     const size_t cells = (size_t)L * N * H * sizeof(float);
     const sb200_zfilter nozf = {nullptr, 1e-5f};
-    float* save[SB200_MAX_LAYERS] = {nullptr, nullptr, nullptr, nullptr};
-    int64_t lds[SB200_MAX_LAYERS] = {0, 0, 0, 0};
-    int rc = SB200_OK;
-    if (stem) {
-        const size_t frame_bytes = (size_t)a->frame_c * a->frame_h * a->frame_w;
-        if (a->frames_host != nullptr)
-            SB200_CUDA(cudaMemcpyAsync(a->frames, a->frames_host, (size_t)N * frame_bytes, cudaMemcpyHostToDevice, st));
+    if (a->obs_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+    if (a->frames_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(a->frames, a->frames_host, (size_t)N * a->frame_c * a->frame_h * a->frame_w,
+                                   cudaMemcpyHostToDevice, st));
+    if (rnn) {
         SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
         SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
+    }
+    int rc = SB200_OK;
+    if (stem) {
         rc = sb200_conv_forward_f32(1, a->frames, 1, N, a->frame_c, a->frame_h, a->frame_w, a->conv_w1, a->conv_b1,
                                     1.0 / 255.0, a->a1, stream);
         if (rc != SB200_OK) return rc;
         rc = sb200_conv_forward_f32(2, a->a1, 0, N, 16, H1, W1, a->conv_w2, a->conv_b2, 1.0, a->a2, stream);
         if (rc != SB200_OK) return rc;
-        const sb200_rows fin = {a->a2, nullptr, a->fc->dims[0], N, 0, nullptr, 0, nullptr, 0};
-        save[0] = a->xf;
-        lds[0] = a->ld_xf;
-        rc = sb200_mlp_forward_f32(a->fc, &nozf, &fin, save, lds, stream);
-    } else {
-        if (a->obs_host != nullptr)
-            SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
-        SB200_CUDA(cudaMemcpyAsync(a->h_before, a->h, cells, cudaMemcpyDeviceToDevice, st));
-        SB200_CUDA(cudaMemcpyAsync(a->c_before, a->c, cells, cudaMemcpyDeviceToDevice, st));
+        rc = sb200_forward_out(a->fc, &nozf, a->a2, a->fc->dims[0], N, a->xf, a->ld_xf, stream);
+    } else if (rnn) {
         rc = sb200_rows_zfilter_f32(a->obs, D, a->ld_obs, N, 1, D, a->zf.stats, (double)a->zf.eps, a->xf, a->ld_xf, stream);
     }
     if (rc != SB200_OK) return rc;
-    sb200_rows in = {a->xf, nullptr, a->ld_xf, N, 0, nullptr, 0, nullptr, 0};
+    // the MLP policy's head reads the observation rows and applies the z-filter itself
+    const float* x = (stem || rnn) ? a->xf : a->obs;
+    int64_t ldx = (stem || rnn) ? a->ld_xf : a->ld_obs;
     for (int k = 0; k < L; ++k) {
-        save[0] = a->pre_x;
-        lds[0] = 4 * H;
-        rc = sb200_mlp_forward_f32(a->ih[k], &nozf, &in, save, lds, stream);
+        rc = sb200_forward_out(a->ih[k], &nozf, x, ldx, N, a->pre_x, 4 * H, stream);
         if (rc != SB200_OK) return rc;
         float* ho = a->h_out[(L - 1 - k) & 1];
         float* hk = a->h + (size_t)k * N * H;
@@ -621,14 +564,16 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
         rc = sb200_lstm_forward_f32(a->pre_x, a->whh[k], a->bhh[k], hk, ck, H, N, 1, H, a->ldh, ho, nullptr, nullptr, nullptr,
                                     hk, ck, stream);
         if (rc != SB200_OK) return rc;
-        in.x = ho;
-        in.ldx = a->ldh;
+        x = ho;
+        ldx = a->ldh;
     }
-    save[0] = nullptr;
-    lds[0] = 0;
-    save[a->head->n_layers - 1] = a->mean;
-    lds[a->head->n_layers - 1] = A;
-    rc = sb200_mlp_forward_f32(a->head, &nozf, &in, save, lds, stream);
+    const sb200_zfilter* zf = (stem || rnn) ? &nozf : &a->zf;
+    if (a->head_packed != nullptr) {
+        const sb200_rows in = {x, nullptr, ldx, N, 0, nullptr, 0, nullptr, 0};
+        rc = sb200_mlp_forward_packed_f32(a->head, a->head_packed, zf, &in, a->mean, A, stream);
+    } else {
+        rc = sb200_forward_out(a->head, zf, x, ldx, N, a->mean, A, stream);
+    }
     if (rc != SB200_OK) return rc;
     rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed, a->step_counter,
                               a->action, a->pd, a->stage, a->assign_slots, stream);
@@ -639,6 +584,41 @@ extern "C" int sb200_ppo_act_rnn_f32(const sb200_ppo_act_rnn* a, void* stream) {
         SB200_CUDA(cudaMemcpyAsync(a->h_before_host, a->h_before, cells, cudaMemcpyDeviceToHost, st));
         SB200_CUDA(cudaMemcpyAsync(a->c_before_host, a->c_before, cells, cudaMemcpyDeviceToHost, st));
     }
+    SB200_CUDA(cudaStreamSynchronize(st));
+    return SB200_OK;
+}
+
+extern "C" int sb200_ddpg_act_f32(const sb200_ddpg_act* a, void* stream) {
+    SB200_REQUIRE(a != nullptr && a->net != nullptr && a->net->n_layers >= 1 && a->net->n_layers <= SB200_MAX_LAYERS);
+    const int N = a->N, D = a->net->dims[0], A = a->net->dims[a->net->n_layers];
+    SB200_REQUIRE(N >= 1 && A >= 1 && a->obs && a->ld_obs >= D && (a->obs_host == nullptr || a->ld_obs == D));
+    SB200_REQUIRE(a->mean && a->action && (a->ou_state != nullptr ? a->sigma64 != nullptr : a->sigma != nullptr));
+    SB200_REQUIRE(a->forward == SB200_DDPG_FWD_FUSED || (a->forward == SB200_DDPG_FWD_PACKED && a->packed) ||
+                  (a->forward == SB200_DDPG_FWD_PER_ACTOR && a->actor_stride >= 0 && a->actor_stride % 4 == 0 &&
+                   (a->shared == nullptr || (a->dist && a->pn_state && a->dist_interval >= 1))));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (a->obs_host != nullptr)
+        SB200_CUDA(cudaMemcpyAsync(a->obs, a->obs_host, (size_t)N * D * sizeof(float), cudaMemcpyHostToDevice, st));
+    const sb200_zfilter nozf = {nullptr, 1e-5f};
+    int rc;
+    if (a->forward == SB200_DDPG_FWD_PER_ACTOR) {
+        rc = sb200_mlp_forward_per_actor_f32(a->net, a->actor_stride, a->obs, a->ld_obs, N, a->mean, A, a->shared, a->dist,
+                                             a->dist_interval, a->pn_state, stream);
+    } else if (a->forward == SB200_DDPG_FWD_PACKED) {
+        const sb200_rows in = {a->obs, nullptr, a->ld_obs, N, 0, nullptr, 0, nullptr, 0};
+        rc = sb200_mlp_forward_packed_f32(a->net, a->packed, &nozf, &in, a->mean, A, stream);
+    } else {
+        rc = sb200_forward_out(a->net, &nozf, a->obs, a->ld_obs, N, a->mean, A, stream);
+    }
+    if (rc != SB200_OK) return rc;
+    if (a->ou_state != nullptr)
+        rc = sb200_ddpg_ou_noise_f32(a->mean, A, a->sigma64, a->unit_noise, N, A, a->deterministic, a->seed, a->step_counter,
+                                     a->theta, a->dt, a->ou_state, a->action, stream);
+    else
+        rc = sb200_ddpg_noise_f32(a->mean, A, a->sigma, a->unit_noise, N, A, a->deterministic, a->seed, a->step_counter,
+                                  a->action, stream);
+    if (rc != SB200_OK || a->action_host == nullptr) return rc;
+    SB200_CUDA(cudaMemcpyAsync(a->action_host, a->action, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaStreamSynchronize(st));
     return SB200_OK;
 }

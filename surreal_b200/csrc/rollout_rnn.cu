@@ -1,6 +1,6 @@
 // Persistent rollout of the recurrent (LSTM) PPO policy: T env steps of ALL co-located actors in ONE launch.
 //
-// The per-step chain of the LSTM policy (sb200_ppo_act_rnn_f32 + the synthetic env step + sb200_ppo_window_step_f32)
+// The per-step chain of the LSTM policy (sb200_ppo_act_f32 + the synthetic env step + sb200_ppo_window_step_f32)
 // is about 9 launches per step, and every step moves each actor's [L][H] cells through HBM (copied to h_before /
 // c_before, read and rewritten by every layer, read again by the window commit) while each launch re-fetches its
 // weights from L2.  Actors are independent, so the loop over time moves inside the kernel:

@@ -414,33 +414,57 @@ def test_default_ddpg_config_host_env_end_to_end():
 
 
 def test_one_call_per_step_launch_counts():
-    """A host RNN act() launches 2 * rnn_layer + 3 kernels (z-filter, per layer input projection + LSTM step, head,
-    sample-assign) -- as many as the device-observation act(); a host wrapper step launches as many as a device one (the
-    commit kernel; the slots were assigned while sampling).  DDPG: 2 kernels per host act() and per host step."""
+    """A host act() launches as many kernels as the device-observation act(): the MLP policy 2 (head, sample-assign), the
+    RNN policy 2 * rnn_layer + 3 (z-filter, per layer input projection + LSTM step, head, sample-assign), the CNN policy 5
+    and the CNN + LSTM policy 7 (conv1, conv2, fc in place of the z-filter); a host wrapper step launches as many
+    as a device one (the commit kernel; the slots were assigned while sampling).  DDPG: 2 kernels per host act() and per
+    host step.  DQN: one kernel per tower and the epsilon-greedy kernel, host and device alike."""
     from surreal_b200 import _lib
-    from surreal_b200.agent import PPOAgent, DDPGAgent
+    from surreal_b200.agent import PPOAgent, DDPGAgent, QAgent
     from surreal_b200.replay import FIFOReplay, UniformReplay
+    from test_pixel_rnn_gpu import _cfg as pixel_cfg
+    from test_dqn_gpu import dqn_configs
     N, D, A, H = 64, 13, 3, 24
-    for layers in (1, 2):
+
+    def kernels(fn):
+        torch.cuda.synchronize()
+        _lib.reset_call_counter()
+        r = fn()
+        k = _lib.call_counter_kernels()
+        torch.cuda.synchronize()
+        return r, k
+    for layers in (0, 1, 2):
         counts = []
         for host in (True, False):
             s = Stream(N, D, 4, seed=1)
             lc, ec, sc = _rnn_configs(D, A, H, layers, N, memory_size=4 * N)
+            lc.algo.rnn.if_rnn_policy = layers > 0
             FIFOReplay(lc, ec, sc)
             ag = PPOAgent(lc, ec, sc, 0, 'training')
             ag.env = w = ag.prepare_env_agent(NumpyEnv(s, A) if host else TorchEnv(s, A))
             obs, _ = w.reset()
             a = ag.act(obs)
             obs, _, _, _ = w.step(a)                               # warm: pinned buffers and device staging exist
-            torch.cuda.synchronize()
-            _lib.reset_call_counter()
-            a = ag.act(obs)
-            k_act = _lib.call_counter_kernels()
-            _lib.reset_call_counter()
-            w.step(a)
-            k_step = _lib.call_counter_kernels()
+            a, k_act = kernels(lambda: ag.act(obs))
+            _, k_step = kernels(lambda: w.step(a))
             counts.append((k_act, k_step))
-        assert counts[0] == counts[1] == (2 * layers + 3, 1), counts
+        assert counts[0] == counts[1] == (2 * layers + 3 if layers else 2, 1), (layers, counts)
+    for rnn, want in ((False, 5), (True, 7)):
+        lc, ec, sc = pixel_cfg(2, 20, 12, A, [32, 24], [28, 20], 4, N, 'clip', 1e-4, 64, 2, 6, 1, N=N)
+        lc.algo.rnn.if_rnn_policy = rnn
+        ag = PPOAgent(lc, ec, sc, 0, 'training')
+        fr = torch.randint(0, 256, (N, 2, 20, 20), dtype=torch.uint8)
+        for obs in (fr.numpy(), fr.cuda()):
+            ag.act(obs)
+            assert kernels(lambda: ag.act(obs))[1] == want, (rnn, type(obs))
+    for dueling in (True, False):
+        lc, ec, sc = dqn_configs(D=D, dueling=dueling)
+        ec.num_envs = N
+        ag = QAgent(lc, ec, sc, 0, 'training')
+        x = torch.randn(N, D)
+        for obs in (x.numpy(), x.cuda()):
+            ag.act(obs)
+            assert kernels(lambda: ag.act(obs))[1] == (3 if dueling else 2), (dueling, type(obs))
     s = Stream(N, D, 4, seed=2)
     lc, ec, sc = ddpg_configs(D=D, A=A, n_step=3, memory_size=100, start=0)
     ec.num_envs = N
@@ -449,10 +473,6 @@ def test_one_call_per_step_launch_counts():
     ag.env = w = ag.prepare_env_agent(NumpyEnv(s, A, rew64=True))
     obs, _ = w.reset()
     obs, _, _, _ = w.step(ag.act(obs))
-    torch.cuda.synchronize()
-    _lib.reset_call_counter()
-    a = ag.act(obs)
-    assert _lib.call_counter_kernels() == 2
-    _lib.reset_call_counter()
-    w.step(a)
-    assert _lib.call_counter_kernels() == 2
+    a, k = kernels(lambda: ag.act(obs))
+    assert k == 2
+    assert kernels(lambda: w.step(a))[1] == 2

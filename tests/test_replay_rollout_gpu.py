@@ -479,7 +479,7 @@ def test_host_env_actor_loop_stages_windows_in_hbm():
     torch.cuda.synchronize()
     st = R._read_state()
     assert st['count'] == N * (T // n) and int(w.step_counter.item()) == T
-    # the one-call host path (sb200_ppo_act_host_f32) and the generic device-tensor path compute the same policy output
+    # numpy and device-tensor observations, through the same act entry, give the same policy output
     ag.agent_mode = 'eval_deterministic'
     o = env._obs(3)
     np.testing.assert_array_equal(ag.act(o), ag.act(torch.tensor(o, device=DEV)).cpu().numpy().astype(np.float64))
