@@ -8,6 +8,8 @@ snapshot into this agent's own model, so between fetches the actors run lagged w
 Surreal's do (fetch cadence: session_config.agent.fetch_parameter_mode/interval, base.py:182-207)."""
 import time
 
+import numpy as np
+
 from .. import utils as U
 from ..distributed import ParameterClient, ModuleDict, LocalHub
 
@@ -39,7 +41,6 @@ class Agent(metaclass=U.AutoInitializeMeta):
         self.actions_since_param_update = 0
         self.episodes_since_param_update = 0
         self.env = None
-        self._obs_pin = self._obs_dev = None   # host observations' pinned staging and device copy (_host_obs)
         self._rollout_graphs = {}
         self._in_chunk = False                 # True while main_loop() records / runs a multi-step chunk
 
@@ -157,27 +158,16 @@ class Agent(metaclass=U.AutoInitializeMeta):
         self._obs = obs
         self.post_episode()
 
-    def _host_obs(self, x, shape, dtype='float32'):
+    def _host_obs(self, x, shape, dtype=np.float32):
         """(host pointer, device buffer) of a numpy observation batch ``x`` ([N, D] rows, or uint8 frames) for the one-call
         act entries: (None, the wrapper's device copy) when the wrapper already uploaded this very array
-        (``cached_device_obs``), else ``x`` itself when it lives in pinned memory, else a pinned staging copy of it; the
-        entry uploads into ``self._obs_dev``."""
-        import numpy as np
-        import torch
+        (``cached_device_obs``), else the address the entry uploads from (staging.Staging.host_ptr) and the buffer it
+        uploads into."""
         env = self.env
         cached = env.cached_device_obs(x) if hasattr(env, 'cached_device_obs') else None
         if cached is not None:
             return None, cached
-        if self._obs_dev is None:
-            t = torch.from_numpy(np.empty(0, dtype)).dtype
-            self._obs_pin = torch.empty(shape, dtype=t, pin_memory=True)
-            self._obs_dev = torch.empty(shape, dtype=t, device=self.device)
-        src = x if (x.dtype == dtype and x.flags['C_CONTIGUOUS'] and x.flags['WRITEABLE'] and
-                    torch.from_numpy(x).is_pinned()) else None
-        if src is None:
-            self._obs_pin.numpy()[...] = np.asarray(x, dtype=dtype).reshape(shape)
-            src = self._obs_pin.numpy()
-        return src.ctypes.data, self._obs_dev
+        return self._staging.host_ptr('obs', x, shape, dtype), self._staging.device('obs', shape, dtype)
 
     def _device_resident(self, obs):
         """The chunked path needs every buffer of the step to live at a fixed device address: true for the in-tree

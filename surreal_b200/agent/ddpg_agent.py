@@ -24,16 +24,14 @@ from .. import _lib, ops
 from .._lib import check
 from ..model.ddpg_net import DDPGModel
 from ..env import ExpSenderWrapperSSARNStepBootstrap
+from ..ops import _ptr
 from ..session import ConfigError
+from ..staging import Staging
 from .base import Agent
 
 
 PARAM_NOISE_TYPES = ('normal', 'adaptive_normal')
 PARAM_NOISE_DIST_INTERVAL = 10          # AdaptiveNormalParameterNoise(compute_dist_interval=10), param_noise.py:31
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def param_noise_stride(actor_size):
@@ -48,6 +46,7 @@ class DDPGAgent(Agent):
         if not torch.cuda.is_available():
             raise RuntimeError('surreal_b200.DDPGAgent needs a CUDA device (there is no CPU fallback)')
         self.device = torch.device('cuda', torch.cuda.current_device())
+        self._staging = Staging(self.device)
         self.action_dim = self.env_config.action_spec.dim[0]
         self.obs_spec = self.env_config.obs_spec
         self.use_layernorm = self.learner_config.model.use_layernorm
@@ -118,8 +117,8 @@ class DDPGAgent(Agent):
             un = torch.from_numpy(z).to(self.device)
         d = actor.desc()
         check(_lib.lib().sb200_ddpg_param_noise_apply_f32(
-            C.byref(d), N, _p(self._pn_images), self.param_noise_stride, _p(self._pn_sigma), _p(un), self.seed,
-            self._pn_fetches, _p(self._pn_dist), _p(self._pn_state), self.param_noise_alpha,
+            C.byref(d), N, _ptr(self._pn_images), self.param_noise_stride, _ptr(self._pn_sigma), _ptr(un), self.seed,
+            self._pn_fetches, _ptr(self._pn_dist), _ptr(self._pn_state), self.param_noise_alpha,
             self.param_noise_target_stddev, ops._stream()), 'sb200_ddpg_param_noise_apply_f32')
         self._pn_fetches += 1
         if not self._pn_applied:
@@ -157,9 +156,7 @@ class DDPGAgent(Agent):
             x = np.asarray(x)
             a.obs_host, obs_dev = self._host_obs(x, (N, D))
             a.obs, a.ld_obs = obs_dev.data_ptr(), D
-            if getattr(self, '_act_pin', None) is None:
-                self._act_pin = torch.empty(N, A, dtype=torch.float32, pin_memory=True)
-            a.action_host = self._act_pin.data_ptr()
+            a.action_host = self._staging.pinned('action', (N, A)).data_ptr()
         else:
             x = x.reshape(N, D)
             if x.stride(1) != 1:
@@ -194,7 +191,7 @@ class DDPGAgent(Agent):
             self._counter += 1
         if not host:
             return self._action
-        act = self._act_pin.numpy().copy()
+        act = self._staging.pinned('action', (N, A)).numpy().copy()
         return act.reshape(-1) if (N == 1 and x.ndim == 1) else act
 
     def pre_episode(self):

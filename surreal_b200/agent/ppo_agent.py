@@ -14,11 +14,8 @@ from .. import _lib, ops
 from .._lib import check
 from ..model.ppo_net import PPOModel, DiagGauss
 from ..env import ExpSenderWrapperMultiStepMovingWindowWithInfo
+from ..staging import Staging
 from .base import Agent
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 class PPOAgent(Agent):
@@ -28,6 +25,7 @@ class PPOAgent(Agent):
         if not torch.cuda.is_available():
             raise RuntimeError('surreal_b200.PPOAgent needs a CUDA device (there is no CPU fallback)')
         self.device = torch.device('cuda', torch.cuda.current_device())
+        self._staging = Staging(self.device)
         self.action_dim = self.env_config.action_spec.dim[0]
         self.obs_spec = self.env_config.obs_spec
         self.use_z_filter = self.learner_config.algo.use_z_filter
@@ -55,7 +53,6 @@ class PPOAgent(Agent):
         self._packed = ops.PackedWeights(self.model.actor)          # per-step inference copy of the policy weights
         self._action = torch.zeros(N, A, device=self.device)
         self._pd = torch.zeros(N, 2 * A, device=self.device)
-        self._out_pin = None
         self._counter = torch.zeros(1, dtype=torch.int64, device=self.device)
         self.seed = 2 + 1000003 * int(agent_id)
 
@@ -133,13 +130,11 @@ class PPOAgent(Agent):
         if xf is not None:
             a.xf, a.ld_xf = xf.data_ptr(), xf.stride(0)
         if host:
-            out = self._pinned_out()
-            a.action_host, a.pd_host = out[0].data_ptr(), out[1].data_ptr()
+            st = self._staging
+            a.action_host, a.pd_host = st.pinned('action', (N, A)).data_ptr(), st.pinned('pd', (N, 2 * A)).data_ptr()
             if training and stem is not None:
-                if getattr(self, '_cells_pin', None) is None:
-                    self._cells_pin = (torch.empty(L, N, H, dtype=torch.float32, pin_memory=True),
-                                       torch.empty(L, N, H, dtype=torch.float32, pin_memory=True))
-                a.h_before_host, a.c_before_host = self._cells_pin[0].data_ptr(), self._cells_pin[1].data_ptr()
+                a.h_before_host = st.pinned('h_before', (L, N, H)).data_ptr()
+                a.c_before_host = st.pinned('c_before', (L, N, H)).data_ptr()
         head = m.actor.desc()
         a.head = C.pointer(head)
         a.zf = ops.zfilter_desc(m.z_stats, m.z_eps)
@@ -167,7 +162,8 @@ class PPOAgent(Agent):
             return self._result(self._action, self._pd, [self._hs_before.transpose(0, 1), self._cs_before.transpose(0, 1)])
         onetime = None
         if training:                                                # [N, layers, H]
-            onetime = [self._cells_pin[0].numpy().transpose(1, 0, 2).copy(), self._cells_pin[1].numpy().transpose(1, 0, 2).copy()]
+            onetime = [self._staging.pinned(k, (L, N, H)).numpy().transpose(1, 0, 2).copy()
+                       for k in ('h_before', 'c_before')]
             if N == 1:
                 onetime = [onetime[0][0], onetime[1][0]]
         return self._host_result(N == 1, onetime)
@@ -190,18 +186,12 @@ class PPOAgent(Agent):
         if not staged and counter is self._counter:
             self._counter += 1
 
-    def _pinned_out(self):
-        if self._out_pin is None:
-            N, A = self.num_envs, self.action_dim
-            self._out_pin = (torch.empty(N, A, dtype=torch.float32, pin_memory=True),
-                             torch.empty(N, 2 * A, dtype=torch.float32, pin_memory=True))
-        return self._out_pin
-
     def _host_result(self, single, onetime):
         """act()'s numpy result from the pinned outputs the C call has filled: float64 actions, as the reference hands the
         env (ppo_net.py:83); ``single``: one actor's unbatched observation gives unbatched results."""
-        out = self._pinned_out()
-        action, pd = out[0].numpy().astype(np.float64), out[1].numpy().copy()
+        N, A = self.num_envs, self.action_dim
+        action = self._staging.pinned('action', (N, A)).numpy().astype(np.float64)
+        pd = self._staging.pinned('pd', (N, 2 * A)).numpy().copy()
         if single:
             action, pd = action.reshape(-1), pd.reshape(-1)
         return self._result(action, pd, onetime)
@@ -324,7 +314,7 @@ class PPOAgent(Agent):
             a.D = w.D                              # the records carry the cells: [obs | h | c]
         else:
             check(L.sb200_ppo_rollout_f32(C.byref(a), st), 'sb200_ppo_rollout_f32')
-        check(L.sb200_ppo_rollout_commit_f32(C.byref(a), _p(ob['scratch']), st), 'sb200_ppo_rollout_commit_f32')
+        check(L.sb200_ppo_rollout_commit_f32(C.byref(a), ops._ptr(ob['scratch']), st), 'sb200_ppo_rollout_commit_f32')
         return True
 
     def module_dict(self):

@@ -18,6 +18,7 @@ from .._lib import check
 from ..env import ExpSenderWrapperSSARNStepBootstrap
 from ..learner.dqn import check_dqn_config
 from ..model.q_net import QModel
+from ..staging import Staging
 from .base import Agent
 
 DETERMINISTIC_MODES = ('eval_deterministic', 'eval_deterministic_local')
@@ -54,6 +55,7 @@ class QAgent(Agent):
             raise RuntimeError('surreal_b200.QAgent needs a CUDA device (there is no CPU fallback)')
         check_dqn_config(self.learner_config, self.env_config)
         self.device = torch.device('cuda', torch.cuda.current_device())
+        self._staging = Staging(self.device)
         self.sleep_time = self.env_config.sleep_time
         self.n_actions = n = int(self.env_config.action_spec.dim[0])
         lc = self.learner_config
@@ -75,7 +77,6 @@ class QAgent(Agent):
         self._action = f(N, 1)                                   # the record's action field: the index as a float
         self._one_hot = f(N, n)                                  # what the device env steps with
         self._action_i64 = torch.zeros(N, dtype=torch.int64, device=self.device)
-        self._act_pin = None
         self._counter = torch.zeros(1, dtype=torch.int64, device=self.device)      # T of q_agent.py:45
         self.seed = 11 + 1000003 * int(agent_id)
 
@@ -105,9 +106,8 @@ class QAgent(Agent):
             x = np.asarray(x)
             a.obs_host, obs_dev = self._host_obs(x, (N, D))
             a.obs, a.ld_obs = obs_dev.data_ptr(), D
-            if self._act_pin is None:
-                self._act_pin = torch.empty(N, dtype=torch.int64, pin_memory=True)
-            a.action_i64, a.action_host = self._action_i64.data_ptr(), self._act_pin.data_ptr()
+            a.action_i64 = self._action_i64.data_ptr()
+            a.action_host = self._staging.pinned('action', (N,), np.int64).data_ptr()
         else:
             x = x.reshape(N, D)
             if x.stride(1) != 1:
@@ -132,7 +132,7 @@ class QAgent(Agent):
         self._counter += 1
         if not host:
             return self._one_hot, self._action
-        act = self._act_pin.numpy().copy()
+        act = self._staging.pinned('action', (N,), np.int64).numpy().copy()
         return act[0] if (N == 1 and x.ndim == 1) else act
 
     def module_dict(self, model=None):

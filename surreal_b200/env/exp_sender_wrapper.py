@@ -7,22 +7,16 @@ that copies the record into the HBM replay's ring in (step, actor) order, and th
 overlapping windows (exp_sender.py:10-59) has nothing left to do."""
 import ctypes as C
 
+import numpy as np
 import torch
 
 from .. import _lib
 from .._lib import check
 from ..distributed import LocalHub
+from ..ops import _ptr, _stream
 from ..session import ConfigError
+from ..staging import Staging
 from ..utils import obs_flat, obs_source, record_action_dim
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def _st():
-    from ..ops import _stream
-    return _stream()
 
 
 class _WrapperBase:
@@ -43,49 +37,10 @@ class _WrapperBase:
         # a batched HOST env (numpy in / numpy out, attributes N, D, A) has no device: the staging lives with the replay
         self.device = env.device if hasattr(env, 'device') else self.replay.device
         self.host_env = not hasattr(env, 'device')
-        self._pins, self._devs = {}, {}
+        self._staging = Staging(self.device)            # host rows' pinned copies and their device landing buffers
         self._last_obs_host, self._last_obs_dev = None, None
         if not hasattr(env, 'step_counter'):
             self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)   # Philox step counter
-
-    def _h2d(self, name, arr, shape):
-        """numpy -> device through a persistent pinned staging buffer (skipped when ``arr`` already is pinned)."""
-        import numpy as np
-        dev = self._devs.get(name)
-        if dev is None:
-            dev = self._devs[name] = torch.zeros(*shape, dtype=torch.float32, device=self.device)
-        src = None
-        if isinstance(arr, np.ndarray) and arr.dtype == np.float32 and arr.flags['C_CONTIGUOUS'] and arr.flags['WRITEABLE']:
-            t = torch.from_numpy(arr)
-            if t.is_pinned():
-                src = t.view(*shape)
-        if src is None:
-            pin = self._pins.get(name)
-            if pin is None:
-                pin = self._pins[name] = torch.empty(*shape, dtype=torch.float32, pin_memory=True)
-            pin.numpy()[...] = np.asarray(arr, dtype=np.float32).reshape(shape)
-            src = pin
-        dev.copy_(src, non_blocking=True)
-        return dev
-
-    def _dev(self, name, shape, dtype=torch.float32):
-        dev = self._devs.get(name)
-        if dev is None:
-            dev = self._devs[name] = torch.zeros(*shape, dtype=dtype, device=self.device)
-        return dev
-
-    def _pinned(self, name, arr, shape, dtype=torch.float32):
-        """Address (c_void_p) of ``arr`` if it already lives in pinned memory, else of a pinned staging copy."""
-        import numpy as np
-        npt = np.float64 if dtype == torch.float64 else np.float32
-        if isinstance(arr, np.ndarray) and arr.dtype == npt and arr.flags['C_CONTIGUOUS'] and arr.flags['WRITEABLE'] \
-                and torch.from_numpy(arr).is_pinned():
-            return C.c_void_p(arr.ctypes.data)
-        pin = self._pins.get(name)
-        if pin is None:
-            pin = self._pins[name] = torch.empty(*shape, dtype=dtype, pin_memory=True)
-        pin.numpy()[...] = np.asarray(arr, dtype=npt).reshape(shape)
-        return C.c_void_p(pin.data_ptr())
 
     def cached_device_obs(self, obs_arr):
         """The device copy of the observation the last step() returned (the agent's next act() input), if
@@ -144,7 +99,8 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         o = obs_flat(obs)
         row0 = self.stage_obs[:, 0]
         if self.host_env:
-            d = self._h2d('obs', o, (self.N, self.obs_dim))
+            d = self._staging.device('obs', (self.N, self.obs_dim))
+            self._staging.upload('obs', o, d)
             row0[:, :self.obs_dim].copy_(d)
             self._last_obs_host, self._last_obs_dev = obs_source(obs), d
         else:
@@ -198,16 +154,18 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
             # host env: this step's successor observation / reward / done cross PCIe (uint8 frames as their 32-bit words),
             # issued with the staging kernels from ONE C call; the device copy of the next observation is handed to the
             # agent's next act() (cached_device_obs, keyed by the array the env returned)
-            rows.obs_reset_host = self._pinned('obs', o, (N, Do))
-            rows.obs_next_host = rows.obs_reset_host if on is o else self._pinned('obs_next', on, (N, Do))
-            rows.reward_host, rows.done_host = self._pinned('rew', reward, (N,)), self._pinned('done', done, (N,))
-            d_o = self._dev('obs', (N, Do))
-            rows.obs_reset, rows.obs_next = d_o.data_ptr(), self._dev('obs_next', (N, Do)).data_ptr()
-            rows.reward, rows.done = self._dev('rew', (N,)).data_ptr(), self._dev('done', (N,)).data_ptr()
+            st = self._staging
+            rows.obs_reset_host = st.host_ptr('obs', o, (N, Do))
+            rows.obs_next_host = rows.obs_reset_host if on is o else st.host_ptr('obs_next', on, (N, Do))
+            rows.reward_host, rows.done_host = st.host_ptr('rew', reward, (N,)), st.host_ptr('done', done, (N,))
+            d_o = st.device('obs', (N, Do))
+            rows.obs_reset, rows.obs_next = d_o.data_ptr(), st.device('obs_next', (N, Do)).data_ptr()
+            rows.reward, rows.done = st.device('rew', (N,)).data_ptr(), st.device('done', (N,)).data_ptr()
         else:
             rows.obs_next, rows.obs_reset, rows.reward, rows.done = on.data_ptr(), o.data_ptr(), reward.data_ptr(), done.data_ptr()
         rows.slots_assigned, rows.force_wide = int(ready), int(self.wide_commit)
-        check(_lib.lib().sb200_ppo_window_step_f32(C.byref(self.windows), C.byref(rows), _st()), 'sb200_ppo_window_step_f32')
+        check(_lib.lib().sb200_ppo_window_step_f32(C.byref(self.windows), C.byref(rows), _stream()),
+              'sb200_ppo_window_step_f32')
         if self.host_env:
             self._last_obs_host, self._last_obs_dev = obs_source(obs), d_o
         return obs, reward, done, info
@@ -239,9 +197,8 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         obs, info = self.env.reset()
         self.dq_len.zero_()
         if self.host_env:
-            import numpy as np
             o = obs_flat(obs)
-            self._obs.copy_(torch.from_numpy(np.ascontiguousarray(o, dtype=np.float32)).view(self.N, self.D))
+            self._staging.upload('obs', o, self._obs)
             self._last_obs_host, self._last_obs_dev = o, self._obs
         else:
             self._obs.copy_(obs['low_dim']['flat_inputs'])
@@ -256,8 +213,8 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         if self.host_env:
             self._step_host(obs, action, reward, done, info)
             return obs, reward, done, info
-        check(_lib.lib().sb200_ssar_step_f32(C.byref(self.ssar), _p(self._obs), _p(action), _p(info['obs_next']), _p(reward),
-                                             _p(done), _st()), 'sb200_ssar_step_f32')
+        check(_lib.lib().sb200_ssar_step_f32(C.byref(self.ssar), _ptr(self._obs), _ptr(action), _ptr(info['obs_next']),
+                                             _ptr(reward), _ptr(done), _stream()), 'sb200_ssar_step_f32')
         self.replay.mark_device_inserts()
         self._obs.copy_(obs['low_dim']['flat_inputs'])             # s_t of the next transition (reset obs where done)
         return obs, reward, done, info
@@ -269,11 +226,13 @@ class ExpSenderWrapperSSARNStepBootstrap(_WrapperBase):
         N, D, A = self.N, self.D, self.A
         o = obs_flat(obs)
         on = info['obs_next'] if (isinstance(info, dict) and 'obs_next' in info) else o
-        h_o = self._pinned('obs', o, (N, D))
-        h_on = h_o if on is o else self._pinned('obs_next', on, (N, D))
+        st = self._staging
+        h_o = st.host_ptr('obs', o, (N, D))
+        h_on = h_o if on is o else st.host_ptr('obs_next', on, (N, D))
         check(_lib.lib().sb200_ssar_step_host_f32(
-            C.byref(self.ssar), h_on, h_o, self._pinned('act', action, (N, A)), self._pinned('rew', reward, (N,), torch.float64),
-            self._pinned('done', done, (N,)), _p(self._obs), _p(self._dev('obs_next', (N, D))), _p(self._dev('act', (N, A))),
-            _p(self._dev('rew', (N,), torch.float64)), _p(self._dev('done', (N,))), _st()), 'sb200_ssar_step_host_f32')
+            C.byref(self.ssar), h_on, h_o, st.host_ptr('act', action, (N, A)), st.host_ptr('rew', reward, (N,), np.float64),
+            st.host_ptr('done', done, (N,)), _ptr(self._obs), _ptr(st.device('obs_next', (N, D))),
+            _ptr(st.device('act', (N, A))), _ptr(st.device('rew', (N,), np.float64)), _ptr(st.device('done', (N,))),
+            _stream()), 'sb200_ssar_step_host_f32')
         self.replay.mark_device_inserts()
         self._last_obs_host, self._last_obs_dev = o, self._obs

@@ -12,11 +12,7 @@ import torch
 
 from .. import _lib
 from .._lib import check
-from ..ops import _stream
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+from ..ops import _ptr, _stream
 
 
 class SyntheticEnv:
@@ -61,8 +57,8 @@ class SyntheticEnv:
         if isinstance(action, tuple):
             action = action[0]
         check(_lib.lib().sb200_synth_env_step_f32(
-            _p(self.state), _p(action), _p(self.WsT), _p(self.WaT), self.N, self.D, self.A, self.max_steps,
-            _p(self.ep_step), self.seed + 7, _p(self.step_counter), _p(self.obs_next), _p(self.reward), _p(self.done),
+            _ptr(self.state), _ptr(action), _ptr(self.WsT), _ptr(self.WaT), self.N, self.D, self.A, self.max_steps,
+            _ptr(self.ep_step), self.seed + 7, _ptr(self.step_counter), _ptr(self.obs_next), _ptr(self.reward), _ptr(self.done),
             _stream()), 'sb200_synth_env_step_f32')
         return {'low_dim': {'flat_inputs': self.state}}, self.reward, self.done, {'obs_next': self.obs_next}
 
@@ -70,8 +66,8 @@ class SyntheticEnv:
         """step() fused with the commit half of ExpSenderWrapperMultiStepMovingWindowWithInfo.step (``w``), for
         steps whose replay slots the sampling kernel has already assigned."""
         check(_lib.lib().sb200_synth_env_window_step_f32(
-            _p(self.state), _p(action), _p(self.WsT), _p(self.WaT), self.N, self.D, self.A, self.max_steps,
-            _p(self.ep_step), self.seed + 7, _p(self.step_counter), _p(self.obs_next), _p(self.reward), _p(self.done),
+            _ptr(self.state), _ptr(action), _ptr(self.WsT), _ptr(self.WaT), self.N, self.D, self.A, self.max_steps,
+            _ptr(self.ep_step), self.seed + 7, _ptr(self.step_counter), _ptr(self.obs_next), _ptr(self.reward), _ptr(self.done),
             C.byref(w.windows), _stream()), 'sb200_synth_env_window_step_f32')
         return {'low_dim': {'flat_inputs': self.state}}, self.reward, self.done, {'obs_next': self.obs_next}
 
@@ -138,8 +134,8 @@ class SyntheticPixelEnv:
         if isinstance(action, tuple):
             action = action[0]
         check(_lib.lib().sb200_synth_pixel_env_step_u8(
-            _p(self.state), _p(action), self.N, self.frame_bytes, self.A, self.max_steps, _p(self.ep_step), self.seed + 7,
-            _p(self.step_counter), _p(self.obs_next), _p(self.reward), _p(self.done), _stream()), 'sb200_synth_pixel_env_step_u8')
+            _ptr(self.state), _ptr(action), self.N, self.frame_bytes, self.A, self.max_steps, _ptr(self.ep_step), self.seed + 7,
+            _ptr(self.step_counter), _ptr(self.obs_next), _ptr(self.reward), _ptr(self.done), _stream()), 'sb200_synth_pixel_env_step_u8')
         return self._obs(self.state), self.reward, self.done, {'obs_next': self._obs(self.obs_next)}
 
     def close(self):

@@ -11,6 +11,7 @@ import torch
 from .. import _lib, ops
 from .._lib import check
 from ..ops import _ptr
+from ..staging import Staging
 from .base import Learner
 
 _HEAD = 16                          # read-back block: int64 target counter [0:8], int32 stop flag [8:12], statistics [16:]
@@ -32,7 +33,7 @@ class OffPolicyLearner(Learner):
                          dones=f(B, 1))
         self._w = f(B, 1)                                      # learn(): the batch's importance weights
         self._prio = f(B)
-        self._pin = {}
+        self._staging = Staging(self.device)              # numpy batches: pinned copies of ``_own``
         self._bad = workspace[bad_offset:bad_offset + 4].view(torch.int32)
         self._block = torch.zeros(_HEAD + 4 * n_stats, dtype=torch.uint8, device=self.device)
         self._counter = self._block[0:8].view(torch.int64)
@@ -52,21 +53,7 @@ class OffPolicyLearner(Learner):
         flat = lambda o: o['low_dim']['flat_inputs'] if isinstance(o, dict) else o  # noqa: E731
         src = dict(obs=flat(get('obs')), obs_next=flat(get('obs_next')), actions=get('actions'),
                    rewards=get('rewards'), dones=get('dones'))
-        nbytes = 0
-        for k, v in src.items():
-            dst = self._own[k]
-            if isinstance(v, torch.Tensor):
-                if v.data_ptr() != dst.data_ptr():
-                    dst.copy_(v.reshape(dst.shape), non_blocking=True)
-                    if not v.is_cuda:
-                        nbytes += dst.numel() * 4
-                continue
-            if k not in self._pin:
-                self._pin[k] = torch.empty(dst.shape, dtype=torch.float32, pin_memory=True)
-            self._pin[k].numpy()[...] = np.asarray(v).reshape(tuple(dst.shape))
-            dst.copy_(self._pin[k], non_blocking=True)
-            nbytes += dst.numel() * 4
-        self.last_h2d_bytes = nbytes
+        self.last_h2d_bytes = sum(self._staging.upload(k, v, self._own[k]) for k, v in src.items())
         return batch
 
     def replay_out_buffers(self):

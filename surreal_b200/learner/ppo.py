@@ -19,6 +19,7 @@ from ..model.ppo_net import PPOModel, DiagGauss
 from ..model.stem_chain import ChainTrainer, StemChain
 from ..ops import _ptr
 from ..session import ConfigError
+from ..staging import Staging
 from .aggregator import MultistepAggregatorWithInfo
 from .base import Learner
 from .scheduler import make_lr_scheduler
@@ -173,7 +174,7 @@ class PPOLearner(Learner):
         self._side_stream = None
         self._rfilter_stats = torch.tensor([1e-5, 0.0, 0.0], dtype=torch.float32, device=dev) \
             if self.use_r_filter else None
-        self._pin = {}
+        self._staging = Staging(dev)                     # numpy batches: pinned copies of the fields above
         self._gae_ws = torch.zeros(int(L.sb200_gae_workspace_bytes(B, n, n)), dtype=torch.uint8, device=dev)
         self.use_cuda_graph = ops.graphs_enabled()
         # policy || value epochs as concurrent graph branches -- not with stems, which both optimisers update
@@ -203,18 +204,6 @@ class PPOLearner(Learner):
         self._hyper.copy_(torch.tensor([getattr(self, 'clip_epsilon', 0.0), getattr(self, 'beta', 0.0)],
                                        dtype=torch.float64))
 
-    def _h2d(self, name, arr, dst):
-        """numpy -> pinned staging -> device buffer (non-blocking); CUDA tensors are copied device-side."""
-        if isinstance(arr, torch.Tensor):
-            dst.copy_(arr.reshape(dst.shape), non_blocking=True)
-            return 0 if arr.is_cuda else dst.numel() * 4
-        a = np.asarray(arr)
-        if name not in self._pin:
-            self._pin[name] = torch.empty(dst.shape, dtype=torch.float32, pin_memory=True)
-        self._pin[name].numpy()[...] = a.reshape(tuple(dst.shape))      # float64 -> float32 like torch.tensor(..)
-        dst.copy_(self._pin[name], non_blocking=True)
-        return dst.numel() * 4
-
     def _low_dim(self, obs):
         if isinstance(obs, dict):
             # the reference concatenates in obs_spec order (ppo_net.py:168-178), not in the batch dict's order
@@ -231,25 +220,13 @@ class PPOLearner(Learner):
         return isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() \
             and tuple(t.shape) == tuple(shape)
 
-    def _put_cells(self, row0, get):
-        """RNN mode: onetime_infos = [h0, c0] [B, layers, H], the cells of every window's first step, into the cell
-        columns of the records' row 0 ``row0`` (device rows, or numpy rows of the pinned staging)."""
-        cl = self.cell_layout
-        if cl is None:
-            return
-        hc, shape = get('onetime_infos'), (self.batch_size, cl.layers * cl.hidden)
-        for dst, src in ((cl.h(row0), hc[0]), (cl.c(row0), hc[1])):
-            if isinstance(dst, np.ndarray):
-                dst[...] = np.asarray(src, dtype=np.float32).reshape(shape)
-            else:
-                dst.copy_(torch.as_tensor(src).reshape(shape), non_blocking=True)
-
     def _preprocess_batch_ppo(self, batch):
         """ppo.py:420-484: everything becomes fp32 on the device.  The learner's working layout is
         obs_full [B, n+1, D] (row n = obs_next), i.e. the reference's cat([obs, obs_next], 1) (ppo.py:380)
         done once at ingest.  A device batch from the HBM replay (which already stores windows that way) is
-        used in place -- zero copies; a host batch goes through pinned staging.  Reward scaling happens inside
-        the GAE / reward-filter kernel."""
+        used in place -- zero copies; a host batch is copied into our buffers: numpy records are packed in pinned memory
+        (utils.pack_window_records) and cross in one copy, torch records are packed straight into the device buffer.
+        Reward scaling happens inside the GAE / reward-filter kernel."""
         get = (lambda k: batch[k]) if isinstance(batch, dict) else (lambda k: getattr(batch, k))
         B, n, A, D = self.batch_size, self.n_step, self.action_dim, self.low_dim
         pinfo = get('persistent_infos')
@@ -271,46 +248,27 @@ class PPOLearner(Learner):
             return batch
         self._obs_full, self._actions, self._pds = own['obs_full'], own['actions'], own['pds']
         self._rewards, self._dones = own['rewards'], own['dones']
-        nbytes = 0
-        od = self.obs_dim
+        st = self._staging
         if isinstance(full, torch.Tensor) and not full.is_cuda and tuple(full.shape) == (B, n + 1, D):
             # host batch already in the working layout (ideally pinned): one DMA, no staging copy
-            own['obs_full'].copy_(full, non_blocking=True)
-            nbytes += own['obs_full'].numel() * 4
-        elif self.pixel:
-            fo, fn = get('obs')['pixel']['camera0'], get('obs_next')['pixel']['camera0']
-            u8 = own['obs_full'].view(torch.uint8).view(B, n + 1, -1)[:, :, :4 * od]
-            self._put_cells(own['obs_full'][:, 0], get)
-            if isinstance(fo, torch.Tensor):
-                u8[:, :n].copy_(fo.reshape(B, n, -1), non_blocking=True)
-                u8[:, n:].copy_(fn.reshape(B, 1, -1), non_blocking=True)
-            else:
-                if 'frames' not in self._pin:
-                    self._pin['frames'] = torch.empty(B, n + 1, u8.shape[-1], dtype=torch.uint8, pin_memory=True)
-                pf = self._pin['frames'].numpy()
-                pf[:, :n] = np.asarray(fo, dtype=np.uint8).reshape(B, n, -1)
-                pf[:, n:] = np.asarray(fn, dtype=np.uint8).reshape(B, 1, -1)
-                u8.copy_(self._pin['frames'], non_blocking=True)
-                nbytes += u8.numel()
+            nbytes = st.upload('obs_full', full, own['obs_full'])
         else:
-            obs, obs_next = self._low_dim(get('obs')), self._low_dim(get('obs_next'))
-            if isinstance(obs, torch.Tensor):
-                own['obs_full'][:, :n, :od].copy_(obs.reshape(B, n, od), non_blocking=True)
-                own['obs_full'][:, n:, :od].copy_(obs_next.reshape(B, 1, od), non_blocking=True)
-                self._put_cells(own['obs_full'][:, 0], get)
+            if self.pixel:
+                obs, obs_next = get('obs')['pixel']['camera0'], get('obs_next')['pixel']['camera0']
             else:
-                if 'obs_full' not in self._pin:
-                    self._pin['obs_full'] = torch.zeros(B, n + 1, D, dtype=torch.float32).pin_memory()
-                pf = self._pin['obs_full'].numpy()
-                pf[:, :n, :od] = np.asarray(obs).reshape(B, n, od)
-                pf[:, n:, :od] = np.asarray(obs_next).reshape(B, 1, od)
-                self._put_cells(pf[:, 0], get)
-                own['obs_full'].copy_(self._pin['obs_full'], non_blocking=True)
-                nbytes += own['obs_full'].numel() * 4
-        nbytes += self._h2d('actions', get('actions'), own['actions'])
-        nbytes += self._h2d('rewards', get('rewards'), own['rewards'])
-        nbytes += self._h2d('dones', get('dones'), own['dones'])
-        nbytes += self._h2d('pds', pinfo[-1], own['pds'])
+                obs, obs_next = self._low_dim(get('obs')), self._low_dim(get('obs_next'))
+            cells = get('onetime_infos') if self.cell_layout is not None else None
+            nbytes = 0
+            if isinstance(obs, torch.Tensor):
+                U.pack_window_records(own['obs_full'], obs, obs_next, self.pixel, self.cell_layout, cells)
+            else:
+                rows = st.pinned('obs_full', (B, n + 1, D))
+                U.pack_window_records(rows.numpy(), obs, obs_next, self.pixel, self.cell_layout, cells)
+                nbytes = st.upload('obs_full', rows, own['obs_full'])
+        nbytes += st.upload('actions', get('actions'), own['actions'])
+        nbytes += st.upload('rewards', get('rewards'), own['rewards'])
+        nbytes += st.upload('dones', get('dones'), own['dones'])
+        nbytes += st.upload('pds', pinfo[-1], own['pds'])
         self.last_h2d_bytes = nbytes
         return batch
 

@@ -13,10 +13,7 @@ import torch
 
 from .. import _lib, ops
 from .._lib import check
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+from ..ops import _ptr
 
 
 def _conv_out(h, k, s):
@@ -95,10 +92,10 @@ class CNNStem:
         rows = frames.shape[0]
         L, st = _lib.lib(), ops._stream()
         P = self.params if params is None else params
-        check(L.sb200_conv_forward_f32(1, _p(frames), 1, rows, self.C, self.H, self.W, _p(self.seg('w1', P)), _p(self.seg('b1', P)),
-                                       1.0 / 255.0, _p(bufs['a1']), st), 'sb200_conv_forward_f32(1)')
-        check(L.sb200_conv_forward_f32(2, _p(bufs['a1']), 0, rows, self.C1, self.H1, self.W1, _p(self.seg('w2', P)),
-                                       _p(self.seg('b2', P)), 1.0, _p(bufs['a2']), st), 'sb200_conv_forward_f32(2)')
+        check(L.sb200_conv_forward_f32(1, _ptr(frames), 1, rows, self.C, self.H, self.W, _ptr(self.seg('w1', P)), _ptr(self.seg('b1', P)),
+                                       1.0 / 255.0, _ptr(bufs['a1']), st), 'sb200_conv_forward_f32(1)')
+        check(L.sb200_conv_forward_f32(2, _ptr(bufs['a1']), 0, rows, self.C1, self.H1, self.W1, _ptr(self.seg('w2', P)),
+                                       _ptr(self.seg('b2', P)), 1.0, _ptr(bufs['a2']), st), 'sb200_conv_forward_f32(2)')
         ops.mlp_forward(self.fc, bufs['a2'], params=self.seg('fc', P), out=bufs['feat'])
         return bufs['feat']
 
@@ -132,19 +129,19 @@ class StemTrainer:
         o_fc = s.off['fc'][0]
         lay = s.fc.layout[0]
         # Linear: dW / db into the slabs, dX (times relu'(a2)) -> conv2's pre-activation gradient
-        check(L.sb200_linear_bwd_dw_f32(_p(b['a2']), b['a2'].stride(0), _p(d_feat_pre), d_feat_pre.stride(0),
+        check(L.sb200_linear_bwd_dw_f32(_ptr(b['a2']), b['a2'].stride(0), _ptr(d_feat_pre), d_feat_pre.stride(0),
                                         C.c_void_p(base + 4 * (o_fc + lay['w'])), C.c_void_p(base + 4 * (o_fc + lay['b'])),
                                         s.size, self.splits, lay['ldw'], M, s.flat, s.d_out, st), 'sb200_linear_bwd_dw_f32(stem fc)')
-        check(L.sb200_linear_bwd_dx_f32(_p(d_feat_pre), d_feat_pre.stride(0), C.c_void_p(s.fc.params.data_ptr() + 4 * lay['w']),
-                                        lay['ldw'], _p(b['a2']), b['a2'].stride(0), _p(self.d_a2), self.d_a2.stride(0), M, s.d_out,
+        check(L.sb200_linear_bwd_dx_f32(_ptr(d_feat_pre), d_feat_pre.stride(0), C.c_void_p(s.fc.params.data_ptr() + 4 * lay['w']),
+                                        lay['ldw'], _ptr(b['a2']), b['a2'].stride(0), _ptr(self.d_a2), self.d_a2.stride(0), M, s.d_out,
                                         s.flat, st), 'sb200_linear_bwd_dx_f32(stem fc)')
         o_w2, o_b2 = s.off['w2'][0], s.off['b2'][0]
-        check(L.sb200_conv_backward_dw_f32(2, _p(b['a1']), 0, _p(self.d_a2), M, s.C1, s.H1, s.W1, 1.0, C.c_void_p(base + 4 * o_w2),
+        check(L.sb200_conv_backward_dw_f32(2, _ptr(b['a1']), 0, _ptr(self.d_a2), M, s.C1, s.H1, s.W1, 1.0, C.c_void_p(base + 4 * o_w2),
                                            C.c_void_p(base + 4 * o_b2), s.size, self.splits, st), 'sb200_conv_backward_dw_f32(2)')
-        check(L.sb200_conv_backward_dx_f32(2, _p(self.d_a2), _p(s.seg('w2')), _p(b['a1']), M, s.C1, s.H1, s.W1, _p(self.d_a1), st),
+        check(L.sb200_conv_backward_dx_f32(2, _ptr(self.d_a2), _ptr(s.seg('w2')), _ptr(b['a1']), M, s.C1, s.H1, s.W1, _ptr(self.d_a1), st),
               'sb200_conv_backward_dx_f32')
         o_w1, o_b1 = s.off['w1'][0], s.off['b1'][0]
-        check(L.sb200_conv_backward_dw_f32(1, _p(self.frames), 1, _p(self.d_a1), M, s.C, s.H, s.W, 1.0 / 255.0,
+        check(L.sb200_conv_backward_dw_f32(1, _ptr(self.frames), 1, _ptr(self.d_a1), M, s.C, s.H, s.W, 1.0 / 255.0,
                                            C.c_void_p(base + 4 * o_w1), C.c_void_p(base + 4 * o_b1), s.size, self.splits, st),
               'sb200_conv_backward_dw_f32(1)')
 
@@ -168,13 +165,13 @@ def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None, adam_eps=1e-
     nh = head.net.size
     segs, o = [(head.net.params, grad[:nh], head.exp_avg, head.exp_avg_sq, nh, norm_out)], nh
     sf = C.c_void_p(stop_flag.data_ptr()) if stop_flag is not None else None
-    check(L.sb200_grad_reduce_norm_f32(_p(head.slabs), nh, head.splits, _p(grad[:nh]), nh, 1.0, 0, _p(head.ws), sf, st),
+    check(L.sb200_grad_reduce_norm_f32(_ptr(head.slabs), nh, head.splits, _ptr(grad[:nh]), nh, 1.0, 0, _ptr(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(head)')
     for tr in stem_trs:
         stem = tr.stem if hasattr(tr, 'stem') else tr.net
         ns = stem.size
         gs = grad[o:o + ns]
-        check(L.sb200_grad_reduce_norm_f32(_p(tr.slabs), ns, tr.splits, _p(gs), ns, 1.0, 0, _p(head.ws), sf, st),
+        check(L.sb200_grad_reduce_norm_f32(_ptr(tr.slabs), ns, tr.splits, _ptr(gs), ns, 1.0, 0, _ptr(head.ws), sf, st),
               'sb200_grad_reduce_norm_f32(stem)')
         segs.append((stem.params, gs, tr.exp_avg, tr.exp_avg_sq, ns, None))
         o += ns
@@ -183,8 +180,8 @@ def joint_step(head, stem_trs, grad, norm_out=None, stop_flag=None, adam_eps=1e-
     if dp is not None:
         dp.sum_(grad)
         scale = 1.0 / dp.world
-    check(L.sb200_grad_reduce_norm_f32(_p(grad), o, 1, _p(grad), o, scale, 1, _p(head.ws), sf, st),
+    check(L.sb200_grad_reduce_norm_f32(_ptr(grad), o, 1, _ptr(grad), o, scale, 1, _ptr(head.ws), sf, st),
           'sb200_grad_reduce_norm_f32(joint norm)')
     for params, g, m, v, n, no in segs:
-        check(L.sb200_clip_adam_f32(_p(params), _p(g), _p(m), _p(v), n, _p(head.lr), 0.9, 0.999, adam_eps, head.weight_decay,
-                                    head.clip_mode, head.clip_value, _p(head.ws), _p(no), sf, st), 'sb200_clip_adam_f32')
+        check(L.sb200_clip_adam_f32(_ptr(params), _ptr(g), _ptr(m), _ptr(v), n, _ptr(head.lr), 0.9, 0.999, adam_eps, head.weight_decay,
+                                    head.clip_mode, head.clip_value, _ptr(head.ws), _ptr(no), sf, st), 'sb200_clip_adam_f32')

@@ -18,10 +18,7 @@ import torch
 
 from .. import _lib, ops
 from .._lib import check
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+from ..ops import _ptr
 
 
 def _sfx(k):
@@ -121,9 +118,9 @@ class LSTMStem:
             lay = self.hhs[k].layout[0]
             hh = self.seg('hh' + _sfx(k), P)
             check(_lib.lib().sb200_lstm_forward_f32(
-                _p(bufs['pre_x']), C.c_void_p(hh.data_ptr() + 4 * lay['w']), C.c_void_p(hh.data_ptr() + 4 * lay['b']), _p(h0[k]),
-                _p(c0[k]), int(ld_cells), B, L, self.H, lb['h_out'].stride(0), _p(lb['h_out']), _p(lb.get('h_prev')),
-                _p(lb.get('gates')), _p(lb.get('c_seq')), _p(h_last[k]), _p(c_last[k]), ops._stream()), 'sb200_lstm_forward_f32')
+                _ptr(bufs['pre_x']), C.c_void_p(hh.data_ptr() + 4 * lay['w']), C.c_void_p(hh.data_ptr() + 4 * lay['b']), _ptr(h0[k]),
+                _ptr(c0[k]), int(ld_cells), B, L, self.H, lb['h_out'].stride(0), _ptr(lb['h_out']), _ptr(lb.get('h_prev')),
+                _ptr(lb.get('gates')), _ptr(lb.get('c_seq')), _ptr(h_last[k]), _ptr(c_last[k]), ops._stream()), 'sb200_lstm_forward_f32')
             x = lb['h_out']
         return x
 
@@ -163,22 +160,22 @@ class RnnTrainer:
             lb, dpre = s.layer_bufs(self.bufs, k), self.dpres[k]
             ih, hh = s.ihs[k], s.hhs[k]
             lay_h, lay_i = hh.layout[0], ih.layout[0]
-            check(L_.sb200_lstm_backward_f32(_p(dh), dh.stride(0), _p(lb['gates']), _p(lb['c_seq']), _p(c0[k]), int(self.ld_cells),
-                                             C.c_void_p(hh.params.data_ptr() + 4 * lay_h['w']), self.B, self.L, s.H, _p(dpre), st),
+            check(L_.sb200_lstm_backward_f32(_ptr(dh), dh.stride(0), _ptr(lb['gates']), _ptr(lb['c_seq']), _ptr(c0[k]), int(self.ld_cells),
+                                             C.c_void_p(hh.params.data_ptr() + 4 * lay_h['w']), self.B, self.L, s.H, _ptr(dpre), st),
                   'sb200_lstm_backward_f32')
             X = self.xf if k == 0 else s.layer_bufs(self.bufs, k - 1)['h_out']
             o_ih, o_hh = s.off['ih' + _sfx(k)][0], s.off['hh' + _sfx(k)][0]
-            check(L_.sb200_linear_bwd_dw_f32(_p(X), X.stride(0), _p(dpre), G, C.c_void_p(base + 4 * (o_ih + lay_i['w'])),
+            check(L_.sb200_linear_bwd_dw_f32(_ptr(X), X.stride(0), _ptr(dpre), G, C.c_void_p(base + 4 * (o_ih + lay_i['w'])),
                                              C.c_void_p(base + 4 * (o_ih + lay_i['b'])), s.size, self.splits, lay_i['ldw'], R,
                                              ih.dims[0], G, st), 'sb200_linear_bwd_dw_f32(lstm ih)')
             hp = lb['h_prev']
-            check(L_.sb200_linear_bwd_dw_f32(_p(hp), hp.stride(0), _p(dpre), G, C.c_void_p(base + 4 * (o_hh + lay_h['w'])),
+            check(L_.sb200_linear_bwd_dw_f32(_ptr(hp), hp.stride(0), _ptr(dpre), G, C.c_void_p(base + 4 * (o_hh + lay_h['w'])),
                                              C.c_void_p(base + 4 * (o_hh + lay_h['b'])), s.size, self.splits, lay_h['ldw'], R, s.H, G, st),
                   'sb200_linear_bwd_dw_f32(lstm hh)')
             if k > 0:                                             # dh_out of layer k-1 = dpre_k . W_ih_k (no activation)
                 dh = self.dh[k - 1]
-                check(L_.sb200_linear_bwd_dx_f32(_p(dpre), G, C.c_void_p(ih.params.data_ptr() + 4 * lay_i['w']), lay_i['ldw'], None, 0,
-                                                 _p(dh), dh.stride(0), R, G, s.H, st), 'sb200_linear_bwd_dx_f32(lstm layer input)')
+                check(L_.sb200_linear_bwd_dx_f32(_ptr(dpre), G, C.c_void_p(ih.params.data_ptr() + 4 * lay_i['w']), lay_i['ldw'], None, 0,
+                                                 _ptr(dh), dh.stride(0), R, G, s.H, st), 'sb200_linear_bwd_dx_f32(lstm layer input)')
 
     def backward_input(self, dx, x_act):
         """After ``backward``: the gradient w.r.t. layer 0's input, dpre_0 . W_ih_0, masked by relu'(x_act) -- i.e. w.r.t.
@@ -186,8 +183,8 @@ class RnnTrainer:
         stem's features) -- into ``dx`` [B*L, >= D]."""
         s, R, G = self.stem, self.B * self.L, 4 * self.stem.H
         ih, lay = s.ihs[0], s.ihs[0].layout[0]
-        check(_lib.lib().sb200_linear_bwd_dx_f32(_p(self.dpres[0]), G, C.c_void_p(ih.params.data_ptr() + 4 * lay['w']), lay['ldw'],
-                                                 _p(x_act), x_act.stride(0), _p(dx), dx.stride(0), R, G, s.D, ops._stream()),
+        check(_lib.lib().sb200_linear_bwd_dx_f32(_ptr(self.dpres[0]), G, C.c_void_p(ih.params.data_ptr() + 4 * lay['w']), lay['ldw'],
+                                                 _ptr(x_act), x_act.stride(0), _ptr(dx), dx.stride(0), R, G, s.D, ops._stream()),
               'sb200_linear_bwd_dx_f32(lstm stem input)')
 
     def state_dict(self):
@@ -200,6 +197,6 @@ class RnnTrainer:
 
 def rows_zfilter(x, row_stride, batch_stride, B, L, D, zf_stats, zf_eps, out):
     """out[b*L + t, :D] = zfilter(x[b*batch_stride + t*row_stride : +D]) (plain gather when zf_stats is None)."""
-    check(_lib.lib().sb200_rows_zfilter_f32(_p(x), int(row_stride), int(batch_stride), B, L, D, _p(zf_stats), float(zf_eps), _p(out),
+    check(_lib.lib().sb200_rows_zfilter_f32(_ptr(x), int(row_stride), int(batch_stride), B, L, D, _ptr(zf_stats), float(zf_eps), _ptr(out),
                                             out.stride(0), ops._stream()), 'sb200_rows_zfilter_f32')
     return out

@@ -8,23 +8,15 @@ arrival order out, silent drop of the OLDEST at capacity, ready when len >= batc
 
 ``sample()`` pops the oldest ``batch_size`` windows and gathers them into the learner-facing batch
 (the aggregator's layout, aggregator.py:176-183) as CUDA tensors."""
-import ctypes as C
-
 import numpy as np
 import torch
 
 from .. import _lib
 from .._lib import check
+from ..ops import _ptr, _stream
+from ..staging import Staging
+from ..utils import pack_window_records
 from .base import Replay, gather_fields
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def _st():
-    from ..ops import _stream
-    return _stream()
 
 
 class FIFOReplay(Replay):
@@ -59,7 +51,7 @@ class FIFOReplay(Replay):
         self._idx = torch.zeros(max(self.batch_size, 1), dtype=torch.int32, device=self.device)
         self._status = torch.zeros(1, dtype=torch.int32, device=self.device)
         self._slots = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self._pin = None
+        self._staging = Staging(self.device)                    # host inserts: the record, pinned and on the device
         self.check_underflow = True
 
     # -- control block ---------------------------------------------------------------------------------
@@ -82,40 +74,28 @@ class FIFOReplay(Replay):
         """``exp``: the dict ExpSenderWrapperMultiStepMovingWindowWithInfo.send emits
         (exp_sender_wrapper.py:244-264): obs [n dicts], obs_next, actions, rewards, dones, persistent_infos."""
         n, D, A = self.n_step, self.D, self.A
-        if self.pixel_shape is not None:       # uint8 frame -> the same bytes viewed as float32 words
-            flat = lambda o: np.ascontiguousarray(np.asarray(o['pixel']['camera0'], dtype=np.uint8)).reshape(-1).view(np.float32)  # noqa: E731
+        frames = self.pixel_shape is not None
+        if frames:
+            obs = lambda o: np.asarray(o['pixel']['camera0'], dtype=np.uint8)  # noqa: E731
         else:
-            flat = lambda o: np.concatenate([np.asarray(o['low_dim'][k], dtype=np.float32).reshape(-1)  # noqa: E731
-                                             for k in o['low_dim']])
+            obs = lambda o: np.concatenate([np.asarray(o['low_dim'][k], dtype=np.float32).reshape(-1)  # noqa: E731
+                                            for k in o['low_dim']])
         assert len(exp['obs']) == n, 'window length %d != n_step %d' % (len(exp['obs']), n)
-        rec = n * (D + A + 2 * A + 2) + D
-        if self._pin is None:
-            self._pin = torch.empty(rec, dtype=torch.float32, pin_memory=True)
-            self._stage = torch.empty(rec, dtype=torch.float32, device=self.device)
-        buf = self._pin.numpy()
-        o = 0
-        rows = np.zeros((n + 1, D), dtype=np.float32)
-        od = self.obs_dim
-        rows[:n, :od] = np.stack([flat(x) for x in exp['obs']])
-        rows[n, :od] = flat(exp['obs_next'])
-        cl = self.cells
-        if cl is not None and exp.get('onetime_infos'):         # [h, c] [L, H] of the window's first step (ppo_agent.py:133-137)
-            for i, blk in enumerate((cl.h(rows[0]), cl.c(rows[0]))):
-                v = np.asarray(exp['onetime_infos'][i], dtype=np.float32)
-                if v.size != blk.size:
-                    raise ValueError('onetime_infos[%d] holds %d floats; a %d-layer LSTM(%d) window carries [%d, %d]'
-                                     % (i, v.size, cl.layers, cl.hidden, cl.layers, cl.hidden))
-                blk[:] = v.reshape(-1)
-        buf[o:o + (n + 1) * D] = rows.reshape(-1); o += (n + 1) * D
+        pin = self._staging.pinned('record', (n * (D + A + 2 * A + 2) + D,))
+        buf = pin.numpy()
+        o = (n + 1) * D
+        # the cells [h, c], each [L, H], of the window's first step (ppo_agent.py:133-137); zeros when the window has none
+        pack_window_records(buf[:o].reshape(1, n + 1, D), np.stack([obs(x) for x in exp['obs']]), obs(exp['obs_next']),
+                            frames, self.cells, exp.get('onetime_infos') or None)
         buf[o:o + n * A] = np.stack(exp['actions']).astype(np.float32).reshape(-1); o += n * A
         buf[o:o + n * 2 * A] = np.stack([p[-1] for p in exp['persistent_infos']]).astype(np.float32).reshape(-1)
         o += n * 2 * A
         buf[o:o + n] = np.asarray(exp['rewards'], dtype=np.float32); o += n
         buf[o:o + n] = np.asarray(exp['dones'], dtype=np.float32)
-        self._stage.copy_(self._pin, non_blocking=True)
-        check(_lib.lib().sb200_fifo_push(_p(self.state), 1, _p(self._slots), _st()), 'sb200_fifo_push')
-        slot = int(self._slots.item())
-        s = self._stage
+        s = self._staging.device('record', pin.shape)
+        self._staging.upload('record', pin, s)
+        check(_lib.lib().sb200_fifo_push(_ptr(self.state), 1, _ptr(self._slots), _stream()), 'sb200_fifo_push')
+        slot = int(self._slots.item())                          # host sync: the pinned record may be rewritten after it
         o = 0
         self.r_obs[slot].view(-1).copy_(s[o:o + (n + 1) * D]); o += (n + 1) * D
         self.r_act[slot].view(-1).copy_(s[o:o + n * A]); o += n * A
@@ -131,7 +111,7 @@ class FIFOReplay(Replay):
         n, D, A = self.n_step, self.D, self.A
         if self._idx.numel() < batch_size:
             self._idx = torch.zeros(batch_size, dtype=torch.int32, device=self.device)
-        check(L.sb200_fifo_pop(_p(self.state), batch_size, _p(self._idx), _p(self._status), _st()), 'sb200_fifo_pop')
+        check(L.sb200_fifo_pop(_ptr(self.state), batch_size, _ptr(self._idx), _ptr(self._status), _stream()), 'sb200_fifo_pop')
         if out is None:
             f = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)  # noqa: E731
             out = dict(obs_full=f(batch_size, n + 1, D), actions=f(batch_size, n, A), pd=f(batch_size, n, 2 * A),

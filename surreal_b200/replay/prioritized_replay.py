@@ -23,7 +23,8 @@ import torch
 
 from .. import _lib
 from .._lib import check
-from .uniform_replay import UniformReplay, _p, _st
+from ..ops import _ptr, _stream
+from .uniform_replay import UniformReplay
 
 # learner_config.replay keys read when present (the reference's PrioritizedReplay / DQN 'prioritized' defaults); a
 # learner config with an algo.prioritized block (DQN) takes all four from there instead
@@ -69,11 +70,11 @@ class PrioritizedReplay(UniformReplay):
     # -- trees -------------------------------------------------------------------------------------------
     def admit(self):
         """Give every record inserted since the last admit max_priority^alpha, then rebuild the trees (device only)."""
-        check(_lib.lib().sb200_per_admit(C.byref(self.tree), _p(self.state), self.alpha, _st()), 'sb200_per_admit')
+        check(_lib.lib().sb200_per_admit(C.byref(self.tree), _ptr(self.state), self.alpha, _stream()), 'sb200_per_admit')
 
     def rebuild(self, full=False):
         """Recompute the internal nodes of the dirty subtrees (all of them with ``full``) and the levels above."""
-        check(_lib.lib().sb200_per_rebuild(C.byref(self.tree), int(bool(full)), _st()), 'sb200_per_rebuild')
+        check(_lib.lib().sb200_per_rebuild(C.byref(self.tree), int(bool(full)), _stream()), 'sb200_per_rebuild')
 
     def priorities(self):
         """-> float32 numpy [memory_size]: the leaves p^alpha (0 for a slot never inserted).  Host read: synchronises."""
@@ -119,9 +120,9 @@ class PrioritizedReplay(UniformReplay):
         outs = (C.c_void_p * n)(*[p[1].data_ptr() for p in pairs])
         recs = (C.c_int64 * n)(*[int(p[2]) for p in pairs])
         anneal = -1.0 if self.beta_anneal_iters is None else self.beta_anneal_iters
-        check(_lib.lib().sb200_per_sample_gather_f32(C.byref(self.tree), srcs, outs, recs, n, _p(view), self.sampler_seed,
-                                                     _p(self.sampler), int(batch_size), self.beta0, anneal,
-                                                     float(beta_override), _p(idx), _p(w), _st()),
+        check(_lib.lib().sb200_per_sample_gather_f32(C.byref(self.tree), srcs, outs, recs, n, _ptr(view), self.sampler_seed,
+                                                     _ptr(self.sampler), int(batch_size), self.beta0, anneal,
+                                                     float(beta_override), _ptr(idx), _ptr(w), _stream()),
               'sb200_per_sample_gather_f32')
         return {'obs': {'low_dim': {'flat_inputs': out['obs']}}, 'obs_next': {'low_dim': {'flat_inputs': out['obs_next']}},
                 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'], 'indices': idx,
@@ -148,8 +149,8 @@ class PrioritizedReplay(UniformReplay):
     def update_priorities_device(self, indices, priorities, stop_flag=None):
         """leaf[indices[b]] = priorities[b]^alpha (the last of equal indices wins), max_priority = max(it, priorities),
         then the rebuild; a no-op while ``stop_flag`` (int32 device flag) is set.  Device tensors, capturable."""
-        check(_lib.lib().sb200_per_update_f32(C.byref(self.tree), _p(indices), _p(priorities), int(indices.numel()),
-                                              self.alpha, _p(stop_flag), _st()), 'sb200_per_update_f32')
+        check(_lib.lib().sb200_per_update_f32(C.byref(self.tree), _ptr(indices), _ptr(priorities), int(indices.numel()),
+                                              self.alpha, _ptr(stop_flag), _stream()), 'sb200_per_update_f32')
 
     def update_priorities(self, indices, priorities):
         """prioritized_replay.py:124-143 for host input (lists, numpy or CPU tensors), checked as the reference does

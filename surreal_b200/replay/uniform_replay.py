@@ -21,17 +21,10 @@ import torch
 
 from .. import _lib
 from .._lib import check
+from ..ops import _ptr, _stream
+from ..staging import Staging
 from ..utils import record_action_dim
 from .base import Replay, gather_fields
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
-
-
-def _st():
-    from ..ops import _stream
-    return _stream()
 
 
 class PyRandomStream:
@@ -79,10 +72,8 @@ class UniformReplay(Replay):
         self._host_next = 0
         self._dirty = False
         self.stream = PyRandomStream()
-        self._idx_pin = None
+        self._staging = Staging(self.device)    # host inserts: the record; sample: the indices
         self._idx_event = None
-        self._idx_dev = None
-        self._pin = None
         # device sampler: the view {start, count, capacity} it draws from, its {draw counter, status} block and the seed
         rc = self.learner_config.replay
         self.sampler_seed = int(rc.sampler_seed) if 'sampler_seed' in rc else 0
@@ -117,14 +108,13 @@ class UniformReplay(Replay):
         D, A = self.D, self.A
         flat = lambda o: np.concatenate([np.asarray(o['low_dim'][k], dtype=np.float32).reshape(-1)  # noqa: E731
                                          for k in o['low_dim']])
-        rec = 2 * D + A + 2
-        if self._pin is None:
-            self._pin = torch.empty(rec, dtype=torch.float32, pin_memory=True)
-        buf = self._pin.numpy()
+        pin = self._staging.pinned('record', (2 * D + A + 2,))
+        buf = pin.numpy()
         buf[:D], buf[D:2 * D] = flat(exp['obs'][0]), flat(exp['obs'][1])
         buf[2 * D:2 * D + A] = np.asarray(exp['action'], dtype=np.float32)
         buf[2 * D + A], buf[2 * D + A + 1] = np.float32(exp['reward']), np.float32(exp['done'])
-        stage = self._pin.to(self.device, non_blocking=False)
+        stage = self._staging.device('record', pin.shape)
+        stage.copy_(pin)                                          # synchronous: the next insert rewrites the pinned record
         slot = self._host_next
         self.r_obs[slot].copy_(stage[:D])
         self.r_obs_next[slot].copy_(stage[D:2 * D])
@@ -139,12 +129,9 @@ class UniformReplay(Replay):
     def sample_indices(self, batch_size):
         """-> int64 numpy array: exactly [random.randint(0, len-1) for _ in range(batch_size)]."""
         n = len(self)
-        if self._idx_pin is None or self._idx_pin.numel() < batch_size:
-            self._idx_pin = torch.empty(batch_size, dtype=torch.int64, pin_memory=True)
-            self._idx_dev = torch.empty(batch_size, dtype=torch.int64, device=self.device)
         if self._idx_event is not None:
             self._idx_event.synchronize()                         # the previous batch's H2D copy has consumed the buffer
-        out = self._idx_pin.numpy()[:batch_size]
+        out = self._staging.pinned('indices', (batch_size,), np.int64).numpy()
         self.stream.randint_fill(n, batch_size, out)
         return out
 
@@ -152,12 +139,13 @@ class UniformReplay(Replay):
         L = _lib.lib()
         D, A = self.D, self.A
         self.sample_indices(batch_size)
-        idx = self._idx_dev[:batch_size]
-        idx.copy_(self._idx_pin[:batch_size], non_blocking=True)
+        st = self._staging
+        pin, idx = st.pinned('indices', (batch_size,), np.int64), st.device('indices', (batch_size,), np.int64)
+        st.upload('indices', pin, idx)
         if self._idx_event is None:
             self._idx_event = torch.cuda.Event()
         self._idx_event.record()                                  # refilling the pinned buffer waits for this copy
-        indices = self._idx_pin[:batch_size].clone()              # the caller's copy: later samples do not alias it
+        indices = pin.clone()                                     # the caller's copy: later samples do not alias it
         if out is None:
             f = lambda *s: torch.empty(*s, dtype=torch.float32, device=self.device)  # noqa: E731
             out = dict(obs=f(batch_size, D), obs_next=f(batch_size, D), actions=f(batch_size, A),
@@ -173,7 +161,7 @@ class UniformReplay(Replay):
         """Fix the population ``sample_device`` draws from: every record in the ring now, minus the slots the next
         ``reserve`` inserts can overwrite (sb200_uniform_view).  One one-thread launch on the current stream; call it
         where that stream is ordered after the inserts so far and before the next ones."""
-        check(_lib.lib().sb200_uniform_view(_p(self.state), int(reserve), _p(self.view), _st()), 'sb200_uniform_view')
+        check(_lib.lib().sb200_uniform_view(_ptr(self.state), int(reserve), _ptr(self.view), _stream()), 'sb200_uniform_view')
 
     @property
     def draw_counter(self):
@@ -203,8 +191,8 @@ class UniformReplay(Replay):
         srcs = (C.c_void_p * n)(*[p[0].data_ptr() for p in pairs])
         outs = (C.c_void_p * n)(*[p[1].data_ptr() for p in pairs])
         recs = (C.c_int64 * n)(*[int(p[2]) for p in pairs])
-        check(_lib.lib().sb200_uniform_sample_gather_f32(srcs, outs, recs, n, _p(self.view), self.sampler_seed,
-                                                         _p(self.sampler), int(batch_size), _p(idx), _st()),
+        check(_lib.lib().sb200_uniform_sample_gather_f32(srcs, outs, recs, n, _ptr(self.view), self.sampler_seed,
+                                                         _ptr(self.sampler), int(batch_size), _ptr(idx), _stream()),
               'sb200_uniform_sample_gather_f32')
         return {'obs': {'low_dim': {'flat_inputs': out['obs']}}, 'obs_next': {'low_dim': {'flat_inputs': out['obs_next']}},
                 'actions': out['actions'], 'rewards': out['rewards'], 'dones': out['dones'], 'indices': idx}

@@ -210,6 +210,43 @@ class CellLayout(collections.namedtuple('CellLayout', 'layers hidden obs_dim')):
         return rows[..., o:o + (self.layers * self.hidden if k is None else self.hidden)]
 
 
+def pack_window_records(rows, obs, obs_next, frames=False, layout=None, cells=None):
+    """The host packer of PPO window records ``rows`` [B, n+1, width] (DESIGN §2): ``obs`` [B, n, ...] into rows :n and
+    ``obs_next`` [B, 1, ...] into row n, in the observation columns -- features, or with ``frames`` uint8 frames as their
+    bytes (obs_packed_dim) -- and, for an RNN policy's CellLayout ``layout``, ``cells`` = (h, c), each [B, L, H] (the
+    reference's onetime_infos: the cells of every window's first step), into the cell columns of row 0, zeros when
+    ``cells`` is None.  ``rows`` is a numpy array, written in place, or a torch tensor, whose copies are issued
+    non-blocking on the current stream.  Columns it does not write keep their contents."""
+    import math
+    import numpy as np
+    import torch
+    host = isinstance(rows, np.ndarray)
+    as_array = np.asarray if host else torch.as_tensor
+
+    def put(dst, src):
+        src = as_array(src).reshape(dst.shape)
+        if host:
+            dst[...] = src
+        else:
+            dst.copy_(src, non_blocking=True)
+
+    B, n, od = rows.shape[0], rows.shape[1] - 1, rows.shape[-1] if layout is None else layout.obs_dim
+    obs_cols = rows.view(np.uint8 if host else torch.uint8)[..., :4 * od] if frames else rows[..., :od]
+    put(obs_cols[:, :n], obs)
+    put(obs_cols[:, n:], obs_next)
+    if layout is None:
+        return
+    for i, blk in enumerate((layout.h(rows[:, 0]), layout.c(rows[:, 0]))):
+        if cells is None:
+            blk[...] = 0
+            continue
+        got = math.prod(as_array(cells[i]).shape)
+        if got != B * layout.layers * layout.hidden:
+            raise ValueError('onetime_infos[%d] holds %d floats; %d window(s) of a %d-layer LSTM(%d) carry [%d, %d, %d]'
+                             % (i, got, B, layout.layers, layout.hidden, B, layout.layers, layout.hidden))
+        put(blk, cells[i])
+
+
 def rnn_cell_layout(learner_config, env_config):
     """The CellLayout of an RNN policy's records (None for a feed-forward policy): rnn_layer x rnn_hidden cells behind
     obs_packed_dim observation floats.  Raises ConfigError for rnn_layer < 1."""
