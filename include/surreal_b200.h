@@ -903,7 +903,12 @@ int sb200_per_update_f32(const sb200_per_tree* tree, const int64_t* indices, con
  *   (float64 running n-step sums).  dest / emit [N]: the current step's ring slot and float32 reward of each actor's
  *   emitted record.  Ring r_*: obs / obs_next [C][D], act [C][A], rew / done [C].
  *   uniform_state: sb200_uniform_state_bytes() bytes {int64 next_idx,size,capacity,total_in}.
- *   step_counter: the Philox step counter, advanced by one per step. */
+ *   step_counter: the Philox step counter, advanced by one per step.
+ *   Rounding, as the reference's `e += pow(gamma, n_step - i - 1) * r` on Python floats: gamma^k is libm pow on the
+ *   host, each step's product is rounded to float64, then the sum (no fused multiply-add); the record's reward is the
+ *   sum rounded to float32 once, at emission.  1 <= n_step <= SB200_SSAR_MAX_NSTEP (the gamma^k table is a kernel
+ *   argument); both ssar_step entries refuse a larger n_step with SB200_ERR_ARG before any launch. */
+#define SB200_SSAR_MAX_NSTEP 64
 typedef struct {
     int N, n_step;
     double gamma;
@@ -922,7 +927,7 @@ size_t sb200_uniform_state_bytes(void);
 int sb200_ssar_step_f32(const sb200_ssar* ssar, const float* obs, const float* action, const float* obs_next,
                         const float* reward, const float* done, void* stream);
 /*   ssar_step_host: ssar_step for a host env, one call: H2D of obs_next, action, done and the rewards AS FLOAT64 (the
- *     reference sums Python floats; the record's reward is rounded to float32 once, at emission), then the ssar_step
+ *     reference sums Python floats, with the rounding above), then the ssar_step
  *     kernels, then obs <- the reset observation (obs_reset_host, or obs_next when obs_reset_host == obs_next_host).
  *     obs [N][D] holds s_t on entry and the next s_t on return.  Host pointers must be pinned. */
 int sb200_ssar_step_host_f32(const sb200_ssar* ssar, const float* obs_next_host, const float* obs_reset_host,

@@ -91,11 +91,17 @@ __global__ void __launch_bounds__(256) gather_kernel(const float* __restrict__ s
 // order (uniform_replay.py:36-41).
 // (UniformState {next_idx, size, capacity, total_in}: replay_dev.cuh)
 
+// gamma^k for k < n_step, from the host's libm pow: the function CPython's float.__pow__ calls.
+struct GammaPow {
+    double p[SB200_SSAR_MAX_NSTEP];
+};
+
 // Rew: float for device envs, double for host envs, whose float64 rewards the reference sums as Python floats.
+// Each step's product and sum are rounded separately, as `e += pow(gamma, k) * r` rounds them in Python: no FMA.
 template <typename Rew>
 __global__ void __launch_bounds__(1024) ssar_flags_kernel(const Rew* __restrict__ reward,
                                                           const float* __restrict__ done, int N, int n_step,
-                                                          double gamma, int* __restrict__ dq_len,
+                                                          const GammaPow gp, int* __restrict__ dq_len,
                                                           double* __restrict__ dq_rew, int* __restrict__ dest,
                                                           float* __restrict__ emit_rew, UniformState* us,
                                                           unsigned long long* step_ctr) {
@@ -111,7 +117,7 @@ __global__ void __launch_bounds__(1024) ssar_flags_kernel(const Rew* __restrict_
             const int len = dq_len[i];
             const double r = (double)reward[i];
             double* q = dq_rew + (long long)i * n_step;
-            for (int e = 0; e < len; ++e) q[e] += pow(gamma, (double)(n_step - e - 1)) * r;
+            for (int e = 0; e < len; ++e) q[e] = __dadd_rn(q[e], __dmul_rn(gp.p[n_step - e - 1], r));
             q[len] = r;                                   // append (position len)
             flag = (len + 1 == n_step) ? 1 : 0;
             if (flag) emit_rew[i] = (float)q[0];          // popleft's accumulated reward -> fp32 at the learner
@@ -384,7 +390,8 @@ extern "C" size_t sb200_uniform_state_bytes(void) { return sizeof(UniformState);
 
 // Host check of an SSAR staging descriptor: every buffer present and the shape sane (step_counter may be NULL).
 static bool ssar_ok(const sb200_ssar* s) {
-    return s != nullptr && s->N >= 1 && s->n_step >= 1 && s->D >= 1 && s->A >= 1 && s->dq_len && s->dq_obs && s->dq_act &&
+    return s != nullptr && s->N >= 1 && s->n_step >= 1 && s->n_step <= SB200_SSAR_MAX_NSTEP && s->D >= 1 && s->A >= 1 &&
+           s->dq_len && s->dq_obs && s->dq_act &&
            s->dq_rew && s->dest && s->emit && s->uniform_state && s->r_obs && s->r_obs_next && s->r_act && s->r_rew &&
            s->r_done;
 }
@@ -393,7 +400,9 @@ static bool ssar_ok(const sb200_ssar* s) {
 template <typename Rew>
 static int ssar_launch(const sb200_ssar* s, const float* obs, const float* action, const float* obs_next, const Rew* reward,
                        const float* done, cudaStream_t st) {
-    ssar_flags_kernel<Rew><<<1, 1024, 0, st>>>(reward, done, s->N, s->n_step, s->gamma, s->dq_len, s->dq_rew, s->dest,
+    GammaPow gp = {};
+    for (int k = 0; k < s->n_step; ++k) gp.p[k] = pow(s->gamma, (double)k);
+    ssar_flags_kernel<Rew><<<1, 1024, 0, st>>>(reward, done, s->N, s->n_step, gp, s->dq_len, s->dq_rew, s->dest,
                                                s->emit, (UniformState*)s->uniform_state,
                                                (unsigned long long*)s->step_counter);
     ssar_commit_kernel<<<s->N, 128, 0, st>>>(obs, action, obs_next, done, s->N, s->n_step, s->D, s->A, s->dq_len, s->dq_obs,
