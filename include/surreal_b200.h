@@ -573,6 +573,39 @@ int sb200_ppo_window_step_f32(const sb200_windows* windows, const sb200_window_r
 int sb200_ppo_sample_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
                          const float* eps, int N, int A, int deterministic, uint64_t seed, uint64_t* step_counter,
                          float* action, float* pd, const sb200_windows* stage, int assign_slots, void* stream);
+
+/* Categorical policy of PPO for discrete action spaces (csrc/ppo_cat.cu; semantics: tests/cat_ref.py).  The actor head
+ * outputs K logits (no tanh, no log_var).  pd row = [p_0..p_{K-1} | log p_0..log p_{K-1}] (2K floats) from a
+ * max-subtracted log-softmax; actions are one-hot rows [K]: the window records keep their [A] / [2A] layout with A = K.
+ * likelihood(a) = max(p_a, 1e-5), KL(p0 || p1) = sum p0 (log p0 - log p1), entropy = -sum p log p.  One warp per row.
+ * K: 2 .. SB200_PPO_CAT_MAX_K, the widest layer the fused forward accepts (sb200_mlp_forward_f32).
+ *   cat_sample: logits [N][ldl] -> pd [N][2K], one-hot action [N][K], index [N] int64 (or NULL).  Inverse CDF of one
+ *     uniform per actor, u = (x >> 8) * 2^-24 with x the first word of Philox4x32-10 keyed (seed, *step_counter,
+ *     actor << 16) as ppo_sample keys its normals: the action is the first j with u < c_j, c_j the fp32 running sum of
+ *     p_0..p_j, or K - 1 if none.  deterministic: the argmax of the logits (lowest index among ties).  stage /
+ *     assign_slots exactly as sb200_ppo_sample_f32 (stage->A == K).
+ *   cat_make_pd: logits [B][ldl] -> pd [B][ldp].
+ *   cat_policy_loss: the clip (mode 0) or adapt (mode 1) loss of sb200_ppo_policy_loss_f32 with the categorical
+ *     likelihoods; dlogits [B][ldd] = gradient w.r.t. the logits (padding columns zeroed); the same stats slots
+ *     (ENTROPY = mean entropy of the current policy) and stop_flag no-op.  Adapt needs sb200_ppo_cat_kl_f32(ref, learn)
+ *     on the same workspace first.
+ *   cat_kl: mean KL(p0 || softmax(logits)) -> stats[stat_slot] and the workspace; raises *stop_flag above stop_threshold.
+ *   cat_final_stats: BEHAVE_LIK, IS_WEIGHT and REF_BEHAVE_KL of sb200_ppo_final_stats_f32 (no LOG_SIG).
+ * workspace: sb200_ppo_loss_workspace_bytes(B, K). */
+#define SB200_PPO_CAT_MAX_K 4096
+int sb200_ppo_cat_sample_f32(const float* logits, int64_t ldl, int N, int K, int deterministic, uint64_t seed,
+                             uint64_t* step_counter, float* action, float* pd, int64_t* index, const sb200_windows* stage,
+                             int assign_slots, void* stream);
+int sb200_ppo_cat_make_pd_f32(const float* logits, int64_t ldl, int B, int K, float* pd, int64_t ldp, void* stream);
+int sb200_ppo_cat_policy_loss_f32(int mode, const float* logits, int64_t ldl, const float* actions, int64_t lda,
+                                  const float* adv, const float* behave_pd, int64_t ldb, const float* ref_pd, int64_t ldr,
+                                  int B, int K, const double* hyper, double eta, double kl_target, float* dlogits,
+                                  int64_t ldd, float* stats, void* workspace, const int* stop_flag, void* stream);
+int sb200_ppo_cat_kl_f32(const float* p0, int64_t ld0, const float* logits, int64_t ldl, int B, int K, float* stats,
+                         int stat_slot, double stop_threshold, int* stop_flag, void* workspace, void* stream);
+int sb200_ppo_cat_final_stats_f32(const float* logits, int64_t ldl, const float* actions, int64_t lda,
+                                  const float* behave_pd, int64_t ldb, const float* ref_pd, int64_t ldr, int B, int K,
+                                  float* stats, void* workspace, void* stream);
 int sb200_ddpg_noise_f32(const float* mean, int64_t ldm, const float* sigma, const float* unit_noise, int N,
                          int A, int deterministic, uint64_t seed, const uint64_t* step_counter,
                          float* action, void* stream);
@@ -730,7 +763,13 @@ typedef struct {
     const sb200_mlp* fc;                /* the stem's Linear + ReLU: 32 * H2 * W2 -> D */
     float* a1;                          /* [N][16][H1][W1] */
     float* a2;                          /* [N][32 * H2 * W2] */
+    /* SB200_PD_GAUSSIAN (0): ppo_sample.  SB200_PD_CATEGORICAL: the head outputs K logits into mean [N][K] and the last
+     * stage is sb200_ppo_cat_sample_f32 (action: one-hot rows [N][K], pd [N][2K]; log_var, log_noise and eps are not
+     * read). */
+    int pd_type;
 } sb200_ppo_act;
+#define SB200_PD_GAUSSIAN 0
+#define SB200_PD_CATEGORICAL 1
 int sb200_ppo_act_f32(const sb200_ppo_act* args, void* stream);
 
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N

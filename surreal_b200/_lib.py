@@ -105,7 +105,12 @@ class PPOAct(C.Structure):
                 ('pd_host', C.c_void_p), ('h_before_host', C.c_void_p), ('c_before_host', C.c_void_p),
                 ('frames_host', C.c_void_p), ('frames', C.c_void_p), ('frame_c', C.c_int), ('frame_h', C.c_int),
                 ('frame_w', C.c_int), ('conv_w1', C.c_void_p), ('conv_b1', C.c_void_p), ('conv_w2', C.c_void_p),
-                ('conv_b2', C.c_void_p), ('fc', C.POINTER(Mlp)), ('a1', C.c_void_p), ('a2', C.c_void_p)]
+                ('conv_b2', C.c_void_p), ('fc', C.POINTER(Mlp)), ('a1', C.c_void_p), ('a2', C.c_void_p),
+                ('pd_type', C.c_int)]
+
+
+PD_GAUSSIAN, PD_CATEGORICAL = 0, 1
+PPO_CAT_MAX_K = 4096                    # SB200_PPO_CAT_MAX_K
 
 
 DDPG_FWD_FUSED, DDPG_FWD_PACKED, DDPG_FWD_PER_ACTOR = 0, 1, 2
@@ -231,6 +236,11 @@ def _declare(lib):
         'sb200_value_loss_f32': (I, [P, L, P, I, P, L, P, P, P]),
         'sb200_ppo_final_stats_f32': (I, [P, L, P, P, L, P, L, P, L, I, I, P, P, P]),
         'sb200_ppo_sample_f32': (I, [P, L, P, P, P, I, I, I, C.c_uint64, P, P, P, C.POINTER(Windows), I, P]),
+        'sb200_ppo_cat_sample_f32': (I, [P, L, I, I, I, C.c_uint64, P, P, P, P, C.POINTER(Windows), I, P]),
+        'sb200_ppo_cat_make_pd_f32': (I, [P, L, I, I, P, L, P]),
+        'sb200_ppo_cat_policy_loss_f32': (I, [I, P, L, P, L, P, P, L, P, L, I, I, P, D, D, P, L, P, P, P, P]),
+        'sb200_ppo_cat_kl_f32': (I, [P, L, P, L, I, I, P, I, D, P, P, P]),
+        'sb200_ppo_cat_final_stats_f32': (I, [P, L, P, L, P, L, P, L, I, I, P, P, P]),
         'sb200_ddpg_noise_f32': (I, [P, L, P, P, I, I, I, C.c_uint64, P, P, P]),
         'sb200_ddpg_target2_f32': (I, [P, P, L, P, L, P, P, L, I, I, D, P, P, P, P]),
         'sb200_ddpg_smooth_action_f32': (I, [P, L, P, I, I, D, D, C.c_uint64, P, P, L, P]),

@@ -3,7 +3,11 @@
 ``act(obs)`` runs the fused actor MLP for all N actors in one launch, then one sampling kernel that
 applies each actor's constant exploration scale exp(noise_i) (drawn once, ppo_agent.py:57-61), samples
 N(mean, std), clips to [-1, 1] and records the behaviour policy AFTER scaling (ppo_agent.py:139,149).
-numpy observations (a single actor's [D] vector or an [N, D] batch) are accepted for external CPU envs."""
+numpy observations (a single actor's [D] vector or an [N, D] batch) are accepted for external CPU envs.
+
+A discrete action_spec selects the categorical policy (model.ppo_net.Categorical): the same call samples each actor's
+action from the softmax of its logits.  The per-actor exploration scale has no categorical counterpart: ``noise`` /
+``set_noise`` are kept but ignored by a categorical agent."""
 import ctypes as C
 import time
 
@@ -12,7 +16,7 @@ import torch
 
 from .. import _lib, ops
 from .._lib import check
-from ..model.ppo_net import PPOModel, DiagGauss
+from ..model.ppo_net import PPOModel, Categorical, make_pd
 from ..env import ExpSenderWrapperMultiStepMovingWindowWithInfo
 from ..staging import Staging
 from .base import Agent
@@ -41,12 +45,14 @@ class PPOAgent(Agent):
             self.noise = np.random.uniform(low=-self.log_sig_range, high=self.log_sig_range, size=N)
         self.rnn_config = self.learner_config.algo.rnn
         self.gpu_ids = 'cuda:all'
-        self.pd = DiagGauss(self.action_dim)
+        self.pd = make_pd(self.env_config.action_spec)
+        self.categorical = isinstance(self.pd, Categorical)
         self.cells = None
         pixel = bool(self.env_config.pixel_input) if 'pixel_input' in self.env_config else False
         self.model = PPOModel(obs_spec=self.obs_spec, action_dim=self.action_dim, model_config=self.learner_config.model,
                               use_cuda=True, init_log_sig=self.init_log_sig, use_z_filter=self.use_z_filter,
-                              if_pixel_input=pixel, rnn_config=self.rnn_config, device=self.device)
+                              if_pixel_input=pixel, rnn_config=self.rnn_config, device=self.device,
+                              categorical=self.categorical)
         A = self.action_dim
         self._log_noise = torch.tensor(self.noise, dtype=torch.float32, device=self.device)
         self._mean = torch.zeros(N, A, device=self.device)
@@ -66,7 +72,8 @@ class PPOAgent(Agent):
         [H2D] -> [CNN stem] -> [z-filter -> LSTM layers, each actor's cells updated in place] -> actor head -> sampling
         (ppo_net.py:268-279,317-351,368-375, ppo_agent.py:133-149) -> [D2H, one sync].  The LSTM policy's onetime_infos are
         its cells BEFORE the step.  Device observations give device results; numpy in, numpy out.  Pixel input is uint8
-        frames [N, C, H, W] (device tensor or numpy)."""
+        frames [N, C, H, W] (device tensor or numpy).  The categorical policy's action is one-hot rows [N, K] for device
+        observations (what DiscreteSyntheticEnv.step takes) and int64 indices for host ones; ``eps`` is Gaussian only."""
         from ..model.lstm_stem import _sfx
         N, A, m = self.num_envs, self.action_dim, self.model
         cnn, stem = m.cnn_stem, m.rnn_stem
@@ -144,10 +151,16 @@ class PPOAgent(Agent):
         staged = training and isinstance(env, ExpSenderWrapperMultiStepMovingWindowWithInfo)
         counter = env.step_counter if (env is not None and hasattr(env, 'step_counter')) else self._counter
         eps_dev = None
-        if eps is not None:
-            eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
-            a.eps = eps_dev.data_ptr()
-        a.mean, a.log_var, a.log_noise = self._mean.data_ptr(), m.log_var.data_ptr(), self._log_noise.data_ptr()
+        a.pd_type = self.pd.pd_type
+        a.mean = self._mean.data_ptr()
+        if self.categorical:
+            if eps is not None:
+                raise ValueError('eps (injected N(0,1) draws) belongs to the Gaussian policy')
+        else:
+            if eps is not None:
+                eps_dev = torch.as_tensor(np.asarray(eps, dtype=np.float32).reshape(N, A)).to(self.device)
+                a.eps = eps_dev.data_ptr()
+            a.log_var, a.log_noise = m.log_var.data_ptr(), self._log_noise.data_ptr()
         a.deterministic, a.seed, a.step_counter = int(det), self.seed, counter.data_ptr()
         a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
         if staged:
@@ -190,10 +203,12 @@ class PPOAgent(Agent):
         """act()'s numpy result from the pinned outputs the C call has filled: float64 actions, as the reference hands the
         env (ppo_net.py:83); ``single``: one actor's unbatched observation gives unbatched results."""
         N, A = self.num_envs, self.action_dim
-        action = self._staging.pinned('action', (N, A)).numpy().astype(np.float64)
+        action = self._staging.pinned('action', (N, A)).numpy()
+        # categorical: the index of each one-hot row; Gaussian: float64 actions
+        action = action.argmax(axis=1).astype(np.int64) if self.categorical else action.astype(np.float64)
         pd = self._staging.pinned('pd', (N, 2 * A)).numpy().copy()
         if single:
-            action, pd = action.reshape(-1), pd.reshape(-1)
+            action, pd = (action[0] if self.categorical else action.reshape(-1)), pd.reshape(-1)
         return self._result(action, pd, onetime)
 
     def _result(self, action, pd, onetime):
@@ -224,11 +239,14 @@ class PPOAgent(Agent):
     def rollout_chunk_supported(self):
         """True when ``steps`` consecutive act -> env.step -> staging iterations can run as one persistent rollout
         kernel: training mode, the in-tree device env behind the window wrapper, and a policy that fits the kernel's
-        plan -- the MLP policy on sb200_ppo_rollout_f32, the low-dim LSTM policy on sb200_ppo_rollout_rnn_f32."""
+        plan -- the MLP policy on sb200_ppo_rollout_f32, the low-dim LSTM policy on sb200_ppo_rollout_rnn_f32.  The
+        categorical policy takes the per-step path."""
         import os
         from ..env import SyntheticEnv
         env = self.env
         if self.agent_mode != 'training' or os.environ.get('SB200_PERSISTENT_ROLLOUT', '1') == '0':
+            return False
+        if self.categorical:
             return False
         if self.model.cnn_stem is not None:
             return False                       # pixel policies run on the per-step launch chain
@@ -322,6 +340,20 @@ class PPOAgent(Agent):
 
     def default_config(self):
         return {'model': {'convs': '_list_', 'fc_hidden_sizes': '_list_'}}
+
+    def get_env(self):
+        """The in-tree synthetic env; for a discrete action_spec its discrete form (one-hot action rows), as QAgent's."""
+        if not self.categorical:
+            return super().get_env()
+        from ..env import DiscreteSyntheticEnv
+        from ..utils import obs_is_pixel
+        ec = self.env_config
+        name = ec.env_name if 'env_name' in ec else ''
+        if not str(name).startswith('synthetic') or obs_is_pixel(ec.obs_spec):
+            return super().get_env()
+        D = sum(v[0] for v in ec.obs_spec['low_dim'].values())
+        return DiscreteSyntheticEnv(self.num_envs, D, self.action_dim, ec.limit_episode_length,
+                                    seed=int(ec.seed) if 'seed' in ec else 0)
 
     def reset(self):
         """reset of LSTM hidden and cell states (ppo_agent.py:169-183; nothing in the reference calls it)."""

@@ -13,17 +13,11 @@
 
 namespace {
 
-constexpr int LT = 256;
+using ppo_dev::LT;
 using ppo_dev::MAX_A;
 using ppo_dev::row_loglik;
 using ppo_dev::row_kl;
-
-struct LossWs {
-    unsigned int counter;
-    unsigned int pad;
-    double kl_mean;          // written by the KL kernel, consumed by the adapt loss
-    double partial[1];       // [blocks][slots]
-};
+using ppo_dev::LossWs;
 
 // ------------------------------------------------------------------------------------------------
 // mode 0: clip   mode 1: adapt (needs ws->kl_mean from kl_kernel(ref, learn))
@@ -121,12 +115,8 @@ __global__ void __launch_bounds__(LT) kl_kernel(const float* __restrict__ p0, lo
         if (tid == 0) {
             double acc = 0.0;
             for (unsigned int k = 0; k < gridDim.x; ++k) acc += ws->partial[k];
-            const float klm = (float)(acc / (double)B);        // .mean() in fp32
-            ws->kl_mean = (double)klm;
-            if (defer) return;                                 // data-parallel: all-reduce ws->kl_mean, then kl_apply
-            if (stats != nullptr && slot >= 0) stats[slot] = klm;
-            if (stop != nullptr && stop_threshold > 0.0 && (double)klm > stop_threshold) *stop = 1;
-            if (stats != nullptr && slot == SB200_STAT_KL_POST) stats[SB200_STAT_EPOCHS] += 1.0f;
+            // .mean() in fp32; data-parallel (defer): all-reduce ws->kl_mean, then kl_apply
+            ppo_dev::kl_publish((float)(acc / (double)B), ws, stats, slot, stop_threshold, stop, defer);
         }
     }
 }
@@ -135,11 +125,7 @@ __global__ void __launch_bounds__(LT) kl_kernel(const float* __restrict__ p0, lo
 __global__ void kl_apply_kernel(LossWs* ws, float* __restrict__ stats, int slot, double stop_threshold,
                                 int* __restrict__ stop) {
     if (stop != nullptr && *stop) return;
-    const float klm = (float)ws->kl_mean;
-    ws->kl_mean = (double)klm;
-    if (stats != nullptr && slot >= 0) stats[slot] = klm;
-    if (stop != nullptr && stop_threshold > 0.0 && (double)klm > stop_threshold) *stop = 1;
-    if (stats != nullptr && slot == SB200_STAT_KL_POST) stats[SB200_STAT_EPOCHS] += 1.0f;
+    ppo_dev::kl_publish((float)ws->kl_mean, ws, stats, slot, stop_threshold, stop, 0);
 }
 
 // value loss: mean((v - ret)^2), dv = 2(v-ret)/B, explained variance (ppo.py:323-331)

@@ -7,6 +7,26 @@
 namespace ppo_dev {
 
 constexpr int MAX_A = 64;
+constexpr int LT = 256;      // threads per block of the loss kernels, and batch rows per block (workspace sizing)
+
+// Workspace of the loss / KL / statistics kernels of both policy distributions (sb200_ppo_loss_workspace_bytes).
+struct LossWs {
+    unsigned int counter;
+    unsigned int pad;
+    double kl_mean;          // written by the KL kernel, consumed by the adapt loss
+    double partial[1];       // [blocks][slots]
+};
+
+// Last block of a KL kernel: mean KL `klm` (the fp32 .mean()) -> ws->kl_mean, stats[slot], the early-stop flag above
+// stop_threshold (> 0) and the epoch count (ppo.py:553-557).  defer: data-parallel, leave the local mean for kl_apply.
+__device__ __forceinline__ void kl_publish(float klm, LossWs* ws, float* stats, int slot, double stop_threshold, int* stop,
+                                           int defer) {
+    ws->kl_mean = (double)klm;
+    if (defer) return;
+    if (stats != nullptr && slot >= 0) stats[slot] = klm;
+    if (stop != nullptr && stop_threshold > 0.0 && (double)klm > stop_threshold) *stop = 1;
+    if (stats != nullptr && slot == SB200_STAT_KL_POST) stats[SB200_STAT_EPOCHS] += 1.0f;
+}
 
 __device__ __forceinline__ float row_loglik(const float* a, const float* mu, const float* sg, int A, float c0,
                                             float* quad_out) {

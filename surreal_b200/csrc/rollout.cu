@@ -522,8 +522,12 @@ extern "C" int sb200_ppo_act_f32(const sb200_ppo_act* a, void* stream) {
     }
     SB200_REQUIRE(a->action_host == nullptr || a->pd_host != nullptr);
     SB200_REQUIRE((a->h_before_host == nullptr) == (a->c_before_host == nullptr) && (a->h_before_host == nullptr || rnn));
-    SB200_REQUIRE(sample_args_ok(a->mean, A, a->log_var, N, A, a->step_counter, a->action, a->pd, a->stage,
-                                 a->assign_slots));
+    SB200_REQUIRE(a->pd_type == SB200_PD_GAUSSIAN || a->pd_type == SB200_PD_CATEGORICAL);
+    const bool cat = a->pd_type == SB200_PD_CATEGORICAL;
+    // the categorical sampler checks its own arguments when it is called, after the forward
+    SB200_REQUIRE(cat || sample_args_ok(a->mean, A, a->log_var, N, A, a->step_counter, a->action, a->pd, a->stage,
+                                        a->assign_slots));
+    SB200_REQUIRE(!cat || (A >= 2 && A <= SB200_PPO_CAT_MAX_K && a->mean && a->action && a->pd));
     // no LayerNorm in the recurrent policy's head, input projections or CNN stem
     if ((rnn && sb200_mlp_has_ln(a->head)) || (stem && sb200_mlp_has_ln(a->fc))) return SB200_ERR_UNSUPPORTED;
     for (int k = 0; k < L; ++k)
@@ -575,8 +579,12 @@ extern "C" int sb200_ppo_act_f32(const sb200_ppo_act* a, void* stream) {
         rc = sb200_forward_out(a->head, zf, x, ldx, N, a->mean, A, stream);
     }
     if (rc != SB200_OK) return rc;
-    rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed, a->step_counter,
-                              a->action, a->pd, a->stage, a->assign_slots, stream);
+    if (cat)
+        rc = sb200_ppo_cat_sample_f32(a->mean, A, N, A, a->deterministic, a->seed, a->step_counter, a->action, a->pd, nullptr,
+                                      a->stage, a->assign_slots, stream);
+    else
+        rc = sb200_ppo_sample_f32(a->mean, A, a->log_var, a->log_noise, a->eps, N, A, a->deterministic, a->seed,
+                                  a->step_counter, a->action, a->pd, a->stage, a->assign_slots, stream);
     if (rc != SB200_OK || a->action_host == nullptr) return rc;
     SB200_CUDA(cudaMemcpyAsync(a->action_host, a->action, (size_t)N * A * sizeof(float), cudaMemcpyDeviceToHost, st));
     SB200_CUDA(cudaMemcpyAsync(a->pd_host, a->pd, (size_t)N * 2 * A * sizeof(float), cudaMemcpyDeviceToHost, st));

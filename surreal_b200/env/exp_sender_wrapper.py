@@ -64,6 +64,8 @@ class ExpSenderWrapperMultiStepMovingWindowWithInfo(_WrapperBase):
         self.cells = cells
         extra = 0 if cells is None else 2 * cells[0].shape[0] * cells[0].shape[2]
         super().__init__(env, learner_config, session_config, replay, obs_extra=extra)
+        # PPO windows stage a discrete spec's actions as one-hot rows (the categorical policy): K floats, like the ring's
+        self.A = int(self.replay.env_config.action_spec['dim'][0])
         self.n_step = self.learner_config.algo.n_step
         self.stride = self.learner_config.algo.stride
         if self.stride < 1:

@@ -7,9 +7,12 @@ import collections
 import numpy as np
 
 
+def _action_type(action_spec):
+    return str(action_spec['type'] if isinstance(action_spec, dict) else action_spec.type)
+
+
 def _check_continuous(action_spec):
-    t = action_spec['type'] if isinstance(action_spec, dict) else action_spec.type
-    if str(t) != 'continuous':
+    if _action_type(action_spec) != 'continuous':
         raise NotImplementedError('action_spec unsupported ' + str(action_spec))
 
 
@@ -45,12 +48,32 @@ class SSARAggregator:
 
 
 class MultistepAggregatorWithInfo:
-    """n-step windows with per-step policy info -> batched arrays (aggregator.py:151-262)."""
+    """n-step windows with per-step policy info -> batched arrays (aggregator.py:151-262).  A discrete action_spec (the
+    categorical PPO policy) takes integer actions and hands the learner one-hot rows [B, n, K] float32, the layout of
+    the window records."""
 
     def __init__(self, obs_spec, action_spec):
         assert isinstance(obs_spec, dict) and isinstance(action_spec, dict)
-        _check_continuous(action_spec)
+        t = _action_type(action_spec)
+        if t not in ('continuous', 'discrete'):
+            raise NotImplementedError('action_spec unsupported ' + str(action_spec))
         self.obs_spec, self.action_spec = obs_spec, action_spec
+        self.n_actions = int(action_spec['dim'][0]) if t == 'discrete' else None
+
+    def _actions(self, exp_list):
+        acts = np.stack([np.stack(e['actions']) for e in exp_list])
+        if self.n_actions is None:
+            return acts
+        K = self.n_actions
+        idx = np.asarray(acts).reshape(acts.shape[0], -1)
+        if idx.dtype.kind == 'f' and not np.array_equal(idx, np.round(idx)):
+            raise ValueError('discrete actions must be integers')
+        idx = idx.astype(np.int64)
+        if idx.size and (idx.min() < 0 or idx.max() >= K):
+            raise ValueError('discrete action out of range [0, %d)' % K)
+        out = np.zeros(idx.shape + (K,), dtype=np.float32)
+        np.put_along_axis(out, idx[..., None], 1.0, axis=-1)
+        return out
 
     def _batch_obs(self, traj_list):
         out = {}
@@ -71,7 +94,7 @@ class MultistepAggregatorWithInfo:
         return {
             'obs': self._batch_obs([e['obs'] for e in exp_list]),
             'obs_next': self._batch_obs([[e['obs_next']] for e in exp_list]),
-            'actions': np.stack([np.stack(e['actions']) for e in exp_list]),
+            'actions': self._actions(exp_list),
             'rewards': np.stack([np.array(e['rewards']) for e in exp_list]),
             'persistent_infos': persistent,
             'onetime_infos': onetime,

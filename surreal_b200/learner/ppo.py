@@ -15,7 +15,7 @@ from .. import _lib, ops
 from .. import utils as U
 from .._lib import check
 from ..model.lstm_stem import rows_zfilter
-from ..model.ppo_net import PPOModel, DiagGauss
+from ..model.ppo_net import PPOModel, Categorical, make_pd
 from ..model.stem_chain import ChainTrainer, StemChain
 from ..ops import _ptr
 from ..session import ConfigError
@@ -83,11 +83,15 @@ class PPOLearner(Learner):
 
         self.exp_counter = 0
         self.kl_record = []
+        # a discrete action_spec: the categorical policy (K = action_dim logits, one-hot action rows, pd rows [p | log p]);
+        # it runs on the launch chain (csrc/ppo_cat.cu), never on the one-launch epoch kernel
+        self.pd = make_pd(self.env_config.action_spec)
+        self.categorical = isinstance(self.pd, Categorical)
 
         pixel = bool(self.env_config.pixel_input) if 'pixel_input' in self.env_config else False
         mk = dict(obs_spec=self.obs_spec, action_dim=self.action_dim, model_config=lc.model, use_cuda=True,
                   init_log_sig=self.init_log_sig, use_z_filter=self.use_z_filter, if_pixel_input=pixel,
-                  rnn_config=lc.algo.rnn, device=self.device)
+                  rnn_config=lc.algo.rnn, device=self.device, categorical=self.categorical)
         self.model = PPOModel(**mk)
         self.ref_target_model = PPOModel(**mk)
         self.ref_target_model.update_target_params(self.model)
@@ -156,7 +160,6 @@ class PPOLearner(Learner):
                                                      update_freq=an.lr_update_frequency, min_lr=an.min_lr)
 
         self.aggregator = MultistepAggregatorWithInfo(self.env_config.obs_spec, self.env_config.action_spec)
-        self.pd = DiagGauss(self.action_dim)
         self.cells = None
 
         # ---- device state of one learn(): allocated once, reused (graph-friendly, no allocator traffic)
@@ -189,7 +192,8 @@ class PPOLearner(Learner):
         self.dp_v = None
         # all epochs of BOTH optimisers as ONE persistent kernel (csrc/epoch2.cu) instead of ~10 launches per epoch;
         # SB200_EPOCH_KERNEL=0 selects the launch chain (always the path of the pixel / RNN stems)
-        self.use_epoch_kernel = os.environ.get('SB200_EPOCH_KERNEL', '2') != '0' and self.chain is None
+        self.use_epoch_kernel = os.environ.get('SB200_EPOCH_KERNEL', '2') != '0' and self.chain is None and \
+            not self.categorical
         self._ek = None
         self.epoch_kernel_gen = 2 if self.use_epoch_kernel else 0
         self.epoch_history = []
@@ -378,12 +382,19 @@ class PPOLearner(Learner):
         mode = 0 if self.ppo_mode == 'clip' else 1
         if mode == 1:
             self._kl(mean, S['KL_PRE'], 0.0, stop)
-        dlog_var = tr.slabs[0, m.actor.extra_off:m.actor.extra_off + A]
-        check(L.sb200_ppo_policy_loss_f32(mode, _ptr(mean), mean.stride(0), _ptr(m.log_var), _ptr(acts), lda,
-                                          _ptr(self._adv), _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, M, A,
-                                          _ptr(self._hyper), float(self.eta), float(self.kl_target), _ptr(tr.d[-1]),
-                                          tr.d[-1].stride(0), _ptr(dlog_var), _ptr(self._stats), _ptr(self._loss_ws),
-                                          _ptr(stop), st), 'sb200_ppo_policy_loss_f32')
+        if self.categorical:                                      # mean: the K logits; no log_var
+            check(L.sb200_ppo_cat_policy_loss_f32(mode, _ptr(mean), mean.stride(0), _ptr(acts), lda, _ptr(self._adv),
+                                                  _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, M, A, _ptr(self._hyper),
+                                                  float(self.eta), float(self.kl_target), _ptr(tr.d[-1]),
+                                                  tr.d[-1].stride(0), _ptr(self._stats), _ptr(self._loss_ws), _ptr(stop),
+                                                  st), 'sb200_ppo_cat_policy_loss_f32')
+        else:
+            dlog_var = tr.slabs[0, m.actor.extra_off:m.actor.extra_off + A]
+            check(L.sb200_ppo_policy_loss_f32(mode, _ptr(mean), mean.stride(0), _ptr(m.log_var), _ptr(acts), lda,
+                                              _ptr(self._adv), _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, M, A,
+                                              _ptr(self._hyper), float(self.eta), float(self.kl_target), _ptr(tr.d[-1]),
+                                              tr.d[-1].stride(0), _ptr(dlog_var), _ptr(self._stats), _ptr(self._loss_ws),
+                                              _ptr(stop), st), 'sb200_ppo_policy_loss_f32')
         tr.backward()
         self._step(tr, self._actor_chain, self._stats[S['GN_ACTOR']:S['GN_ACTOR'] + 1], stop)
         # post-step KL(ref || current) (ppo.py:553-556)
@@ -396,6 +407,10 @@ class PPOLearner(Learner):
         L = _lib.lib()
         B, A, m, st = self._rows, self.action_dim, self.model, ops._stream()
         dp = self.dp
+        if self.categorical:                                      # KL(ref || softmax(logits)); never data-parallel
+            check(L.sb200_ppo_cat_kl_f32(_ptr(self._ref_pd), 2 * A, _ptr(mean), mean.stride(0), B, A, _ptr(self._stats),
+                                         slot, float(threshold), _ptr(stop), _ptr(self._loss_ws), st), 'sb200_ppo_cat_kl_f32')
+            return
         check(L.sb200_ppo_kl_f32(_ptr(self._ref_pd), 2 * A, _ptr(mean), mean.stride(0), _ptr(m.log_var), B, A,
                                  _ptr(self._stats), slot, float(threshold), _ptr(stop), 0 if dp is None else 1,
                                  _ptr(self._loss_ws), st), 'sb200_ppo_kl_f32')
@@ -409,6 +424,8 @@ class PPOLearner(Learner):
         shard / B local windows; gradients, advantage moments, the KL scalar, z-filter sums and statistics are
         all-reduced.  Parameters start from rank 0's initialisation."""
         from ..parallel import LearnerDP
+        if self.categorical:
+            raise NotImplementedError('categorical policy + data parallel')
         if self.use_r_filter:
             raise NotImplementedError('reward filter + data parallel')
         if self.rnn:
@@ -470,7 +487,7 @@ class PPOLearner(Learner):
         else:
             ops.mlp_forward(ref.actor, self._obs_full, zf_stats=ref.z_stats, zf_eps=ref.z_eps, rows=B, ldx=(n + 1) * D,
                             out=self._ref_mean)
-        ops.make_pd(self._ref_mean, ref.log_var, self._rows, A, self._ref_pd)
+        ref.policy_pd(self._ref_mean, self._rows, self._ref_pd)
         self._stats.zero_()
         self._stop.zero_()
 
@@ -482,9 +499,15 @@ class PPOLearner(Learner):
             for _ in range(self.epoch_baseline):
                 self._value_epoch()
         acts, lda, pds, ldp = self._upd
-        check(L.sb200_ppo_final_stats_f32(_ptr(self._cur_mean), self._cur_mean.stride(0), _ptr(m.log_var),
-                                          _ptr(acts), lda, _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, self._rows, A,
-                                          _ptr(self._stats), _ptr(self._loss_ws), st), 'sb200_ppo_final_stats_f32')
+        if self.categorical:
+            check(L.sb200_ppo_cat_final_stats_f32(_ptr(self._cur_mean), self._cur_mean.stride(0), _ptr(acts), lda,
+                                                  _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, self._rows, A,
+                                                  _ptr(self._stats), _ptr(self._loss_ws), st),
+                  'sb200_ppo_cat_final_stats_f32')
+        else:
+            check(L.sb200_ppo_final_stats_f32(_ptr(self._cur_mean), self._cur_mean.stride(0), _ptr(m.log_var),
+                                              _ptr(acts), lda, _ptr(pds), ldp, _ptr(self._ref_pd), 2 * A, self._rows, A,
+                                              _ptr(self._stats), _ptr(self._loss_ws), st), 'sb200_ppo_final_stats_f32')
         if self.use_z_filter:
             # the rows the updates trained on (step 0 of every window; the first eff_len steps in RNN mode), AFTER the
             # updates (ppo.py:578)
@@ -644,7 +667,8 @@ class PPOLearner(Learner):
         if self.clip_critic_gradient:
             stats['grad_norm_critic'] = float(s[S['GN_CRITIC']])
         stats['_avg_return_targ'] = float(s[S['RET_MEAN']])
-        stats['_avg_log_sig'] = float(s[S['LOG_SIG']])
+        if not self.categorical:                                  # no log_var: no _avg_log_sig
+            stats['_avg_log_sig'] = float(s[S['LOG_SIG']])
         stats['_avg_behave_likelihood'] = float(s[S['BEHAVE_LIK']])
         stats['_avg_is_weight'] = float(s[S['IS_WEIGHT']])
         stats['_ref_behave_diff'] = float(s[S['REF_BEHAVE']])

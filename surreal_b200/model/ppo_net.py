@@ -4,14 +4,40 @@ import collections
 
 import torch
 
-from .. import ops
+from .. import _lib, ops
 
 
 class DiagGauss:
     """Shape bookkeeping only; the distribution math runs inside the loss kernels (csrc/ppo_loss.cu)."""
+    pd_type = _lib.PD_GAUSSIAN
 
     def __init__(self, action_dim):
         self.d = action_dim
+
+
+class Categorical:
+    """Categorical policy of a discrete action space over ``n_actions`` logits (tests/cat_ref.py): pd rows
+    [p | log p], one-hot action rows.  Shape bookkeeping only; the math runs in csrc/ppo_cat.cu."""
+    pd_type = _lib.PD_CATEGORICAL
+
+    def __init__(self, n_actions):
+        self.d = n_actions
+
+
+def make_pd(action_spec):
+    """The policy distribution of an action_spec: Categorical for {'type': 'discrete', 'dim': (K,)}, 2 <= K <=
+    SB200_PPO_CAT_MAX_K, else DiagGauss."""
+    from ..session import ConfigError
+    t = str(action_spec['type'] if isinstance(action_spec, dict) else action_spec.type)
+    d = int((action_spec['dim'] if isinstance(action_spec, dict) else action_spec.dim)[0])
+    if t == 'continuous':
+        return DiagGauss(d)
+    if t != 'discrete':
+        raise ConfigError('action_spec.type must be "continuous" or "discrete", got %r' % t)
+    if not 2 <= d <= _lib.PPO_CAT_MAX_K:
+        raise ConfigError('a discrete action_spec needs 2 <= dim <= %d (the widest layer the fused forward accepts), '
+                          'got %d' % (_lib.PPO_CAT_MAX_K, d))
+    return Categorical(d)
 
 
 def _default_linear_init(dims, seed_gen=None):
@@ -30,13 +56,15 @@ class PPOModel:
     its features through the LSTM stem, and the heads read the LSTM's output."""
 
     def __init__(self, obs_spec, action_dim, model_config, use_cuda=True, init_log_sig=0, use_z_filter=False,
-                 if_pixel_input=False, rnn_config=None, device=None):
+                 if_pixel_input=False, rnn_config=None, device=None, categorical=False):
         self.device = torch.device(device if device is not None else 'cuda')
         if self.device.type != 'cuda':
             raise RuntimeError('surreal_b200 has no CPU path: PPOModel needs a CUDA device')
         self.obs_spec, self.action_dim, self.model_config = obs_spec, action_dim, model_config
         self.use_z_filter, self.init_log_sig = use_z_filter, init_log_sig
         self.if_pixel_input, self.rnn_config = if_pixel_input, rnn_config
+        # categorical: the actor head's last layer is linear with action_dim outputs (the logits) and there is no log_var
+        self.categorical = bool(categorical)
         self.cnn_stem = None
         self.rnn_stem = None
         self.if_rnn = bool(rnn_config is not None and rnn_config.if_rnn_policy)
@@ -66,9 +94,13 @@ class PPOModel:
         D, A = in_dim, action_dim
         ah, ch = list(model_config.actor_fc_hidden_sizes), list(model_config.critic_fc_hidden_sizes)
         R, T, N = ops.ACT_RELU, ops.ACT_TANH, ops.ACT_NONE
-        self.actor = ops.FlatNet([D] + ah + [A], [R] * len(ah) + [T], self.device, extra=A)
+        if self.categorical:
+            self.actor = ops.FlatNet([D] + ah + [A], [R] * len(ah) + [N], self.device)
+            self.actor.load_layers(_default_linear_init(self.actor.dims))
+        else:
+            self.actor = ops.FlatNet([D] + ah + [A], [R] * len(ah) + [T], self.device, extra=A)
+            self.actor.load_layers(_default_linear_init(self.actor.dims), extra=torch.zeros(A) + init_log_sig)
         self.critic = ops.FlatNet([D] + ch + [1], [R] * len(ch) + [N], self.device)
-        self.actor.load_layers(_default_linear_init(self.actor.dims), extra=torch.zeros(A) + init_log_sig)
         self.critic.load_layers(_default_linear_init(self.critic.dims))
         self.z_eps = 1e-5
         self.z_stats = None
@@ -80,7 +112,8 @@ class PPOModel:
     # -- parameters --------------------------------------------------------------------------------
     @property
     def log_var(self):
-        return self.actor.extra_view()
+        """The Gaussian policy's log_var; None for the categorical policy."""
+        return None if self.categorical else self.actor.extra_view()
 
     def update_target_params(self, net):
         """ppo_net.py:226-242: actor, critic and z-filter."""
@@ -120,7 +153,7 @@ class PPOModel:
 
     def state_dict(self):
         """Keys follow the reference module tree (actor.log_var, actor.model.*, critic.model.*, z_filter.*);
-        Linear weights are exported in torch's [out, in] convention."""
+        Linear weights are exported in torch's [out, in] convention.  The categorical policy has no actor.log_var."""
         sd = collections.OrderedDict()
         if self.cnn_stem is not None:
             for k, v in self.cnn_stem.state_items():
@@ -128,7 +161,8 @@ class PPOModel:
         if self.rnn_stem is not None:
             for k, v in self.rnn_stem.state_items():
                 sd[k] = v
-        sd['actor.log_var'] = self.log_var.detach().clone().view(1, -1)
+        if not self.categorical:
+            sd['actor.log_var'] = self.log_var.detach().clone().view(1, -1)
         for name, net in (('actor', self.actor), ('critic', self.critic)):
             for l in range(net.n_layers):
                 w, b = net.get_layer(l)
@@ -143,11 +177,16 @@ class PPOModel:
 
     def load_state_dict(self, sd):
         g = lambda k: torch.as_tensor(sd[k], dtype=torch.float32)  # noqa: E731
+        if ('actor.log_var' in sd) == self.categorical:
+            have, want = ('Gaussian', 'categorical') if self.categorical else ('categorical', 'Gaussian')
+            raise ValueError('state_dict holds a %s policy (%s actor.log_var) but this PPOModel has a %s policy'
+                             % (have, 'with' if have == 'Gaussian' else 'without', want))
         if self.cnn_stem is not None:
             self.cnn_stem.load_state(sd)
         if self.rnn_stem is not None:
             self.rnn_stem.load_torch(sd, prefix='rnn_stem.')
-        self.log_var.copy_(g('actor.log_var').reshape(-1).to(self.device))
+        if not self.categorical:
+            self.log_var.copy_(g('actor.log_var').reshape(-1).to(self.device))
         for name, net in (('actor', self.actor), ('critic', self.critic)):
             for l in range(net.n_layers):
                 net.set_layer(l, g('%s.model.seq.%d.weight' % (name, 2 * l)), g('%s.model.seq.%d.bias' % (name, 2 * l)))
@@ -178,22 +217,25 @@ class PPOModel:
                                       'acts through PPOAgent.act and trains through PPOLearner')
 
     def forward_actor(self, obs, cells=None, out_pd=None):
-        """-> [rows, 2A] = cat(mean, std) (builders.py:114-132)."""
+        """-> [rows, 2A] = cat(mean, std) (builders.py:114-132), or [p | log p] of the categorical policy."""
         self._no_rnn()
         if self.cnn_stem is not None:
-            x2 = self._features(obs)
-            mean = ops.mlp_forward(self.actor, x2)
-            B, A = mean.shape[0], self.action_dim
-            pd = out_pd if out_pd is not None else torch.empty(B, 2 * A, dtype=torch.float32, device=self.device)
-            ops.make_pd(mean, self.log_var, B, A, pd)
-            return pd
-        x = self._flat(obs)
-        x2 = x.reshape(-1, x.shape[-1])
-        mean = ops.mlp_forward(self.actor, x2, zf_stats=self.z_stats, zf_eps=self.z_eps)
+            mean = ops.mlp_forward(self.actor, self._features(obs))
+        else:
+            x = self._flat(obs)
+            x2 = x.reshape(-1, x.shape[-1])
+            mean = ops.mlp_forward(self.actor, x2, zf_stats=self.z_stats, zf_eps=self.z_eps)
         B, A = mean.shape[0], self.action_dim
         pd = out_pd if out_pd is not None else torch.empty(B, 2 * A, dtype=torch.float32, device=self.device)
-        ops.make_pd(mean, self.log_var, B, A, pd)
+        self.policy_pd(mean, B, pd)
         return pd
+
+    def policy_pd(self, head_out, B, pd):
+        """pd rows of the actor head's output rows: [mean | exp(log_var)], or [p | log p] of the logits."""
+        if self.categorical:
+            ops.cat_make_pd(head_out, B, self.action_dim, pd)
+        else:
+            ops.make_pd(head_out, self.log_var, B, self.action_dim, pd)
 
     def forward_critic(self, obs, cells=None):
         self._no_rnn()

@@ -685,5 +685,11 @@ def make_pd(mean, log_var, B, A, pd, log_noise=None):
     return pd
 
 
+def cat_make_pd(logits, B, K, pd):
+    """pd rows [p | log p] of the categorical policy from its logits (sb200_ppo_cat_make_pd_f32)."""
+    check(_lib.lib().sb200_ppo_cat_make_pd_f32(_ptr(logits), logits.stride(0), B, K, _ptr(pd), pd.stride(0), _stream()),
+          'sb200_ppo_cat_make_pd_f32')
+
+
 def zfilter_update(x, rows, D, ldx, stats):
     check(_lib.lib().sb200_zfilter_update_f32(_ptr(x), ldx, rows, D, _ptr(stats), _stream()), 'sb200_zfilter_update_f32')
