@@ -275,9 +275,10 @@ __device__ __forceinline__ void hidden_layer(const Sm& sm, const float* As, int 
     }
 }
 
-// ---- one batch row of the policy loss on a whole warp: lane j holds action dimension j (NO <= 32).  The arithmetic is that
-// of ppo_dev::policy_row / policy_dlogvar / row_kl -- the per-dimension terms are formed in parallel and summed in index
-// order through shuffles (the serial version is a chain of ~1.5 K dependent instructions per row on one lane).
+// ---- one batch row of the policy loss on a whole warp: lane j holds action dimension j (NO <= 32).  The Gaussian terms are
+// those of ppo_loss.cu's policy_row / policy_dlogvar / row_kl, formed in parallel and summed in index order through
+// shuffles (the serial version is a chain of ~1.5 K dependent instructions per row on one lane); the surrogate and c_kl
+// come from ppo_loss_dev.cuh.
 __device__ __forceinline__ float seq_sum(float term, int n) {
     float s = 0.0f;
     for (int j = 0; j < n; ++j) s += __shfl_sync(0xffffffffu, term, j);
@@ -301,55 +302,29 @@ __device__ __forceinline__ float row_kl_warp(const float* rp, const float* mu, c
     return t1 + t2 - 0.5f * (float)A;
 }
 struct RowOut {
-    float surr, rowloss, klrow, dlogvar;      // dlogvar: this lane's dimension
+    float surr, rowloss, dlogvar;             // dlogvar: this lane's dimension
 };
 __device__ __forceinline__ RowOut policy_row_warp(int mode, const float* mu_, const float* act_, const float* s_sig, const float* bp,
-                                                  const float* rp, float ad, int A, float c0, double invB, const double* hyper, double eta,
-                                                  double kl_target, double kl_mean, float* dpre_row, int ldd, int lane) {
+                                                  const float* rp, float ad, int A, float c0, double invB, const double* hyper,
+                                                  float c_kl, float* dpre_row, int ldd, int lane) {
     const bool on = lane < A;
     const float a = on ? act_[lane] : 0.0f, mu = on ? mu_[lane] : 0.0f, sg = on ? s_sig[lane] : 1.0f;
     const float bm = on ? bp[lane] : 0.0f, bs = on ? bp[A + lane] : 1.0f, rm = on ? rp[lane] : 0.0f, rs = on ? rp[A + lane] : 1.0f;
-    RowOut o = {0.0f, 0.0f, 0.0f, 0.0f};
     const float z = (a - mu) / sg;
     const float ll = -0.5f * seq_sum_sq(z, A) - c0 - seq_sum(logf(sg), A);
-    const float Pl = expf(ll);
-    const float Ll = fmaxf(Pl, 1e-5f);
-    const bool live = Pl >= 1e-5f;                                    // clamp(min) passes grad where x >= min
     const float zb = (a - bm) / bs;
     const float llb = -0.5f * seq_sum_sq(zb, A) - c0 - seq_sum(logf(bs), A);
-    const float Lb = fmaxf(expf(llb), 1e-5f);
-    float g_ll = 0.0f, c_kl = 0.0f;
-    if (mode == 0) {
-        const float lo = (float)(1.0 - hyper[0]), hi = (float)(1.0 + hyper[0]);
-        const float ratio = Ll / Lb;
-        const float cr = fminf(fmaxf(ratio, lo), hi);
-        o.surr = -ratio * ad;
-        const float cs = -cr * ad;
-        o.rowloss = fmaxf(o.surr, cs);
-        const float g_ratio = (o.surr >= cs) ? -ad : 0.0f;            // max(1) routes grad to the first max
-        g_ll = live ? (float)((double)g_ratio * invB) * (Pl / Lb) : 0.0f;
-    } else {
-        const float d = rm - mu;
-        o.klrow = seq_sum(logf(sg / rs), A) + seq_sum((rs * rs + d * d) / (2.0f * sg * sg), A) - 0.5f * (float)A;
-        const float den = fmaxf(Lb, 1e-2f);
-        o.surr = -ad * (Ll / den);
-        o.rowloss = o.surr;
-        g_ll = live ? (float)((double)(-ad / den) * invB) * Pl : 0.0f;
-        double ck = hyper[1];
-        if (kl_mean - 2.0 * kl_target > 0.0) ck += 2.0 * eta * (kl_mean - 2.0 * kl_target);
-        c_kl = (float)(ck * invB);
-    }
+    const ppo_dev::Surrogate sr = ppo_dev::surrogate(mode, expf(ll), expf(llb), ad, invB, hyper);
     // gradient w.r.t. the pre-tanh output (mean = tanh(pre)) and this dimension's share of d loss / d log_var
-    float dmu = g_ll * z / sg;
-    float dl = g_ll * (z * z - 1.0f);
+    float dmu = sr.g_ll * z / sg;
+    float dl = sr.g_ll * (z * z - 1.0f);
     if (mode == 1) {
         const float d = rm - mu;
         dmu += c_kl * (-(rm - mu) / (sg * sg));
         dl += c_kl * (1.0f - (rs * rs + d * d) / (sg * sg));
     }
     if (lane < ldd) dpre_row[lane] = on ? dmu * (1.0f - mu * mu) : 0.0f;
-    o.dlogvar = on ? dl : 0.0f;
-    return o;
+    return {sr.surr, sr.rowloss, on ? dl : 0.0f};
 }
 
 // ---- P1a: forward of one row block; leaves xs / h1s / h2s / outs in shared memory and the KL partial in kl_part[rb]
@@ -492,6 +467,7 @@ __device__ void bwd_item(const Job& p, const Sm& sm, int rb, bool resident, doub
     __syncthreads();
     const double invM = 1.0 / (double)M;
     const float c0 = (float)(0.5 * 1.8378770664093453 * (double)NO);
+    const float c_kl = (p.mode == 1) ? ppo_dev::adapt_ckl(kl_mean_now, invM, p.hyper, p.eta, p.kl_target) : 0.0f;
     // loss rows.  Policy: a warp per row, lane j = action dimension j (policy_row_warp).  Value: lanes 0 / 1 of every warp take
     // rows warp / warp + 8 together.  Operands and results live in shared memory: no local arrays.
     double acc_slot[4] = {0.0, 0.0, 0.0, 0.0};
@@ -505,12 +481,11 @@ __device__ void bwd_item(const Job& p, const Sm& sm, int rb, bool resident, doub
                 continue;
             }
             const RowOut o = policy_row_warp(p.mode, sm.outs + r * E2_MAX_OUT, sm.acts + r * E2_MAX_OUT, s_sig, sm.behs + r * 2 * E2_MAX_OUT,
-                                             sm.refs + r * 2 * E2_MAX_OUT, sm.advs[r], NO, c0, invM, p.hyper, p.eta, p.kl_target,
-                                             kl_mean_now, dp, p.ld_out, lane);
+                                             sm.refs + r * 2 * E2_MAX_OUT, sm.advs[r], NO, c0, invM, p.hyper, c_kl, dp, p.ld_out,
+                                             lane);
             if (lane == 0) {
                 acc_slot[0] += (double)o.surr;
                 acc_slot[1] += (double)o.rowloss;
-                acc_slot[2] += (double)o.klrow;
             }
             dl_acc += (double)o.dlogvar;
             __syncwarp();
@@ -521,12 +496,10 @@ __device__ void bwd_item(const Job& p, const Sm& sm, int rb, bool resident, doub
         if (lane < 2 && my_r < RB) {
             float* dp = sm.dps + my_r * E2_MAX_OUT;
             for (int j = 0; j < p.ld_out; ++j) dp[j] = 0.0f;
-            if (m0 + my_r < M) {                             // value_loss_kernel's arithmetic (ppo.py:311-332)
-                const float vv = sm.outs[my_r * E2_MAX_OUT], rr = sm.advs[my_r];
-                const float df = vv - rr;
-                const double d = (double)(rr - vv), rd = (double)rr;
-                dp[0] = (float)(2.0 * (double)df / (double)M);
-                acc_slot[0] = d; acc_slot[1] = d * d; acc_slot[2] = rd; acc_slot[3] = rd * rd;
+            if (m0 + my_r < M) {
+                const ppo_dev::ValueRow vr = ppo_dev::value_row(sm.outs[my_r * E2_MAX_OUT], sm.advs[my_r], M);
+                dp[0] = vr.dpre;
+                acc_slot[0] = vr.d; acc_slot[1] = vr.d * vr.d; acc_slot[2] = vr.r; acc_slot[3] = vr.r * vr.r;
                 for (int j = 0; j < p.ld_out; ++j) p.dpre[(long long)(m0 + my_r) * p.ld_out + j] = dp[j];
             }
         }
@@ -555,7 +528,7 @@ __device__ void bwd_item(const Job& p, const Sm& sm, int rb, bool resident, doub
     }
     {
         double* part = p.loss_part + (size_t)rb * E2_SLOTS;
-        const int ns = policy ? 3 : 4;
+        const int ns = policy ? 2 : 4;                       // policy: [surr, rowloss, unused, unused] + dlog_var
         for (int s = 0; s < ns; ++s) {
             const double t = block_sum(acc_slot[s], s_red);
             if (tid == 0) part[s] = t;
@@ -825,8 +798,6 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
             if (stop_now || !train[j]) {
                 left[j] = true;
                 train[j] = false;
-            } else if (p.mode == 1 && c == 0 && tid == 0) {
-                p.stats[SB200_STAT_KL_PRE] = (float)klm[j];
             }
         }
         // ---------------- adapt mode: the loss needs the KL mean (ppo.py:262-270) -> second half of P1 now
@@ -860,7 +831,7 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
                     __syncthreads();
                     for (int s0 = 0; s0 < 4 + NO; s0 += E2T >> 3) {               // 8 lanes per statistic, uniform trip count
                         const int s = s0 + (tid >> 3);
-                        const bool on = s < 4 + NO && s != 3;
+                        const bool on = s < 4 + NO && (s < 2 || s >= 4);
                         double acc = 0.0;
                         if (on)
                             for (int k = tid & 7; k < p.n_rb; k += 8) acc += __ldcg(&p.loss_part[(size_t)k * E2_SLOTS + s]);
@@ -869,39 +840,16 @@ __global__ void __launch_bounds__(E2T, 1) ppo_epochs2_kernel(const __grid_consta
                         acc += __shfl_xor_sync(0xffffffffu, acc, 1);
                         if (!on || (tid & 7) != 0) continue;
                         if (s >= 4) p.slabs[p.extra_off + (s - 4)] = (float)acc;
-                        if (s == 0) p.stats[SB200_STAT_SURR] = (float)(acc * invM);
-                        if (s == 1 && p.mode == 0) p.stats[SB200_STAT_LOSS] = (float)(acc * invM);
-                        if (s == 0 && p.mode == 1) {
-                            const double kl = klm[j];
-                            double loss = acc * invM + p.hyper[1] * kl;
-                            if (kl - 2.0 * p.kl_target > 0.0) loss += p.eta * (kl - 2.0 * p.kl_target) * (kl - 2.0 * p.kl_target);
-                            p.stats[SB200_STAT_LOSS] = (float)loss;
-                        }
+                        else ppo_dev::loss_stats(p.mode, s, acc, invM, p.hyper, p.eta, p.kl_target, klm[j], p.stats);
                     }
-                    if (tid == 0) {
-                        float slog = 0.0f;
-                        for (int jj = 0; jj < NO; ++jj) slog += logf(s_sig[jj]);
-                        p.stats[SB200_STAT_ENTROPY] = 0.5f * slog + (float)(0.5 * 2.8378770664093453 * (double)NO);   // ppo_net.py:72
-                    }
+                    if (tid == 0) p.stats[SB200_STAT_ENTROPY] = ppo_dev::gauss_entropy(s_sig, NO);
                     __syncthreads();
                 } else if (tid < 32) {
                     double s[4] = {0, 0, 0, 0};
                     for (int k = tid; k < p.n_rb; k += 32)
                         for (int q = 0; q < 4; ++q) s[q] += __ldcg(&p.loss_part[(size_t)k * E2_SLOTS + q]);
                     for (int q = 0; q < 4; ++q) s[q] = warp_sum(s[q]);
-                    if (tid != 0) continue;
-                    const double n = (double)p.M;
-                    const double var_d = (s[1] - s[0] * s[0] / n) / (n - 1.0);
-                    const double var_r = (s[3] - s[2] * s[2] / n) / (n - 1.0);
-                    p.stats[SB200_STAT_VAL_LOSS] = (float)(s[1] / n);
-                    p.stats[SB200_STAT_EXPLAINED_VAR] = (float)(1.0 - var_d / var_r);
-                    p.stats[SB200_STAT_RETURN_MEAN] = (float)(s[2] / n);
-                    for (int q = 0; q < 4; ++q) {
-                        const double mq = s[q] / n;
-                        const float hi = (float)mq;
-                        p.stats[SB200_STAT_VAL_MOMENTS + 2 * q] = hi;
-                        p.stats[SB200_STAT_VAL_MOMENTS + 2 * q + 1] = (float)(mq - (double)hi);
-                    }
+                    if (tid == 0) ppo_dev::value_stats(s, (double)p.M, p.stats);
                 }
             }
         }

@@ -14,6 +14,8 @@ namespace {
 
 using ppo_dev::LossWs;
 using ppo_dev::LT;
+using ppo_dev::put_partial;
+using ppo_dev::grid_sums;
 constexpr int WARPS = LT / 32;
 constexpr int ROWS_PER_WARP = LT / WARPS;
 
@@ -149,10 +151,8 @@ __global__ void __launch_bounds__(LT) cat_make_pd_kernel(const float* __restrict
 // order; the caller reduces the warps' sums in warp order.
 __device__ __forceinline__ int warp_row0(int w) { return blockIdx.x * LT + w * ROWS_PER_WARP; }
 
-// Sum over the block of one value per warp (lane 0's), in warp order; every thread gets it.
-__device__ __forceinline__ double block_warp_sum(double v, double* sh) {
-    return block_sum((threadIdx.x & 31) == 0 ? v : 0.0, sh);
-}
+// A warp's per-row sums are the same on every lane: lane 0 alone brings them into a block partial (put_partial).
+__device__ __forceinline__ double lane0(double v) { return (threadIdx.x & 31) == 0 ? v : 0.0; }
 
 // mode 0: clip (hyper[0] = clip_epsilon)   mode 1: adapt (hyper[1] = beta; ws->kl_mean from cat_kl_kernel(ref, learn))
 __global__ void __launch_bounds__(LT) cat_policy_loss_kernel(int mode, const float* __restrict__ logits, long long ldl,
@@ -169,12 +169,7 @@ __global__ void __launch_bounds__(LT) cat_policy_loss_kernel(int mode, const flo
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const double invB = 1.0 / (double)B;
     const double kl_mean = ws->kl_mean;
-    float c_kl = 0.0f;
-    if (mode == 1) {
-        double ck = hyper[1];
-        if (kl_mean - 2.0 * kl_target > 0.0) ck += 2.0 * eta * (kl_mean - 2.0 * kl_target);
-        c_kl = (float)(ck * invB);
-    }
+    const float c_kl = (mode == 1) ? ppo_dev::adapt_ckl(kl_mean, invB, hyper, eta, kl_target) : 0.0f;
     double s_surr = 0.0, s_loss = 0.0, s_ent = 0.0;
     for (int r = 0; r < ROWS_PER_WARP; ++r) {
         const int b = warp_row0(w) + r;
@@ -194,60 +189,28 @@ __global__ void __launch_bounds__(LT) cat_policy_loss_kernel(int mode, const flo
         pa = warp_sum(pa);
         pb = warp_sum(pb);
         ent = warp_sum(ent);
-        const float Ll = fmaxf(pa, 1e-5f);
-        const bool live = pa >= 1e-5f;                                   // clamp(min) passes grad where x >= min
-        const float Lb = fmaxf(pb, 1e-5f);
-        const float ad = adv[b];
-        float surr, rowloss, g_ll;
-        if (mode == 0) {
-            const float lo = (float)(1.0 - hyper[0]), hi = (float)(1.0 + hyper[0]);
-            const float ratio = Ll / Lb;
-            const float cs = -fminf(fmaxf(ratio, lo), hi) * ad;
-            surr = -ratio * ad;
-            rowloss = fmaxf(surr, cs);
-            const float g_ratio = (surr >= cs) ? -ad : 0.0f;             // max(1) routes grad to the first max
-            g_ll = live ? (float)((double)g_ratio * invB) * (pa / Lb) : 0.0f;
-        } else {
-            const float den = fmaxf(Lb, 1e-2f);
-            surr = -ad * (Ll / den);
-            rowloss = surr;
-            g_ll = live ? (float)((double)(-ad / den) * invB) * pa : 0.0f;
-        }
+        const ppo_dev::Surrogate o = ppo_dev::surrogate(mode, pa, pb, adv[b], invB, hyper);
         // d/dl_j: g_ll * (a_j - p_j) through log p_a, c_kl * (p_j - r_j) through KL(ref || learn)
         float* dr = dlogits + (long long)b * ldd;
         for (int j = lane; j < K; j += 32) {
             const float pj = sm.p(l[j]);
-            float d = g_ll * (a[j] - pj);
+            float d = o.g_ll * (a[j] - pj);
             if (mode == 1) d += c_kl * (pj - rp[j]);
             dr[j] = d;
         }
         for (int j = K + lane; j < ldd; j += 32) dr[j] = 0.0f;
-        s_surr += (double)surr;
-        s_loss += (double)rowloss;
+        s_surr += (double)o.surr;
+        s_loss += (double)o.rowloss;
         s_ent += (double)ent;
     }
-    double* part = ws->partial + (size_t)blockIdx.x * 3;
-    double t;
-    t = block_warp_sum(s_surr, sh);
-    if (threadIdx.x == 0) part[0] = t;
-    t = block_warp_sum(s_loss, sh);
-    if (threadIdx.x == 0) part[1] = t;
-    t = block_warp_sum(s_ent, sh);
-    if (threadIdx.x == 0) part[2] = t;
+    put_partial(ws, 3, 0, lane0(s_surr), sh);
+    put_partial(ws, 3, 1, lane0(s_loss), sh);
+    put_partial(ws, 3, 2, lane0(s_ent), sh);
     if (last_block_ticket(&ws->counter, gridDim.x) && threadIdx.x == 0) {
-        double s[3] = {0.0, 0.0, 0.0};
-        for (unsigned int k = 0; k < gridDim.x; ++k)
-            for (int q = 0; q < 3; ++q) s[q] += ws->partial[(size_t)k * 3 + q];
-        stats[SB200_STAT_SURR] = (float)(s[0] * invB);
+        double s[3];
+        grid_sums(ws, 3, 0, s);
+        for (int q = 0; q < 2; ++q) ppo_dev::loss_stats(mode, q, s[q], invB, hyper, eta, kl_target, kl_mean, stats);
         stats[SB200_STAT_ENTROPY] = (float)(s[2] * invB);
-        if (mode == 0) {
-            stats[SB200_STAT_LOSS] = (float)(s[1] * invB);
-        } else {
-            double loss = s[0] * invB + hyper[1] * kl_mean;
-            if (kl_mean - 2.0 * kl_target > 0.0) loss += eta * (kl_mean - 2.0 * kl_target) * (kl_mean - 2.0 * kl_target);
-            stats[SB200_STAT_LOSS] = (float)loss;
-            stats[SB200_STAT_KL_PRE] = (float)kl_mean;
-        }
     }
 }
 
@@ -277,12 +240,11 @@ __global__ void __launch_bounds__(LT) cat_kl_kernel(const float* __restrict__ p0
         if (b >= B) break;
         acc += (double)row_cat_kl(p0 + (long long)b * ld0, logits + (long long)b * ldl, false, K, lane);
     }
-    const double t = block_warp_sum(acc, sh);
-    if (threadIdx.x == 0) ws->partial[blockIdx.x] = t;
+    put_partial(ws, 1, 0, lane0(acc), sh);
     if (last_block_ticket(&ws->counter, gridDim.x) && threadIdx.x == 0) {
-        double s = 0.0;
-        for (unsigned int k = 0; k < gridDim.x; ++k) s += ws->partial[k];
-        ppo_dev::kl_publish((float)(s / (double)B), ws, stats, slot, stop_threshold, stop, 0);
+        double s[1];
+        grid_sums(ws, 1, 0, s);
+        ppo_dev::kl_publish((float)(s[0] / (double)B), ws, stats, slot, stop_threshold, stop, 0);
     }
 }
 
@@ -314,21 +276,13 @@ __global__ void __launch_bounds__(LT) cat_final_stats_kernel(const float* __rest
         isw += (double)(Lc / (Lb + 1e-4f));
         kd += (double)row_cat_kl(ref + (long long)b * ldr, bp, true, K, lane);
     }
-    double* part = ws->partial + (size_t)blockIdx.x * 3;
-    double t;
-    t = block_warp_sum(lb, sh);
-    if (threadIdx.x == 0) part[0] = t;
-    t = block_warp_sum(isw, sh);
-    if (threadIdx.x == 0) part[1] = t;
-    t = block_warp_sum(kd, sh);
-    if (threadIdx.x == 0) part[2] = t;
+    put_partial(ws, 3, 0, lane0(lb), sh);
+    put_partial(ws, 3, 1, lane0(isw), sh);
+    put_partial(ws, 3, 2, lane0(kd), sh);
     if (last_block_ticket(&ws->counter, gridDim.x) && threadIdx.x == 0) {
-        double s[3] = {0.0, 0.0, 0.0};
-        for (unsigned int k = 0; k < gridDim.x; ++k)
-            for (int q = 0; q < 3; ++q) s[q] += ws->partial[(size_t)k * 3 + q];
-        stats[SB200_STAT_BEHAVE_LIK] = (float)(s[0] / B);
-        stats[SB200_STAT_IS_WEIGHT] = (float)(s[1] / B);
-        stats[SB200_STAT_REF_BEHAVE_KL] = (float)(s[2] / B);
+        double s[3];
+        grid_sums(ws, 3, 0, s);
+        ppo_dev::closing_stats(s, B, stats);
     }
 }
 

@@ -15,9 +15,63 @@ namespace {
 
 using ppo_dev::LT;
 using ppo_dev::MAX_A;
-using ppo_dev::row_loglik;
-using ppo_dev::row_kl;
 using ppo_dev::LossWs;
+using ppo_dev::put_partial;
+using ppo_dev::grid_sums;
+
+__device__ __forceinline__ float row_loglik(const float* a, const float* mu, const float* sg, int A, float c0) {
+    // ppo_net.py:39-40:  -0.5*sum(((a-mu)/std)^2) - 0.5*log(2pi)*d - sum(log std)
+    float quad = 0.0f, slog = 0.0f;
+    for (int j = 0; j < A; ++j) {
+        const float z = (a[j] - mu[j]) / sg[j];
+        quad += z * z;
+        slog += logf(sg[j]);
+    }
+    return -0.5f * quad - c0 - slog;
+}
+
+__device__ __forceinline__ float row_kl(const float* m0, const float* s0, const float* m1, const float* s1, int A) {
+    // ppo_net.py:61-62: KL(p0 || p1)
+    float t1 = 0.0f, t2 = 0.0f;
+    for (int j = 0; j < A; ++j) {
+        t1 += logf(s1[j] / s0[j]);
+        const float d = m0[j] - m1[j];
+        t2 += (s0[j] * s0[j] + d * d) / (2.0f * s1[j] * s1[j]);
+    }
+    return t1 + t2 - 0.5f * (float)A;
+}
+
+// One batch row of the policy loss and its gradient w.r.t. the pre-tanh head output (dpre_row[0..ldd), zero padded).
+// c_kl: adapt mode's ppo_dev::adapt_ckl.
+__device__ __forceinline__ ppo_dev::Surrogate policy_row(int mode, const float* mu, const float* act, const float* s_sig,
+                                                         const float* bp, const float* rp, float ad, int A, float c0,
+                                                         double invB, const double* hyper, float c_kl, float* dpre_row,
+                                                         int ldd) {
+    const float P = expf(row_loglik(act, mu, s_sig, A, c0));
+    const float Pb = expf(row_loglik(act, bp, bp + A, A, c0));
+    const ppo_dev::Surrogate o = ppo_dev::surrogate(mode, P, Pb, ad, invB, hyper);
+    // gradient w.r.t. the pre-tanh output (mean = tanh(pre))
+    for (int j = 0; j < A; ++j) {
+        const float z = (act[j] - mu[j]) / s_sig[j];
+        float dmu = o.g_ll * z / s_sig[j];
+        if (mode == 1) dmu += c_kl * (-(rp[j] - mu[j]) / (s_sig[j] * s_sig[j]));
+        dpre_row[j] = dmu * (1.0f - mu[j] * mu[j]);
+    }
+    for (int j = A; j < ldd; ++j) dpre_row[j] = 0.0f;
+    return o;
+}
+
+// this row's contribution to d loss / d log_var[j]
+__device__ __forceinline__ float policy_dlogvar(int mode, int j, const float* mu, const float* act, const float* s_sig,
+                                                const float* rp, float g_ll, float c_kl, int A) {
+    const float z = (act[j] - mu[j]) / s_sig[j];
+    float dl = g_ll * (z * z - 1.0f);
+    if (mode == 1) {
+        const float d = rp[j] - mu[j];
+        dl += c_kl * (1.0f - (rp[A + j] * rp[A + j] + d * d) / (s_sig[j] * s_sig[j]));
+    }
+    return dl;
+}
 
 // ------------------------------------------------------------------------------------------------
 // mode 0: clip   mode 1: adapt (needs ws->kl_mean from kl_kernel(ref, learn))
@@ -36,61 +90,41 @@ __global__ void __launch_bounds__(LT) policy_loss_kernel(int mode, const float* 
     __shared__ float s_sig[MAX_A];
     const int tid = threadIdx.x;
     const int b = blockIdx.x * LT + tid;
-    const int nslots = 3 + A;
+    const int nslots = 3 + A;                                            // [surr, rowloss, unused] + dlog_var[A]
     for (int j = tid; j < A; j += LT) s_sig[j] = expf(log_var[j]);       // builders.py:127: std = exp(log_var)
     __syncthreads();
     const float c0 = (float)(0.5 * 1.8378770664093453 * (double)A);      // 0.5*log(2*pi)*d
     const double invB = 1.0 / (double)B;
+    const float c_kl = (mode == 1) ? ppo_dev::adapt_ckl(ws->kl_mean, invB, hyper, eta, kl_target) : 0.0f;
 
     float mu[MAX_A], act[MAX_A];
-    ppo_dev::PolicyRow pr = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    ppo_dev::Surrogate pr = {0.0f, 0.0f, 0.0f};
     const bool live_row = b < B;
+    const float* rp = ref + (long long)b * ldr;
     if (live_row) {
         for (int j = 0; j < A; ++j) {
             mu[j] = mean[(long long)b * ldm + j];
             act[j] = actions[(long long)b * lda + j];
         }
-        pr = ppo_dev::policy_row(mode, mu, act, s_sig, behave + (long long)b * ldb, ref + (long long)b * ldr, adv[b], A, c0,
-                                 invB, hyper, eta, kl_target, ws->kl_mean, dpre + (long long)b * ldd, (int)ldd);
+        pr = policy_row(mode, mu, act, s_sig, behave + (long long)b * ldb, rp, adv[b], A, c0, invB, hyper, c_kl,
+                        dpre + (long long)b * ldd, (int)ldd);
     }
-    const float surr = pr.surr, rowloss = pr.rowloss, klrow = pr.klrow;
-    // ---- block partials: [surr, rowloss, kl] + dlog_var[A]
-    double* part = ws->partial + (size_t)blockIdx.x * nslots;
-    double t;
-    t = block_sum(live_row ? (double)surr : 0.0, sh);
-    if (tid == 0) part[0] = t;
-    t = block_sum(live_row ? (double)rowloss : 0.0, sh);
-    if (tid == 0) part[1] = t;
-    t = block_sum(live_row ? (double)klrow : 0.0, sh);
-    if (tid == 0) part[2] = t;
+    put_partial(ws, nslots, 0, live_row ? (double)pr.surr : 0.0, sh);
+    put_partial(ws, nslots, 1, live_row ? (double)pr.rowloss : 0.0, sh);
     for (int j = 0; j < A; ++j) {
         float dl = 0.0f;
-        if (live_row) dl = ppo_dev::policy_dlogvar(mode, j, mu, act, s_sig, ref + (long long)b * ldr, pr, A);
-        t = block_sum((double)dl, sh);
-        if (tid == 0) part[3 + j] = t;
+        if (live_row) dl = policy_dlogvar(mode, j, mu, act, s_sig, rp, pr.g_ll, c_kl, A);
+        put_partial(ws, nslots, 3 + j, (double)dl, sh);
     }
     if (last_block_ticket(&ws->counter, gridDim.x)) {
         for (int s = tid; s < nslots; s += LT) {
-            double acc = 0.0;
-            for (unsigned int k = 0; k < gridDim.x; ++k) acc += ws->partial[(size_t)k * nslots + s];
-            if (s >= 3) dlog_var[s - 3] = (float)acc;
-            if (s == 0) stats[SB200_STAT_SURR] = (float)(acc * invB);
-            if (s == 1 && mode == 0) stats[SB200_STAT_LOSS] = (float)(acc * invB);
-            if (s == 2 && mode == 1) stats[SB200_STAT_KL_PRE] = (float)ws->kl_mean;
+            if (s == 2) continue;
+            double acc[1];
+            grid_sums(ws, nslots, s, acc);
+            if (s >= 3) dlog_var[s - 3] = (float)acc[0];
+            else ppo_dev::loss_stats(mode, s, acc[0], invB, hyper, eta, kl_target, ws->kl_mean, stats);
         }
-        if (tid == 0) {
-            float slog = 0.0f;
-            for (int j = 0; j < A; ++j) slog += logf(s_sig[j]);
-            stats[SB200_STAT_ENTROPY] = 0.5f * slog + (float)(0.5 * 2.8378770664093453 * (double)A);   // ppo_net.py:72
-            if (mode == 1) {
-                double surr_sum = 0.0;
-                for (unsigned int k = 0; k < gridDim.x; ++k) surr_sum += ws->partial[(size_t)k * nslots + 0];
-                const double kl = ws->kl_mean;
-                double loss = surr_sum * invB + hyper[1] * kl;
-                if (kl - 2.0 * kl_target > 0.0) loss += eta * (kl - 2.0 * kl_target) * (kl - 2.0 * kl_target);
-                stats[SB200_STAT_LOSS] = (float)loss;
-            }
-        }
+        if (tid == 0) stats[SB200_STAT_ENTROPY] = ppo_dev::gauss_entropy(s_sig, A);
     }
 }
 
@@ -109,15 +143,12 @@ __global__ void __launch_bounds__(LT) kl_kernel(const float* __restrict__ p0, lo
     __syncthreads();
     float kl = 0.0f;
     if (b < B) kl = row_kl(p0 + (long long)b * ld0, p0 + (long long)b * ld0 + A, mean + (long long)b * ldm, s_sig, A);
-    const double t = block_sum((double)kl, sh);
-    if (tid == 0) ws->partial[blockIdx.x] = t;
-    if (last_block_ticket(&ws->counter, gridDim.x)) {
-        if (tid == 0) {
-            double acc = 0.0;
-            for (unsigned int k = 0; k < gridDim.x; ++k) acc += ws->partial[k];
-            // .mean() in fp32; data-parallel (defer): all-reduce ws->kl_mean, then kl_apply
-            ppo_dev::kl_publish((float)(acc / (double)B), ws, stats, slot, stop_threshold, stop, defer);
-        }
+    put_partial(ws, 1, 0, (double)kl, sh);
+    // .mean() in fp32; data-parallel (defer): all-reduce ws->kl_mean, then kl_apply
+    if (last_block_ticket(&ws->counter, gridDim.x) && tid == 0) {
+        double s[1];
+        grid_sums(ws, 1, 0, s);
+        ppo_dev::kl_publish((float)(s[0] / (double)B), ws, stats, slot, stop_threshold, stop, defer);
     }
 }
 
@@ -137,39 +168,20 @@ __global__ void __launch_bounds__(LT) value_loss_kernel(const float* __restrict_
     const int tid = threadIdx.x, b = blockIdx.x * LT + tid;
     double d = 0.0, r = 0.0;
     if (b < B) {
-        const float vv = v[(long long)b * ldv], rr = ret[b];
-        const float df = vv - rr;
-        d = (double)(rr - vv);
-        r = (double)rr;
-        dpre[(long long)b * ldd] = (float)(2.0 * (double)df / (double)B);
+        const ppo_dev::ValueRow vr = ppo_dev::value_row(v[(long long)b * ldv], ret[b], B);
+        d = vr.d;
+        r = vr.r;
+        dpre[(long long)b * ldd] = vr.dpre;
         for (int j = 1; j < (int)ldd; ++j) dpre[(long long)b * ldd + j] = 0.0f;
     }
-    double* part = ws->partial + (size_t)blockIdx.x * 4;
-    double t;
-    t = block_sum(d, sh);       if (tid == 0) part[0] = t;
-    t = block_sum(d * d, sh);   if (tid == 0) part[1] = t;
-    t = block_sum(r, sh);       if (tid == 0) part[2] = t;
-    t = block_sum(r * r, sh);   if (tid == 0) part[3] = t;
-    if (last_block_ticket(&ws->counter, gridDim.x)) {
-        if (tid == 0) {
-            double s[4] = {0, 0, 0, 0};
-            for (unsigned int k = 0; k < gridDim.x; ++k)
-                for (int q = 0; q < 4; ++q) s[q] += ws->partial[(size_t)k * 4 + q];
-            const double n = (double)B;
-            const double var_d = (s[1] - s[0] * s[0] / n) / (n - 1.0);
-            const double var_r = (s[3] - s[2] * s[2] / n) / (n - 1.0);
-            stats[SB200_STAT_VAL_LOSS] = (float)(s[1] / n);
-            stats[SB200_STAT_EXPLAINED_VAR] = (float)(1.0 - var_d / var_r);
-            stats[SB200_STAT_RETURN_MEAN] = (float)(s[2] / n);
-            // raw moments as (hi, lo) float pairs: a data-parallel learner averages them over ranks and recomputes the
-            // explained variance of the GLOBAL batch (a mean of per-rank ratios is not the ratio of the global moments)
-            for (int q = 0; q < 4; ++q) {
-                const double m = s[q] / n;
-                const float hi = (float)m;
-                stats[SB200_STAT_VAL_MOMENTS + 2 * q] = hi;
-                stats[SB200_STAT_VAL_MOMENTS + 2 * q + 1] = (float)(m - (double)hi);
-            }
-        }
+    put_partial(ws, 4, 0, d, sh);
+    put_partial(ws, 4, 1, d * d, sh);
+    put_partial(ws, 4, 2, r, sh);
+    put_partial(ws, 4, 3, r * r, sh);
+    if (last_block_ticket(&ws->counter, gridDim.x) && tid == 0) {
+        double s[4];
+        grid_sums(ws, 4, 0, s);
+        ppo_dev::value_stats(s, (double)B, stats);
     }
 }
 
@@ -191,29 +203,22 @@ __global__ void __launch_bounds__(LT) final_stats_kernel(const float* __restrict
         const float* a = actions + (long long)b * lda;
         const float* bp = behave + (long long)b * ldb;
         const float* rp = ref + (long long)b * ldr;
-        const float Lb = fmaxf(expf(row_loglik(a, bp, bp + A, A, c0, nullptr)), 1e-5f);
-        const float Lc = fmaxf(expf(row_loglik(a, mean + (long long)b * ldm, s_sig, A, c0, nullptr)), 1e-5f);
+        const float Lb = fmaxf(expf(row_loglik(a, bp, bp + A, A, c0)), 1e-5f);
+        const float Lc = fmaxf(expf(row_loglik(a, mean + (long long)b * ldm, s_sig, A, c0)), 1e-5f);
         lb = (double)Lb;
         isw = (double)(Lc / (Lb + 1e-4f));
         kd = (double)row_kl(rp, rp + A, bp, bp + A, A);
     }
-    double* part = ws->partial + (size_t)blockIdx.x * 3;
-    double t;
-    t = block_sum(lb, sh);  if (tid == 0) part[0] = t;
-    t = block_sum(isw, sh); if (tid == 0) part[1] = t;
-    t = block_sum(kd, sh);  if (tid == 0) part[2] = t;
-    if (last_block_ticket(&ws->counter, gridDim.x)) {
-        if (tid == 0) {
-            double s[3] = {0, 0, 0};
-            for (unsigned int k = 0; k < gridDim.x; ++k)
-                for (int q = 0; q < 3; ++q) s[q] += ws->partial[(size_t)k * 3 + q];
-            stats[SB200_STAT_BEHAVE_LIK] = (float)(s[0] / B);
-            stats[SB200_STAT_IS_WEIGHT] = (float)(s[1] / B);
-            stats[SB200_STAT_REF_BEHAVE_KL] = (float)(s[2] / B);
-            float lv = 0.0f;
-            for (int j = 0; j < A; ++j) lv += log_var[j];
-            stats[SB200_STAT_LOG_SIG] = lv / (float)A;
-        }
+    put_partial(ws, 3, 0, lb, sh);
+    put_partial(ws, 3, 1, isw, sh);
+    put_partial(ws, 3, 2, kd, sh);
+    if (last_block_ticket(&ws->counter, gridDim.x) && tid == 0) {
+        double s[3];
+        grid_sums(ws, 3, 0, s);
+        ppo_dev::closing_stats(s, B, stats);
+        float lv = 0.0f;
+        for (int j = 0; j < A; ++j) lv += log_var[j];
+        stats[SB200_STAT_LOG_SIG] = lv / (float)A;
     }
 }
 
