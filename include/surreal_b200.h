@@ -630,6 +630,32 @@ int sb200_synth_env_window_step_f32(float* state, const float* action, const flo
                                     const uint64_t* step_counter, float* obs_next, float* reward, float* done,
                                     const sb200_windows* windows, void* stream);
 
+/* Classic-control tasks, batched and device-resident (csrc/classic_env.cu; semantics: tests/classic_ref.py).  No
+ * counterpart in the reference, which reaches these tasks through gym.  One thread per actor.
+ *   SB200_CLASSIC_CARTPOLE: CartPole-v1.  state = obs = (x, x_dot, theta, theta_dot) [N][4]; action one-hot rows [N][2]
+ *     (index 1, i.e. a[1] > a[0], pushes right); reward 1; terminal when |x| > 2.4 or |theta| > 12 deg (strict, against
+ *     the fp32 thresholds).  Registered episode limit 500.
+ *   SB200_CLASSIC_PENDULUM: Pendulum-v1.  state (theta, theta_dot) [N][2], obs (cos, sin, theta_dot) [N][3]; action
+ *     [N][1] clipped to [-1, 1] and scaled to the torque 2a; never terminal.  Registered episode limit 200.
+ * ep_step [N] counts the steps of each actor's episode, episode [N] its episode index.  done = terminal or ep_step
+ * reaching max_steps (> 0; <= 0: no cap).  Done actors start episode index + 1 in the same launch.  Reset states are
+ * drawn from Philox4x32-10 keyed (seed ^ const, episode index, actor).
+ *   classic_env_reset: every actor to episode 0, ep_step 0; state and obs drawn.
+ *   classic_env_step: obs [N][D] = what each actor observes next (reset where done), obs_next [N][D] = the true
+ *     successor (terminal where done), reward [N], done [N] (0 / 1).
+ *   classic_env_window_step: classic_env_step fused with the commit half of ppo_window_step (`windows`, whose dest
+ *     ppo_sample has assigned; windows->D and ->A must be the task's). */
+#define SB200_CLASSIC_CARTPOLE 0
+#define SB200_CLASSIC_PENDULUM 1
+int sb200_classic_env_reset_f32(int task, int N, uint64_t seed, float* state, float* obs, int* ep_step, int* episode,
+                                void* stream);
+int sb200_classic_env_step_f32(int task, const float* action, int N, int max_steps, uint64_t seed, float* state,
+                               float* obs, int* ep_step, int* episode, float* obs_next, float* reward, float* done,
+                               void* stream);
+int sb200_classic_env_window_step_f32(int task, const float* action, int N, int max_steps, uint64_t seed, float* state,
+                                      float* obs, int* ep_step, int* episode, float* obs_next, float* reward,
+                                      float* done, const sb200_windows* windows, void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * DDPG parameter-space exploration noise (surreal/agent/param_noise.py:9-74, ddpg_agent.py:136-153,174-175): every
  * actor acts with its own perturbed copy of the policy.  Images are [N][actor_stride] floats, each in the layout of

@@ -114,6 +114,7 @@ PPO_CAT_MAX_K = 4096                    # SB200_PPO_CAT_MAX_K
 
 
 DDPG_FWD_FUSED, DDPG_FWD_PACKED, DDPG_FWD_PER_ACTOR = 0, 1, 2
+CLASSIC_CARTPOLE, CLASSIC_PENDULUM = 0, 1       # SB200_CLASSIC_*
 
 
 class DDPGAct(C.Structure):
@@ -249,6 +250,9 @@ def _declare(lib):
         'sb200_fifo_state_bytes': (S, []),
         'sb200_ppo_window_step_f32': (I, [C.POINTER(Windows), C.POINTER(WindowRows), P]),
         'sb200_synth_env_window_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, C.POINTER(Windows), P]),
+        'sb200_classic_env_reset_f32': (I, [I, I, C.c_uint64, P, P, P, P, P]),
+        'sb200_classic_env_step_f32': (I, [I, P, I, I, C.c_uint64, P, P, P, P, P, P, P, P]),
+        'sb200_classic_env_window_step_f32': (I, [I, P, I, I, C.c_uint64, P, P, P, P, P, P, P, C.POINTER(Windows), P]),
         'sb200_fifo_pop': (I, [P, I, P, P, P]),
         'sb200_fifo_push': (I, [P, I, P, P]),
         'sb200_replay_gather_f32': (I, [P, L, P, P, I, P, P]),

@@ -180,11 +180,15 @@ class Agent(metaclass=U.AutoInitializeMeta):
         return isinstance(x, torch.Tensor) and x.is_cuda
 
     def get_env(self):
-        from ..env import SyntheticEnv
+        from ..env import SyntheticEnv, make_classic_env
         ec = self.env_config
+        env = make_classic_env(ec, self.num_envs)
+        if env is not None:
+            return env
         name = ec.env_name if 'env_name' in ec else ''
         if not str(name).startswith('synthetic'):
-            raise ValueError('only the device-resident synthetic env ships with surreal_b200 (env_name "synthetic"); '
+            raise ValueError('only the device-resident envs ship with surreal_b200 (env_name "synthetic", '
+                             '"classic:CartPole-v1", "classic:Pendulum-v1"); '
                              'gym / dm_control / robosuite adapters are out of scope -- pass your own env to '
                              'main_setup(env)')
         from ..utils import obs_is_pixel

@@ -342,12 +342,16 @@ class PPOAgent(Agent):
         return {'model': {'convs': '_list_', 'fc_hidden_sizes': '_list_'}}
 
     def get_env(self):
-        """The in-tree synthetic env; for a discrete action_spec its discrete form (one-hot action rows), as QAgent's."""
+        """The in-tree device env: a classic-control task, or the synthetic env -- for a discrete action_spec its discrete
+        form (one-hot action rows), as QAgent's."""
         if not self.categorical:
             return super().get_env()
-        from ..env import DiscreteSyntheticEnv
+        from ..env import DiscreteSyntheticEnv, make_classic_env
         from ..utils import obs_is_pixel
         ec = self.env_config
+        env = make_classic_env(ec, self.num_envs)
+        if env is not None:
+            return env
         name = ec.env_name if 'env_name' in ec else ''
         if not str(name).startswith('synthetic') or obs_is_pixel(ec.obs_spec):
             return super().get_env()

@@ -143,8 +143,11 @@ class QAgent(Agent):
                 'eval': {'eps': '_float_'}}
 
     def get_env(self):
-        from ..env import DiscreteSyntheticEnv
+        from ..env import DiscreteSyntheticEnv, make_classic_env
         ec = self.env_config
+        env = make_classic_env(ec, self.num_envs)
+        if env is not None:
+            return env
         name = ec.env_name if 'env_name' in ec else ''
         if not str(name).startswith('synthetic'):
             return super().get_env()

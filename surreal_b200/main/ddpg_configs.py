@@ -87,7 +87,7 @@ class DDPGLauncher:
         from ..agent import DDPGAgent
         from ..learner import DDPGLearner
         from ..replay import UniformReplay, PrioritizedReplay
-        from .ppo_configs import make_synthetic_env_config
+        from .ppo_configs import make_synthetic_env_config, make_classic_env_config
 
         class _DDPGLauncher(SurrealDefaultLauncher):
             def __init__(self):
@@ -96,10 +96,13 @@ class DDPGLauncher:
 
             def setup(self, argv):
                 args = ddpg_argparser().parse_args(args=argv)
-                dims = args.env.split(':')[1:] if ':' in args.env else []
-                D = int(dims[0]) if len(dims) > 0 else 64
-                A = int(dims[1]) if len(dims) > 1 else 8
-                make_synthetic_env_config(self.env_config, args.num_agents, D, A)
+                if args.env.startswith('classic:'):
+                    make_classic_env_config(self.env_config, args.env, args.num_agents)
+                else:
+                    dims = args.env.split(':')[1:] if ':' in args.env else []
+                    D = int(dims[0]) if len(dims) > 0 else 64
+                    A = int(dims[1]) if len(dims) > 1 else 8
+                    make_synthetic_env_config(self.env_config, args.num_agents, D, A)
                 self.env_config.num_agents = args.num_agents
                 self.session_config.folder = args.experiment_folder
                 self.session_config.agent.num_gpus = args.agent_num_gpus

@@ -5,6 +5,7 @@ import argparse
 
 from ..session import Config, BASE_LEARNER_CONFIG
 from .ddpg_configs import DDPG_DEFAULT_ENV_CONFIG, DDPG_DEFAULT_SESSION_CONFIG
+from .ppo_configs import make_classic_env_config
 
 DQN_DEFAULT_LEARNER_CONFIG = Config({
     'model': {'convs': '_list_', 'fc_hidden_sizes': '_list_', 'dueling': '_bool_'},
@@ -37,7 +38,7 @@ def make_discrete_synthetic_env_config(env_config, num_envs, obs_dim=64, n_actio
 
 def dqn_argparser():
     p = argparse.ArgumentParser()
-    p.add_argument('--env', type=str, required=True)            # synthetic[:D[:n_actions]]
+    p.add_argument('--env', type=str, required=True)            # synthetic[:D[:n_actions]] or classic:CartPole-v1
     p.add_argument('--num-agents', type=int, required=True)
     p.add_argument('--experiment-folder', required=True)
     p.add_argument('--restore-folder', type=str, default=None)
@@ -74,10 +75,13 @@ class DQNLauncher:
 
             def setup(self, argv):
                 args = dqn_argparser().parse_args(args=argv)
-                dims = args.env.split(':')[1:] if ':' in args.env else []
-                D = int(dims[0]) if len(dims) > 0 else 64
-                n = int(dims[1]) if len(dims) > 1 else 18
-                make_discrete_synthetic_env_config(self.env_config, args.num_agents, D, n)
+                if args.env.startswith('classic:'):
+                    make_classic_env_config(self.env_config, args.env, args.num_agents)
+                else:
+                    dims = args.env.split(':')[1:] if ':' in args.env else []
+                    D = int(dims[0]) if len(dims) > 0 else 64
+                    n = int(dims[1]) if len(dims) > 1 else 18
+                    make_discrete_synthetic_env_config(self.env_config, args.num_agents, D, n)
                 self.env_config.num_agents = args.num_agents
                 lc = self.learner_config
                 lc.model.convs, lc.model.fc_hidden_sizes = [], list(args.fc_hidden_sizes)

@@ -85,6 +85,23 @@ def make_synthetic_env_config(env_config, num_envs, obs_dim=64, action_dim=8, se
     return env_config
 
 
+def make_classic_env_config(env_config, name, num_envs, seed=0):
+    """obs_spec / action_spec of a classic-control task (``name`` = 'classic:CartPole-v1' or 'classic:Pendulum-v1',
+    env.classic), and limit_episode_length = the task's registered limit (500 / 200), which the PPO env tree's 200 would
+    otherwise cut short; a caller may override it afterwards."""
+    from ..env.classic import classic_env_class
+    cls = classic_env_class(name)
+    if cls is None:
+        raise ValueError('%r is not a classic-control env name (classic:<task>)' % (name,))
+    env_config.env_name = str(name)
+    env_config.num_envs = int(num_envs)
+    env_config.seed = int(seed)
+    env_config.obs_spec = {'low_dim': {'flat_inputs': (cls.D,)}}
+    env_config.action_spec = {'dim': (cls.A,), 'type': cls.ACTION_TYPE}
+    env_config.limit_episode_length = cls.MAX_STEPS
+    return env_config
+
+
 def make_synthetic_pixel_env_config(env_config, num_envs, frame_shape=(4, 84, 84), action_dim=8, seed=0):
     """Pixel flavour (BASELINE configs[3]): obs_spec = {'pixel': {'camera0': (C, H, W)}}, pixel_input on -- what
     surreal.env.make_env_config fills in for a pixel env (docs/env.md:79-108)."""
@@ -114,10 +131,13 @@ class PPOLauncher:
             def setup(self, argv):
                 args = ppo_argparser().parse_args(args=argv)
                 name = args.env
-                dims = name.split(':')[1:] if ':' in name else []
-                D = int(dims[0]) if len(dims) > 0 else 64
-                A = int(dims[1]) if len(dims) > 1 else 8
-                make_synthetic_env_config(self.env_config, args.num_agents, D, A)
+                if name.startswith('classic:'):
+                    make_classic_env_config(self.env_config, name, args.num_agents)
+                else:
+                    dims = name.split(':')[1:] if ':' in name else []
+                    D = int(dims[0]) if len(dims) > 0 else 64
+                    A = int(dims[1]) if len(dims) > 1 else 8
+                    make_synthetic_env_config(self.env_config, args.num_agents, D, A)
                 self.session_config.folder = args.experiment_folder
                 self.session_config.agent.num_gpus = args.agent_num_gpus
                 self.session_config.learner.num_gpus = args.num_gpus
