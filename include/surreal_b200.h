@@ -155,12 +155,6 @@ int sb200_conv_backward_dw_f32(int layer, const void* x, int in_u8, const float*
 int sb200_conv_backward_dx_f32(int layer, const float* dy, const float* Wk, const float* act, int64_t frames, int CIN, int H,
                                int W, float* dx, void* stream);
 
-/* One step of the device-resident synthetic PIXEL env (SURVEY §8d cfg 4: uint8 frames of uniform random bytes, reward
- * -mean(a^2) + 0.1 N(0,1), done at the episode cap): state = the frames the actors observe next, obs_next = true successors. */
-int sb200_synth_pixel_env_step_u8(void* state, const float* action, int N, int64_t frame_bytes, int A, int max_steps,
-                                  int* ep_step, uint64_t seed, const uint64_t* step_counter, void* obs_next, float* reward,
-                                  float* done, void* stream);
-
 /* ---------------------------------------------------------------------------------------------
  * One-shot all-reduce over NVLink peer memory (csrc/peer_allreduce.cu) for the small exchanges of the data-parallel
  * learner (SURVEY §8e; the reference has no collective at all): every rank maps every other rank's "symmetric" buffer
@@ -568,7 +562,7 @@ int sb200_ppo_window_step_f32(const sb200_windows* windows, const sb200_window_r
  *     step_counter == stage->step_counter) fuses the slot assignment of the windows this step completes (it depends only
  *     on the deque lengths, so it can precede the env step): the same launch writes stage->dest, advances fifo_state and
  *     *step_counter (+1, after every block has drawn with the old value).  Follow with ppo_window_step
- *     (slots_assigned = 1) or synth_env_window_step.
+ *     (slots_assigned = 1) or env_step with `windows`.
  *   ddpg_noise: DDPGAgent.act after the network (ddpg_agent.py:176-183): clip -> + sigma_i*N(0,1) -> clip. */
 int sb200_ppo_sample_f32(const float* mean, int64_t ldm, const float* log_var, const float* log_noise,
                          const float* eps, int N, int A, int deterministic, uint64_t seed, uint64_t* step_counter,
@@ -615,46 +609,55 @@ int sb200_ddpg_noise_f32(const float* mean, int64_t ldm, const float* sigma, con
 int sb200_ddpg_ou_noise_f32(const float* mean, int64_t ldm, const double* sigma, const float* unit_noise, int N, int A,
                             int deterministic, uint64_t seed, const uint64_t* step_counter, double theta, double dt,
                             double* ou_state, float* action, void* stream);
-/* Synthetic device-resident environment of the benchmark configs (SURVEY §8d): s' = tanh(Ws s + Wa a) + 0.01 xi,
- * r = -|s|^2/D + 0.1 xi', done at max_steps (MaxStepWrapper, env/wrapper.py:142-163) with auto-reset.
- * state [N,D] is updated in place to what the agent observes next; obs_next is the true successor.
- * Ws / Wa are passed transposed (k-major): WsT [D][D] with WsT[k][d] = Ws[d][k], WaT [A][D]. */
-int sb200_synth_env_step_f32(float* state, const float* action, const float* Ws, const float* Wa, int N,
-                             int D, int A, int max_steps, int* ep_step, uint64_t seed,
-                             const uint64_t* step_counter, float* obs_next, float* reward, float* done,
-                             void* stream);
-/* synth_env_step fused with the commit half of ppo_window_step (`windows`, whose dest ppo_sample has assigned): the
- * successor state is staged straight from shared memory.  One launch per rollout step instead of three. */
-int sb200_synth_env_window_step_f32(float* state, const float* action, const float* Ws, const float* Wa, int N,
-                                    int D, int A, int max_steps, int* ep_step, uint64_t seed,
-                                    const uint64_t* step_counter, float* obs_next, float* reward, float* done,
-                                    const sb200_windows* windows, void* stream);
-
-/* Classic-control tasks, batched and device-resident (csrc/classic_env.cu; semantics: tests/classic_ref.py).  No
- * counterpart in the reference, which reaches these tasks through gym.  One thread per actor.
- *   SB200_CLASSIC_CARTPOLE: CartPole-v1.  state = obs = (x, x_dot, theta, theta_dot) [N][4]; action one-hot rows [N][2]
- *     (index 1, i.e. a[1] > a[0], pushes right); reward 1; terminal when |x| > 2.4 or |theta| > 12 deg (strict, against
- *     the fp32 thresholds).  Registered episode limit 500.
- *   SB200_CLASSIC_PENDULUM: Pendulum-v1.  state (theta, theta_dot) [N][2], obs (cos, sin, theta_dot) [N][3]; action
- *     [N][1] clipped to [-1, 1] and scaled to the torque 2a; never terminal.  Registered episode limit 200.
- * ep_step [N] counts the steps of each actor's episode, episode [N] its episode index.  done = terminal or ep_step
- * reaching max_steps (> 0; <= 0: no cap).  Done actors start episode index + 1 in the same launch.  Reset states are
- * drawn from Philox4x32-10 keyed (seed ^ const, episode index, actor).
- *   classic_env_reset: every actor to episode 0, ep_step 0; state and obs drawn.
- *   classic_env_step: obs [N][D] = what each actor observes next (reset where done), obs_next [N][D] = the true
- *     successor (terminal where done), reward [N], done [N] (0 / 1).
- *   classic_env_window_step: classic_env_step fused with the commit half of ppo_window_step (`windows`, whose dest
- *     ppo_sample has assigned; windows->D and ->A must be the task's). */
-#define SB200_CLASSIC_CARTPOLE 0
-#define SB200_CLASSIC_PENDULUM 1
-int sb200_classic_env_reset_f32(int task, int N, uint64_t seed, float* state, float* obs, int* ep_step, int* episode,
-                                void* stream);
-int sb200_classic_env_step_f32(int task, const float* action, int N, int max_steps, uint64_t seed, float* state,
-                               float* obs, int* ep_step, int* episode, float* obs_next, float* reward, float* done,
-                               void* stream);
-int sb200_classic_env_window_step_f32(int task, const float* action, int N, int max_steps, uint64_t seed, float* state,
-                                      float* obs, int* ep_step, int* episode, float* obs_next, float* reward,
-                                      float* done, const sb200_windows* windows, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * Device-resident envs (csrc/env.cu): all N actors advance in one step call at fixed addresses (CUDA-graph capturable),
+ * and done actors auto-reset inside it.  One descriptor per env, filled once by its owner; `kind` selects the task:
+ *   SB200_ENV_SYNTH: the synthetic env of the benchmark configs (SURVEY §8d): s' = tanh(Ws s + Wa a) + 0.01 xi,
+ *     r = -|s|^2/D + 0.1 xi', done at max_steps (MaxStepWrapper, env/wrapper.py:142-163); a done actor's state is
+ *     re-drawn ~ N(0,1).  state [N][D] = what the agent observes next (obs NULL).  WsT [D][D] / WaT [A][D]: Ws / Wa
+ *     transposed (k-major, WsT[k][d] = Ws[d][k]).  Noise keyed by (seed, *step_counter, actor).
+ *   SB200_ENV_SYNTH_PIXEL: the synthetic PIXEL env (SURVEY §8d cfg 4): every step each actor observes a fresh uint8 frame
+ *     of uniform random bytes; reward -mean(a^2) + 0.1 N(0,1); done at max_steps.  D = the frame's 32-bit words (frame
+ *     bytes / 4, a multiple of 4); state / obs_next [N][D] words hold the frames (obs NULL).  Keyed like SYNTH.
+ *   SB200_ENV_CARTPOLE, SB200_ENV_PENDULUM: classic-control tasks (semantics: tests/classic_ref.py; no counterpart in the
+ *     reference, which reaches them through gym), one thread per actor.  obs [N][D] = what each actor observes next;
+ *     episode [N] = its episode index; done = terminal or ep_step reaching max_steps (<= 0: no cap).  A done actor starts
+ *     episode index + 1 in the same launch, its state drawn from Philox4x32-10 keyed (seed ^ const, episode index, actor).
+ *     step_counter is not read.
+ *     CARTPOLE: CartPole-v1.  state = obs = (x, x_dot, theta, theta_dot) [N][4]; action one-hot rows [N][2] (index 1,
+ *       i.e. a[1] > a[0], pushes right); reward 1; terminal when |x| > 2.4 or |theta| > 12 deg (strict, against the fp32
+ *       thresholds).  Registered episode limit 500.
+ *     PENDULUM: Pendulum-v1.  state (theta, theta_dot) [N][2], obs (cos, sin, theta_dot) [N][3]; action [N][1] clipped
+ *       to [-1, 1] and scaled to the torque 2a; never terminal.  Registered episode limit 200.
+ * Every kind: action [N][A]; ep_step [N] = steps of each actor's episode; obs_next = the true successor (terminal where
+ * done); reward [N]; done [N] (0 / 1).
+ *   env_step: one step.  With `windows` (NULL: none) the step is fused with the commit half of ppo_window_step (`windows`,
+ *     whose dest ppo_sample has assigned; its N / D / A must be the env's): the successor rows are staged straight from
+ *     shared memory.  1 launch; the pixel env: 2, and no fused commit (SB200_ERR_UNSUPPORTED with `windows`).
+ *   env_reset: the classic kinds only: every actor to episode 0, ep_step 0; state and obs drawn.  (The synthetic envs
+ *     reset from the host.) */
+#define SB200_ENV_SYNTH 0
+#define SB200_ENV_SYNTH_PIXEL 1
+#define SB200_ENV_CARTPOLE 2
+#define SB200_ENV_PENDULUM 3
+typedef struct {
+    int kind;                           /* SB200_ENV_* */
+    int N, D, A;
+    int max_steps;
+    uint64_t seed;                      /* the key the kernels draw with */
+    void* state;                        /* fp32 rows, or the pixel env's frames */
+    float* obs;                         /* classic kinds; NULL where the observation is the state */
+    const float* WsT;                   /* SB200_ENV_SYNTH only */
+    const float* WaT;
+    int* ep_step;
+    int* episode;                       /* classic kinds only */
+    const uint64_t* step_counter;       /* the agents' Philox step counter */
+    void* obs_next;
+    float* reward;
+    float* done;
+} sb200_env;
+int sb200_env_step_f32(const sb200_env* env, const float* action, const sb200_windows* windows, void* stream);
+int sb200_env_reset_f32(const sb200_env* env, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * DDPG parameter-space exploration noise (surreal/agent/param_noise.py:9-74, ddpg_agent.py:136-153,174-175): every
@@ -801,8 +804,8 @@ int sb200_ppo_act_f32(const sb200_ppo_act* args, void* stream);
 /* Persistent rollout: T steps of policy forward -> sample -> synthetic env step -> window staging for ALL N
  * actors in ONE launch (a 4-CTA cluster owns 32 actors for the whole chunk; the policy weights stay resident in
  * shared memory, layer outputs cross CTAs through distributed shared memory).  Replaces T x (ppo_sample with
- * assign_slots + synth_env_window_step + the policy forward), i.e. the actor main loop of surreal/agent/base.py:224-271
- * for a device-resident env.  Same sampling / env arithmetic and Philox keys as the per-step entries.
+ * assign_slots + env_step with `windows` + the policy forward), i.e. the actor main loop of surreal/agent/base.py:224-271
+ * for the synthetic env (`env`).  Same sampling / env arithmetic and Philox keys as the per-step entries.
  *   The kernel stages into the window deques of `windows` (whose N / D / A must match) and reads its step counter.
  *   Completed windows are written to a per-actor OUTBOX (o_*: [N*W] records in the record layout of sb200_windows,
  *   ev_step [N*W] = chunk-relative completion step, ev_count [N]); W >= T / stride + 2.
@@ -819,17 +822,9 @@ typedef struct {
     const float* log_noise;             /* [N] or NULL */
     uint64_t agent_seed;
     int deterministic;
-    float* state;                       /* [N][D] env state = next observation, updated in place */
-    const float* WsT;                   /* [D][D] k-major */
-    const float* WaT;                   /* [A][D] k-major */
-    int* ep_step;                       /* [N] */
-    int max_steps;
-    uint64_t env_seed;
+    const sb200_env* env;               /* SB200_ENV_SYNTH, with the rollout's N / D / A; stepped in place */
     float* action;                      /* outputs of the LAST step, like the per-step entries leave them */
     float* pd;
-    float* obs_next;
-    float* reward;
-    float* done;
     const sb200_windows* windows;       /* window staging and FIFO ring (not read by rollout_footprint) */
     float* o_obs;                       /* outbox */
     float* o_act;
@@ -851,9 +846,9 @@ int sb200_ppo_rollout_commit_f32(const sb200_ppo_rollout* args, int* scratch, vo
 
 /* Persistent rollout of the recurrent policy (csrc/rollout_rnn.cu): T steps of z-filter -> LSTM layers -> actor head ->
  * sampling -> synthetic env step -> window staging for ALL N actors in ONE launch.  Replaces T x (sb200_ppo_act_f32
- * with `stage` and assign_slots + sb200_synth_env_step_f32 + sb200_ppo_window_step_f32 with the cells), i.e. the actor
+ * with `stage` and assign_slots + sb200_env_step_f32 + sb200_ppo_window_step_f32 with the cells), i.e. the actor
  * main loop of surreal/agent/base.py:224-271 with the LSTM policy of ppo_net.py:317-351 and ppo_agent.py:84-93,133-154,
- * for a device-resident env.  A CTA owns 8 actors; their
+ * for the synthetic env.  A CTA owns 8 actors; their
  * env state and [L][H] cells stay in shared memory for the whole chunk.  Same records, Philox keys and FIFO order as
  * that chain: the action noise of step t is keyed by *step_counter + t, the env noise by *step_counter + t + 1.
  *   base: a filled sb200_ppo_rollout for the env, sampling, outbox and windows; base->net is the actor head

@@ -65,13 +65,22 @@ class PerTree(C.Structure):
                 ('ctrl', C.c_void_p)]
 
 
+class Env(C.Structure):
+    """sb200_env (include/surreal_b200.h): one device-resident env's task, shape, noise key and buffers."""
+    _fields_ = [('kind', C.c_int), ('N', C.c_int), ('D', C.c_int), ('A', C.c_int), ('max_steps', C.c_int),
+                ('seed', C.c_uint64), ('state', C.c_void_p), ('obs', C.c_void_p), ('WsT', C.c_void_p), ('WaT', C.c_void_p),
+                ('ep_step', C.c_void_p), ('episode', C.c_void_p), ('step_counter', C.c_void_p), ('obs_next', C.c_void_p),
+                ('reward', C.c_void_p), ('done', C.c_void_p)]
+
+
+ENV_SYNTH, ENV_SYNTH_PIXEL, ENV_CARTPOLE, ENV_PENDULUM = 0, 1, 2, 3     # SB200_ENV_*
+
+
 class PPORollout(C.Structure):
     """sb200_ppo_rollout (include/surreal_b200.h)."""
     _fields_ = [('net', C.POINTER(Mlp)), ('zf_stats', C.c_void_p), ('zf_eps', C.c_float), ('log_var', C.c_void_p),
                 ('log_noise', C.c_void_p), ('agent_seed', C.c_uint64), ('deterministic', C.c_int),
-                ('state', C.c_void_p), ('WsT', C.c_void_p), ('WaT', C.c_void_p), ('ep_step', C.c_void_p),
-                ('max_steps', C.c_int), ('env_seed', C.c_uint64), ('action', C.c_void_p), ('pd', C.c_void_p),
-                ('obs_next', C.c_void_p), ('reward', C.c_void_p), ('done', C.c_void_p), ('windows', C.POINTER(Windows)),
+                ('env', C.POINTER(Env)), ('action', C.c_void_p), ('pd', C.c_void_p), ('windows', C.POINTER(Windows)),
                 ('o_obs', C.c_void_p), ('o_act', C.c_void_p), ('o_pd', C.c_void_p), ('o_rew', C.c_void_p),
                 ('o_done', C.c_void_p), ('ev_step', C.c_void_p), ('ev_count', C.c_void_p), ('W', C.c_int), ('N', C.c_int),
                 ('D', C.c_int), ('A', C.c_int), ('T', C.c_int)]
@@ -114,7 +123,6 @@ PPO_CAT_MAX_K = 4096                    # SB200_PPO_CAT_MAX_K
 
 
 DDPG_FWD_FUSED, DDPG_FWD_PACKED, DDPG_FWD_PER_ACTOR = 0, 1, 2
-CLASSIC_CARTPOLE, CLASSIC_PENDULUM = 0, 1       # SB200_CLASSIC_*
 
 
 class DDPGAct(C.Structure):
@@ -185,7 +193,6 @@ def _declare(lib):
         'sb200_mlp_tc5_supported': (I, [C.POINTER(Mlp), L]),
         'sb200_mlp_tc5_workspace_bytes': (S, [C.POINTER(Mlp)]),
         'sb200_mlp_forward_tc5_f32': (I, [C.POINTER(Mlp), C.POINTER(ZFilter), C.POINTER(Rows), P, L, P, I, P]),
-        'sb200_synth_pixel_env_step_u8': (I, [P, P, I, L, I, I, P, C.c_uint64, P, P, P, P, P]),
         'sb200_par_buffer_bytes': (S, [L]),
         'sb200_par_alloc': (I, [L, C.POINTER(C.c_void_p), P]),
         'sb200_par_open': (I, [P, C.POINTER(C.c_void_p)]),
@@ -246,13 +253,10 @@ def _declare(lib):
         'sb200_ddpg_target2_f32': (I, [P, P, L, P, L, P, P, L, I, I, D, P, P, P, P]),
         'sb200_ddpg_smooth_action_f32': (I, [P, L, P, I, I, D, D, C.c_uint64, P, P, L, P]),
         'sb200_ddpg_ou_noise_f32': (I, [P, L, P, P, I, I, I, C.c_uint64, P, D, D, P, P, P]),
-        'sb200_synth_env_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, P]),
         'sb200_fifo_state_bytes': (S, []),
         'sb200_ppo_window_step_f32': (I, [C.POINTER(Windows), C.POINTER(WindowRows), P]),
-        'sb200_synth_env_window_step_f32': (I, [P, P, P, P, I, I, I, I, P, C.c_uint64, P, P, P, P, C.POINTER(Windows), P]),
-        'sb200_classic_env_reset_f32': (I, [I, I, C.c_uint64, P, P, P, P, P]),
-        'sb200_classic_env_step_f32': (I, [I, P, I, I, C.c_uint64, P, P, P, P, P, P, P, P]),
-        'sb200_classic_env_window_step_f32': (I, [I, P, I, I, C.c_uint64, P, P, P, P, P, P, P, C.POINTER(Windows), P]),
+        'sb200_env_step_f32': (I, [C.POINTER(Env), P, C.POINTER(Windows), P]),
+        'sb200_env_reset_f32': (I, [C.POINTER(Env), P]),
         'sb200_fifo_pop': (I, [P, I, P, P, P]),
         'sb200_fifo_push': (I, [P, I, P, P]),
         'sb200_replay_gather_f32': (I, [P, L, P, P, I, P, P]),

@@ -180,25 +180,8 @@ class Agent(metaclass=U.AutoInitializeMeta):
         return isinstance(x, torch.Tensor) and x.is_cuda
 
     def get_env(self):
-        from ..env import SyntheticEnv, make_classic_env
-        ec = self.env_config
-        env = make_classic_env(ec, self.num_envs)
-        if env is not None:
-            return env
-        name = ec.env_name if 'env_name' in ec else ''
-        if not str(name).startswith('synthetic'):
-            raise ValueError('only the device-resident envs ship with surreal_b200 (env_name "synthetic", '
-                             '"classic:CartPole-v1", "classic:Pendulum-v1"); '
-                             'gym / dm_control / robosuite adapters are out of scope -- pass your own env to '
-                             'main_setup(env)')
-        from ..utils import obs_is_pixel
-        if obs_is_pixel(ec.obs_spec):
-            from ..env import SyntheticPixelEnv
-            return SyntheticPixelEnv(self.num_envs, tuple(ec.obs_spec['pixel']['camera0']), ec.action_spec.dim[0],
-                                     ec.limit_episode_length, seed=int(ec.seed) if 'seed' in ec else 0)
-        D = sum(v[0] for v in ec.obs_spec['low_dim'].values())
-        return SyntheticEnv(self.num_envs, D, ec.action_spec.dim[0], ec.limit_episode_length,
-                            seed=int(ec.seed) if 'seed' in ec else 0)
+        from ..env import make_env
+        return make_env(self.env_config, self.num_envs)
 
     def prepare_env(self, env):
         return self.prepare_env_agent(env) if self.agent_mode == 'training' else self.prepare_env_eval(env)

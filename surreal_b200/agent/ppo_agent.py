@@ -277,23 +277,21 @@ class PPOAgent(Agent):
 
     def _rollout_args(self, ob=None, steps=0):
         """sb200_ppo_rollout of this agent's policy, env and window wrapper; with ``ob`` (the wrapper's outbox for chunks of
-        ``steps``) every buffer of a chunk.  ``net`` is the actor (the LSTM policy's head); D the env's observation width."""
+        ``steps``) every buffer of a chunk.  ``net`` is the actor (the LSTM policy's head); D the env's observation width;
+        ``env`` the env's own descriptor."""
         m, w = self.model, self.env
         a = _lib.PPORollout()
         d = m.actor.desc()
         a.net = C.pointer(d)
         a.N, a.D, a.A, a.T = self.num_envs, m.low_dim, self.action_dim, int(steps)
+        a.env = C.pointer(w.env.desc)
         if ob is None:
             return a
-        e = w.env
         a.zf_stats = m.z_stats.data_ptr() if m.z_stats is not None else None
         a.zf_eps = float(m.z_eps)
         a.log_var, a.log_noise = m.log_var.data_ptr(), self._log_noise.data_ptr()
         a.agent_seed, a.deterministic = self.seed, 0
-        a.state, a.WsT, a.WaT, a.ep_step = e.state.data_ptr(), e.WsT.data_ptr(), e.WaT.data_ptr(), e.ep_step.data_ptr()
-        a.max_steps, a.env_seed = e.max_steps, e.seed + 7
         a.action, a.pd = self._action.data_ptr(), self._pd.data_ptr()
-        a.obs_next, a.reward, a.done = e.obs_next.data_ptr(), e.reward.data_ptr(), e.done.data_ptr()
         a.windows = C.pointer(w.windows)           # its step counter is the env's: the wrapper shares it
         a.o_obs, a.o_act, a.o_pd = ob['o_obs'].data_ptr(), ob['o_act'].data_ptr(), ob['o_pd'].data_ptr()
         a.o_rew, a.o_done = ob['o_rew'].data_ptr(), ob['o_done'].data_ptr()
@@ -340,24 +338,6 @@ class PPOAgent(Agent):
 
     def default_config(self):
         return {'model': {'convs': '_list_', 'fc_hidden_sizes': '_list_'}}
-
-    def get_env(self):
-        """The in-tree device env: a classic-control task, or the synthetic env -- for a discrete action_spec its discrete
-        form (one-hot action rows), as QAgent's."""
-        if not self.categorical:
-            return super().get_env()
-        from ..env import DiscreteSyntheticEnv, make_classic_env
-        from ..utils import obs_is_pixel
-        ec = self.env_config
-        env = make_classic_env(ec, self.num_envs)
-        if env is not None:
-            return env
-        name = ec.env_name if 'env_name' in ec else ''
-        if not str(name).startswith('synthetic') or obs_is_pixel(ec.obs_spec):
-            return super().get_env()
-        D = sum(v[0] for v in ec.obs_spec['low_dim'].values())
-        return DiscreteSyntheticEnv(self.num_envs, D, self.action_dim, ec.limit_episode_length,
-                                    seed=int(ec.seed) if 'seed' in ec else 0)
 
     def reset(self):
         """reset of LSTM hidden and cell states (ppo_agent.py:169-183; nothing in the reference calls it)."""

@@ -142,19 +142,6 @@ class QAgent(Agent):
         return {'model': {'convs': '_list_', 'fc_hidden_sizes': '_list_', 'dueling': '_bool_'},
                 'eval': {'eps': '_float_'}}
 
-    def get_env(self):
-        from ..env import DiscreteSyntheticEnv, make_classic_env
-        ec = self.env_config
-        env = make_classic_env(ec, self.num_envs)
-        if env is not None:
-            return env
-        name = ec.env_name if 'env_name' in ec else ''
-        if not str(name).startswith('synthetic'):
-            return super().get_env()
-        D = sum(v[0] for v in ec.obs_spec['low_dim'].values())
-        return DiscreteSyntheticEnv(self.num_envs, D, self.n_actions, ec.limit_episode_length,
-                                    seed=int(ec.seed) if 'seed' in ec else 0)
-
     def prepare_env_agent(self, env):
         env = super().prepare_env_agent(env)
         return ExpSenderWrapperSSARNStepBootstrap(env, self.learner_config, self.session_config)

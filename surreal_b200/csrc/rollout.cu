@@ -1,6 +1,6 @@
-// Actor-side kernels of the batched rollout: policy sampling, exploration noise, the synthetic
-// device-resident environment, and the per-actor experience staging that replaces the Python deques of
-// surreal/env/exp_sender_wrapper.py (windows for PPO, n-step SSAR records for DDPG).
+// Actor-side kernels of the batched rollout: policy sampling, exploration noise, the per-actor experience
+// staging that replaces the Python deques of surreal/env/exp_sender_wrapper.py (windows for PPO, n-step SSAR
+// records for DDPG), and the act entries.  The device-resident envs are in env.cu.
 //
 // All per-actor control state (deque length, episode step, RNG counter) lives in HBM so that a whole
 // T-step rollout is a fixed launch sequence (CUDA-graph capturable) with no host round trip.
@@ -138,99 +138,6 @@ __global__ void __launch_bounds__(RT) ddpg_ou_noise_kernel(const float* __restri
     action[(long long)i * A + j] = fminf(fmaxf(a, -1.0f), 1.0f);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Synthetic environment of SURVEY §8(d) cfg 2/3/5, batched and device-resident:
-//   s' = tanh(Ws s + Wa a) + 0.01*xi,   r = -|s|^2 / D + 0.1*xi',   done when the episode reaches
-//   `max_steps` (MaxStepWrapper, env/wrapper.py:142-163); on done the state is re-drawn ~ N(0,1).
-// One block per 4 actors; the weights are passed TRANSPOSED (WsT [D][D], WaT [A][D]: k-major) so that the
-// threads of a warp read consecutive addresses; they stay L1/L2-resident (18 KB).  obs_next = the true successor (terminal
-// when done), state = what the agent observes next (reset when done).
-// Block-level body (RT threads, 4 actors).  s_n / s_z (optional) receive the successor and the next observed
-// state of the block's actors, s_rew / s_dn their reward and done flag.
-__device__ void synth_env_block(float* __restrict__ state, const float* __restrict__ action,
-                                const float* __restrict__ Ws, const float* __restrict__ Wa, int N, int D, int A,
-                                int max_steps, int* __restrict__ ep_step, unsigned long long seed,
-                                const unsigned long long* __restrict__ step_ctr, float* __restrict__ obs_next,
-                                float* __restrict__ reward, float* __restrict__ done, float* s_s, float* s_a,
-                                float* s_q, float* s_n, float* s_z, float* s_rew, float* s_dn,
-                                unsigned long long ctr_bias) {
-    const int per = 4;
-    const int a0 = blockIdx.x * per;
-    const int tid = threadIdx.x;
-    for (int idx = tid; idx < per * D; idx += RT) {
-        const int q = idx / D, d = idx - q * D;
-        s_s[idx] = (a0 + q < N) ? state[(long long)(a0 + q) * D + d] : 0.0f;
-    }
-    for (int idx = tid; idx < per * A; idx += RT) {
-        const int q = idx / A, j = idx - q * A;
-        s_a[idx] = (a0 + q < N) ? action[(long long)(a0 + q) * A + j] : 0.0f;
-    }
-    __syncthreads();
-    // ctr_bias = -1 in the fused rollout, where the sampling kernel has already advanced the counter: both launch
-    // sequences then draw the same noise for the same step
-    const unsigned long long ctr = ((step_ctr != nullptr) ? *step_ctr : 0ull) + ctr_bias;
-    // reward: -|s|^2/D (+ noise), one warp per actor (warps 0..3)
-    const int warp = tid >> 5, lane = tid & 31;
-    if (warp < per) {
-        float q = 0.0f;
-        for (int d = lane; d < D; d += 32) q += s_s[warp * D + d] * s_s[warp * D + d];
-        q = warp_sum(q);
-        if (lane == 0) s_q[warp] = q;
-    }
-    __syncthreads();
-    for (int idx = tid; idx < per * D; idx += RT) {
-        const int q = idx / D, d = idx - q * D;
-        const int i = a0 + q;
-        if (i >= N) continue;
-        float acc = 0.0f;                                   // WsT / WaT are [k][d]: coalesced across d
-#pragma unroll 8
-        for (int k = 0; k < D; ++k) acc = fmaf(__ldg(Ws + (long long)k * D + d), s_s[q * D + k], acc);
-#pragma unroll 4
-        for (int k = 0; k < A; ++k) acc = fmaf(__ldg(Wa + (long long)k * D + d), s_a[q * A + k], acc);
-        const Philox4 r = env_noise(seed, ctr, i, d);
-        const float2 g = box_muller(r.x, r.y);
-        const float nxt = env_successor(acc, g.x);
-        const bool dn = env_done(ep_step[i] + 1, max_steps);
-        const float st = dn ? env_reset_draw(r) : nxt;
-        obs_next[(long long)i * D + d] = nxt;
-        state[(long long)i * D + d] = st;
-        if (s_n != nullptr) {
-            s_n[idx] = nxt;
-            s_z[idx] = st;
-        }
-        if (d == 0) {
-            const float rw = env_reward(s_q[q], D, g.y);
-            reward[i] = rw;
-            done[i] = dn ? 1.0f : 0.0f;
-            if (s_rew != nullptr) {
-                s_rew[q] = rw;
-                s_dn[q] = dn ? 1.0f : 0.0f;
-            }
-        }
-    }
-    __syncthreads();
-    for (int q = tid; q < per; q += RT) {
-        const int i = a0 + q;
-        if (i < N) {
-            const int t = ep_step[i] + 1;
-            ep_step[i] = env_done(t, max_steps) ? 0 : t;
-        }
-    }
-}
-
-__global__ void __launch_bounds__(RT) synth_env_step_kernel(float* __restrict__ state, const float* __restrict__ action,
-                                                            const float* __restrict__ Ws, const float* __restrict__ Wa,
-                                                            int N, int D, int A, int max_steps,
-                                                            int* __restrict__ ep_step, unsigned long long seed,
-                                                            const unsigned long long* __restrict__ step_ctr,
-                                                            float* __restrict__ obs_next, float* __restrict__ reward,
-                                                            float* __restrict__ done) {
-    extern __shared__ float sm[];                  // [4][D] states, [4][A] actions
-    __shared__ float s_q[4];
-    synth_env_block(state, action, Ws, Wa, N, D, A, max_steps, ep_step, seed, step_ctr, obs_next, reward, done, sm,
-                    sm + 4 * D, s_q, nullptr, nullptr, nullptr, nullptr, 0ull);
-}
-
 __global__ void __launch_bounds__(1024) ppo_window_slots_kernel(int N, int n_step, const int* __restrict__ stage_pos,
                                                                 int* __restrict__ dest, FifoState* fifo,
                                                                 unsigned long long* step_ctr) {
@@ -345,36 +252,6 @@ __global__ void __launch_bounds__(128, 4) ppo_window_commit_rnn_wide_kernel(cons
                                         stage_done, r_obs, r_act, r_pd, r_rew, r_done);
 }
 
-// Fused environment step + window commit for the device-resident synthetic env: the successor state never
-// leaves shared memory before it is staged.  One block per 4 actors, 64 threads per actor in the commit.
-__global__ void __launch_bounds__(RT) synth_env_window_step_kernel(
-    float* __restrict__ state, const float* __restrict__ action, const float* __restrict__ Ws,
-    const float* __restrict__ Wa, int N, int D, int A, int max_steps, int* __restrict__ ep_step,
-    unsigned long long seed, const unsigned long long* __restrict__ step_ctr, float* __restrict__ obs_next,
-    float* __restrict__ reward, float* __restrict__ done, int n_step, int stride, int* __restrict__ stage_pos,
-    float* __restrict__ stage_obs, float* __restrict__ stage_act, float* __restrict__ stage_pd,
-    float* __restrict__ stage_rew, float* __restrict__ stage_done, const int* __restrict__ dest,
-    float* __restrict__ r_obs, float* __restrict__ r_act, float* __restrict__ r_pd, float* __restrict__ r_rew,
-    float* __restrict__ r_done) {
-    extern __shared__ float sm[];                  // [4][D] states, [4][A] actions, [4][D] successor, [4][D] reset
-    const int per = 4;
-    const int a0 = blockIdx.x * per;
-    float* s_s = sm;
-    float* s_a = sm + per * D;
-    float* s_n = s_a + per * A;
-    float* s_z = s_n + per * D;
-    __shared__ float s_q[4], s_rew[4], s_dn[4];
-    const int tid = threadIdx.x;
-    synth_env_block(state, action, Ws, Wa, N, D, A, max_steps, ep_step, seed, step_ctr, obs_next, reward, done, s_s, s_a,
-                    s_q, s_n, s_z, s_rew, s_dn, ~0ull);
-    __syncthreads();
-    const int q = tid >> 6, g = tid & 63;
-    const int i = a0 + q;
-    commit_actor(i < N, i, g, 64, s_n + q * D, s_z + q * D, s_rew[q], s_dn[q], n_step, stride, D, A, stage_pos + min(i, N - 1),
-                 (i < N) ? dest[i] : SLOT_NONE, stage_obs, stage_act, stage_pd, stage_rew, stage_done, r_obs, r_act, r_pd,
-                 r_rew, r_done);
-}
-
 }  // namespace
 
 static bool sample_args_ok(const float* mean, int64_t ldm, const float* log_var, int N, int A,
@@ -416,37 +293,6 @@ extern "C" int sb200_ddpg_ou_noise_f32(const float* mean, int64_t ldm, const dou
     ddpg_ou_noise_kernel<<<(N * A + RT - 1) / RT, RT, 0, (cudaStream_t)stream>>>(
         mean, ldm, sigma, unit_noise, N, A, deterministic, (unsigned long long)seed,
         (const unsigned long long*)step_counter, theta, dt, ou_state, action);
-    return sb200_launch_status();
-}
-
-extern "C" int sb200_synth_env_step_f32(float* state, const float* action, const float* Ws, const float* Wa, int N,
-                                        int D, int A, int max_steps, int* ep_step, uint64_t seed,
-                                        const uint64_t* step_counter, float* obs_next, float* reward, float* done,
-                                        void* stream) {
-    SB200_REQUIRE(state && action && Ws && Wa && ep_step && obs_next && reward && done);
-    SB200_REQUIRE(N >= 1 && D >= 1 && A >= 1 && (size_t)(4 * (D + A)) * 4 <= 40 * 1024);
-    const size_t smem = (size_t)(4 * (D + A)) * sizeof(float);
-    synth_env_step_kernel<<<(N + 3) / 4, RT, smem, (cudaStream_t)stream>>>(
-        state, action, Ws, Wa, N, D, A, max_steps, ep_step, (unsigned long long)seed,
-        (const unsigned long long*)step_counter, obs_next, reward, done);
-    return sb200_launch_status();
-}
-
-static bool env_smem_ok(int D, int A, bool fused) {
-    return (size_t)(4 * (D + A) + (fused ? 8 * D : 0)) * sizeof(float) <= 40 * 1024;
-}
-
-extern "C" int sb200_synth_env_window_step_f32(float* state, const float* action, const float* Ws, const float* Wa,
-                                               int N, int D, int A, int max_steps, int* ep_step, uint64_t seed,
-                                               const uint64_t* step_counter, float* obs_next, float* reward,
-                                               float* done, const sb200_windows* w, void* stream) {
-    SB200_REQUIRE(state && action && Ws && Wa && ep_step && obs_next && reward && done && windows_ok(w));
-    SB200_REQUIRE(w->N == N && w->D == D && w->A == A && env_smem_ok(D, A, true));
-    const size_t smem = (size_t)(4 * (D + A) + 8 * D) * sizeof(float);
-    synth_env_window_step_kernel<<<(N + 3) / 4, RT, smem, (cudaStream_t)stream>>>(
-        state, action, Ws, Wa, N, D, A, max_steps, ep_step, (unsigned long long)seed,
-        (const unsigned long long*)step_counter, obs_next, reward, done, w->n_step, w->stride, w->stage_pos, w->stage_obs,
-        w->stage_act, w->stage_pd, w->stage_rew, w->stage_done, w->dest, w->r_obs, w->r_act, w->r_pd, w->r_rew, w->r_done);
     return sb200_launch_status();
 }
 

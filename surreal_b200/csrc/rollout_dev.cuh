@@ -1,6 +1,6 @@
-// Device-side building blocks shared by the per-step rollout kernels (rollout.cu) and the persistent rollout
-// kernel (rollout_fused.cu): FIFO control block, replay-slot assignment, the sampling and env formulas, per-actor
-// window commit.
+// Device-side building blocks shared by the per-step rollout kernels (rollout.cu), the device envs (env.cu) and the
+// persistent rollout kernels (rollout_fused.cu, rollout_rnn.cu): FIFO control block, replay-slot assignment, the
+// sampling and env formulas, per-actor window commit.
 #pragma once
 #include "common.cuh"
 
@@ -27,6 +27,12 @@ inline bool windows_ok(const sb200_windows* w) {
     return w != nullptr && w->N >= 1 && w->n_step >= 1 && w->stride >= 1 && w->D >= 1 && w->A >= 1 && w->stage_pos &&
            w->stage_obs && w->stage_act && w->stage_pd && w->stage_rew && w->stage_done && w->dest && w->fifo_state &&
            w->r_obs && w->r_act && w->r_pd && w->r_rew && w->r_done;
+}
+
+// Host check of a persistent rollout's env: the synthetic env, stepping the rollout's N actors with its D / A.
+inline bool rollout_env_ok(const sb200_ppo_rollout* a) {
+    const sb200_env* e = a->env;
+    return e != nullptr && e->kind == SB200_ENV_SYNTH && e->N == a->N && e->D == a->D && e->A == a->A;
 }
 
 constexpr int SLOT_NONE = -1;      // deque not full after this step
@@ -96,8 +102,8 @@ __device__ void assign_window_slots(int N, int n_step, const int* __restrict__ s
 __device__ unsigned int* fifo_ticket(FifoState* fifo) { return &fifo->ticket; }
 
 // ------------------------------------------------------------------------------------------------
-// Per-element formulas of PPO sampling and of the synthetic env, used by the per-step kernels (rollout.cu) and by the
-// persistent rollout (rollout_fused.cu), whose results must agree bit for bit.  Each formula is one expression, so
+// Per-element formulas of PPO sampling and of the synthetic env, used by the per-step kernels (rollout.cu, env.cu) and
+// by the persistent rollout (rollout_fused.cu), whose results must agree bit for bit.  Each formula is one expression, so
 // every caller gets the same FMA contraction.
 
 // PPOAgent.act (ppo_agent.py:138-149): std = exp(log_var) * scale, scale = exp(noise_i) (1 without per-actor noise)

@@ -1205,8 +1205,9 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
     RfParams p;
     size_t smem = 0;
     if (!rf_plan(a->net, a->D, a->A, 1, &p, &smem)) return SB200_ERR_UNSUPPORTED;
-    SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->W >= 1 && rollout_windows_ok(a));
-    SB200_REQUIRE(a->state && a->WsT && a->WaT && a->ep_step && a->action && a->pd && a->obs_next && a->reward && a->done);
+    SB200_REQUIRE(a->N >= 1 && a->T >= 1 && a->W >= 1 && rollout_windows_ok(a) && rollout_env_ok(a));
+    const sb200_env* e = a->env;
+    SB200_REQUIRE(e->state && e->WsT && e->WaT && e->ep_step && a->action && a->pd && e->obs_next && e->reward && e->done);
     SB200_REQUIRE(a->log_var);
     SB200_REQUIRE(a->o_obs && a->o_act && a->o_pd && a->o_rew && a->o_done && a->ev_step && a->ev_count);
     for (int l = 0; l < 3; ++l) {
@@ -1216,24 +1217,24 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
         p.act[l] = a->net->act[l];
         SB200_REQUIRE(p.W[l] != nullptr && p.b[l] != nullptr && p.ldw[l] % 4 == 0 && (((uintptr_t)p.W[l]) & 15) == 0);
     }
-    SB200_REQUIRE((((uintptr_t)a->WsT) & 15) == 0 && (((uintptr_t)a->WaT) & 15) == 0 && (((uintptr_t)a->state) & 15) == 0);
+    SB200_REQUIRE((((uintptr_t)e->WsT) & 15) == 0 && (((uintptr_t)e->WaT) & 15) == 0 && (((uintptr_t)e->state) & 15) == 0);
     p.zf = a->zf_stats;
     p.zf_eps = a->zf_eps;
     p.log_var = a->log_var;
     p.log_noise = a->log_noise;
     p.agent_seed = a->agent_seed;
     p.deterministic = a->deterministic;
-    p.state = a->state;
-    p.WsT = a->WsT;
-    p.WaT = a->WaT;
-    p.ep_step = a->ep_step;
-    p.max_steps = a->max_steps;
-    p.env_seed = a->env_seed;
+    p.state = (float*)e->state;
+    p.WsT = e->WsT;
+    p.WaT = e->WaT;
+    p.ep_step = e->ep_step;
+    p.max_steps = e->max_steps;
+    p.env_seed = e->seed;
     p.action = a->action;
     p.pd = a->pd;
-    p.obs_next = a->obs_next;
-    p.reward = a->reward;
-    p.done = a->done;
+    p.obs_next = (float*)e->obs_next;
+    p.reward = e->reward;
+    p.done = e->done;
     const sb200_windows* w = a->windows;
     p.stage_pos = w->stage_pos;
     p.stage_obs = w->stage_obs;
@@ -1270,7 +1271,7 @@ extern "C" int sb200_ppo_rollout_f32(const sb200_ppo_rollout* a, void* stream) {
 }
 
 extern "C" int sb200_ppo_rollout_footprint(const sb200_ppo_rollout* a, int* sms) {
-    SB200_REQUIRE(a != nullptr && a->net != nullptr && sms != nullptr && a->N >= 1);
+    SB200_REQUIRE(a != nullptr && a->net != nullptr && sms != nullptr && a->N >= 1 && rollout_env_ok(a));
     *sms = 0;
     RfParams p;
     size_t smem = 0;

@@ -487,8 +487,9 @@ extern "C" int sb200_ppo_rollout_rnn_f32(const sb200_ppo_rollout_rnn* a, void* s
     SB200_REQUIRE(a != nullptr && a->base != nullptr);
     if (sb200_ppo_rollout_rnn_supported(a) != 1) return SB200_ERR_UNSUPPORTED;
     const sb200_ppo_rollout* b = a->base;
-    SB200_REQUIRE(b->N >= 1 && b->T >= 1 && b->W >= 1 && rr_windows_ok(a));
-    SB200_REQUIRE(b->state && b->WsT && b->WaT && b->ep_step && b->action && b->pd && b->obs_next && b->reward && b->done);
+    SB200_REQUIRE(b->N >= 1 && b->T >= 1 && b->W >= 1 && rr_windows_ok(a) && rollout_env_ok(b));
+    const sb200_env* e = b->env;
+    SB200_REQUIRE(e->state && e->WsT && e->WaT && e->ep_step && b->action && b->pd && e->obs_next && e->reward && e->done);
     SB200_REQUIRE(b->log_var && b->o_obs && b->o_act && b->o_pd && b->o_rew && b->o_done && b->ev_step && b->ev_count);
     SB200_REQUIRE(a->h && a->c && a->h_before && a->c_before);
     RrParams p = {};
@@ -525,17 +526,17 @@ extern "C" int sb200_ppo_rollout_rnn_f32(const sb200_ppo_rollout_rnn* a, void* s
     p.log_noise = b->log_noise;
     p.agent_seed = b->agent_seed;
     p.deterministic = b->deterministic;
-    p.state = b->state;
-    p.WsT = b->WsT;
-    p.WaT = b->WaT;
-    p.ep_step = b->ep_step;
-    p.max_steps = b->max_steps;
-    p.env_seed = b->env_seed;
+    p.state = (float*)e->state;
+    p.WsT = e->WsT;
+    p.WaT = e->WaT;
+    p.ep_step = e->ep_step;
+    p.max_steps = e->max_steps;
+    p.env_seed = e->seed;
     p.action = b->action;
     p.pd = b->pd;
-    p.obs_next = b->obs_next;
-    p.reward = b->reward;
-    p.done = b->done;
+    p.obs_next = (float*)e->obs_next;
+    p.reward = e->reward;
+    p.done = e->done;
     const sb200_windows* w = b->windows;
     p.stage_pos = w->stage_pos;
     p.stage_obs = w->stage_obs;
@@ -564,7 +565,7 @@ extern "C" int sb200_ppo_rollout_rnn_f32(const sb200_ppo_rollout_rnn* a, void* s
 }
 
 extern "C" int sb200_ppo_rollout_rnn_footprint(const sb200_ppo_rollout_rnn* a, int* sms_out) {
-    SB200_REQUIRE(a != nullptr && a->base != nullptr && sms_out != nullptr && a->base->N >= 1);
+    SB200_REQUIRE(a != nullptr && a->base != nullptr && sms_out != nullptr && a->base->N >= 1 && rollout_env_ok(a->base));
     *sms_out = 0;
     if (sb200_ppo_rollout_rnn_supported(a) != 1) return SB200_ERR_UNSUPPORTED;
     int sms = 0;

@@ -294,60 +294,3 @@ extern "C" int sb200_conv_backward_dx_f32(int layer, const float* dy, const floa
     conv_bwd_dx_kernel<4, 2, 32><<<grid, CT, smem, (cudaStream_t)stream>>>(dy, Wk, act, (int)frames, CIN, H, W, dx);
     return sb200_launch_status();
 }
-
-// ------------------------------------------------------------------------------------------------------------------------
-// Synthetic PIXEL environment of BASELINE configs[3] (SURVEY §8d cfg 4): every step each actor observes a fresh frame of
-// uniform random bytes (Philox keyed by (seed, step, actor, word)), reward = -mean(a^2) + 0.1 xi, done at the episode cap.
-// Frames are written as 32-bit words (4 pixels each); `state` = what the actor observes next (a reset frame where done),
-// `obs_next` = the true successor.
-namespace {
-__global__ void __launch_bounds__(256) synth_pixel_env_kernel(unsigned int* __restrict__ state, const float* __restrict__ action, int N,
-                                                              int words, int A, int max_steps, int* __restrict__ ep_step,
-                                                              unsigned long long seed, const unsigned long long* __restrict__ step_ctr,
-                                                              unsigned int* __restrict__ obs_next, float* __restrict__ reward,
-                                                              float* __restrict__ done) {
-    const int i = blockIdx.y;
-    const unsigned long long ctr = (step_ctr != nullptr) ? *step_ctr : 0ull;
-    const int t = ep_step[i] + 1;
-    const bool dn = (max_steps > 0) && (t >= max_steps);
-    const int w4 = words / 4;
-    for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < w4; g += gridDim.x * blockDim.x) {
-        const Philox4 r = philox4x32_10(seed ^ 0x2545F4914F6CDD1Dull, ctr, ((unsigned long long)i << 24) | (unsigned long long)g);
-        uint4 nx = make_uint4(r.x, r.y, r.z, r.w);
-        reinterpret_cast<uint4*>(obs_next + (long long)i * words)[g] = nx;
-        if (dn) {
-            const Philox4 z = philox4x32_10(seed ^ 0x9E3779B97F4A7C15ull, ctr, ((unsigned long long)i << 24) | (unsigned long long)g);
-            nx = make_uint4(z.x, z.y, z.z, z.w);
-        }
-        reinterpret_cast<uint4*>(state + (long long)i * words)[g] = nx;
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        float s = 0.0f;
-        for (int j = 0; j < A; ++j) s += action[(long long)i * A + j] * action[(long long)i * A + j];
-        const Philox4 r = philox4x32_10(seed ^ 0x5851F42D4C957F2Dull, ctr, ((unsigned long long)i << 24) | 0xFFFFFFull);
-        reward[i] = -s / (float)A + 0.1f * box_muller(r.x, r.y).x;
-        done[i] = dn ? 1.0f : 0.0f;
-    }
-}
-// ep_step update must happen after every block has read it: separate tiny kernel
-__global__ void synth_pixel_env_tick_kernel(int N, int max_steps, int* __restrict__ ep_step) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    const int t = ep_step[i] + 1;
-    ep_step[i] = ((max_steps > 0) && (t >= max_steps)) ? 0 : t;
-}
-}  // namespace
-
-extern "C" int sb200_synth_pixel_env_step_u8(void* state, const float* action, int N, int64_t frame_bytes, int A, int max_steps,
-                                             int* ep_step, uint64_t seed, const uint64_t* step_counter, void* obs_next,
-                                             float* reward, float* done, void* stream) {
-    SB200_REQUIRE(state && action && ep_step && obs_next && reward && done && N >= 1 && A >= 1);
-    SB200_REQUIRE(frame_bytes >= 16 && frame_bytes % 16 == 0 && frame_bytes / 16 < (1ll << 24) && N < (1 << 24));
-    const int words = (int)(frame_bytes / 4);
-    dim3 grid((unsigned)((words / 4 + 255) / 256 < 8 ? (words / 4 + 255) / 256 : 8), (unsigned)N);
-    synth_pixel_env_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((unsigned int*)state, action, N, words, A, max_steps, ep_step,
-                                                                   (unsigned long long)seed, (const unsigned long long*)step_counter,
-                                                                   (unsigned int*)obs_next, reward, done);
-    synth_pixel_env_tick_kernel<<<(N + 255) / 256, 256, 0, (cudaStream_t)stream>>>(N, max_steps, ep_step);
-    return sb200_launch_status(2);
-}

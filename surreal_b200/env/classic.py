@@ -1,5 +1,5 @@
 """Classic-control tasks as batched, device-resident envs: CartPole-v1 and Pendulum-v1 with gym's dynamics, one CUDA
-thread per actor (csrc/classic_env.cu; the float64 statement of both tasks is tests/classic_ref.py).  They have
+thread per actor (csrc/env.cu; the float64 statement of both tasks is tests/classic_ref.py).  They have
 SyntheticEnv's interface, so every agent and engine that runs the synthetic env runs them, and unlike it they have a
 known solution: a policy that learns them shows that training works end to end.
 
@@ -13,92 +13,43 @@ import torch
 
 from .. import _lib
 from .._lib import check
-from ..ops import _ptr, _stream
+from ..ops import _stream
+from .base import LowDimEnv
 
 
-class _ClassicEnv:
-    metadata = {}
-    graph_safe = True          # every buffer at a fixed address, no host logic inside step()
-    TASK = S = D = A = MAX_STEPS = ACTION_TYPE = None
+class _ClassicEnv(LowDimEnv):
+    S = MAX_STEPS = ACTION_TYPE = None
     NAME = ''
 
     def __init__(self, num_envs, limit_episode_length=0, seed=0, device=None):
-        if not torch.cuda.is_available():
-            raise RuntimeError('%s is device-resident: a CUDA device is required' % type(self).__name__)
-        self.device = torch.device(device if device is not None else ('cuda:%d' % torch.cuda.current_device()))
-        self.N = int(num_envs)
         lim = int(limit_episode_length)
-        self.max_steps = lim if lim > 0 else self.MAX_STEPS
-        self.seed = int(seed)
+        super().__init__(num_envs, self.D, self.A, lim if lim > 0 else self.MAX_STEPS, seed, device)
         f = lambda *s: torch.zeros(*s, device=self.device)  # noqa: E731
         self.state = f(self.N, self.S)
         self.obs = f(self.N, self.D)
         self.obs_next = f(self.N, self.D)
-        self.reward = f(self.N)
-        self.done = f(self.N)
-        self.ep_step = torch.zeros(self.N, dtype=torch.int32, device=self.device)
         self.episode = torch.zeros(self.N, dtype=torch.int32, device=self.device)
-        self.step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)   # the agents' Philox counter
-
-    def observation_spec(self):
-        return {'low_dim': {'flat_inputs': (self.D,)}}
+        self._describe(self.seed, obs=self.obs, episode=self.episode)
 
     def action_spec(self):
         return {'dim': (self.A,), 'type': self.ACTION_TYPE}
 
-    def _obs(self, x):
-        return {'low_dim': {'flat_inputs': x}}
-
     def reset(self):
-        check(_lib.lib().sb200_classic_env_reset_f32(self.TASK, self.N, self.seed, _ptr(self.state), _ptr(self.obs),
-                                                     _ptr(self.ep_step), _ptr(self.episode), _stream()),
-              'sb200_classic_env_reset_f32')
+        check(_lib.lib().sb200_env_reset_f32(C.byref(self.desc), _stream()), 'sb200_env_reset_f32')
         return self._obs(self.obs), {}
-
-    def _action(self, action):
-        if isinstance(action, tuple):            # QAgent.act: (one-hot rows, indices)
-            action = action[0]
-        if not (isinstance(action, torch.Tensor) and action.is_cuda and action.dtype == torch.float32 and
-                action.is_contiguous() and tuple(action.shape) == (self.N, self.A)):
-            raise ValueError('%s.step takes a contiguous float32 CUDA tensor [%d, %d]' % (type(self).__name__, self.N,
-                                                                                          self.A))
-        return action
-
-    def step(self, action):
-        """Returns (obs, reward, done, info) like SyntheticEnv.step: obs is what every actor observes NEXT (already
-        reset where done), ``info['obs_next']`` the true successor (terminal where done)."""
-        a = self._action(action)
-        check(_lib.lib().sb200_classic_env_step_f32(
-            self.TASK, _ptr(a), self.N, self.max_steps, self.seed, _ptr(self.state), _ptr(self.obs), _ptr(self.ep_step),
-            _ptr(self.episode), _ptr(self.obs_next), _ptr(self.reward), _ptr(self.done), _stream()),
-            'sb200_classic_env_step_f32')
-        return self._obs(self.obs), self.reward, self.done, {'obs_next': self.obs_next}
-
-    def step_and_commit_window(self, action, w):
-        """step() fused with the commit half of ExpSenderWrapperMultiStepMovingWindowWithInfo.step (``w``), for
-        steps whose replay slots the sampling kernel has already assigned."""
-        a = self._action(action)
-        check(_lib.lib().sb200_classic_env_window_step_f32(
-            self.TASK, _ptr(a), self.N, self.max_steps, self.seed, _ptr(self.state), _ptr(self.obs), _ptr(self.ep_step),
-            _ptr(self.episode), _ptr(self.obs_next), _ptr(self.reward), _ptr(self.done), C.byref(w.windows), _stream()),
-            'sb200_classic_env_window_step_f32')
-        return self._obs(self.obs), self.reward, self.done, {'obs_next': self.obs_next}
-
-    def close(self):
-        pass
 
 
 class CartPoleEnv(_ClassicEnv):
     """CartPole-v1: observation (x, x_dot, theta, theta_dot); two discrete actions as one-hot rows [N, 2] (index 1 pushes
     right); reward 1 per step; terminal when |x| > 2.4 or |theta| > 12 degrees."""
-    TASK, S, D, A, MAX_STEPS, ACTION_TYPE = _lib.CLASSIC_CARTPOLE, 4, 4, 2, 500, 'discrete'
+    KIND, S, D, A, MAX_STEPS, ACTION_TYPE = _lib.ENV_CARTPOLE, 4, 4, 2, 500, 'discrete'
     NAME = 'CartPole-v1'
 
 
 class PendulumEnv(_ClassicEnv):
     """Pendulum-v1: observation (cos theta, sin theta, theta_dot); one continuous action in [-1, 1], scaled to the torque
     2a; reward -(theta^2 + 0.1 theta_dot^2 + 0.001 torque^2); never terminal."""
-    TASK, S, D, A, MAX_STEPS, ACTION_TYPE = _lib.CLASSIC_PENDULUM, 2, 3, 1, 200, 'continuous'
+    KIND, S, D, A, MAX_STEPS, ACTION_TYPE = _lib.ENV_PENDULUM, 2, 3, 1, 200, 'continuous'
     NAME = 'Pendulum-v1'
 
 

@@ -2,7 +2,7 @@
 Pendulum-v1 with gym's classic_control dynamics, their episode cap, auto-reset and Philox reset draws.
 
 These tasks have no counterpart in the reference, which reaches them through gym; this module defines the semantics the
-device kernels implement (surreal_b200/csrc/classic_env.cu).  Physics runs in float64 on the given (float32) states;
+device kernels implement (surreal_b200/csrc/env.cu).  Physics runs in float64 on the given (float32) states;
 the reset draws are exact: the kernels form them in float32 with the same roundings.
 
 ``ClassicRef`` is also a batched host env (attributes N, D, A; numpy reset / step), so the host-env path of the agents
@@ -13,7 +13,7 @@ import numpy as np
 
 from oracle.philox import philox4x32_10
 
-CARTPOLE, PENDULUM = 0, 1                   # SB200_CLASSIC_*
+CARTPOLE, PENDULUM = 0, 1                   # task ids of this module
 CLASSIC_KEY = 0xD6E8FEB86659FD93            # the reset stream's key: env seed ^ CLASSIC_KEY
 REGISTERED_LIMIT = {CARTPOLE: 500, PENDULUM: 200}
 DIMS = {CARTPOLE: (4, 4, 2), PENDULUM: (2, 3, 1)}      # state, observation, action widths

@@ -1,6 +1,6 @@
 """CPU checks of the classic-control tasks: the float64 statement (tests/classic_ref.py) against the hand checks, the
 strict termination boundaries, the angle normalisation at +-pi, the episode cap and auto-reset; the env-name routing of
-the configs, launchers and agents; the sm_90a cross-compile of csrc/classic_env.cu."""
+the configs, launchers and agents; the sm_90a cross-compile of csrc/env.cu."""
 import copy
 import math
 import os
@@ -198,8 +198,8 @@ def test_kernels_cross_compile_for_sm_90a(tmp_path):
     assert 'arch=compute_90a,code=sm_90a' in build.FLAGS
     if not os.path.exists(build.NVCC):
         pytest.skip('nvcc not installed')
-    src = os.path.join(build.CSRC, 'classic_env.cu')
-    r = subprocess.run([build.NVCC] + build.FLAGS + ['-c', src, '-o', str(tmp_path / 'classic_env.o')],
+    src = os.path.join(build.CSRC, 'env.cu')
+    r = subprocess.run([build.NVCC] + build.FLAGS + ['-c', src, '-o', str(tmp_path / 'env.o')],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     # one kernel per task and variant, none spilling

@@ -1,4 +1,4 @@
-"""The classic-control tasks on the device (csrc/classic_env.cu, surreal_b200.env.classic):
+"""The classic-control tasks on the device (csrc/env.cu, surreal_b200.env.classic):
 
 1. kernels against the float64 statement of tests/classic_ref.py: one step from random states and actions at several
    actor counts, the termination boundaries, the reset draws bit for bit, episode counters and caps at staggered

@@ -75,7 +75,7 @@ def test_ctypes_signatures_match_header_prototypes():
 STRUCTS = {'sb200_mlp': 'Mlp', 'sb200_zfilter': 'ZFilter', 'sb200_rows': 'Rows', 'sb200_par': 'Par',
            'sb200_epochs': 'Epochs', 'sb200_windows': 'Windows', 'sb200_window_rows': 'WindowRows',
            'sb200_ppo_act': 'PPOAct', 'sb200_ddpg_act': 'DDPGAct', 'sb200_dqn_agent_act': 'DQNAgentAct',
-           'sb200_ppo_rollout': 'PPORollout', 'sb200_ssar': 'Ssar', 'sb200_param_noise_state': None}
+           'sb200_ppo_rollout': 'PPORollout', 'sb200_ssar': 'Ssar', 'sb200_env': 'Env', 'sb200_param_noise_state': None}
 
 
 def _header_structs():

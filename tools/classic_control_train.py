@@ -3,8 +3,8 @@
 
   train   each learning case of tests/classic_learning.py (the configs the learning tests commit): mean first-episode
           return of 64 fresh eval actors against env steps and training wall time (evaluations excluded);
-  env     the env step kernel (sb200_classic_env_step_f32) for CartPole-v1 and Pendulum-v1 at 1024, 16 384 and 65 536
-          actors beside sb200_synth_env_step_f32 (64-dim state, 8-dim action): CUDA events around replays of a graph
+  env     the env step (sb200_env_step_f32) of CartPole-v1 and Pendulum-v1 at 1024, 16 384 and 65 536 actors beside
+          the synthetic env's (64-dim state, 8-dim action): CUDA events around replays of a graph
           of 100 steps after warm-up, cycling through 16 random action sets.
 The card's name, power limit and maximum SM clock are read in the same run.
 
